@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the PIDM training step (BASELINE.json: "train samples/s Darcy 64x64 PIDM at 1/2/4/8 B200;
+"""Benchmark of the PIDM training step (BASELINE.json: "train samples/s Darcy 64x64 PIDM at 1/2/4/8 GPUs;
 residual-kernel HBM GB/s").
 
     python bench.py --gpus N --steps K --warmup W           # this repo's engine (libpidm kernels)
@@ -8,7 +8,9 @@ residual-kernel HBM GB/s").
 One step = one iteration of the reference training loop (main.py:157-183): q_sample -> Unet3D(dim=32) -> x0_hat ->
 Darcy residual -> data + residual loss -> backward -> clip(1.0) -> Adam(1e-4) -> EMA(0.99), batch 32 per GPU,
 synthetic 64x64 fields, random-init weights, bf16 GEMM operands / activations with fp32 accumulation.
-Prints ONE JSON line (rank 0)."""
+Prints ONE JSON line (rank 0).  `--dump-outputs DIR` also writes what the last timed step computed (loss terms, the
+updated weights, a fixed sample of the EMA weights) as DIR/<name>.npy, so that two builds can be compared output for
+output: the weights, the data and the noise stream are seeded, so the same arguments give the same inputs."""
 import argparse
 import json
 import os
@@ -36,12 +38,23 @@ FWD_GFLOP_PER_SAMPLE = 3.98      # SURVEY.md section 3.2 (conv3x3 2.40, 1x1 0.96
 
 
 def peaks():
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm_gbs=d['hbm_gbs'], bf16_tflops=d['bf16_tflops'], bf16_sustained=d.get('bf16_tflops_sustained'),
-                    source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    """NVIDIA data-sheet figures of the H100 SXM (700 W): HBM3 bandwidth and dense BF16 tensor rate.  A card with a
+    lower power limit clocks lower under sustained load, so shares of these peaks are upper-bound references."""
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source='H100 SXM data sheet (700 W)')
+
+
+def dump_outputs(path, out, eng):
+    """What the timed path computed in its last step: the loss terms TrainEngine.step returns, the updated flat weight
+    vector, and a fixed seeded sample of 2^20 entries of the EMA weights (the whole EMA vector would double the size)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    arrays = {'loss': out[0], 'data_loss': out[1], 'residual_abs': out[2], 'weights': eng.fp.flat}
+    ema = eng.fp.ema
+    idx = torch.randperm(ema.numel(), generator=torch.Generator().manual_seed(0))[:1 << 20].to(ema.device)
+    arrays['ema_weights_sample'] = ema[idx]
+    for name, v in arrays.items():
+        v = torch.as_tensor(v).detach().float().cpu().reshape(-1)
+        np.save(os.path.join(path, name + '.npy'), v.numpy())
 
 
 class ClockSampler(threading.Thread):
@@ -125,7 +138,7 @@ def run_reference(args, rank):
 
 def run_side_leg(args):
     """internal legs spawned by the b200 arm: `--impl cpu_extras` (BASELINE.md 3.5 CPU timings) and `--impl torch_cuda`
-    (the reference on the same B200 through stock PyTorch-CUDA)."""
+    (the reference on the same GPU through stock PyTorch-CUDA)."""
     ra = _ref_arm()
     out = ra.cpu_extras() if args.impl == 'cpu_extras' else ra.torch_cuda_baselines(PER_GPU_BATCH)
     print(json.dumps(out), flush=True)
@@ -295,7 +308,7 @@ def sampling_bench(model, dev, n_steps=250, batches=(16, 64, 256)):
 
 
 def mechanics_bench(dev, pk, batch=32, steps=10, warmup=4):
-    """BASELINE.json configs[2]: topology-optimisation (mechanics) 64x64, PIDM loss, batch 32, one B200 -- the model the
+    """BASELINE.json configs[2]: topology-optimisation (mechanics) 64x64, PIDM loss, batch 32, one GPU -- the model the
     reference trains for this study, Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True) (main.py:102-109,
     126), through TrainEngine (CUDA graph), device-timed; plus the matrix-free residual kernel against the HBM roofline
     on a working set larger than L2."""
@@ -337,7 +350,7 @@ def mechanics_bench(dev, pk, batch=32, steps=10, warmup=4):
          'finite': bool(torch.isfinite(out[0]).item())}
     try:      # the same convolution kernels at 128 .. 1024 channels: per-entry-point device time of one step
         agg = breakdown_one_step(eng, inp)
-        peak = pk['bf16_sustained'] or pk['bf16_tflops']
+        peak = pk['bf16_tflops']
         conv = agg.get('pidm_conv2d_tc_general')
         if conv and conv['flop']:
             tf = conv['flop'] / (conv['ms'] * 1e-3) / 1e12
@@ -355,7 +368,7 @@ def mechanics_bench(dev, pk, batch=32, steps=10, warmup=4):
     eng.close()
     del eng, model
     torch.cuda.empty_cache()
-    # ---- residual kernel alone, B = 8192 (1.24 GB working set >> 126 MB L2)
+    # ---- residual kernel alone, B = 8192 (1.24 GB working set >> 50 MB L2)
     Bs = 8192
     u = torch.randn(Bs, 2, 65, 65, device=dev) * 0.1
     rho = torch.rand(Bs, 64, 64, device=dev)
@@ -384,7 +397,7 @@ def mechanics_bench(dev, pk, batch=32, steps=10, warmup=4):
 
 
 def residual_kernel_sweep(pk):
-    """Standalone HBM sweep of the Darcy residual kernel at B = 32768 (2.7 GB working set >> 126 MB L2)."""
+    """Standalone HBM sweep of the Darcy residual kernel at B = 32768 (2.7 GB working set >> 50 MB L2)."""
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200._lib import call, stream
     Bs = 32768
@@ -436,6 +449,7 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-sampling', action='store_true')
     ap.add_argument('--no-mechanics', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the outputs of the last timed step as DIR/<name>.npy')
     args = ap.parse_args()
     rank = int(os.environ.get('RANK', '0'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
@@ -503,6 +517,8 @@ def main():
     clocks = sampler.stop()
     ms = e0.elapsed_time(e1)
     last_loss = float(out[0].item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, eng)
     log(f'device-resident: {ms / args.steps:.3f} ms/step')
     # ---- end to end: pinned host batch -> H2D -> step -> D2H loss, every step ------------------------------------
     for _ in range(3):
@@ -538,10 +554,10 @@ def main():
                         'pidm_conv2d_wgrad_tc')
         if name in tensor_names and d['flop'] > 0:
             ach = d['flop'] / (d['ms'] * 1e-3) / 1e12
-            peak = pk['bf16_sustained'] or pk['bf16_tflops']
+            peak = pk['bf16_tflops']
             roof = {'bound': 'tensor', 'kernel': name, 'achieved': ach, 'peak': peak, 'unit': 'TFLOP/s',
                     'frac': ach / peak, 'traffic': None, 'launches_per_step': d['calls'],
-                    'share_of_step_kernel_time': d['ms'] / total_ms, 'peak_source': pk['source'] + ', sustained figure',
+                    'share_of_step_kernel_time': d['ms'] / total_ms, 'peak_source': pk['source'],
                     'how': 'algorithmic 2*M*N*K FLOPs of every launch of this entry point in one step / device time of '
                            'those launches (each distinct call replayed from a CUDA graph, CUDA events on its stream)'}
             if d.get('bytes'):
@@ -550,19 +566,6 @@ def main():
                 roof['algorithmic_bytes'] = d['bytes']
                 roof['hbm_view'] = {'achieved': d['bytes'] / (d['ms'] * 1e-3) / 1e9, 'peak': pk['hbm_gbs'], 'unit': 'GB/s',
                                     'frac': d['bytes'] / (d['ms'] * 1e-3) / 1e9 / pk['hbm_gbs']}
-            prof = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles')
-            tpath = next((os.path.join(prof, f) for f in ('r02_step_traffic.json', 'r01_step_traffic.json')
-                          if os.path.exists(os.path.join(prof, f))), None)
-            if tpath:
-                prefix = {'pidm_conv2d_tc_general': 'conv_tc_kernel',
-                          'pidm_conv2d_wgrad_tc': 'wgrad'}.get(name)
-                if prefix:
-                    tr = json.load(open(tpath))
-                    roof['traffic'] = sum(v['dram_bytes'] for k, v in tr.items() if k.startswith(prefix))
-                    roof['traffic_note'] = ('STATIC, not measured in this run: dram__bytes_read.sum + dram__bytes_write.sum summed '
-                                            'over the launches of this kernel in ONE step, from the committed ncu launch '
-                                            f'list profiles/{os.path.basename(tpath)} (same command, scripts/gpu_final.sh); '
-                                            'compare with algorithmic_bytes')
         else:
             roof = {'bound': 'hbm', 'kernel': name, 'achieved': None, 'peak': pk['hbm_gbs'], 'unit': 'GB/s', 'frac': None,
                     'traffic': None, 'share_of_step_kernel_time': d['ms'] / total_ms}
@@ -608,7 +611,7 @@ def main():
                           'global_batch': world * B, 'per_gpu_batch': B, 'parallelism': f'dp{world}',
                           'cuda_graph': not args.no_graph,
                           'l2': 'no explicit flush: one step streams >1 GB of activations and gradients (dqkv alone 201 MB) '
-                                'through the 126 MB L2, so weights/activations are cold at every layer',
+                                'through the 50 MB L2, so weights/activations are cold at every layer',
                           'model_tflops_at_value': tflops, 'last_loss': last_loss},
                'clocks': clocks,
                'e2e': {'value': sps_e2e, 'unit': 'samples/s', 'ms_per_step': ms_e2e / args.steps,

@@ -1,4 +1,4 @@
-/* libpidm -- C ABI of the B200-native physics-informed-diffusion hot path.
+/* libpidm -- C ABI of the H100-native physics-informed-diffusion hot path.
  *
  * The reference (jhbastek/PhysicsInformedDiffusionModels) has no FFI: its boundary is the Python class
  * surface used by main.py / sample.py (SURVEY.md section 8b).  This header is the operator interface those
@@ -120,7 +120,7 @@ int pidm_conv2d_wgrad_simt(const void* x, const void* dy, float* dw, float* dbia
                            long long w_stride_n, long long w_stride_c, int dtype, void* stream);
 /* debugging aid: device buffer (>= 4096 int64) receiving a clock64 timeline of CTA 0 of every tensor-core conv launch */
 int pidm_debug_set_trace(void* buf);
-/* tcgen05 + TMA implicit-GEMM convolution, bf16 operands, fp32 TMEM accumulation; same contract as pidm_conv2d_simt
+/* wgmma + TMA implicit-GEMM convolution, bf16 operands, fp32 register accumulation; same contract as pidm_conv2d_simt
  * (requires Cin % 32 == 0, Cout % 32 == 0): stride-1/2 regular convolution (input sampled through TMA elementStrides) and the
  * stride-2 transposed gather (ConvTranspose forward / dgrad of the stride-2 conv) as 4 output-parity classes.
  * gn_sums (optional, [B, gn_groups, 2]): per-(sample, group) sum and sum of squares of the fp32 output, accumulated in
@@ -131,7 +131,7 @@ int pidm_conv2d_tc_general(const void* x, const void* w_packed, const float* bia
                            int transposed, float* gn_sums, int gn_groups, int gn_sums_zeroed, void* stream);
 int pidm_conv2d_tc_general_supported(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW, int stride,
                                      int pad, int transposed);
-/* wgrad on tcgen05: D[(tap,cA)][cB] = sum over grid pixels g of a[a_stride*g - pad + tap][cA] * b[g][cB], MN-major
+/* wgrad on the tensor cores (wgmma): D[(tap,cA)][cB] = sum over grid pixels g of a[a_stride*g - pad + tap][cA] * b[g][cB], MN-major
  * (pixel-strided) TMA operands, split over pixel ranges, red.global.add into dw[cA*s_row + cB*s_col + tap] (fp32,
  * ACCUMULATED).  Regular conv: a = x, b = dy.  ConvTranspose: a = dy (a_stride 2), b = x.  Rows cA >= CA_real (channel
  * padding) are dropped. */

@@ -1,11 +1,11 @@
 """Golden-vector generator.  TEST INFRASTRUCTURE ONLY; runs in the build container, not on the GPU box.
 
-Imports the UNMODIFIED reference modules from /root/reference through the import shims in
-oracle/ref_shims/ (SURVEY.md section 8c), runs them on seeded CPU inputs and writes small fixtures
+Imports the UNMODIFIED reference modules from a checkout of the original project (path in PIDM_REFERENCE) through
+the import shims in oracle/ref_shims/ (SURVEY.md section 8c), runs them on seeded CPU inputs and writes small fixtures
 to tests/golden/.  The weights are not stored: both sides rebuild them with
-oracle.pidm_oracle.make_test_state_dict(cfg, seed).
+oracle.pidm_oracle.make_test_state_dict(cfg, seed).  Large tensors are stored as oracle.pidm_oracle.golden_sample().
 
-    python oracle/make_golden.py            # rewrites tests/golden/*.pt
+    PIDM_REFERENCE=<checkout of the original project> python oracle/make_golden.py      # rewrites tests/golden/*.pt
 """
 import os
 import sys
@@ -18,7 +18,7 @@ from torch.nn.functional import pad as F_pad
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.environ.get('PIDM_REFERENCE', '/root/reference')
+REF = os.environ['PIDM_REFERENCE']
 # NOTE: the repo root must NOT be importable here: its `src/` drop-in package (a regular package) would shadow
 # the reference's `src/` (a namespace package) regardless of path order.
 sys.path = [p for p in sys.path if os.path.abspath(p or '.') != ROOT]
@@ -121,7 +121,7 @@ def main():
     for h in hs:
         h.remove()
     assert torch.equal(y, y_bxyc)
-    save('unet_darcy_fwd.pt', dict(x=x, t=t, y=y, **{'tap_' + k: v for k, v in taps.items()}))
+    save('unet_darcy_fwd.pt', dict(x=x, t=t, y=y, **{'tap_' + k: O.golden_sample(v) for k, v in taps.items()}))
 
     # ---- Darcy residual on given fields (A7-A9) -----------------------------------------------
     res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
@@ -160,7 +160,7 @@ def main():
             'ups.0.3.weight', 'ups.3.2.fn.norm.gamma', 'final_conv.1.weight', 'final_conv.1.bias',
             'downs.3.1.block2.norm.weight', 'ups.1.0.res_conv.weight']
     named = dict(model.named_parameters())
-    grads = {'grad_' + k: named[k].grad.clone() for k in keys}
+    grads = {'grad_' + k: O.golden_sample(named[k].grad) for k in keys}
     gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).float()
     nograd = sorted(k for k, p in named.items() if p.grad is None)
     save('darcy_loss_mean.pt', dict(x0=x0, t=t_l, noise=e_l, loss=loss.detach(), data_loss=torch.tensor(data_l),

@@ -6,13 +6,13 @@ path: only `tests/`, `__graft_entry__.smoke()` and `bench.py` (cpu_baseline / `-
 legs) may import it.  The product package never imports anything from `oracle/`.
 
 Pinned against the real reference: `oracle/make_golden.py` imports the untouched reference modules
-from /root/reference (through the import shims in `oracle/ref_shims/`), runs them on seeded inputs
+from the original project (through the import shims in `oracle/ref_shims/`), runs them on seeded inputs
 and writes `tests/golden/*.pt`; `tests/test_oracle_golden.py` checks every function below against
 those fixtures.  Where the reference's own third-party dependency is absent (findiff stencil
 tables, solidspy Q4 stiffness, the authors' mesh files) parity is pinned analytically only -- see
 DESIGN.md "Oracle" for the list.
 
-Each function cites the reference file:line it follows (paths relative to /root/reference).
+Each function cites the reference file:line it follows (paths relative to the original project's root).
 """
 import math
 from collections import OrderedDict
@@ -23,6 +23,17 @@ import torch.nn.functional as F
 # --------------------------------------------------------------------------------------------
 # A1/A2  schedule tables            (src/denoising_utils.py:315-370, extract :302-306)
 # --------------------------------------------------------------------------------------------
+
+
+def golden_sample(t, n=8192):
+    """Fixed, seeded sample of n elements of a flattened tensor (all of it when it is smaller).  The large activation
+    taps and weight gradients in tests/golden are stored this way so that every fixture stays small; the tests compare
+    the same elements of what they compute."""
+    flat = t.reshape(-1)
+    if flat.numel() <= n:
+        return flat.clone()
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n]
+    return flat[idx.to(flat.device)]
 
 
 def cosine_betas(n_steps, s=0.008):

@@ -4,13 +4,12 @@ Runs the UNMODIFIED reference modules (jhbastek/PhysicsInformedDiffusionModels `
 oracle/ref_shims/ (SURVEY.md section 8c: einops_exts, rotary_embedding_torch, findiff, solidspy, matplotlib, imageio):
 
 * on the host CPU cores  -> `bench.py --impl reference` / the `cpu_baseline` block       (kind = "reference")
-* on the B200 through stock PyTorch-CUDA (cuDNN / cuBLAS) -> the `torch_cuda_baseline` block, the comparison point
+* on the GPU through stock PyTorch-CUDA (cuDNN / cuBLAS) -> the `torch_cuda_baseline` block, the comparison point
   SURVEY 2b / BASELINE.md 3.7 ask for (the reference ships no GPU kernels of its own)
 
-The reference sources are NOT part of this repository: `__graft_entry__.build()` copies /root/reference/{src,*.py,
-model.yaml} into the git-ignored baseline/_ref/reference/ when /root/reference exists (build container); the directory
-travels to the GPU box with the snapshot.  When it is absent every function here falls back to the oracle port
-(oracle/pidm_oracle.py, kind = "port") and says so.
+The reference sources are NOT part of this repository.  A user who wants the unmodified reference in these legs places
+a checkout of it (its src/, *.py and model.yaml) in the git-ignored baseline/_ref/reference/.  When that directory is
+absent every function here falls back to the oracle port (oracle/pidm_oracle.py, kind = "port") and says so.
 
 This module must be loaded BY FILE PATH in a process whose sys.path does not contain the repo root: the repo's `src/`
 drop-in package (a regular package) would shadow the reference's `src/` (a namespace package) regardless of order.
@@ -257,7 +256,7 @@ def cpu_extras(budget_s=120.0):
 
 
 def torch_cuda_baselines(batch=32, steps=10, warmup=3):
-    """The same reference code on the B200 via stock PyTorch-CUDA kernels: eager fp32 (TF32 off), TF32, bf16 autocast
+    """The same reference code on the GPU via stock PyTorch-CUDA kernels: eager fp32 (TF32 off), TF32, bf16 autocast
     (+ channels_last for the port), and the port under a CUDA graph.  Device-timed per step."""
     import torch
     assert torch.cuda.is_available()

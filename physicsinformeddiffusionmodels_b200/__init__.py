@@ -1,4 +1,4 @@
-"""B200-native engine for the physics-informed-diffusion hot path (see DESIGN.md).
+"""H100-native engine for the physics-informed-diffusion hot path (see DESIGN.md).
 
 Host code is Python/PyTorch (device memory, streams, autograd bookkeeping, torch.distributed);
 every per-step operation is a hand-written sm_100a CUDA kernel in libpidm.so behind the C ABI of

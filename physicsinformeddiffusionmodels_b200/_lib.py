@@ -84,7 +84,7 @@ _VALUE_RETURN = {'pidm_pack_entry_size', 'pidm_pack_pair_entry_size', 'pidm_mlp_
                  'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported'}
 
 if not os.path.exists(LIB_PATH):
-    raise ImportError(f'{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_100a). '
+    raise ImportError(f'{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). '
                       'There is no CPU / PyTorch fallback for the PIDM hot path.')
 
 _lib = ctypes.CDLL(LIB_PATH)

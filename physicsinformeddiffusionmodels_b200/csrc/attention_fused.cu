@@ -314,8 +314,7 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
 }
 
 // ---- out[n,h,e] = sum_d softmax_d(q[n,:])[d] * s * ctx[h][d][e],  q projected from xn --------------------------------
-constexpr int LFO_STAGES = 2;      // 61 KB per CTA: three CTAs (24 warps) per SM -- ncu (r02): the kernel is bound by
-                                   // fixed-latency dependencies (stall_wait 2.0 per issue at 16 warps per SM)
+constexpr int LFO_STAGES = 2;      // 61 KB per CTA: three CTAs (24 warps) per SM
 __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
                                                       const float* __restrict__ ctx, __nv_bfloat16* __restrict__ out, int N,
                                                       int chunk_px, float scale) {
@@ -383,8 +382,8 @@ __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __res
 
 // ---- backward per pixel: dq | dk | dv from xn, dout, ctx, dctx and the saved column statistics -------------------------
 // 217 registers (the nine loop-invariant 32x32 B-operand fragment sets live in registers): one CTA = 8 warps per SM.
-// Capping the kernel at 128 registers for two CTAs per SM was measured (round 2): ptxas spills ~70 fragment registers to
-// local memory and the 64x64 layer goes from 104 to 154 us -- occupancy does not pay for re-reading the operands.
+// Capping the kernel at 128 registers for two CTAs per SM makes ptxas spill ~70 fragment registers to local memory:
+// occupancy does not pay for re-reading the operands.
 constexpr int LFB_ROWS = 16;
 constexpr int LFB_STAGES = 4;
 constexpr int LFB_STAGE_ELEMS = 2 * LFB_ROWS * LW_PITCH;          // xn tile | dout tile
@@ -554,7 +553,7 @@ static int laf_attrs() {
 
 static int laf_chunk_px(int B, int N, int ctas_per_sm) {
     // chunks are per sample: k chunks per sample with B * k <= resident CTA slots (one wave), 32-pixel granularity
-    int k = (148 * ctas_per_sm) / B;
+    int k = (num_sms() * ctas_per_sm) / B;
     if (k < 1) k = 1;
     int px = ((N + k - 1) / k + 31) / 32 * 32;
     if (px < 64) px = 64;

@@ -6,8 +6,8 @@
 //   dP = dout v^T   dS = P * (dP - sum_j P dP)      dq = s dS k     dk = s dS^T q     dv = P^T dout
 //
 // The CUDA-core version of these kernels (attention.cu: attn_fwd_kernel / attn_bwd_kernel, still used for fp32
-// activations and for fewer than 64 tokens) spends ~3.8 k shared-memory loads per thread on five 64x64x32 products
-// (19.5 us forward / 39 us backward per step at batch 32); here the five products are 40 MMAs per warp, the probabilities
+// activations and for fewer than 64 tokens) spends ~3.8 k shared-memory loads per thread on five 64x64x32 products;
+// here the five products are 40 MMAs per warp, the probabilities
 // never leave the registers in forward, and backward stages P and dS once (bf16) for the two key-side products.
 #define PIDM_PDL_GROUP 1
 #include "common.cuh"

@@ -1,12 +1,12 @@
 // Linear attention (reference unet_model.py:286-297) on the tensor cores for bf16 activations, heads = 8, dim_head = 32.
 //
-// The per-(sample, head) products are 32x32 blocks -- too small for tcgen05 (UMMA M >= 64) and HBM-bound anyway
+// The per-(sample, head) products are 32x32 blocks -- too small for wgmma (M = 64 per warpgroup) and HBM-bound anyway
 // (the whole qkv row of a pixel, 8 heads x 3 x 32 channels = 1536 B, is streamed once), so these kernels use
 // warp-level mma.sync m16n8k16 (bf16 in, fp32 accumulate) with ldmatrix-fed fragments.  One warp per head, and the
 // eight warps of a CTA are fully DECOUPLED: every warp streams its own head's 64-byte slice of each pixel row through
 // a private cp.async ring in shared memory, transforms it in place (one lane per pixel row) and feeds the tensor cores;
 // only __syncwarp is used in the loops.  (The first version staged whole 512-byte rows for all heads behind two
-// __syncthreads per tile: ncu showed 12 % occupancy with every warp stalled on the barriers / scoreboard.)
+// __syncthreads per tile, which left every warp stalled on the barriers.)
 //   la_ctx_mma<0>: ctx[h][d][e]  += sum_n exp(k[n,d]-M_d) v[n,e]      (scaled by 1/(Z_d N) in the epilogue)
 //   la_ctx_mma<1>: dctx[h][d][e] += sum_n softmax_d(q[n,:])[d]*s * dout[n,e]
 //   la_out_mma   : out[n,h,e]     = sum_d softmax_d(q[n,:])[d]*s * ctx[h][d][e]
@@ -358,7 +358,7 @@ static int la_mma_attrs() {
 // pixels per CTA: about two CTAs per SM over the whole batch, a multiple of 32, never more than the image
 static int la_chunk_px(int B, int N, int ctas_per_sm) {
     // chunks are per sample: k chunks per sample with B * k <= resident CTA slots (one wave), 32-pixel granularity
-    int k = (148 * ctas_per_sm) / B;
+    int k = (num_sms() * ctas_per_sm) / B;
     if (k < 1) k = 1;
     int px = ((N + k - 1) / k + 31) / 32 * 32;
     if (px < 64) px = 64;

@@ -8,8 +8,8 @@
 //
 // Why: at these sizes a (sample, head) problem is 64..256 tokens x 96 channels = 12..48 KB, and the streaming
 // formulation (column statistics -> context -> output, and dcontext -> per-token gradients for the backward: 3 + 2
-// dependent kernels plus two memsets, each a grid-wide pass) was pure launch / dependency latency: 16.6-18.7 us
-// forward and 20.1-20.7 us backward per layer for 6..25 MB of traffic.  Here the whole chain runs inside one CTA on
+// dependent kernels plus two memsets, each a grid-wide pass) is pure launch / dependency latency for 6..25 MB of
+// traffic.  Here the whole chain runs inside one CTA on
 // CUDA cores (the products are 32-wide: 2 MFLOP per CTA), 256 CTAs = one wave.
 // (A one-CTA backward was built and measured too: no faster than the streaming backward at 64 tokens, slower at 256.)
 #define PIDM_PDL_GROUP 1
@@ -177,8 +177,6 @@ static size_t ls_smem(int N, bool bwd) {
 }
 
 // entry points used by attention.cu
-// Measured at B = 32 (graph-replayed, us per layer, streaming kernels -> this file):
-//   N =  64: forward 16.3 -> 8.7, backward 20.0 -> 19.9        N = 256: forward 18.5 -> 26.9, backward 20.7 -> 48.3
 // At 256 tokens the 32-wide products (0.7 GFLOP per layer) are CUDA-core FLOP-bound here while the streaming kernels
 // run them on mma.sync, so only the 8x8 level takes this path, and only where it wins (forward).
 bool la_small_supported(int N, int dtype) { return dtype == PIDM_BF16 && N >= 32 && N <= 64; }

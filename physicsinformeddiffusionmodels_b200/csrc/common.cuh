@@ -1,4 +1,4 @@
-// Shared device/host helpers for libpidm (sm_100a only).
+// Shared device/host helpers for libpidm (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -117,10 +117,13 @@ __device__ __forceinline__ float silu_grad_f(float z) {
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// streaming multiprocessors of the current device (queried once; sizes persistent grids and one-wave splits)
+int num_sms();
+
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------------------
 // The step is a chain of ~420 dependent kernels, many of them a few microseconds long: the kernel-to-kernel launch
 // latency is a first-order cost.  Kernels launched through launch_pdl() may start while their predecessor is still
-// draining: they run their prologue (barrier init, TMEM allocation, tensor-map prefetch, parameter loads that do not
+// draining: they run their prologue (barrier init, tensor-map prefetch, parameter loads that do not
 // depend on the predecessor) and then block in pdl_wait() until the predecessor grid has completed and flushed.
 // Every kernel calls pdl_trigger() first so that ITS successor can be scheduled as early as possible.  Both
 // instructions are no-ops for kernels launched without the attribute.  PIDM_PDL=0 disables the attribute.
@@ -128,9 +131,8 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // PIDM_PDL = bit mask of kernel groups launched with the attribute: 0 conv / wgrad / norm, 1 attention,
-// 2 element-wise, 3 linear / optimizer / residual.  Default 1: on one B200 the step takes 4.34 ms without PDL, 4.02 ms
-// with group 0 only, 4.15 ms with all groups (kernels whose first instruction is the wait gain nothing and their
-// early-scheduled CTAs only take SM slots from the forked weight-gradient stream).
+// 2 element-wise, 3 linear / optimizer / residual.  Default 1: group 0 only (kernels whose first instruction is the
+// wait gain nothing and their early-scheduled CTAs only take SM slots from the forked weight-gradient stream).
 #ifndef PIDM_PDL_GROUP
 #define PIDM_PDL_GROUP 0
 #endif

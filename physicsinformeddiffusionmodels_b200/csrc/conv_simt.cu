@@ -1,7 +1,7 @@
 // Generic implicit-GEMM convolution on NHWC activations (fp32 accumulate, CUDA cores).
 // This is the geometry-complete path: any KHxKW / stride / padding, regular ("gather from input") or
 // transposed addressing, forward / dgrad / wgrad, fp32 or bf16 activations.  It is the parity anchor
-// for the tcgen05 tile kernel in conv_tc.cu (which takes the stride-1 layers that carry the FLOPs) and
+// for the tensor-core (wgmma) tile kernel in conv_tc.cu (which takes the stride-1 layers that carry the FLOPs) and
 // runs the layers that kernel does not cover (7x7 stem, 4x4/s2 down, 4x4/s2 transposed up, wgrad).
 //
 //   y[m, n] = sum_k A(m, k) * Wp[n, k] (+ bias[n]) (+ residual[m, n]),  m = (b, oh, ow),  k = tap*Cin + c
@@ -196,7 +196,7 @@ struct PackEntry {
 };
 
 // two consecutive packed channels per thread (Cpad is even): 32-bit index arithmetic (the 64-bit divisions of the first
-// version cost more than the memory traffic: 62 us for 83 MB), one 4- or 8-byte store
+// version cost more than the memory traffic), one 4- or 8-byte store
 template <typename T>
 __global__ void pack_weights_kernel(const PackEntry* __restrict__ table) {
     const PackEntry e = table[blockIdx.y];
@@ -224,8 +224,8 @@ __global__ void pack_weights_kernel(const PackEntry* __restrict__ table) {
 // master weights: it reads the block as 32 contiguous runs of 32 * taps floats, keeps it in shared memory in the
 // activation dtype and writes the forward operand Wp_f[co][tap * Cin + ci] and the dgrad operand
 // Wp_d[ci][tap' * Cout + co] (tap' = taps - 1 - tap for stride-1 layers) as 64 / 128-byte row segments.  The generic
-// kernel above reads every source element twice with a stride of `taps` floats between neighbouring threads
-// (68 us per step for 10.4 M parameters); this one moves 41.5 MB in and 2 x 20.8 MB out once.
+// kernel above reads every source element twice with a stride of `taps` floats between neighbouring threads; this one
+// moves 41.5 MB in and 2 x 20.8 MB out once.
 struct PackPairEntry {
     const float* src;
     void* dst_f;
@@ -346,7 +346,7 @@ extern "C" int pidm_conv2d_wgrad_simt(const void* x, const void* dy, float* dw, 
     long long M = (long long)B * Ho * Wo;
     int K = KH * KW * Cin;
     int tiles = ceil_div(K, CS_BM) * ceil_div(Cout, CS_BN);
-    int splits = (148 * 4 + tiles - 1) / tiles;
+    int splits = (num_sms() * 4 + tiles - 1) / tiles;
     long long max_splits = (M + 255) / 256;
     if (splits > max_splits) splits = (int)max_splits;
     if (splits < 1) splits = 1;

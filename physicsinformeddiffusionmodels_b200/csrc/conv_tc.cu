@@ -1,5 +1,5 @@
-// Convolutions of the U-Net on NHWC bf16 activations as implicit GEMMs on the 5th-generation tensor cores (tcgen05),
-// operands staged by TMA, fp32 accumulators in tensor memory (TMEM).
+// Convolutions of the U-Net on NHWC bf16 activations as implicit GEMMs on the Hopper tensor cores (wgmma), operands
+// staged by TMA through an mbarrier ring, fp32 accumulators in registers.
 //
 //   y[b,h,w,n] = sum_{r,q,c} x[b, s*h+r-pad, s*w+q-pad, c] * Wp[n][(r*KW+q)*Cin + c] (+ bias[n]) (+ residual[b,h,w,n])
 //
@@ -16,95 +16,25 @@
 //                    that one shared-memory tile (a shift of 8 pixels = one swizzle period), so L2 -> SM operand
 //                    traffic drops from KH*KW to KW*(16+KH-1)/16 tiles per output tile.
 //   The B operand (K-major packed weights) is a 2-D TMA box per tap, or resident in shared memory for the whole kernel
-//   when the layer has a single n-tile.  Both land in the canonical K-major swizzled layout that the UMMA descriptors
+//   when the layer has a single n-tile.  Both land in the canonical K-major swizzled layout that the wgmma descriptors
 //   expect: no thread ever touches the operands.
 //
-// Persistent, warp-specialised (256 threads, one CTA per SM, tiles walked with stride gridDim.x):
-//   warps 0,2,3  TMA producers (one elected lane each, K-step i belongs to producer i % 3), <= 12-stage mbarrier ring
+// Persistent, warp-specialised (512 threads, one CTA per SM, tiles walked with stride gridDim.x):
+//   warps 0-3    TMA producers (one elected lane each, K-step i belongs to producer i % 4), <= 12-stage mbarrier ring
 //                that runs across tile boundaries
-//   warp 1       MMA issuer: ONE thread, tcgen05.mma.cta_group::1.kind::f16 M128 x BN x K16, descriptors advanced by
-//                integer adds; tcgen05.commit releases ring stages / publishes the accumulator
-//   warp 2       also allocates TMEM (2 x BN columns: the epilogue of tile i overlaps the mainloop of tile i+1)
-//   warps 4-7    epilogue: tcgen05.ld -> +bias +residual -> GroupNorm sum / sum-of-squares (optional) -> bf16 ->
-//                XOR-swizzled smem transpose -> 64/128-byte coalesced row-segment stores
-// What bounds it (clock64 traces, scripts/trace_conv.py; profiles/r02_conv_splitk_trace.txt): the K-step cadence of the
-// main loop is set by the copy engine, not by the tensor pipe -- ~427 cycles per (128-row im2col box + weight box) at the
-// 8x8 level whatever the n-tile width, ~770 cycles per 144-row halo box of 64-byte rows at Cin = 32 (5.3 cycles per row) --
-// while the four to six MMAs of a K-step issue in 190-290 cycles; a launch costs >= 4.3 us (1x1 conv at 8x8).
-// Two alternatives were built and measured in round 2 and are NOT in this file (git history: c60b6e5, c86e22a): split-K
-// over a thread-block cluster with a DSMEM exchange of the partial accumulators (main loop 3.3x shorter, but the cluster
-// barrier absorbs ~6.5 k cycles of CTA start skew and the exchange 5-12 k: 11.9 -> 12.8 us per 8x8x256 layer) and
-// cp.async producer warps for the A operand instead of TMA (2100-2400 cycles per K-step: 12.8 -> 44-49 us).  Carrying
-// them as opt-in paths cost the default path 3 % (register pressure in the issue loops), so they were removed.
-#include "common.cuh"
+//   warps 4-11   two consumer warpgroups, wgmma.m64nBNk16 on rows 0-63 / 64-127 of the tile, descriptors advanced by
+//                integer adds; each warp releases a ring stage once the wgmma group that read it has retired
+//   warps 12-15  epilogue: parked fp32 tile -> +bias +residual -> GroupNorm sum / sum-of-squares (optional) -> bf16 ->
+//                XOR-swizzled smem transpose -> 64/128-byte coalesced row-segment stores; it overlaps the main loop of
+//                the next tile
+#include "hopper.cuh"
 #include "pidm.h"
-#include <cuda.h>
 #include <stdlib.h>
 
 namespace pidm {
 
 constexpr int TC_BM = 128;
-constexpr int TC_THREADS = 256;
-
-__device__ __forceinline__ uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void tc_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void tc_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(tc_smem_u32(bar)), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
-                                            int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-            tc_smem_u32(dst)),
-        "l"(map), "r"(tc_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            tc_smem_u32(dst)),
-        "l"(map), "r"(tc_smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-// K-major, swizzled UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4, [16,30) LBO>>4 (unused for swizzled K-major, 1), [32,46) SBO>>4 = 8 rows * swizzle span,
-//   [46,48) version = 1, [61,64) layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B
-template <int SWIZZLE_BYTES>
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr) {
-    constexpr uint64_t layout = SWIZZLE_BYTES == 128 ? 2 : (SWIZZLE_BYTES == 64 ? 4 : 6);
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)((8 * SWIZZLE_BYTES) >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= layout << 61;
-    return d;
-}
+constexpr int TC_THREADS = 512;
 
 struct TcClass {             // one output-parity class of a transposed (stride-2) gather: <= 16 taps
     int n_taps, off_h, off_w;
@@ -199,40 +129,39 @@ template <int BN, int BK>
 struct TcCfg {
     static constexpr int SW = BK * 2;                                     // swizzle span in bytes (128 or 64)
     static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int ACC_STAGES = 2;                                  // TMEM accumulators: epilogue(i) || mainloop(i+1)
-    static constexpr int TMEM_COLS = ACC_STAGES * BN;                     // 64 .. 512, power of two
+    static constexpr int ACC_PITCH = BN + 4;                              // fp32 staging row: conflict-free float4 rows
+    static constexpr int ACC_BYTES = TC_BM * ACC_PITCH * 4;
+    static constexpr int SMEM_BYTES = 227 * 1024;                         // the per-block maximum of sm_90
 };
-// persistent kernel, one CTA per SM: the operand ring takes (almost) all shared memory so that the TMA producers
-// run many K-steps (and tiles) ahead of the tensor pipe; latency is hidden by the ring, not by co-resident CTAs
+// persistent kernel, one CTA per SM: the operand ring takes most of the shared memory so that the TMA producers run
+// many K-steps (and tiles) ahead of the tensor cores; latency is hidden by the ring, not by co-resident CTAs
 constexpr int TC_MAX_STAGES = 12;
 constexpr int TC_RING_STAGES = 12;      // default ring depth (PIDM_TC_STAGES overrides)
-constexpr int TC_OPERAND_BYTES = 200 * 1024;                              // resident weights + ring
-constexpr int TC_SMEM_BYTES = TC_OPERAND_BYTES + 1024 /*align slack*/ + 512 /*barriers*/ + 4 * 4096 /*epilogue staging*/;
 
 // Persistent, warp-specialised implicit-GEMM convolution.  Tiles (m_tile, n_tile, class) are walked with a static
 // stride of gridDim.x by all three roles in lock step:
-//   warp 0   TMA producer : keeps the smem ring full across tile boundaries
-//   warp 1   MMA issuer   : tcgen05.mma into TMEM accumulator (tile & 1); commits free ring slots / publish the tile
-//   warp 2   TMEM allocator
-//   warps 4-7 epilogue    : drain accumulator (tile & 1) while the tensor pipe already works on the next tile
+//   warps 0-3   TMA producers: keep the smem ring full across tile boundaries
+//   warps 4-11  two consumer warpgroups: wgmma of output rows 0-63 / 64-127 of the tile into register accumulators,
+//               then the fp32 tile is parked in shared memory (acc_full) and the next tile's main loop starts
+//   warps 12-15 epilogue: drain the parked tile while the tensor cores already work on the next one
 template <int BN, int BK>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap map_x,
                                                                 const __grid_constant__ CUtensorMap map_w, TcParams p) {
     using Cfg = TcCfg<BN, BK>;
     extern __shared__ unsigned char smem_raw[];
     // 1024-byte aligned operand ring (required by the 128B swizzle atoms)
-    const uint32_t raw_addr = tc_smem_u32(smem_raw);
+    const uint32_t raw_addr = smem_u32(smem_raw);
     const uint32_t pad_bytes = (1024 - (raw_addr & 1023)) & 1023;
     unsigned char* wres = smem_raw + pad_bytes;              // resident weights (res_bytes, may be 0)
     unsigned char* ring = wres + p.res_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + pad_bytes + p.operand_bytes);
     uint64_t* full = bars;                                   // [TC_MAX_STAGES]
     uint64_t* empty = bars + TC_MAX_STAGES;                  // [TC_MAX_STAGES]
-    uint64_t* acc_full = bars + 2 * TC_MAX_STAGES;           // [ACC_STAGES]
-    uint64_t* acc_empty = acc_full + Cfg::ACC_STAGES;        // [ACC_STAGES]
-    uint64_t* wfull = acc_empty + Cfg::ACC_STAGES;           // resident weights have landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
+    uint64_t* acc_full = bars + 2 * TC_MAX_STAGES;           // the accumulator tile is parked in shared memory
+    uint64_t* acc_empty = acc_full + 1;                      // ... and has been read back by the epilogue
+    uint64_t* wfull = acc_empty + 1;                         // resident weights have landed
     unsigned char* stage_base = smem_raw + pad_bytes + p.operand_bytes + 512;   // 4 warps x 4 KB epilogue staging
+    float* acc_tile = reinterpret_cast<float*>(stage_base + 4 * 4096);          // [TC_BM][ACC_PITCH] fp32
     const int n_stages = p.stages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -245,32 +174,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     }
     if (warp == 1 && lane == 0) {
-        for (int s = 0; s < n_stages; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 1); }
-        for (int s = 0; s < Cfg::ACC_STAGES; ++s) { tc_mbar_init(&acc_full[s], 1); tc_mbar_init(&acc_empty[s], 128); }
-        tc_mbar_init(wfull, 1);
+        // a ring stage is free once all 8 consumer warps have retired the wgmmas that read it
+        for (int s = 0; s < n_stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+        mbar_init(acc_full, 256);
+        mbar_init(acc_empty, 128);
+        mbar_init(wfull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {   // TMEM allocation (power of two >= 32 columns), whole warp executes
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(tmem_slot)),
-                     "r"(Cfg::TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();                 // prologue done; everything below reads what the previous kernel wrote
 
-    if (warp == 0 || warp == 2 || warp == 3) {
-        // ===== TMA producers: three warps, one elected lane each, K-step `git` belongs to producer git % 3 ===========
-        // (a single thread can only issue a K-step every ~600 cycles -- wait + expect_tx + 2 TMA -- which starved the
-        //  tensor pipe on the small-channel layers; the three issue streams are independent)
-        const uint32_t pidx = (warp == 0) ? 0u : (uint32_t)(warp - 1);
+    if (warp < 4) {
+        // ===== TMA producers: four warps, one elected lane each, K-step `git` belongs to producer git % 4 ============
+        // (a single thread can only issue a K-step every ~600 cycles -- wait + expect_tx + 2 TMA -- which starves the
+        //  tensor cores on the small-channel layers; the issue streams are independent)
+        const uint32_t pidx = (uint32_t)warp;
         if (elect_one()) {
             if (p.resident && pidx == 0) {
                 // all K tiles of the (single) n-tile: [tap][kc] boxes of BN x BK
                 const int n_k = p.KH * p.KW * kc_per_tap;
-                tc_mbar_expect_tx(wfull, (uint32_t)(n_k * Cfg::B_BYTES));
+                mbar_expect_tx(wfull, (uint32_t)(n_k * Cfg::B_BYTES));
                 for (int i = 0; i < n_k; ++i) tma_load_2d(wres + (size_t)i * Cfg::B_BYTES, &map_w, wfull, i * BK, 0);
             }
             // ring position (stage, phase, whose turn) is carried incrementally: no integer divisions in the loop
@@ -303,9 +226,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     int kcol = ktap * p.Cin;
                     for (int kc = 0; kc < kc_per_tap; ++kc, kcol += BK) {
                         if (turn == pidx) {
-                            tc_mbar_wait(&empty[st], ph ^ 1);
+                            mbar_wait(&empty[st], ph ^ 1);
                             if (tracing && git < 1000) p.trace[6144 + git] = clock64();
-                            tc_mbar_expect_tx(&full[st], (uint32_t)p.stage_bytes);
+                            mbar_expect_tx(&full[st], (uint32_t)p.stage_bytes);
                             tma_load_4d(a_dst, &map_x, &full[st], kc * BK, ww0 + dw, hh0 + dh, b0);
                             if (!p.resident) {
                                 unsigned char* b_dst = a_dst + p.a_bytes;
@@ -315,7 +238,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                             }
                         }
                         ++git;
-                        if (++turn == 3u) turn = 0;
+                        if (++turn == 4u) turn = 0;
                         if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_dst = ring; } else a_dst += p.stage_bytes;
                     }
                 }
@@ -323,84 +246,77 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 if (tile_m >= p.m_tiles) { tile_m -= p.m_tiles; ++rest; }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-        // A,B K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-        constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                                   ((uint32_t)(TC_BM >> 4) << 24);
-        // One elected thread runs the whole loop.  The loop body is kept free of integer divisions and descriptor
-        // re-encoding: a clock64 trace showed ~500 cycles of scalar overhead per K-step in the naive form, more than
-        // the MMAs themselves on the narrow (N = 32) tiles.
-        if (elect_one()) {
-            const bool tracing = p.trace != nullptr && blockIdx.x == 0;
-            // descriptor = hi(constant: SBO, version, swizzle) : lo(start >> 4 | LBO = 1 << 16)
-            const uint32_t desc_hi = (uint32_t)(umma_desc<Cfg::SW>(0) >> 32);
-            const uint32_t ring_lo = ((tc_smem_u32(ring) & 0x3FFFF) >> 4) | (1u << 16);
-            const uint32_t wres_lo = ((tc_smem_u32(wres) & 0x3FFFF) >> 4) | (1u << 16);
-            const uint32_t stage_lo = (uint32_t)p.stage_bytes >> 4;
-            const uint32_t a_shift_lo = (uint32_t)(p.TW * BK * 2) >> 4;      // one tile row of pixels
-            const uint32_t b_off_lo = (uint32_t)p.a_bytes >> 4;
-            constexpr uint32_t b_tile_lo = (uint32_t)Cfg::B_BYTES >> 4;
-            const uint32_t res_j_lo = (uint32_t)(p.KW * kc_per_tap) * b_tile_lo;   // resident: next kernel row
-            const int groups_m0 = p.rg ? p.KW : p.KH * p.KW;
-            const int nb = p.nb;
-            const bool resident = p.resident != 0;
-            uint32_t st = 0, ph = 0, a_lo = ring_lo, git = 0;
-            int rest = blockIdx.x / p.m_tiles, tile_m = blockIdx.x % p.m_tiles;
-            const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
-            int lt = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-                const int n_iters = ((p.mode == 0) ? groups_m0 : p.cls[rest / p.n_tiles].n_taps) * kc_per_tap;
-                const int as = lt & 1;
-                if (tracing && lt < 64) p.trace[1024 + lt * 4] = clock64();
-                if (lt == 0 && resident) tc_mbar_wait(wfull, 0);
-                tc_mbar_wait(&acc_empty[as], ((lt >> 1) & 1) ^ 1);   // epilogue has drained this accumulator
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (tracing && lt < 64) p.trace[1024 + lt * 4 + 1] = clock64();
-                const uint32_t tmem_acc = tmem_base + (uint32_t)(as * BN);
-                uint32_t accum = 0;
-                uint32_t res_lo = wres_lo;                           // resident weights: tile (it) of kernel row 0
-                for (int it = 0; it < n_iters; ++it, res_lo += b_tile_lo) {
-                    tc_mbar_wait(&full[st], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    if (tracing && git < 1000) p.trace[4096 + git * 2] = clock64();
-                    uint32_t aj = a_lo;
-                    uint32_t bj = resident ? res_lo : a_lo + b_off_lo;
-                    const uint32_t bj_step = resident ? res_j_lo : b_tile_lo;
-                    for (int j = 0; j < nb; ++j, aj += a_shift_lo, bj += bj_step) {
+    } else if (warp < 12) {
+        // ===== consumers: warpgroup cg computes output rows [64 cg, 64 cg + 64) of every tile =====
+        // The loop body is kept free of integer divisions and descriptor re-encoding: descriptors are advanced by adds
+        // to their low word (16-byte units).  One wgmma group is kept in flight: the stage of K-step i - 1 is released
+        // once the group of K-step i has been issued and the older one has retired.
+        const int cg = (warp - 4) >> 2;
+        const bool tracing = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 128;
+        constexpr uint32_t desc_hi = gmma_desc_hi<Cfg::SW>();
+        const uint32_t row_half_lo = (uint32_t)(64 * BK * 2) >> 4;           // 64 pixel rows of the A tile
+        const uint32_t ring_lo = gmma_desc_lo(smem_u32(ring), 16) + (uint32_t)cg * row_half_lo;
+        const uint32_t wres_lo = gmma_desc_lo(smem_u32(wres), 16);
+        const uint32_t stage_lo = (uint32_t)p.stage_bytes >> 4;
+        const uint32_t a_shift_lo = (uint32_t)(p.TW * BK * 2) >> 4;      // one tile row of pixels
+        const uint32_t b_off_lo = ((uint32_t)p.a_bytes >> 4) - (uint32_t)cg * row_half_lo;
+        constexpr uint32_t b_tile_lo = (uint32_t)Cfg::B_BYTES >> 4;
+        const uint32_t res_j_lo = (uint32_t)(p.KW * kc_per_tap) * b_tile_lo;   // resident: next kernel row
+        const int groups_m0 = p.rg ? p.KW : p.KH * p.KW;
+        const int nb = p.nb;
+        const bool resident = p.resident != 0;
+        // fragment -> staging tile: this thread's rows 64 cg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
+        float* acc_row = acc_tile + (size_t)(64 * cg + 16 * (warp & 3) + (lane >> 2)) * Cfg::ACC_PITCH + 2 * (lane & 3);
+        uint32_t st = 0, ph = 0, a_lo = ring_lo, git = 0;
+        int rest = blockIdx.x / p.m_tiles, tile_m = blockIdx.x % p.m_tiles;
+        const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
+        int lt = 0;
+        float acc[BN / 2];
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+            const int n_iters = ((p.mode == 0) ? groups_m0 : p.cls[rest / p.n_tiles].n_taps) * kc_per_tap;
+            if (tracing && lt < 64) p.trace[1024 + lt * 4] = clock64();
+            if (lt == 0 && resident) mbar_wait(wfull, 0);
+            uint32_t accum = 0;
+            uint32_t res_lo = wres_lo;                           // resident weights: tile (it) of kernel row 0
+            uint32_t prev_st = 0;
+            for (int it = 0; it < n_iters; ++it, res_lo += b_tile_lo) {
+                mbar_wait(&full[st], ph);
+                if (tracing && git < 1000) p.trace[4096 + git * 2] = clock64();
+                uint32_t aj = a_lo;
+                uint32_t bj = resident ? res_lo : a_lo + b_off_lo;
+                const uint32_t bj_step = resident ? res_j_lo : b_tile_lo;
+                wgmma_fence();
+                for (int j = 0; j < nb; ++j, aj += a_shift_lo, bj += bj_step) {
 #pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            const uint64_t da = ((uint64_t)desc_hi << 32) | (uint64_t)(aj + 2 * k);
-                            const uint64_t db = ((uint64_t)desc_hi << 32) | (uint64_t)(bj + 2 * k);
-                            asm volatile(
-                                "{\n\t.reg .pred p;\n\t"
-                                "setp.ne.b32 p, %4, 0;\n\t"
-                                "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_acc),
-                                "l"(da), "l"(db), "r"(idesc), "r"(accum)
-                                : "memory");
-                            accum = 1;
-                        }
+                    for (int k = 0; k < BK / 16; ++k) {
+                        wgmma_bf16<0>(acc, gmma_desc(desc_hi, aj + 2 * k), gmma_desc(desc_hi, bj + 2 * k), accum);
+                        accum = 1;
                     }
-                    // release the smem stage once the MMAs that read it have completed
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                     tc_smem_u32(&empty[st]))
-                                 : "memory");
-                    if (tracing && git < 1000) p.trace[4096 + git * 2 + 1] = clock64();
-                    ++git;
-                    if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_lo = ring_lo; } else a_lo += stage_lo;
                 }
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                 tc_smem_u32(&acc_full[as]))
-                             : "memory");
-                if (tracing && lt < 64) p.trace[1024 + lt * 4 + 3] = clock64();
-                tile_m += step_m; rest += step_r;
-                if (tile_m >= p.m_tiles) { tile_m -= p.m_tiles; ++rest; }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (it > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
+                if (tracing && git < 1000) p.trace[4096 + git * 2 + 1] = clock64();
+                prev_st = st;
+                ++git;
+                if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_lo = ring_lo; } else a_lo += stage_lo;
             }
+            wgmma_wait<0>();
+            if (n_iters > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
+            if (tracing && lt < 64) p.trace[1024 + lt * 4 + 1] = clock64();
+            mbar_wait(acc_empty, (lt & 1) ^ 1);                 // the epilogue has read the previous tile back
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                *reinterpret_cast<float2*>(acc_row + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                *reinterpret_cast<float2*>(acc_row + 8 * Cfg::ACC_PITCH + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            }
+            mbar_arrive(acc_full);
+            if (tracing && lt < 64) p.trace[1024 + lt * 4 + 3] = clock64();
+            tile_m += step_m; rest += step_r;
+            if (tile_m >= p.m_tiles) { tile_m -= p.m_tiles; ++rest; }
         }
-        __syncwarp();
-    } else if (warp >= 4) {
-        // ===== epilogue: TMEM -> registers (+bias, +residual, GroupNorm statistics) -> bf16 -> smem transpose -> global
+    } else {
+        // ===== epilogue: parked fp32 tile -> registers (+bias, +residual, GroupNorm statistics) -> bf16 -> global
         // A lane owns one accumulator row (pixel).  Writing its row straight to global memory would make every store
         // instruction touch 32 different lines (16 bytes each): the LSU, not HBM, bounds the wide-N layers that way.
         // Instead each warp stages its 32 rows x CH columns in a private, XOR-swizzled shared-memory tile and writes it
@@ -409,15 +325,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         constexpr int CH = BN >= 64 ? 64 : 32;        // columns per pass
         constexpr int LPR = CH / 8;                   // 16-byte units per staged row = lanes per row when storing
         constexpr int RPI = 32 / LPR;                 // rows per store instruction
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
+        const int quarter = warp & 3;                 // rows [32 quarter, 32 quarter + 32) of the tile
         uint4* stage = reinterpret_cast<uint4*>(stage_base) + quarter * (32 * 8);
         const int m = quarter * 32 + lane;            // accumulator row = pixel within the tile
+        const float* acc_src = acc_tile + (size_t)m * Cfg::ACC_PITCH;
         const int tn = m / (p.TH * p.TW);
         const int rem = m - tn * p.TH * p.TW;
         const int th = rem / p.TW, tw = rem - th * p.TW;
         const int my_sw = (LPR == 8) ? (lane & 7) : ((lane >> 1) & 3);
         const int sr = lane / LPR, su = lane % LPR;   // store phase: row within the group of RPI rows, 16-byte unit
-        const bool tracing = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 128;
+        const bool tracing = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 384;
         int tile_m = blockIdx.x % p.m_tiles, rest = blockIdx.x / p.m_tiles;
         const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
         int lt = 0;
@@ -435,38 +352,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             long long st_off[LPR];
 #pragma unroll
             for (int it = 0; it < LPR; ++it) st_off[it] = __shfl_sync(0xffffffffu, row_off, it * RPI + sr);
-            const int as = lt & 1;
             if (tracing && lt < 64) p.trace[2048 + lt * 4] = clock64();
-            tc_mbar_wait(&acc_full[as], (lt >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            mbar_wait(acc_full, lt & 1);
             if (tracing && lt < 64) p.trace[2048 + lt * 4 + 1] = clock64();
 #pragma unroll 1
             for (int c = 0; c < BN; c += CH) {
                 float f[CH];
 #pragma unroll
-                for (int hh = 0; hh < CH / 32; ++hh) {
-                    uint32_t v[32];
-                    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * BN + c + hh * 32);
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-                          "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-                          "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-                          "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                        : "r"(taddr));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[hh * 32 + j] = row_ok ? __uint_as_float(v[j]) : 0.f;
+                for (int j = 0; j < CH; j += 4) {
+                    const float4 v = *reinterpret_cast<const float4*>(acc_src + c + j);
+                    f[j] = row_ok ? v.x : 0.f; f[j + 1] = row_ok ? v.y : 0.f;
+                    f[j + 2] = row_ok ? v.z : 0.f; f[j + 3] = row_ok ? v.w : 0.f;
                 }
                 if (tracing && lt < 64 && c == 0) p.trace[3072 + lt * 4] = clock64();
-                if (c + CH >= BN) {
-                    // the last columns of this accumulator are in registers: hand the TMEM stage back to the MMA warp
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc_smem_u32(&acc_empty[as])) : "memory");
-                }
+                // the last columns of the parked tile are in registers: hand the staging tile back to the consumers
+                if (c + CH >= BN) mbar_arrive(acc_empty);
                 if (p.bias && row_ok) {
 #pragma unroll
                     for (int j = 0; j < CH; j += 4) {
@@ -534,19 +434,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             if (tile_m >= p.m_tiles) { tile_m -= p.m_tiles; ++rest; }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(Cfg::TMEM_COLS));
-    }
 }
 
 // ---- host side ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
+EncodeTiledFn tensor_map_encoder() {
     static EncodeTiledFn fn = nullptr;
     if (!fn) {
         void* p = nullptr;
@@ -558,10 +449,12 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
+// resident weights + operand ring of an n-tile width (TcCfg<BN, *>::OPERAND_BYTES)
+static int tc_operand_bytes(int bn) { return (227 * 1024 - 1024 - 512 - 4 * 4096 - TC_BM * (bn + 4) * 4) / 1024 * 1024; }
+
 struct TcPlan {
     int TW, TH, TN, BN, BK;
     int rg, nb, a_bytes, stage_bytes, stages, resident, res_bytes, operand_bytes;
-    int cps;                 // CTAs per SM the launch is sized for (grid = SMs * cps persistent CTAs)
 };
 
 // GH x GW = pixel grid of the GEMM (output grid for regular convs, input grid for the transposed gather)
@@ -588,11 +481,12 @@ static bool tc_plan(int B, int GH, int GW, int Cin, int Cout, int KH, int KW, in
     pl.a_bytes = (pl.TH + (pl.rg ? KH - 1 : 0)) * pl.TW * pl.TN * pl.BK * 2;
     const long long K = (long long)KH * KW * Cin;
     const long long m_tiles = (long long)((B + pl.TN - 1) / pl.TN) * (GH / pl.TH) * (GW / pl.TW) * classes;
-    const int cands[4] = {256, 128, 64, 32};
+    // n-tile widths: a consumer warpgroup holds 64 x BN fp32 accumulators in registers, BN / 2 per thread
+    const int cands[3] = {128, 64, 32};
     static int force_bn = -1;                       // debugging aid: PIDM_TC_BN pins the n-tile width
     if (force_bn < 0) { const char* ev = getenv("PIDM_TC_BN"); force_bn = ev ? atoi(ev) : 0; }
     pl.BN = 0;
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < 3; ++i) {
         const int bn = cands[i];
         if (Cout % bn != 0) continue;
         if (force_bn > 0 && bn != force_bn && Cout % force_bn == 0) continue;
@@ -600,30 +494,17 @@ static bool tc_plan(int B, int GH, int GW, int Cin, int Cout, int KH, int KW, in
         const long long wbytes = (long long)bn * K * 2;
         int resident = (mode == 0 && Cout == bn && wbytes <= 100 * 1024) ? 1 : 0;
         int stage = pl.a_bytes + (resident ? 0 : pl.nb * bn * pl.BK * 2);
-        int stages = (int)((TC_OPERAND_BYTES - (resident ? wbytes : 0)) / stage);
+        int stages = (int)((tc_operand_bytes(bn) - (resident ? wbytes : 0)) / stage);
         if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
         if (stages < 3) continue;
         static int stage_cap = -1;                  // tuning aid: PIDM_TC_STAGES caps the ring depth
         if (stage_cap < 0) { const char* ev = getenv("PIDM_TC_STAGES"); stage_cap = ev ? atoi(ev) : TC_RING_STAGES; }
         if (stage_cap >= 3 && stages > stage_cap) stages = stage_cap;
-        // Two CTAs per SM for the narrow layers with resident weights (BN = 32: 126 registers, 64 TMEM columns): these
-        // layers are bound by per-CTA issue chains as much as by the SM's copy engine -- measured (B200, batch 32) 64x64x32
-        // 3x3 10.5 -> 8.0 us, 4x4/s2 32->32 10.7 -> 7.7 us, 1x1 256->32 13.8 -> 11.1 us with two half-size rings, while
-        // layers that stream their weights (several n-tiles) or already run wide tiles do not gain.  PIDM_TC_CTAS=1 disables.
-        static int max_cps = -1;
-        if (max_cps < 0) { const char* ev = getenv("PIDM_TC_CTAS"); max_cps = ev ? atoi(ev) : 2; if (max_cps < 1) max_cps = 1; }
-        int cps = 1;
-        if (max_cps >= 2 && bn == 32 && resident) {
-            const long long fixed = (long long)wbytes + 1024 + 512 + 4 * 4096 + 1024;       // + 1 KB reserved per CTA
-            const int s2 = (int)(((227 * 1024) / 2 - fixed) / stage);
-            if (s2 >= 3) { cps = 2; if (stages > s2) stages = s2; }
-        }
-        pl.cps = cps;
         pl.BN = bn; pl.resident = resident; pl.res_bytes = resident ? (int)wbytes : 0;
         pl.stage_bytes = stage; pl.stages = stages;
         pl.operand_bytes = (int)(((resident ? wbytes : 0) + (long long)stages * stage + 1023) / 1024 * 1024);
-        // widest tile that still (nearly) fills the machine: 128 tiles of N = 64 beat 256 tiles of N = 32 = 1.7 waves
-        // (16x16x128 3x3: 8.5 -> 6.2 us), while 64 tiles of N = 64 lose to 128 of N = 32 (8x8x256: 11.5 vs 11.6 us)
+        // widest tile that still (nearly) fills the machine (one persistent CTA per SM): fewer, wider tiles re-read
+        // the A operand less often, but a grid well short of one wave leaves SMs idle
         if (m_tiles * (Cout / bn) >= 128) break;
     }
     return pl.BN != 0;
@@ -634,10 +515,11 @@ static int launch_tc(const CUtensorMap& mx, const CUtensorMap& mw, const TcParam
     static bool attr = false;
     if (!attr) {
         PIDM_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       TC_SMEM_BYTES));
+                                       TcCfg<BN, BK>::SMEM_BYTES));
         attr = true;
     }
-    const size_t smem = (size_t)p.operand_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + 4 * 4096 /*epilogue staging*/;
+    const size_t smem = (size_t)p.operand_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + 4 * 4096 /*epilogue staging*/ +
+                        TcCfg<BN, BK>::ACC_BYTES;
     PIDM_CUDA(launch_pdl(conv_tc_kernel<BN, BK>, grid, dim3(TC_THREADS), smem, st, mx, mw, p));
     PIDM_LAUNCH_CHECK("conv2d_tc");
     return 0;
@@ -697,7 +579,7 @@ static int tc_run(const void* x, const void* w_packed, const float* bias, const 
         PIDM_CUDA(cudaFree(0));
         ctx_bound = true;
     }
-    EncodeTiledFn enc = get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     PIDM_REQUIRE(enc != nullptr, "conv2d_tc: cuTensorMapEncodeTiled is not available from the driver");
     PIDM_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0, "conv2d_tc: operands must be 16-byte aligned");
     CUtensorMap mx, mw;
@@ -739,18 +621,12 @@ static int tc_run(const void* x, const void* w_packed, const float* bias, const 
     p.m_tiles = ((B + pl.TN - 1) / pl.TN) * p.tiles_h * p.tiles_w;
     p.n_tiles = Cout / pl.BN;
     p.n_classes = classes;
-    static int sm_count = 0;
-    if (!sm_count) {
-        int dev = 0;
-        PIDM_CUDA(cudaGetDevice(&dev));
-        PIDM_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-    }
     const int total_tiles = p.m_tiles * p.n_tiles * p.n_classes;
-    const int slots = sm_count * pl.cps;
+    const int slots = num_sms();
     dim3 grid(total_tiles < slots ? total_tiles : slots);
 #define TC_CASE(bn, bk) if (pl.BN == bn && pl.BK == bk) return launch_tc<bn, bk>(mx, mw, p, grid, st)
-    TC_CASE(256, 64); TC_CASE(128, 64); TC_CASE(64, 64); TC_CASE(32, 64);
-    TC_CASE(256, 32); TC_CASE(128, 32); TC_CASE(64, 32); TC_CASE(32, 32);
+    TC_CASE(128, 64); TC_CASE(64, 64); TC_CASE(32, 64);
+    TC_CASE(128, 32); TC_CASE(64, 32); TC_CASE(32, 32);
 #undef TC_CASE
     return set_error(2, "conv2d_tc: no kernel for BN=%d BK=%d", pl.BN, pl.BK);
 }

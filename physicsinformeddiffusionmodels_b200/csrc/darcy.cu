@@ -6,7 +6,7 @@
 //   r[b, i*P+j, 1] = (i==0 ? -p_0 : i==P-1 ? +p_0 : 0)
 //   r[b, i*P+j, 2] = (j==0 ? +s p_1 : j==P-1 ? -s p_1 : 0),  s = +1 if reverse_d1 else -1
 //
-// B200 design: HBM-bound (about 2 flop/byte).  Persistent CTAs; every sample (p-plane + K-plane,
+// Design: HBM-bound (about 2 flop/byte).  Persistent CTAs; every sample (p-plane + K-plane,
 // 2*P*P*4 = 32 KiB contiguous in NCHW) is staged into shared memory by ONE bulk-async (TMA) copy
 // that completes on an mbarrier, double-buffered so the copy of sample n+1 overlaps the stencil math
 // of sample n.  All stencils read shared memory (the halo is the plane itself: one-sided stencils at
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_fwd_kernel(const float* _
 // Phase 1 evaluates the residual of a quad of pixels (all derivatives of p and K are already in registers there) and
 // leaves A, U0, U1, V0, V1 in shared-memory planes; phase 2 gathers the <= 5-point adjoint stencils from those planes.
 // (The first version re-derived K_0 / K_1 / p_0 / p_1 at every neighbour inside the gather -- ~60 shared-memory loads
-// per pixel -- and ran at 18 % of the HBM roofline; it also used 256 threads per sample, 25 us in the training step.)
+// per pixel -- and used 256 threads per sample.)
 constexpr int DG_THREADS = 512;
 constexpr int DG_QUADS = PP / 4 / DG_THREADS;      // quads per thread per sample (2)
 
@@ -611,7 +611,7 @@ extern "C" int pidm_fd_stencil(const float* u, float* out, int planes, int pixel
                                void* stream) {
     PIDM_REQUIRE(pixels == P, "fd_stencil is built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(mode >= 0 && mode <= 4, "fd_stencil: mode must be 0..4 (d_d0, d_d1, d_d00, d_d11, d_d01)");
-    int grid = planes < 148 * 4 ? planes : 148 * 4;
+    int grid = planes < num_sms() * 4 ? planes : num_sms() * 4;
     PIDM_CUDA(launch_pdl(fd_stencil_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, u, out, planes, mode, 1.f / d0, 1.f / d1));
     PIDM_LAUNCH_CHECK("fd_stencil");
     return 0;

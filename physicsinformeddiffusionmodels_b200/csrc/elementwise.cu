@@ -380,7 +380,7 @@ __global__ void head_bwd_kernel(const T* __restrict__ x, const float* __restrict
 // pixel rows (8 pixels x 64 B at C = 32: fully coalesced), a thread keeps the weight-gradient partials of ITS octet in
 // registers over all its pixels and the lanes that share an octet are combined ONCE at the end (log2(32 / LPP) shuffles
 // per value) -- the kernel above reduces every (o, c) product over the warp for every 32 pixels (320 shuffles + 64
-// shared-memory atomics per warp iteration: 25 us for the 9 MB head of the Darcy model; this one is a streaming pass).
+// shared-memory atomics per warp iteration; this one is a streaming pass).
 // Requires LPP = C / 8 to be a power of two <= 32.
 template <typename T, int O>
 __global__ void __launch_bounds__(256) head_bwd_octet_kernel(const T* __restrict__ x, const float* __restrict__ w,
@@ -456,8 +456,9 @@ __global__ void __launch_bounds__(256) head_bwd_octet_kernel(const T* __restrict
     if (threadIdx.x < O) atomicAdd(&db[threadIdx.x], sdb[threadIdx.x]);
 }
 
-static inline int grid_for(long long n, int block, int cap = 148 * 16) {
+static inline int grid_for(long long n, int block, int cap = 0) {    // cap 0: 16 CTAs per SM
     long long g = (n + block - 1) / block;
+    if (cap <= 0) cap = num_sms() * 16;
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return (int)g;
@@ -617,7 +618,7 @@ extern "C" int pidm_head_bwd(const void* x, const float* w, const float* y, cons
     if (lpp <= 32 && (lpp & (lpp - 1)) == 0) {
         const long long items = M * lpp;
 #define HEAD_BO(OO)                                                                                    \
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_bwd_octet_kernel<T, OO>, dim3(grid_for(items, 256, 148 * 4)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_bwd_octet_kernel<T, OO>, dim3(grid_for(items, 256, num_sms() * 4)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
                                    (const T*)x, w, y, dy, (T*)dx, dw, db, C, HW, M, sigmoid_last)))
         switch (O) { case 1: HEAD_BO(1); break; case 2: HEAD_BO(2); break; case 3: HEAD_BO(3); break; default: HEAD_BO(4); }
 #undef HEAD_BO
@@ -625,7 +626,7 @@ extern "C" int pidm_head_bwd(const void* x, const float* w, const float* y, cons
         return 0;
     }
 #define HEAD_B(OO)                                                                                     \
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_bwd_kernel<T, OO>, dim3(grid_for(M, 256, 148 * 2)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_bwd_kernel<T, OO>, dim3(grid_for(M, 256, num_sms() * 2)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
                                    (const T*)x, w, y, dy, (T*)dx, dw, db, C, HW, M, sigmoid_last)))
     switch (O) { case 1: HEAD_B(1); break; case 2: HEAD_B(2); break; case 3: HEAD_B(3); break; default: HEAD_B(4); }
 #undef HEAD_B

@@ -37,7 +37,7 @@ __global__ void time_embed_fwd_kernel(const long long* __restrict__ t, const flo
     }
     __syncthreads();
     // thread j owns output row j: its weight row is read as 16-byte vectors, 16 loads in flight (the scalar loop issued
-    // td dependent-latency batches: 13 us for two 128-wide products)
+    // td dependent-latency batches)
     float acc = b1[j];
     {
         const float4* wr = reinterpret_cast<const float4*>(W1 + (size_t)j * dim);
@@ -90,7 +90,7 @@ __global__ void time_embed_bwd_act_kernel(const float* __restrict__ d_silu, cons
 
 // backward, stage 2 (one CTA per output row j, blockDim = td = columns k): the weight gradients are small
 // [td x B] x [B x td] products -- every element is owned by exactly one thread, so they are accumulated with plain
-// read-modify-writes (the first version issued td + dim contended atomics per thread from B CTAs: 26 us).
+// read-modify-writes (rather than td + dim contended atomics per thread from B CTAs).
 //   dW2[j,k] += sum_b dt[b,j] gelu(h1[b,k]);  db2[j] += sum_b dt[b,j];  dW1[j,k<dim] += sum_b dh[b,j] emb[b,k];  db1[j] += ...
 __global__ void time_embed_bwd_wgrad_kernel(const float* __restrict__ dt, const float* __restrict__ dh,
                                             const float* __restrict__ emb, const float* __restrict__ h1,
@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256) block_mlps_wgrad_kernel(const MlpEntry* _
 // Thread = k keeps 32 sample accumulators; W rows are read once (coalesced over k), dout comes from shared memory as
 // broadcast float4 reads, one atomicAdd per (sample, k) and CTA at the end.  ds zeroed by the caller.  (The first version
 // gave each of 37 CTAs a 128-row chunk found by scanning the table: 18 dependent table loads + 16 serial batches of
-// weight loads per CTA = 27 us for a 30 MFLOP problem; now ~120 CTAs with 4 batches each, addressed directly.)
+// weight loads per CTA for a 30 MFLOP problem; now ~120 CTAs with 4 batches each, addressed directly.)
 __global__ void block_mlps_dgrad_kernel(const MlpEntry* __restrict__ table, float* __restrict__ ds, int B, int td) {
     pdl_trigger();
     pdl_wait();

@@ -312,7 +312,7 @@ extern "C" int pidm_mechanics_residual_bwd(const float* u, const float* rho, con
 extern "C" int pidm_bilinear_resize_fwd(const float* x, float* y, int planes, int in, int out, void* stream) {
     long long total = (long long)planes * out * out;
     int grid = (int)((total + 255) / 256);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > num_sms() * 8) grid = num_sms() * 8;
     bilinear_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, y, planes, in, out);
     PIDM_LAUNCH_CHECK("bilinear_resize_fwd");
     return 0;
@@ -324,7 +324,7 @@ extern "C" int pidm_bilinear_resize_bwd(const float* dy, float* dx, int planes, 
     PIDM_CUDA(cudaMemsetAsync(dx, 0, (size_t)planes * in * in * sizeof(float), st));
     long long total = (long long)planes * out * out;
     int grid = (int)((total + 255) / 256);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > num_sms() * 8) grid = num_sms() * 8;
     bilinear_bwd_kernel<<<grid, 256, 0, st>>>(dy, dx, planes, in, out);
     PIDM_LAUNCH_CHECK("bilinear_resize_bwd");
     return 0;

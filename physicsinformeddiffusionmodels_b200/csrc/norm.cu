@@ -295,8 +295,8 @@ __global__ void __launch_bounds__(NORM_THREADS, 2) gn_bwd_piece_packed_kernel(
 
 // The piece kernel for pieces of MORE than 4 vectors per thread (the 64x64 levels): x and dy are streamed twice (the second
 // pass hits L2).  Compared with gn_bwd_piece_kernel<T, 2, false>, which it replaces, the loops are written for instruction
-// count -- ncu (r02) shows that variant issue-bound as much as latency-bound: 29 instructions per element and phase, a third
-// of them 64-bit address arithmetic and predicate bookkeeping.  Here a thread walks its vectors with three running
+// count -- that variant spends 29 instructions per element and phase, a third of them 64-bit address arithmetic and
+// predicate bookkeeping.  Here a thread walks its vectors with three running
 // pointers, per-channel constants are folded (xhat = x * rs - mr, z = xhat * A + Bc, dx = dz * Ap - m1p - xhat * m2p), the
 // next two vector pairs are fetched (raw, 16 registers) while the current two are processed, and the first pass parks dz in
 // the dx buffer (activation dtype) so that the second pass needs no SiLU' (it reads x and dz, overwrites dz with dx).
@@ -630,10 +630,9 @@ __global__ void gn_bwd_dx_kernel(const T* __restrict__ x, const T* __restrict__ 
 //   phase 2: dx = rstd * (gamma*(1+scale)*dz - m1 - xhat*m2), FiLM / affine / bias gradients
 // KEEP = true (<= 2 vectors per thread): xhat and dz stay in REGISTERS between the phases, x and dy are read once.
 // KEEP = false: phase 2 re-reads the thread's own vectors (L1 / L2 hits: the CTA touched them a few microseconds
-// earlier), two vectors at a time -- holding 4 x 8 x 2 fp32 values per thread cost 156 registers = one CTA per SM and
-// 35 us at 64x64x32.
+// earlier), two vectors at a time -- holding 4 x 8 x 2 fp32 values per thread costs 156 registers = one CTA per SM.
 // Either way the grid has 256..512 CTAs at every level of the U-Net (the first version ran one CTA or one 8-CTA cluster
-// per SAMPLE: 32 CTAs on 148 SMs at the 8x8 level, 14 us for 1 MB; ncu: warps_active 12 %, waves_per_multiprocessor 0.05).
+// per SAMPLE: 32 CTAs for the whole GPU at the 8x8 level, a small fraction of one wave).
 // Element-wise arithmetic is the same, in the same order, as in gn_bwd_reduce_kernel + gn_bwd_dx_kernel.
 template <typename T, int V, bool KEEP>
 __global__ void __launch_bounds__(NORM_THREADS, 2) gn_bwd_piece_kernel(
@@ -1058,11 +1057,11 @@ extern "C" int pidm_groupnorm_silu_fwd(const void* x, const float* gamma, const 
         PIDM_REQUIRE(ov <= NORM_THREADS && NORM_THREADS % ov == 0, "groupnorm: C=%d is not supported by the apply kernel", C);
         const int rpp = NORM_THREADS / ov;
         int ach = ceil_div(HW, rpp * GN_APPLY_UNR);
-        for (int u = GN_APPLY_UNR; u > 1 && (long long)B * ach < 148 * 2; u /= 2) ach = ceil_div(HW, rpp * (u / 2));
-        while (ach > 1 && (long long)B * ach > 148 * 8) ach = (ach + 1) / 2;
+        for (int u = GN_APPLY_UNR; u > 1 && (long long)B * ach < num_sms() * 2; u /= 2) ach = ceil_div(HW, rpp * (u / 2));
+        while (ach > 1 && (long long)B * ach > num_sms() * 8) ach = (ach + 1) / 2;
         // ~123 registers: two CTAs per SM are resident.  Between one and two waves the second wave runs mostly empty
-        // (ncu r02: 512 CTAs = 1.73 waves at 64x64x32, batch 32): size the grid to one wave and let the CTAs loop
-        if ((long long)B * ach > 148 * 2 && (long long)B * ach < 148 * 4 && B <= 148 * 2) ach = (148 * 2) / B;
+        // (e.g. 512 CTAs at 64x64x32, batch 32): size the grid to one wave and let the CTAs loop
+        if ((long long)B * ach > num_sms() * 2 && (long long)B * ach < num_sms() * 4 && B <= num_sms() * 2) ach = (num_sms() * 2) / B;
         PIDM_CUDA(launch_pdl(gn_apply_kernel<T>, dim3(ach, B), dim3(NORM_THREADS), 0, st, (const T*)x, (const float*)sums,
                              gamma, beta, scale_shift, (const T*)residual, (T*)y, HW, C, G, eps));
     });
@@ -1091,11 +1090,11 @@ extern "C" int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const floa
             const long long nv = (long long)HW * so;            // 16-byte vectors per (sample, slab)
             int threads = NORM_THREADS;
             while (threads > 32 && threads / 2 >= nv && (threads / 2) % so == 0) threads /= 2;
-            // CTAs per piece.  Measured (B200, B = 32): a CTA of this kernel is a ~4 us latency chain whatever its size, a
+            // CTAs per piece.  A CTA of this kernel is a latency chain of a few microseconds whatever its size, a
             // second wave of CTAs doubles the launch and a cluster costs ~1 us extra -- so: no cluster unless a piece
             // has more than 8 vectors per thread, never more CTAs than are resident at once (2 per SM), and otherwise
             // as many CTAs as that allows.
-            const int resident = 148 * 2;
+            const int resident = num_sms() * 2;
             int cl = 1;
             while (cl < 8 && nv > (long long)cl * threads * 8) cl *= 2;
             while (cl < 8 && (long long)B * nslab * cl * 2 <= resident && nv > (long long)cl * threads) cl *= 2;
@@ -1142,8 +1141,7 @@ extern "C" int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const floa
                                  scale_shift, (T*)dx, d_scale_shift, dgamma, dbeta, dbias_of_producer, HW, C, G, eps,    \
                                  S, cl, rows_per_cta))
                 // three shapes of a piece: <= 2 vectors per thread stay in registers unpacked between the phases; 3-4 vectors are
-                // held packed (measured 11.6 -> 10.5 us at 32x32x64; with 8 vectors that variant spills: 15.5 -> 29 us at
-                // 64x64x32); larger pieces are streamed twice (12.5 us at 64x64x32)
+                // held packed (with 8 vectors that variant spills); larger pieces are streamed twice
                 if (keep) {
                     PIDM_DISPATCH_DTYPE(dtype, { GN_PIECE_CASE(1, true) else GN_PIECE_CASE(2, true) });
                 } else if (v <= 4) {
@@ -1181,10 +1179,10 @@ extern "C" int pidm_layernorm_c_fwd(const void* x, const float* gamma, void* y, 
     int oct = C / 8, L = 1;
     while (L < 32 && L < oct) L <<= 1;
     long long groups = (M + (32 / L) * 8 - 1) / ((32 / L) * 8);
-    int grid = (int)(groups < 148 * 8 ? (groups < 1 ? 1 : groups) : 148 * 8);
+    int grid = (int)(groups < num_sms() * 8 ? (groups < 1 ? 1 : groups) : num_sms() * 8);
     if (L == oct) {          // one octet per lane: register-resident kernel
         long long g1 = (M + (32 / L) * 8 * LN_UNR - 1) / ((32 / L) * 8 * LN_UNR);
-        int grid1 = (int)(g1 < 148 * 8 ? (g1 < 1 ? 1 : g1) : 148 * 8);
+        int grid1 = (int)(g1 < num_sms() * 8 ? (g1 < 1 ? 1 : g1) : num_sms() * 8);
         PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(ln1_kernel<T, false>, dim3(grid1), dim3(256), 0, (cudaStream_t)stream,
                                                         (const T*)x, (const T*)nullptr, gamma, (T*)y, (float*)nullptr,
                                                         (const T*)nullptr, M, C, eps)));
@@ -1205,10 +1203,10 @@ extern "C" int pidm_layernorm_c_bwd(const void* x, const void* dy, const float* 
     int oct = C / 8, L = 1;
     while (L < 32 && L < oct) L <<= 1;
     long long groups = (M + (32 / L) * 8 - 1) / ((32 / L) * 8);
-    int grid = (int)(groups < 148 * 4 ? (groups < 1 ? 1 : groups) : 148 * 4);
+    int grid = (int)(groups < num_sms() * 4 ? (groups < 1 ? 1 : groups) : num_sms() * 4);
     if (L == oct) {
         long long g1 = (M + (32 / L) * 8 * LN_UNR - 1) / ((32 / L) * 8 * LN_UNR);
-        int grid1 = (int)(g1 < 148 * 4 ? (g1 < 1 ? 1 : g1) : 148 * 4);
+        int grid1 = (int)(g1 < num_sms() * 4 ? (g1 < 1 ? 1 : g1) : num_sms() * 4);
         PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(ln1_kernel<T, true>, dim3(grid1), dim3(256), C * sizeof(float),
                                                         (cudaStream_t)stream, (const T*)x, (const T*)dy, gamma, (T*)dx,
                                                         dgamma, (const T*)dx_residual, M, C, eps)));

@@ -20,6 +20,16 @@ bool pdl_enabled(int group) {
     return ((mask >> group) & 1) != 0;
 }
 
+int num_sms() {
+    static int n = 0;
+    if (!n) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+            n = 132;
+    }
+    return n;
+}
+
 int set_error(int code, const char* fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
@@ -173,7 +183,7 @@ extern "C" int pidm_adam_ema_step(float* param, float* grad, float* exp_avg, flo
                    (uintptr_t)(ema_first_step > 0 ? ema_shadow : param)) & 15) == 0, "adam: buffers must be 16-byte aligned");
     if (step_counter_dev) PIDM_CUDA(launch_pdl(incr_kernel, dim3(1), dim3(1), (size_t)(0), (cudaStream_t)stream, step_counter_dev));   // counter holds steps done so far
     int grid = (int)((n / 4 + 255) / 256);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > num_sms() * 8) grid = num_sms() * 8;
     if (grid < 1) grid = 1;
     PIDM_CUDA(launch_pdl(adam_ema_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, param, grad, exp_avg, exp_avg_sq, ema_shadow, n, lr, beta1,
                                                            beta2, eps, step, step_counter_dev, grad_norm_sq_dev, grad_scale,

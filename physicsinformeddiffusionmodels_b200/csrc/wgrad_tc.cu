@@ -1,73 +1,24 @@
-// Weight gradient of a stride-1 "same" KxK convolution on the tcgen05 tensor cores.
+// Weight gradient of a stride-1 "same" KxK convolution on the Hopper tensor cores (wgmma).
 //
 //   dW[co][ci][tap] += sum_{pixels m} dy[m][co] * x[m shifted by tap][ci]
 //
 // GEMM view: D[M' = (tap, ci)][N' = co] = A^T B with the reduction dimension K' = pixels.  Both operands live in
 // HBM pixel-major (NHWC), i.e. the M'/N' dimension (channels) is contiguous and K' (pixels) is strided: they are
-// "MN-major" UMMA operands.  One K' step = one 128-pixel box (TN x TH x TW) fetched by TMA:
+// "MN-major" wgmma operands.  One K' step = one 128-pixel box (TN x TH x TW) fetched by TMA:
 //   A: 128/ATOM_A shifted boxes of x  {ATOM_A channels, TW, TH, TN}, one per (tap, channel-chunk) pair of this M' tile
 //   B: NP/ATOM_B boxes of dy          {ATOM_B channels, TW, TH, TN}
 // Each box lands as [128 pixel rows][ATOM channels] with the 128B/64B swizzle = one column of MN-major swizzle atoms
 // (8 pixel rows x ATOM channels); atoms along M'/N' are LBO = one box apart, along K' SBO = 8 rows apart.
-// The 8 MMAs of a stage (K'=16 pixels each) accumulate into TMEM; CTAs split the pixel range (split-K) and add their
-// partial D into the fp32 gradient with red.global.add (framework layout through strides).
-#include "common.cuh"
+// Warp 0 produces the ring; two consumer warpgroups each own 64 rows of M' and issue the 8 wgmmas (K' = 16 pixels
+// each) of a stage into register accumulators.  CTAs split the pixel range (split-K) and add their partial D into the
+// fp32 gradient with red.global.add (framework layout through strides), straight from the accumulator fragments.
+#include "hopper.cuh"
 #include "pidm.h"
-#include <cuda.h>
 #include <stdlib.h>
 
 namespace pidm {
 
-constexpr int WG_THREADS = 256;
-
-__device__ __forceinline__ uint32_t wg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void wg_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(wg_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void wg_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(wg_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void wg_mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(wg_smem_u32(bar)), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-__device__ __forceinline__ void wg_tma_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-            wg_smem_u32(dst)),
-        "l"(map), "r"(wg_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ bool wg_elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-// MN-major swizzled UMMA descriptor: LBO = byte stride between swizzle atoms along M/N, SBO = between 8-row K groups
-template <int ROW_BYTES>
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-    constexpr uint64_t layout = ROW_BYTES == 128 ? 2 : (ROW_BYTES == 64 ? 4 : 6);
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((8 * ROW_BYTES) >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= layout << 61;
-    return d;
-}
+constexpr int WG_THREADS = 384;
 
 struct WgParams {
     int B, Cin, Cout;            // Cin = channels of the A-side (gathered) tensor, Cout = channels of the B-side tensor
@@ -94,13 +45,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(const __grid_co
                                                                  const __grid_constant__ CUtensorMap map_dy, WgParams p) {
     using Cfg = WgCfg<NP, ATOM_A, ATOM_B>;
     extern __shared__ unsigned char smem_raw[];
-    const uint32_t raw_addr = wg_smem_u32(smem_raw);
+    const uint32_t raw_addr = smem_u32(smem_raw);
     unsigned char* ring = smem_raw + ((1024 - (raw_addr & 1023)) & 1023);
     uint64_t* bars = reinterpret_cast<uint64_t*>(ring + Cfg::STAGES * Cfg::STAGE_BYTES);
     uint64_t* full = bars;
     uint64_t* empty = bars + Cfg::STAGES;
-    uint64_t* acc_full = bars + 2 * Cfg::STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger();
@@ -117,125 +66,85 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(const __grid_co
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_dy) : "memory");
     }
     if (warp == 1 && lane == 0) {
-        for (int s = 0; s < Cfg::STAGES; ++s) { wg_mbar_init(&full[s], 1); wg_mbar_init(&empty[s], 1); }
-        wg_mbar_init(acc_full, 1);
+        // a stage is free once all 8 consumer warps have retired the wgmmas that read it
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(wg_smem_u32(tmem_slot)),
-                     "r"(NP));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();
 
-    if (n_iters > 0) {
-        if (warp == 0) {
-            if (wg_elect_one()) {
-                // per-box coordinates of this M' tile are loop invariant: resolve (tap, chunk) -> (c0, dw, dh) once
-                int ac[Cfg::NA], aw[Cfg::NA], ah[Cfg::NA];
+    if (n_iters <= 0) return;
+    if (warp == 0) {
+        if (elect_one()) {
+            // per-box coordinates of this M' tile are loop invariant: resolve (tap, chunk) -> (c0, dw, dh) once
+            int ac[Cfg::NA], aw[Cfg::NA], ah[Cfg::NA];
 #pragma unroll
-                for (int j = 0; j < Cfg::NA; ++j) {
-                    int pr = mt * Cfg::NA + j;
-                    if (pr >= n_pairs) pr = n_pairs - 1;          // padding rows of the last M' tile (discarded later)
-                    const int tap = pr / chunks, ch = pr - tap * chunks;
-                    const int r = tap / p.KW, q = tap - r * p.KW;
-                    ac[j] = ch * ATOM_A; aw[j] = q - p.pad; ah[j] = r - p.pad;
-                }
-                int tb = pt_begin / p.tiles_h, th_idx = pt_begin - tb * p.tiles_h;
-                uint32_t st = 0, ph = 0;
-                unsigned char* a_dst = ring;
-                for (int it = 0; it < n_iters; ++it) {
-                    wg_mbar_wait(&empty[st], ph ^ 1);
-                    const int b0 = tb * p.TN, h0 = th_idx * p.TH;
-                    unsigned char* b_dst = a_dst + Cfg::NA * Cfg::A_TILE;
-                    wg_mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
-#pragma unroll
-                    for (int j = 0; j < Cfg::NA; ++j)
-                        wg_tma_4d(a_dst + j * Cfg::A_TILE, &map_x, &full[st], ac[j], aw[j], p.a_stride * h0 + ah[j], b0);
-#pragma unroll
-                    for (int j = 0; j < Cfg::NB; ++j)
-                        wg_tma_4d(b_dst + j * Cfg::B_TILE, &map_dy, &full[st], n0 + j * ATOM_B, 0, h0, b0);
-                    if (++th_idx == p.tiles_h) { th_idx = 0; ++tb; }
-                    if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; a_dst = ring; } else a_dst += Cfg::STAGE_BYTES;
-                }
+            for (int j = 0; j < Cfg::NA; ++j) {
+                int pr = mt * Cfg::NA + j;
+                if (pr >= n_pairs) pr = n_pairs - 1;          // padding rows of the last M' tile (discarded later)
+                const int tap = pr / chunks, ch = pr - tap * chunks;
+                const int r = tap / p.KW, q = tap - r * p.KW;
+                ac[j] = ch * ATOM_A; aw[j] = q - p.pad; ah[j] = r - p.pad;
             }
-        } else if (warp == 1) {
-            // D = f32, A = B = bf16, both MN-major (bits 15, 16), N>>3 at [17,23), M>>4 at [24,29)
-            constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) |
-                                       ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            if (wg_elect_one()) {          // one thread runs the whole issue loop; descriptors advance by adds only
-                const uint64_t da0 = umma_desc_mn<ATOM_A * 2>(wg_smem_u32(ring), Cfg::A_TILE);
-                const uint64_t db0 = umma_desc_mn<ATOM_B * 2>(wg_smem_u32(ring) + Cfg::NA * Cfg::A_TILE, Cfg::B_TILE);
-                constexpr uint32_t stage_lo = Cfg::STAGE_BYTES >> 4;
-                constexpr uint32_t ka_lo = (16 * ATOM_A * 2) >> 4, kb_lo = (16 * ATOM_B * 2) >> 4;
-                uint32_t st = 0, ph = 0, off_lo = 0, accum = 0;
-                for (int it = 0; it < n_iters; ++it) {
-                    wg_mbar_wait(&full[st], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            int tb = pt_begin / p.tiles_h, th_idx = pt_begin - tb * p.tiles_h;
+            uint32_t st = 0, ph = 0;
+            unsigned char* a_dst = ring;
+            for (int it = 0; it < n_iters; ++it) {
+                mbar_wait(&empty[st], ph ^ 1);
+                const int b0 = tb * p.TN, h0 = th_idx * p.TH;
+                unsigned char* b_dst = a_dst + Cfg::NA * Cfg::A_TILE;
+                mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) {      // 8 x 16 pixels
-                        const uint64_t da = da0 + (uint64_t)(off_lo + k * ka_lo);
-                        const uint64_t db = db0 + (uint64_t)(off_lo + k * kb_lo);
-                        asm volatile(
-                            "{\n\t.reg .pred p;\n\t"
-                            "setp.ne.b32 p, %4, 0;\n\t"
-                            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_base),
-                            "l"(da), "l"(db), "r"(idesc), "r"(accum)
-                            : "memory");
-                        accum = 1;
-                    }
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                     wg_smem_u32(&empty[st]))
-                                 : "memory");
-                    if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; off_lo = 0; } else off_lo += stage_lo;
-                }
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                 wg_smem_u32(acc_full))
-                             : "memory");
+                for (int j = 0; j < Cfg::NA; ++j)
+                    tma_load_4d(a_dst + j * Cfg::A_TILE, &map_x, &full[st], ac[j], aw[j], p.a_stride * h0 + ah[j], b0);
+#pragma unroll
+                for (int j = 0; j < Cfg::NB; ++j)
+                    tma_load_4d(b_dst + j * Cfg::B_TILE, &map_dy, &full[st], n0 + j * ATOM_B, 0, h0, b0);
+                if (++th_idx == p.tiles_h) { th_idx = 0; ++tb; }
+                if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; a_dst = ring; } else a_dst += Cfg::STAGE_BYTES;
             }
-            __syncwarp();
-        } else if (warp >= 4) {
-            const int quarter = warp & 3;
-            const int mrow = quarter * 32 + lane;             // accumulator row = (pair j, channel within atom)
+        }
+    } else if (warp >= 4) {
+        // ===== consumer warpgroup cg: M' rows [64 cg, 64 cg + 64) =====
+        const int cg = (warp - 4) >> 2;
+        // rows 64 cg.. start (64 / ATOM_A) * cg atoms into the A boxes
+        const uint32_t a_lo0 = gmma_desc_lo(smem_u32(ring) + cg * (64 / ATOM_A) * Cfg::A_TILE, Cfg::A_TILE);
+        const uint32_t b_lo0 = gmma_desc_lo(smem_u32(ring) + Cfg::NA * Cfg::A_TILE, Cfg::B_TILE);
+        constexpr uint32_t a_hi = gmma_desc_hi<ATOM_A * 2>(), b_hi = gmma_desc_hi<ATOM_B * 2>();
+        constexpr uint32_t stage_lo = Cfg::STAGE_BYTES >> 4;
+        constexpr uint32_t ka_lo = (16 * ATOM_A * 2) >> 4, kb_lo = (16 * ATOM_B * 2) >> 4;
+        float acc[NP / 2];
+        uint32_t st = 0, ph = 0, off_lo = 0, prev_st = 0;
+        for (int it = 0; it < n_iters; ++it) {
+            mbar_wait(&full[st], ph);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 8; ++k)        // 8 x 16 pixels
+                wgmma_bf16<1>(acc, gmma_desc(a_hi, a_lo0 + off_lo + k * ka_lo), gmma_desc(b_hi, b_lo0 + off_lo + k * kb_lo),
+                              (it | k) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (it > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
+            prev_st = st;
+            if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; off_lo = 0; } else off_lo += stage_lo;
+        }
+        wgmma_wait<0>();
+        // fragment rows: 64 cg + 16 (warp % 4) + lane / 4 + 8 i; columns 8 j + 2 (lane % 4) + e
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int mrow = 64 * cg + 16 * (warp & 3) + (lane >> 2) + 8 * i;    // = (pair j, channel within atom)
             const int j = mrow / ATOM_A, cl = mrow - j * ATOM_A;
             const int pr = mt * Cfg::NA + j;
             const int tap = (pr < n_pairs) ? pr / chunks : 0;
             const int ci = (pr < n_pairs) ? (pr - tap * chunks) * ATOM_A + cl : 0;
-            const bool row_ok = (pr < n_pairs) && (ci < p.c_real);
-            float* dst = p.dw + (long long)ci * p.s_row + tap;
-            wg_mbar_wait(acc_full, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int c = 0; c < NP; c += 32) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c;
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                      "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-                      "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-                      "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-                      "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (row_ok) {
+            if (pr >= n_pairs || ci >= p.c_real) continue;
+            float* dst = p.dw + (long long)ci * p.s_row + tap + (long long)(n0 + 2 * (lane & 3)) * p.s_col;
 #pragma unroll
-                    for (int n = 0; n < 32; ++n)
-                        atomicAdd(dst + (long long)(n0 + c + n) * p.s_col, __uint_as_float(v[n]));
-                }
+            for (int jj = 0; jj < NP / 8; ++jj) {
+                atomicAdd(dst + (long long)(8 * jj) * p.s_col, acc[4 * jj + 2 * i]);
+                atomicAdd(dst + (long long)(8 * jj + 1) * p.s_col, acc[4 * jj + 2 * i + 1]);
             }
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(NP));
     }
 }
 
@@ -251,7 +160,7 @@ __global__ void colsum_kernel(const T* __restrict__ dy, float* __restrict__ out,
     __syncthreads();
     float a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     // four independent row loads in flight per thread (one load per iteration left the kernel waiting on one memory
-    // round trip per ~38 k rows: 4.7 us for 8 MB)
+    // round trip per ~38 k rows)
     const long long stride = (long long)gridDim.x * rows;
     for (long long m = (long long)blockIdx.x * rows + r0; m < M; m += 4 * stride) {
         float v[4][8];
@@ -274,21 +183,6 @@ __global__ void colsum_kernel(const T* __restrict__ dy, float* __restrict__ out,
     }
     __syncthreads();
     for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(&out[i], sacc[i]);
-}
-
-typedef CUresult (*WgEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static WgEncodeFn wg_get_encode() {
-    static WgEncodeFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (WgEncodeFn)ptr;
-    }
-    return fn;
 }
 
 struct WgPlan { int TW, TH, TN, NP, AA, AB; };
@@ -314,7 +208,7 @@ static bool wg_plan(int B, int GH, int GW, int CA, int CB, int a_stride, WgPlan&
 
 static int wg_encode(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int atom, int TW, int TH, int TN,
                      int es_) {
-    WgEncodeFn enc = wg_get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     PIDM_REQUIRE(enc != nullptr, "wgrad_tc: cuTensorMapEncodeTiled is not available from the driver");
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
@@ -385,9 +279,9 @@ extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int
     const int n_pairs = KH * KW * (CA / pl.AA);
     const int m_tiles = (n_pairs + na - 1) / na;
     const int n_tiles = CB / pl.NP;
-    // split the pixel range so that the grid is one wave of the 148 SMs (one CTA per SM: the ring takes the shared
-    // memory); fewer, longer CTAs also mean fewer red.global.add of partial tiles
-    int splits = 148 / (m_tiles * n_tiles);
+    // split the pixel range so that the grid is one wave (one CTA per SM: the ring takes the shared memory); fewer,
+    // longer CTAs also mean fewer red.global.add of partial tiles
+    int splits = num_sms() / (m_tiles * n_tiles);
     if (splits > p.n_pix_tiles) splits = p.n_pix_tiles;
     if (splits < 1) splits = 1;
     p.tiles_per_split = (p.n_pix_tiles + splits - 1) / splits;
@@ -406,7 +300,7 @@ extern "C" int pidm_colsum(const void* x, float* out, long long M, int C, int dt
     int oct = C / 8, rows = 256 / oct;
     if (rows < 1) rows = 1;
     int grid1 = (int)((M + rows * 8 - 1) / (rows * 8));
-    if (grid1 > 148 * 4) grid1 = 148 * 4;
+    if (grid1 > num_sms() * 4) grid1 = num_sms() * 4;
     if (grid1 < 1) grid1 = 1;
     PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(colsum_kernel<T>, dim3(grid1), dim3(oct * rows), C * sizeof(float),
                                                     (cudaStream_t)stream, (const T*)x, out, M, C)));

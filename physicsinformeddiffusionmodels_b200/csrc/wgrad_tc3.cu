@@ -1,4 +1,4 @@
-// Weight gradient of a stride-1 3x3 convolution on tcgen05, "tap-complete" tiling.
+// Weight gradient of a stride-1 3x3 convolution on the Hopper tensor cores (wgmma), "tap-complete" tiling.
 //
 //   dW[co][ci][tap] += sum_{pixels m} dy[m][co] * x[m shifted by tap][ci]
 //
@@ -6,7 +6,8 @@
 // MANY input channels, their addresses in the framework layout [co][ci][tap] are 9 floats apart, and the split-K
 // epilogue degenerates into scattered 4-byte red.global.add (16 K transactions per CTA; it dominated every layer
 // with few pixels).  Here a CTA owns ALL nine taps of a 32-channel chunk of ci and an NP-wide tile of co:
-//   * three TMEM accumulators (M = 128 rows each = 4 atoms of 32 channels),
+//   * three accumulators (M = 128 rows each = 4 atoms of 32 channels; each of the two consumer warpgroups holds
+//     rows 0-63 or 64-127 of all three in registers, so NP <= 64),
 //   * for a fixed co its 9 x 32 results are 288 CONTIGUOUS floats of dW: the epilogue transposes through shared
 //     memory and issues fully coalesced 128-byte reductions,
 //   * the dy tile (B operand) is fetched once per K' step for all nine taps (it was fetched by three CTAs before).
@@ -15,61 +16,12 @@
 //              three kernel rows r are row-shifted views of it -- atom j of accumulator q starts j * 8 pixel rows
 //              further down, which the MN-major descriptor expresses as LBO = 8 rows (the 4th atom is discarded).
 //   RG = false (small images, e.g. 8x8): nine separate boxes of 64 pixels, 12 atom slots (3 unused).
-#include "common.cuh"
+#include "hopper.cuh"
 #include "pidm.h"
-#include <cuda.h>
 
 namespace pidm {
 
-constexpr int W3_THREADS = 256;
-
-__device__ __forceinline__ uint32_t w3_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void w3_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(w3_smem(bar)), "r"(count));
-}
-__device__ __forceinline__ void w3_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(w3_smem(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void w3_mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(w3_smem(bar)), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-__device__ __forceinline__ void w3_tma_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-            w3_smem(dst)),
-        "l"(map), "r"(w3_smem(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ bool w3_elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-// MN-major swizzled UMMA descriptor: LBO = byte stride between swizzle atoms along M/N, SBO = between 8-row K groups
-template <int ROW_BYTES>
-__device__ __forceinline__ uint64_t w3_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-    constexpr uint64_t layout = ROW_BYTES == 128 ? 2 : (ROW_BYTES == 64 ? 4 : 6);
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((8 * ROW_BYTES) >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= layout << 61;
-    return d;
-}
+constexpr int W3_THREADS = 384;
 
 struct W3Params {
     int B, pad;
@@ -93,7 +45,6 @@ struct W3Cfg {
     static constexpr int TX_BYTES = B_BYTES + (RG ? 3 * A_BOX_RG : 9 * A_ATOM);
     static constexpr int STAGES_RAW = (184 * 1024) / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 4 ? 4 : STAGES_RAW;
-    static constexpr int TMEM_COLS = 3 * NP <= 128 ? 128 : (3 * NP <= 256 ? 256 : 512);
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
     static_assert(STAGES * STAGE_BYTES >= 32 * 288 * 4, "epilogue staging must fit in the ring");
 };
@@ -103,13 +54,11 @@ __global__ void __launch_bounds__(W3_THREADS, 1) wgrad3_kernel(const __grid_cons
                                                                const __grid_constant__ CUtensorMap map_dy, W3Params p) {
     using Cfg = W3Cfg<NP, AB, RG>;
     extern __shared__ unsigned char smem_raw[];
-    const uint32_t raw_addr = w3_smem(smem_raw);
+    const uint32_t raw_addr = smem_u32(smem_raw);
     unsigned char* ring = smem_raw + ((1024 - (raw_addr & 1023)) & 1023);
     uint64_t* bars = reinterpret_cast<uint64_t*>(ring + Cfg::STAGES * Cfg::STAGE_BYTES);
     uint64_t* full = bars;
     uint64_t* empty = bars + Cfg::STAGES;
-    uint64_t* acc_full = bars + 2 * Cfg::STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger();
@@ -124,162 +73,115 @@ __global__ void __launch_bounds__(W3_THREADS, 1) wgrad3_kernel(const __grid_cons
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_dy) : "memory");
     }
     if (warp == 1 && lane == 0) {
-        for (int s = 0; s < Cfg::STAGES; ++s) { w3_mbar_init(&full[s], 1); w3_mbar_init(&empty[s], 1); }
-        w3_mbar_init(acc_full, 1);
+        // a stage is free once all 8 consumer warps have retired the wgmmas that read it
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(w3_smem(tmem_slot)),
-                     "r"(Cfg::TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();
 
-    if (n_iters > 0) {
-        if (warp == 0) {
-            if (w3_elect_one()) {
-                // pixel tile index -> (sample group, tile row, tile column), walked incrementally
-                int tw_idx = pt_begin % p.tiles_w;
-                int t2 = pt_begin / p.tiles_w;
-                int th_idx = t2 % p.tiles_h, tb = t2 / p.tiles_h;
-                uint32_t st = 0, ph = 0;
-                unsigned char* stage = ring;
-                for (int it = 0; it < n_iters; ++it) {
-                    w3_mbar_wait(&empty[st], ph ^ 1);
-                    const int b0 = tb * p.TN, h0 = th_idx * p.TH, w0 = tw_idx * p.TW;
-                    unsigned char* a_dst = stage + Cfg::B_BYTES;
-                    w3_mbar_expect_tx(&full[st], Cfg::TX_BYTES);
+    if (n_iters <= 0) return;
+    if (warp == 0) {
+        if (elect_one()) {
+            // pixel tile index -> (sample group, tile row, tile column), walked incrementally
+            int tw_idx = pt_begin % p.tiles_w;
+            int t2 = pt_begin / p.tiles_w;
+            int th_idx = t2 % p.tiles_h, tb = t2 / p.tiles_h;
+            uint32_t st = 0, ph = 0;
+            unsigned char* stage = ring;
+            for (int it = 0; it < n_iters; ++it) {
+                mbar_wait(&empty[st], ph ^ 1);
+                const int b0 = tb * p.TN, h0 = th_idx * p.TH, w0 = tw_idx * p.TW;
+                unsigned char* a_dst = stage + Cfg::B_BYTES;
+                mbar_expect_tx(&full[st], Cfg::TX_BYTES);
 #pragma unroll
-                    for (int j = 0; j < Cfg::NBOX; ++j)
-                        w3_tma_4d(stage + j * Cfg::B_TILE, &map_dy, &full[st], n0 + j * AB, w0, h0, b0);
-                    if (RG) {
+                for (int j = 0; j < Cfg::NBOX; ++j)
+                    tma_load_4d(stage + j * Cfg::B_TILE, &map_dy, &full[st], n0 + j * AB, w0, h0, b0);
+                if (RG) {
 #pragma unroll
-                        for (int q = 0; q < 3; ++q)
-                            w3_tma_4d(a_dst + q * Cfg::A_RG_ALLOC, &map_x, &full[st], c0, w0 + q - p.pad, h0 - p.pad, b0);
-                    } else {
+                    for (int q = 0; q < 3; ++q)
+                        tma_load_4d(a_dst + q * Cfg::A_RG_ALLOC, &map_x, &full[st], c0, w0 + q - p.pad, h0 - p.pad, b0);
+                } else {
 #pragma unroll
-                        for (int tap = 0; tap < 9; ++tap)
-                            w3_tma_4d(a_dst + tap * Cfg::A_ATOM, &map_x, &full[st], c0, w0 + tap % 3 - p.pad,
-                                      h0 + tap / 3 - p.pad, b0);
-                    }
-                    if (++tw_idx == p.tiles_w) { tw_idx = 0; if (++th_idx == p.tiles_h) { th_idx = 0; ++tb; } }
-                    if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; stage = ring; } else stage += Cfg::STAGE_BYTES;
+                    for (int tap = 0; tap < 9; ++tap)
+                        tma_load_4d(a_dst + tap * Cfg::A_ATOM, &map_x, &full[st], c0, w0 + tap % 3 - p.pad,
+                                    h0 + tap / 3 - p.pad, b0);
                 }
+                if (++tw_idx == p.tiles_w) { tw_idx = 0; if (++th_idx == p.tiles_h) { th_idx = 0; ++tb; } }
+                if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; stage = ring; } else stage += Cfg::STAGE_BYTES;
             }
-        } else if (warp == 1) {
-            // D = f32, A = B = bf16, both MN-major (bits 15, 16), N>>3 at [17,23), M>>4 at [24,29)
-            constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) |
-                                       ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            if (w3_elect_one()) {
-                const uint32_t ring_addr = w3_smem(ring);
-                // accumulator t: RG -> halo box of kernel column t, atoms (kernel rows) 8 pixel rows = 512 B apart;
-                //                else -> atom slots 4t .. 4t+3, one atom apart
-                constexpr uint32_t a_lbo = RG ? 8 * 64 : Cfg::A_ATOM;
-                constexpr uint32_t a_acc_stride = RG ? Cfg::A_RG_ALLOC : 4 * Cfg::A_ATOM;
-                const uint64_t da0 = w3_desc_mn<64>(ring_addr + Cfg::B_BYTES, a_lbo);
-                const uint64_t db0 = w3_desc_mn<AB * 2>(ring_addr, Cfg::B_TILE);
-                constexpr uint32_t stage_lo = Cfg::STAGE_BYTES >> 4;
-                constexpr uint32_t ka_lo = (16 * 64) >> 4, kb_lo = (16 * AB * 2) >> 4, acc_lo = a_acc_stride >> 4;
-                uint32_t st = 0, ph = 0, off_lo = 0, accum = 0;
-                for (int it = 0; it < n_iters; ++it) {
-                    w3_mbar_wait(&full[st], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        }
+    } else if (warp >= 4) {
+        // ===== consumer warpgroup cg: rows [64 cg, 64 cg + 64) = atoms 2 cg, 2 cg + 1 of each accumulator =====
+        const int cg = (warp - 4) >> 2;
+        const uint32_t ring_addr = smem_u32(ring);
+        // accumulator t: RG -> halo box of kernel column t, atoms (kernel rows) 8 pixel rows = 512 B apart;
+        //                else -> atom slots 4t .. 4t+3, one atom apart
+        constexpr uint32_t a_lbo = RG ? 8 * 64 : Cfg::A_ATOM;
+        constexpr uint32_t a_acc_stride = RG ? Cfg::A_RG_ALLOC : 4 * Cfg::A_ATOM;
+        const uint32_t a_lo0 = gmma_desc_lo(ring_addr + Cfg::B_BYTES + 2 * cg * a_lbo, a_lbo);
+        const uint32_t b_lo0 = gmma_desc_lo(ring_addr, Cfg::B_TILE);
+        constexpr uint32_t a_hi = gmma_desc_hi<64>(), b_hi = gmma_desc_hi<AB * 2>();
+        constexpr uint32_t stage_lo = Cfg::STAGE_BYTES >> 4;
+        constexpr uint32_t ka_lo = (16 * 64) >> 4, kb_lo = (16 * AB * 2) >> 4, acc_lo = a_acc_stride >> 4;
+        float acc[3][NP / 2];
+        uint32_t st = 0, ph = 0, off_lo = 0, prev_st = 0;
+        for (int it = 0; it < n_iters; ++it) {
+            mbar_wait(&full[st], ph);
+            wgmma_fence();
 #pragma unroll
-                    for (int t = 0; t < 3; ++t) {
+            for (int t = 0; t < 3; ++t) {
 #pragma unroll
-                        for (int k = 0; k < Cfg::PX / 16; ++k) {
-                            const uint64_t da = da0 + (uint64_t)(off_lo + t * acc_lo + k * ka_lo);
-                            const uint64_t db = db0 + (uint64_t)(off_lo + k * kb_lo);
-                            const uint32_t acc_k = (k == 0) ? accum : 1u;
-                            asm volatile(
-                                "{\n\t.reg .pred p;\n\t"
-                                "setp.ne.b32 p, %4, 0;\n\t"
-                                "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_base + (uint32_t)(t * NP)),
-                                "l"(da), "l"(db), "r"(idesc), "r"(acc_k)
-                                : "memory");
-                        }
-                    }
-                    accum = 1;
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                     w3_smem(&empty[st]))
-                                 : "memory");
-                    if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; off_lo = 0; } else off_lo += stage_lo;
-                }
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                                 w3_smem(acc_full))
-                             : "memory");
+                for (int k = 0; k < Cfg::PX / 16; ++k)
+                    wgmma_bf16<1>(acc[t], gmma_desc(a_hi, a_lo0 + off_lo + t * acc_lo + k * ka_lo),
+                                  gmma_desc(b_hi, b_lo0 + off_lo + k * kb_lo), (it | k) != 0);
             }
-            __syncwarp();
-        } else if (warp >= 4) {
-            // ===== epilogue: warp q reads atom slot q of every accumulator (TMEM lane quarter q), lane = channel ci
-            const int quarter = warp & 3;
-            float* S = reinterpret_cast<float*>(ring);             // [32 co][288] staging, the ring is idle by now
-            w3_mbar_wait(acc_full, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int c = 0; c < NP; c += 32) {
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (it > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
+            prev_st = st;
+            if (++st == (uint32_t)Cfg::STAGES) { st = 0; ph ^= 1; off_lo = 0; } else off_lo += stage_lo;
+        }
+        wgmma_wait<0>();
+        // ===== epilogue: both warpgroups are done with the ring, which now stages S[32 co][ci * 9 + tap]
+        named_bar(1, 256);
+        float* S = reinterpret_cast<float*>(ring);
+        const int cw = warp - 4;                                   // consumer warp 0..7
+#pragma unroll
+        for (int c = 0; c < NP; c += 32) {
+            // fragment rows 64 cg + 16 (warp % 4) + lane / 4 + 8 i = (atom quarter, channel ci); columns 8 j + 2 (lane % 4)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int row = 64 * cg + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                const int quarter = row >> 5, ci = row & 31;
 #pragma unroll
                 for (int t = 0; t < 3; ++t) {
                     const int tap = RG ? quarter * 3 + t : t * 4 + quarter;        // RG: (r = quarter, q = t)
-                    const bool valid = RG ? quarter < 3 : tap < 9;                 // warp-uniform
+                    const bool valid = RG ? quarter < 3 : tap < 9;
                     if (!valid) continue;
-                    uint32_t v[32];
-                    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(t * NP + c);
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-                          "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-                          "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-                          "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                        : "r"(taddr));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    // S[co][ci * 9 + tap]: lanes are 9 floats apart -> conflict-free
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) S[j * 288 + lane * 9 + tap] = __uint_as_float(v[j]);
+                    for (int j = c / 8; j < c / 8 + 4; ++j) {
+                        const int col = 8 * j + 2 * (lane & 3) - c;
+                        S[col * 288 + ci * 9 + tap] = acc[t][4 * j + 2 * i];
+                        S[(col + 1) * 288 + ci * 9 + tap] = acc[t][4 * j + 2 * i + 1];
+                    }
                 }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                // 288 contiguous floats of dW per co: coalesced reductions, 8 output channels per warp
-#pragma unroll 1
-                for (int j = quarter; j < 32; j += 4) {
-                    float* dst = p.dw + (long long)(n0 + c + j) * p.s_col + (long long)c0 * 9;
-#pragma unroll
-                    for (int i = 0; i < 9; ++i) atomicAdd(dst + i * 32 + lane, S[j * 288 + i * 32 + lane]);
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
             }
+            named_bar(1, 256);
+            // 288 contiguous floats of dW per co: coalesced reductions, 4 output channels per warp
+#pragma unroll 1
+            for (int j = cw; j < 32; j += 8) {
+                float* dst = p.dw + (long long)(n0 + c + j) * p.s_col + (long long)c0 * 9;
+#pragma unroll
+                for (int i = 0; i < 9; ++i) atomicAdd(dst + i * 32 + lane, S[j * 288 + i * 32 + lane]);
+            }
+            named_bar(1, 256);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(Cfg::TMEM_COLS));
-    }
-}
-
-typedef CUresult (*W3EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static W3EncodeFn w3_get_encode() {
-    static W3EncodeFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (W3EncodeFn)ptr;
-    }
-    return fn;
 }
 
 static int w3_encode(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int atom, int bw, int bh, int bn) {
-    W3EncodeFn enc = w3_get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     PIDM_REQUIRE(enc != nullptr, "wgrad3: cuTensorMapEncodeTiled is not available from the driver");
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
@@ -340,13 +242,13 @@ int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, i
     }
     p.tiles_h = GH / p.TH; p.tiles_w = GW / p.TW;
     p.n_pix_tiles = (B / p.TN) * p.tiles_h * p.tiles_w;
-    const int NP = (CB % 128 == 0) ? 128 : ((CB % 64 == 0) ? 64 : 32);
+    const int NP = (CB % 64 == 0) ? 64 : 32;          // 3 x NP / 2 accumulator registers per consumer thread
     const int AB = (CB % 64 == 0) ? 64 : 32;
     CUtensorMap mx, my;
     if (int e = w3_encode(&mx, a, B, HA, WA, CA, 32, p.TW, rg ? p.TH + 3 : p.TH, p.TN)) return e;
     if (int e = w3_encode(&my, b, B, GH, GW, CB, AB, p.TW, p.TH, p.TN)) return e;
     const int chunks = CA / 32, n_tiles = CB / NP;
-    int splits = 148 / (chunks * n_tiles);
+    int splits = num_sms() / (chunks * n_tiles);
     if (splits > p.n_pix_tiles) splits = p.n_pix_tiles;
     if (splits < 1) splits = 1;
     p.tiles_per_split = (p.n_pix_tiles + splits - 1) / splits;
@@ -354,7 +256,7 @@ int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, i
     dim3 grid(chunks, n_tiles, splits);
 #define W3_CASE(np, ab) \
     if (NP == np && AB == ab) return rg ? w3_launch<np, ab, true>(mx, my, p, grid, st) : w3_launch<np, ab, false>(mx, my, p, grid, st)
-    W3_CASE(128, 64); W3_CASE(64, 64); W3_CASE(32, 32);
+    W3_CASE(64, 64); W3_CASE(32, 32);
 #undef W3_CASE
     return set_error(2, "wgrad3: no kernel for NP=%d AB=%d", NP, AB);
 }

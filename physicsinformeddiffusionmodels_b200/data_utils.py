@@ -1,5 +1,5 @@
 """Dataset classes with the reference's names and file formats (reference src/data_utils.py:31-119) and the host -> HBM
-staging the training loop needs on a B200 (`DevicePrefetcher`).
+staging the training loop needs on the GPU (`DevicePrefetcher`).
 
 * `Dataset`        one CSV per channel, one flattened P*P sample per row -> [N, C, P, P] held in RAM (Darcy study)
 * `Dataset_Paths`  one .npy per sample ([65, 65, 10], channels last on disk) -> [10, 65, 65] (mechanics study)

@@ -1,4 +1,4 @@
-"""Training-step engine: the body of the reference's loop (main.py:157-183) as a B200-native step.
+"""Training-step engine: the body of the reference's loop (main.py:157-183) as a H100-native step.
 
     q_sample -> U-Net -> x0_hat -> Darcy residual + loss (fused) -> backward -> [NCCL all-reduce of ONE flat
     fp32 gradient buffer] -> global-norm clip + Adam + EMA (one fused kernel over the flat buffers)
@@ -124,8 +124,7 @@ class TrainEngine:
         # bucketed_allreduce=False selects the single all-reduce behind the last weight gradient): the flat gradient is
         # laid out in three readiness groups and a group is all-reduced on its own stream as soon as backward has crossed
         # the matching boundary of the U-Net.  scripts/check_ddp.py (2 GPUs): ranks stay bitwise identical, exchanged
-        # gradient equal to the single all-reduce to 2e-5 (fp32 atomics), eager and CUDA graph.  Measured per step at
-        # batch 32 per GPU: N = 2 3.800 -> 3.767 ms, N = 8 3.815 -> 3.781 ms (single GPU 3.58 ms).
+        # gradient equal to the single all-reduce to 2e-5 (fp32 atomics), eager and CUDA graph.
         if bucketed_allreduce is None:
             import os
             bucketed_allreduce = world > 1 and os.environ.get('PIDM_BUCKET_AR', '1') != '0'
@@ -260,7 +259,7 @@ class TrainEngine:
 
 
 class SampleEngine:
-    """B200-native ancestral sampling loop (reference denoising_utils.py:388-545 p_sample / p_sample_loop, called from
+    """H100-native ancestral sampling loop (reference denoising_utils.py:388-545 p_sample / p_sample_loop, called from
     sample.py:145): the same per-step work as DenoisingDiffusion.p_sample -- x0 estimate through the residual object
     (network call, or the DDIM walk when use_ddim_x0), Darcy residual, posterior step with sigma_t = sqrt(beta_t) --
     but with the time index and the posterior coefficients living on the DEVICE, so that a captured CUDA graph of

@@ -49,7 +49,7 @@ def _grad_buffer(p):
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError('physicsinformeddiffusionmodels_b200 runs on CUDA (B200) only: got a CPU tensor. '
+            raise RuntimeError('physicsinformeddiffusionmodels_b200 runs on CUDA (H100) only: got a CPU tensor. '
                                'There is no CPU fallback on the product path.')
 
 

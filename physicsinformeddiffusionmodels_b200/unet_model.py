@@ -389,7 +389,7 @@ class Unet3D(nn.Module):
         elif x.dim() != 4:
             raise ValueError('Input must be image [BxCxPxP] or image sequence [BxCxFxPxP].')
         if not x.is_cuda:
-            raise RuntimeError('Unet3D (B200 engine) needs CUDA tensors: no CPU fallback on the product path')
+            raise RuntimeError('Unet3D (CUDA engine) needs CUDA tensors: no CPU fallback on the product path')
         dt = ops.act_dtype()
         # the weight re-packing (one launch over all layers) runs on a forked stream and overlaps the input layout
         # change and the time-conditioning MLPs; it is joined before the first convolution

@@ -1,4 +1,4 @@
-"""configs[2] (topology optimisation / linear elasticity): the mechanics branch of the training loss through the B200
+"""configs[2] (topology optimisation / linear elasticity): the mechanics branch of the training loss through the
 engine against the UNMODIFIED reference (tests/golden/mechanics_loss.pt, dense 8450 x 8450 assembly) and against the CPU
 oracle at the reference's model size (Unet3D dim=128, channels=10, out_dim=3; main.py:102-109,126), and the
 TrainEngine (flat buffers, fused Adam/EMA, CUDA graph) on that branch."""

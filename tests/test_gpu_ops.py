@@ -111,7 +111,7 @@ TC_CASES = [
 
 @pytest.mark.parametrize('case', TC_CASES, ids=[f'B{c[0]}_H{c[1]}_C{c[2]}x{c[3]}_k{c[4]}' for c in TC_CASES])
 def test_conv_tcgen05_matches_reference(pk, case):
-    """tcgen05/TMA kernel vs fp32 F.conv2d on bf16-representable operands: only accumulation order and the bf16
+    """wgmma/TMA kernel vs fp32 F.conv2d on bf16-representable operands: only accumulation order and the bf16
     rounding of the OUTPUT differ -> 1e-2 relative (bf16 has 8 mantissa bits: 2^-9 per element)."""
     ops, packing = pk
     from physicsinformeddiffusionmodels_b200._lib import call
@@ -142,7 +142,7 @@ def test_conv_tcgen05_matches_reference(pk, case):
     torch.cuda.synchronize()
     e_tc, e_simt = rel(nchw(y), yr), rel(nchw(y_simt), yr)
     assert e_simt < 1e-2, f'simt reference itself off: {e_simt}'
-    assert e_tc < 1e-2, f'tcgen05 conv off: rel {e_tc} (simt {e_simt})'
+    assert e_tc < 1e-2, f'tensor-core conv off: rel {e_tc} (simt {e_simt})'
 
 
 def test_conv_tcgen05_dgrad(pk):
@@ -557,7 +557,7 @@ WG_CASES = [
 
 @pytest.mark.parametrize('case', WG_CASES, ids=[f'B{c[0]}_H{c[1]}_C{c[2]}x{c[3]}_k{c[4]}' for c in WG_CASES])
 def test_wgrad_tcgen05_matches_reference(pk, case):
-    """tcgen05 wgrad (MN-major TMA operands, split over pixels, fp32 atomics) vs autograd of F.conv2d on
+    """wgmma wgrad (MN-major TMA operands, split over pixels, fp32 atomics) vs autograd of F.conv2d on
     bf16-representable operands: fp32 accumulation both sides -> 2e-3 (summation order over up to 131072 pixels)."""
     ops, packing = pk
     from physicsinformeddiffusionmodels_b200._lib import call, stream
@@ -599,7 +599,7 @@ TC_GENERAL_CASES = [
 @pytest.mark.parametrize('case', TC_GENERAL_CASES, ids=[c[0] for c in TC_GENERAL_CASES])
 def test_conv_tcgen05_strided_transposed_and_stem(pk, case):
     """Stride-2 conv (TMA elementStrides), stride-2 transposed conv (4 output-parity classes) and the channel-padded
-    7x7 stem through the tcgen05 kernels: forward, dgrad and wgrad vs autograd of torch conv ops on bf16-representable
+    7x7 stem through the tensor-core (wgmma) kernels: forward, dgrad and wgrad vs autograd of torch conv ops on bf16-representable
     operands (1e-2: bf16 rounding of outputs)."""
     ops, packing = pk
     from physicsinformeddiffusionmodels_b200._lib import call
