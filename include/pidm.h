@@ -167,14 +167,18 @@ int pidm_layernorm_c_bwd(const void* x, const void* dy, const float* gamma, void
 /* Linear attention fused with its to_qkv 1x1 projection (C = 32 input channels, 8 heads, bf16): q, k, v are recomputed
  * per head on the tensor cores from xn = PreNorm(x) instead of being materialised (reference unet_model.py:275-297 --
  * `qkv = self.to_qkv(x)` and everything after it).  w_qkv = packed to_qkv weights [768][32] bf16 (pidm_pack_weights).
- * Forward keeps ctx / kmax / kzinv for backward; backward returns dqkv [B,N,768] (gradient w.r.t. xn W^T) for the
- * ordinary dgrad / wgrad of to_qkv.  dctx is scratch. */
+ * Forward keeps ctx / kmax / kzinv for backward.  Backward writes dxn [B,N,32] bf16 (gradient w.r.t. xn through
+ * qkv = xn W^T) and fills dctx [B,8,32,32]; the weight-gradient pass then reads dctx and ACCUMULATES the to_qkv weight
+ * gradient into grad_w (fp32, element [n][c] at n * w_stride_n + c * w_stride_c).  Neither materialises dqkv. */
 int pidm_linattn_fused_supported(int C, int heads, int N, int dtype);
 int pidm_linattn_fused_workspace_floats(int B, int N);
 int pidm_linattn_fused_fwd(const void* xn, const void* w_qkv, void* out, float* ctx, float* kmax, float* kzinv,
                            float* workspace, int B, int N, void* stream);
 int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const void* dout, const float* ctx, const float* kmax,
-                           const float* kzinv, void* dqkv, float* dctx, int B, int N, void* stream);
+                           const float* kzinv, void* dxn, float* dctx, int B, int N, void* stream);
+int pidm_linattn_fused_wgrad(const void* xn, const void* w_qkv, const void* dout, const float* ctx, const float* dctx,
+                             const float* kmax, const float* kzinv, float* grad_w, int B, int N, long long w_stride_n,
+                             long long w_stride_c, void* stream);
 int pidm_linattn_workspace_floats(int B, int N, int heads);
 int pidm_linattn_fwd(const void* qkv, void* out, float* ctx, float* kmax, float* kzinv, float* workspace, int B, int N,
                      int heads, int dtype, void* stream);

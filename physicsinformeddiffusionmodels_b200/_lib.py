@@ -58,6 +58,7 @@ _SIGS = {
     'pidm_linattn_fused_workspace_floats': [I, I],
     'pidm_linattn_fused_fwd': [P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_fused_bwd': [P, P, P, P, P, P, P, P, I, I, P],
+    'pidm_linattn_fused_wgrad': [P, P, P, P, P, P, P, P, I, I, L, L, P],
     'pidm_linattn_fwd': [P, P, P, P, P, P, I, I, I, I, P],
     'pidm_linattn_bwd': [P, P, P, P, P, P, P, I, I, I, I, P],
     'pidm_attn_fwd': [P, P, I, I, I, I, P],

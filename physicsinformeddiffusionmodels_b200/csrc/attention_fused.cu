@@ -5,7 +5,9 @@
 // streaming it back through the statistics / context / output / backward kernels was ~1.2 GB of HBM traffic per layer.
 // Here every warp (one head) recomputes its q / k / v slices on the tensor cores from the 64-byte pixel rows of the
 // normalised input xn -- a 32x32x32 mma.sync product per 32 pixels -- so that forward reads xn (8 MB) and writes
-// `out` only, and backward reads xn + dout and writes dqkv once (consumed by the unchanged dgrad / wgrad of to_qkv).
+// `out` only.  Backward recomputes them the same way in two passes over (xn, dout): one multiplies dq | dk | dv by W
+// and writes dxn (8 MB), the other multiplies them by xn into the to_qkv weight gradient; the [B, N, 768] dqkv is
+// never written either.
 // All intermediate tiles stay in registers: accumulator fragments are converted to A fragments directly and to
 // transposed (K-major) fragments with movmatrix; only xn / dout tiles and the output staging touch shared memory.
 // The two paths differ only by the bf16 rounding of the (here never materialised) q, k, v.
@@ -380,59 +382,157 @@ __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __res
     }
 }
 
-// ---- backward per pixel: dq | dk | dv from xn, dout, ctx, dctx and the saved column statistics -------------------------
-// 217 registers (the nine loop-invariant 32x32 B-operand fragment sets live in registers): one CTA = 8 warps per SM.
-// Capping the kernel at 128 registers for two CTAs per SM makes ptxas spill ~70 fragment registers to local memory:
-// occupancy does not pay for re-reading the operands.
+// ---- backward: dq | dk | dv per 16-pixel tile from xn, dout, ctx, dctx and the saved column statistics ----------------
+//   dq = s p (dp - sum_d p dp),  dp = dout ctx^T,  p = softmax_d(q)
+//   dk = k~ (dk~ - cd),          dk~ = (v / N) dctx^T,  k~ = exp(k - M) Zinv,  cd[d] = sum_e dctx[d][e] ctx[d][e]
+//   dv = (k~ dctx) / N
+// Neither pass below writes dq, dk or dv: the input-gradient pass multiplies them by W on the spot, the weight-gradient
+// pass multiplies them by xn.  They enter those products as bf16 tensor-core operands, like every other mma operand.
 constexpr int LFB_ROWS = 16;
 constexpr int LFB_STAGES = 4;
-constexpr int LFB_STAGE_ELEMS = 2 * LFB_ROWS * LW_PITCH;          // xn tile | dout tile
-constexpr int LFB_OUT_ELEMS = 3 * LFB_ROWS * LW_PITCH;            // dq | dk | dv staging
+constexpr int LFB_TILE = LFB_ROWS * LW_PITCH;                       // one [16 px][32] bf16 tile
+
+struct LfbTile {                     // what every head needs from one 16-pixel tile (A fragments of xn and of dout)
+    uint32_t ax[1][2][4], ag[2][4];
+};
+// dq (fp32 accumulator fragment [16 px][32 d])
+__device__ __forceinline__ void lfb_dq(float (&dq)[4][4], const LfbTile& tl, const uint32_t (&wq)[2][4][2],
+                                       const uint32_t (&bc)[2][4][2], float scale) {
+    float c1[1][4][4], c2[4][4];
+    project<1>(c1, tl.ax, wq);
+    frag_softmax(c1[0], 1.f);
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) c2[nt][i] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) mma_bf16(c2[nt], tl.ag[ks], bc[ks][nt][0], bc[ks][nt][1]);
+    }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        float dot = 0.f;
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+            dot += c1[0][nt][half * 2] * c2[nt][half * 2] + c1[0][nt][half * 2 + 1] * c2[nt][half * 2 + 1];
+        dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+        dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) dq[nt][half * 2 + j] = scale * c1[0][nt][half * 2 + j] * (c2[nt][half * 2 + j] - dot);
+    }
+}
+// dk and dv (fp32 accumulator fragments [16 px][32 d])
+__device__ __forceinline__ void lfb_dkdv(float (&dk)[4][4], float (&dv)[4][4], const uint32_t (&ax)[1][2][4],
+                                         const uint32_t (&wk)[2][4][2], const uint32_t (&wv)[2][4][2],
+                                         const uint32_t (&bd)[2][4][2], const uint32_t (&bt)[2][4][2],
+                                         const float (&Mc)[8], const float (&Zc)[8], const float (&cdc)[8], float invN) {
+    float c1[1][4][4];
+    uint32_t a[2][4];
+    project<1>(c1, ax, wv);
+    c_to_a(a, c1[0]);
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) {               // dk~ N = v dctx^T
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dk[nt][i] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) mma_bf16(dk[nt], a[ks], bd[ks][nt][0], bd[ks][nt][1]);
+    }
+    project<1>(c1, ax, wk);
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            c1[0][nt][i] = __expf(c1[0][nt][i] - Mc[nt * 2 + (i & 1)]) * Zc[nt * 2 + (i & 1)];
+            dk[nt][i] = c1[0][nt][i] * (dk[nt][i] * invN - cdc[nt * 2 + (i & 1)]);
+        }
+    c_to_a(a, c1[0]);
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dv[nt][i] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) mma_bf16(dv[nt], a[ks], bt[ks][nt][0], bt[ks][nt][1]);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dv[nt][i] *= invN;
+    }
+}
+// loop-invariant per-head operands: cd (through a 32-float shared scratch), column statistics, B fragments of ctx / dctx
+__device__ __forceinline__ void lfb_cd(float (&cdc)[8], float* scd, const float* __restrict__ cg, const float* __restrict__ dg,
+                                       int lane) {
+    float s = 0.f;                     // cd[d] = sum_e dctx[d][e] ctx[d][e]   (lane = d)
+#pragma unroll
+    for (int e = 0; e < LM_D; e += 4) {
+        const float4 x = *reinterpret_cast<const float4*>(dg + lane * LM_D + e);
+        const float4 y = *reinterpret_cast<const float4*>(cg + lane * LM_D + e);
+        s += x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
+    }
+    scd[lane] = s;
+    __syncwarp();
+    load_cols(cdc, scd, lane);
+}
+
+// ---- pass A (input gradient): dxn = sum_h dq_h Wq_h + dk_h Wk_h + dv_h Wv_h -----------------------------------------
+// The eight warps (= heads) of a CTA step through the same 16-pixel tiles, sharing one xn tile.  A warp multiplies its
+// head's dq | dk | dv by its 32-row slices of W at once (B fragments [k = d][n = c] by ldmatrix.trans from a shared
+// copy of W), leaving a [16 px][32] fp32 partial; the eight partials are summed through shared memory and dxn is
+// written once, in bf16.  The nine loop-invariant 32x32 B-operand fragment sets stay in registers: one CTA per SM.
+constexpr int LFB_STAGE_ELEMS = (1 + LM_HEADS) * LFB_TILE;         // xn tile | the eight heads' dout tiles
+constexpr int LFB_W_PITCH = LF_C + 8;                              // W copy [768][40] bf16: conflict-free ldmatrix
+constexpr int LFB_R_PITCH = LF_C + 8;                              // fp32 partial rows: conflict-free float2 stores
+constexpr size_t LAF_BWD_SMEM = (size_t)LFB_STAGES * LFB_STAGE_ELEMS * 2 + (size_t)3 * LM_HID * LFB_W_PITCH * 2 +
+                                (size_t)LM_HEADS * LFB_ROWS * LFB_R_PITCH * 4 + (size_t)LM_HEADS * LM_D * 4;
+
+// c[16 px][32 c] += g[16 px][32 d] Wh[d][c]   (g as A fragments; Wh = one head's 32 rows of the shared W copy)
+__device__ __forceinline__ void mma_w(float (&c)[4][4], const uint32_t (&g)[2][4], const __nv_bfloat16* Wh, int lane) {
+#pragma unroll
+    for (int kd = 0; kd < 2; ++kd)
+#pragma unroll
+        for (int np = 0; np < 2; ++np) {
+            uint32_t bw[4];
+            frag_b_krows(bw, Wh, LFB_W_PITCH, kd * 16, np * 16, lane);
+            mma_bf16(c[2 * np], g[kd], bw[0], bw[1]);
+            mma_bf16(c[2 * np + 1], g[kd], bw[2], bw[3]);
+        }
+}
+
 __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
                                                       const __nv_bfloat16* __restrict__ dout, const float* __restrict__ ctx,
                                                       const float* __restrict__ dctx, const float* __restrict__ kmax,
-                                                      const float* __restrict__ kzinv, __nv_bfloat16* __restrict__ dqkv,
+                                                      const float* __restrict__ kzinv, __nv_bfloat16* __restrict__ dxn,
                                                       int N, int chunk_px, float scale) {
     pdl_trigger();
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFB_STAGES * LFB_STAGE_ELEMS + LFB_OUT_ELEMS);
-    __nv_bfloat16* Os = ring + LFB_STAGES * LFB_STAGE_ELEMS;
-    float* scd = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * (LFB_STAGES * LFB_STAGE_ELEMS + LFB_OUT_ELEMS) * 2) + h * LM_D;
+    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw);
+    __nv_bfloat16* Ws = ring + LFB_STAGES * LFB_STAGE_ELEMS;
+    float* R = reinterpret_cast<float*>(Ws + 3 * LM_HID * LFB_W_PITCH);
+    float* scd = R + LM_HEADS * LFB_ROWS * LFB_R_PITCH + h * LM_D;
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / LFB_ROWS;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
     const __nv_bfloat16* gsrc = dout + pix0 * LM_HID + h * LM_D;
-    __nv_bfloat16* ddst = dqkv + pix0 * 3 * LM_HID + h * LM_D;
+    for (int i = threadIdx.x; i < 3 * LM_HID * (LF_C / 8); i += blockDim.x)      // W -> smem: the oldest copy group
+        cp_async16(Ws + (i >> 2) * LFB_W_PITCH + (i & 3) * 8, W + (size_t)(i >> 2) * LF_C + (i & 3) * 8);
+    cp_commit();
     auto issue = [&](int it) {
         if (it < n_tiles) {
             __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * LFB_STAGE_ELEMS;
-            lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-            lw_issue<LFB_ROWS>(buf + LFB_ROWS * LW_PITCH, gsrc + (size_t)it * LFB_ROWS * LM_HID, LM_HID, lane);
+            if (h == 0) lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
+            lw_issue<LFB_ROWS>(buf + (1 + h) * LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LM_HID, LM_HID, lane);
         }
         cp_commit();
     };
 #pragma unroll
-    for (int s = 0; s < LFB_STAGES; ++s) issue(s);
+    for (int s = 0; s < LFB_STAGES - 1; ++s) issue(s);
     const float* cg = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
     const float* dg = dctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
-    {
-        float s = 0.f;                 // cd[d] = sum_e dctx[d][e] ctx[d][e]   (lane = d)
-#pragma unroll
-        for (int e = 0; e < LM_D; e += 4) {
-            const float4 x = *reinterpret_cast<const float4*>(dg + lane * LM_D + e);
-            const float4 y = *reinterpret_cast<const float4*>(cg + lane * LM_D + e);
-            s += x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
-        }
-        scd[lane] = s;
-    }
-    __syncwarp();
     float Mc[8], Zc[8], cdc[8];
+    lfb_cd(cdc, scd, cg, dg, lane);
     load_cols(Mc, kmax + (size_t)b * LM_HID + h * LM_D, lane);
     load_cols(Zc, kzinv + (size_t)b * LM_HID + h * LM_D, lane);
-    load_cols(cdc, scd, lane);
     uint32_t wq[2][4][2], wk[2][4][2], wv[2][4][2];
     load_w_frags(wq, W + (size_t)(h * LM_D) * LF_C, lane);
     load_w_frags(wk, W + (size_t)(LM_HID + h * LM_D) * LF_C, lane);
@@ -448,95 +548,197 @@ __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __res
         }
     const int g = lane >> 2, t = lane & 3;
     const float invN = 1.f / (float)N;
-    __nv_bfloat16* Oq = Os;
-    __nv_bfloat16* Ok = Os + LFB_ROWS * LW_PITCH;
-    __nv_bfloat16* Ov = Os + 2 * LFB_ROWS * LW_PITCH;
+    const __nv_bfloat16* Wq = Ws + (size_t)(h * LM_D) * LFB_W_PITCH;
+    const __nv_bfloat16* Wk = Wq + (size_t)LM_HID * LFB_W_PITCH;
+    const __nv_bfloat16* Wv = Wk + (size_t)LM_HID * LFB_W_PITCH;
+    float* Rw = R + h * LFB_ROWS * LFB_R_PITCH;
+    const int rrow = threadIdx.x >> 4, rcol = (threadIdx.x & 15) * 2;     // the two dxn elements this thread sums
     for (int it = 0; it < n_tiles; ++it) {
-        cp_wait<LFB_STAGES - 1>();
-        __syncwarp();
+        cp_wait<LFB_STAGES - 2>();
+        __syncthreads();                           // tile `it` is visible to every warp; slot (it - 1) is free
+        issue(it + LFB_STAGES - 1);
         const __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * LFB_STAGE_ELEMS;
-        uint32_t ax[1][2][4], ag[2][4];
-        load_x_frags<1>(ax, buf, lane);
-        frag_a_rowmajor(ag[0], buf + LFB_ROWS * LW_PITCH, LW_PITCH, 0, 0, lane);      // dout [px][e]
-        frag_a_rowmajor(ag[1], buf + LFB_ROWS * LW_PITCH, LW_PITCH, 0, 16, lane);
-        __syncwarp();                              // the tile is in registers
-        issue(it + LFB_STAGES);
-        float c1[1][4][4], c2[4][4];
-        // ---- dq = s * p * (dp - sum_d p dp),  dp = dout ctx^T,  p = softmax_d(q) (bf16-rounded like the unfused path)
-        project<1>(c1, ax, wq);
-        frag_softmax(c1[0], 1.f);
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) c2[nt][i] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) mma_bf16(c2[nt], ag[ks], bc[ks][nt][0], bc[ks][nt][1]);
-        }
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            float dot = 0.f;
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-                dot += c1[0][nt][half * 2] * c2[nt][half * 2] + c1[0][nt][half * 2 + 1] * c2[nt][half * 2 + 1];
-            dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-            dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-                *reinterpret_cast<uint32_t*>(Oq + (g + half * 8) * LW_PITCH + nt * 8 + 2 * t) =
-                    pack_bf16(scale * c1[0][nt][half * 2] * (c2[nt][half * 2] - dot),
-                              scale * c1[0][nt][half * 2 + 1] * (c2[nt][half * 2 + 1] - dot));
-        }
-        // ---- dk = k~ * (dk~ - cd),  dk~ = (v / N) dctx^T,  k~ = exp(k - M) Zinv
-        uint32_t av[2][4], ak[2][4];
-        project<1>(c1, ax, wv);
-        c_to_a(av, c1[0]);
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) c2[nt][i] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) mma_bf16(c2[nt], av[ks], bd[ks][nt][0], bd[ks][nt][1]);
-        }
-        project<1>(c1, ax, wk);
+        LfbTile tl;
+        load_x_frags<1>(tl.ax, buf, lane);
+        frag_a_rowmajor(tl.ag[0], buf + (1 + h) * LFB_TILE, LW_PITCH, 0, 0, lane);      // dout [px][e]
+        frag_a_rowmajor(tl.ag[1], buf + (1 + h) * LFB_TILE, LW_PITCH, 0, 16, lane);
+        float dx[4][4];
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-                c1[0][nt][i] = __expf(c1[0][nt][i] - Mc[nt * 2 + (i & 1)]) * Zc[nt * 2 + (i & 1)];
-        c_to_a(ak, c1[0]);
-#pragma unroll
-        for (int half = 0; half < 2; ++half)
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-                *reinterpret_cast<uint32_t*>(Ok + (g + half * 8) * LW_PITCH + nt * 8 + 2 * t) =
-                    pack_bf16(c1[0][nt][half * 2] * (c2[nt][half * 2] * invN - cdc[nt * 2]),
-                              c1[0][nt][half * 2 + 1] * (c2[nt][half * 2 + 1] * invN - cdc[nt * 2 + 1]));
-        // ---- dv = (k~ dctx) / N
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) c2[nt][i] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) mma_bf16(c2[nt], ak[ks], bt[ks][nt][0], bt[ks][nt][1]);
+            for (int i = 0; i < 4; ++i) dx[nt][i] = 0.f;
+        uint32_t a[2][4];
+        {
+            float dq[4][4];
+            lfb_dq(dq, tl, wq, bc, scale);
+            c_to_a(a, dq);
+            mma_w(dx, a, Wq, lane);
+        }
+        {
+            float dk[4][4], dv[4][4];
+            lfb_dkdv(dk, dv, tl.ax, wk, wv, bd, bt, Mc, Zc, cdc, invN);
+            c_to_a(a, dk);
+            mma_w(dx, a, Wk, lane);
+            c_to_a(a, dv);
+            mma_w(dx, a, Wv, lane);
         }
 #pragma unroll
-        for (int half = 0; half < 2; ++half)
+        for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-                *reinterpret_cast<uint32_t*>(Ov + (g + half * 8) * LW_PITCH + nt * 8 + 2 * t) =
-                    pack_bf16(c2[nt][half * 2] * invN, c2[nt][half * 2 + 1] * invN);
+            for (int half = 0; half < 2; ++half)
+                *reinterpret_cast<float2*>(Rw + (g + half * 8) * LFB_R_PITCH + nt * 8 + 2 * t) =
+                    make_float2(dx[nt][half * 2], dx[nt][half * 2 + 1]);
+        __syncthreads();                           // the eight head partials of this tile are in R
+        float sx = 0.f, sy = 0.f;
+#pragma unroll
+        for (int w = 0; w < LM_HEADS; ++w) {
+            const float2 v = *reinterpret_cast<const float2*>(R + (w * LFB_ROWS + rrow) * LFB_R_PITCH + rcol);
+            sx += v.x;
+            sy += v.y;
+        }
+        *reinterpret_cast<uint32_t*>(dxn + (pix0 + (size_t)it * LFB_ROWS + rrow) * LF_C + rcol) = pack_bf16(sx, sy);
+    }
+}
+
+// ---- pass B (weight gradient): dW_h = [dq | dk | dv]_h^T xn over the CTA's pixels, one reduction per CTA ---------------
+// PART 0 accumulates dWq (reads xn and dout), PART 1 dWk and dWv (reads xn only): split so that neither instantiation
+// holds more than 64 accumulators next to its operand fragments.  Warps are independent (one head each, own tiles).
+// The [32 d][32 c] sums leave through shared memory as coalesced 128-byte red.global.add rows of the fp32 gradient.
+template <int PART>
+struct LfwCfg {
+    static constexpr int MATS = PART == 0 ? 1 : 2;
+    static constexpr int STAGE_ELEMS = (PART == 0 ? 2 : 1) * LFB_TILE;     // xn tile (| dout tile)
+    static constexpr int S_PITCH = LM_D + 1;                                 // epilogue staging [32 d][33] fp32
+    static_assert(LFB_STAGES * STAGE_ELEMS * 2 >= LM_D * S_PITCH * 4, "the epilogue staging reuses the tile ring");
+    static constexpr size_t SMEM = (size_t)LM_HEADS * (LFB_STAGES * STAGE_ELEMS * 2 + LM_D * 4);
+};
+
+// acc[32 d][32 c] += gf^T x over one 16-pixel tile: gf = accumulator fragment [16 px][32 d], bx = B fragments
+// [k = px][n = c] of the xn tile (two n-tile pairs)
+__device__ __forceinline__ void acc_gtx(float (&acc)[2][4][4], const float (&gf)[4][4], const uint32_t (&bx)[2][4]) {
+#pragma unroll
+    for (int md = 0; md < 2; ++md) {               // A[d][px]: transposed 8x8 blocks of the accumulator fragment
+        uint32_t a[4];
+        a[0] = movm_t(pack_bf16(gf[2 * md][0], gf[2 * md][1]));
+        a[1] = movm_t(pack_bf16(gf[2 * md + 1][0], gf[2 * md + 1][1]));
+        a[2] = movm_t(pack_bf16(gf[2 * md][2], gf[2 * md][3]));
+        a[3] = movm_t(pack_bf16(gf[2 * md + 1][2], gf[2 * md + 1][3]));
+#pragma unroll
+        for (int np = 0; np < 2; ++np) {
+            mma_bf16(acc[md][2 * np], a, bx[np][0], bx[np][1]);
+            mma_bf16(acc[md][2 * np + 1], a, bx[np][2], bx[np][3]);
+        }
+    }
+}
+
+template <int PART>
+__global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
+                                                        const __nv_bfloat16* __restrict__ dout, const float* __restrict__ ctx,
+                                                        const float* __restrict__ dctx, const float* __restrict__ kmax,
+                                                        const float* __restrict__ kzinv, float* __restrict__ grad_w, int N,
+                                                        int chunk_px, long long w_stride_n, long long w_stride_c, float scale) {
+    pdl_trigger();
+    pdl_wait();
+    extern __shared__ __align__(16) unsigned char raw[];
+    constexpr int MATS = LfwCfg<PART>::MATS, STAGE_ELEMS = LfwCfg<PART>::STAGE_ELEMS, S_PITCH = LfwCfg<PART>::S_PITCH;
+    const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
+    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFB_STAGES * STAGE_ELEMS);
+    float* scd = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFB_STAGES * STAGE_ELEMS * 2) + h * LM_D;
+    const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
+    const int n_tiles = (n_end - n_begin) / LFB_ROWS;
+    const size_t pix0 = (size_t)b * N + n_begin;
+    const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
+    const __nv_bfloat16* gsrc = dout + pix0 * LM_HID + h * LM_D;
+    auto issue = [&](int it) {
+        if (it < n_tiles) {
+            __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * STAGE_ELEMS;
+            lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
+            if (PART == 0) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LM_HID, LM_HID, lane);
+        }
+        cp_commit();
+    };
+#pragma unroll
+    for (int s = 0; s < LFB_STAGES; ++s) issue(s);
+    const float* cg = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
+    const float* dg = dctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
+    float Mc[8], Zc[8], cdc[8];
+    uint32_t w0[2][4][2], w1[2][4][2];             // PART 0: Wq, (unused)   PART 1: Wk, Wv
+    uint32_t b0[2][4][2], b1[2][4][2];             // PART 0: ctx^T, (unused)   PART 1: dctx^T, dctx
+    if (PART == 0) {
+        load_w_frags(w0, W + (size_t)(h * LM_D) * LF_C, lane);
+    } else {
+        lfb_cd(cdc, scd, cg, dg, lane);
+        load_cols(Mc, kmax + (size_t)b * LM_HID + h * LM_D, lane);
+        load_cols(Zc, kzinv + (size_t)b * LM_HID + h * LM_D, lane);
+        load_w_frags(w0, W + (size_t)(LM_HID + h * LM_D) * LF_C, lane);
+        load_w_frags(w1, W + (size_t)(2 * LM_HID + h * LM_D) * LF_C, lane);
+    }
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+            frag_b_global<false>(b0[ks][nt], PART == 0 ? cg : dg, ks * 16, nt * 8, lane);
+            if (PART == 1) frag_b_global<true>(b1[ks][nt], dg, ks * 16, nt * 8, lane);
+        }
+    const float invN = 1.f / (float)N;
+    float acc[MATS][2][4][4];
+#pragma unroll
+    for (int m = 0; m < MATS; ++m)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int k = 0; k < 4; ++k) acc[m][i][j][k] = 0.f;
+    for (int it = 0; it < n_tiles; ++it) {
+        cp_wait<LFB_STAGES - 1>();
         __syncwarp();
-        __nv_bfloat16* d = ddst + (size_t)it * LFB_ROWS * 3 * LM_HID;
-        lw_store<LFB_ROWS>(d, 3 * LM_HID, Oq, lane);
-        lw_store<LFB_ROWS>(d + LM_HID, 3 * LM_HID, Ok, lane);
-        lw_store<LFB_ROWS>(d + 2 * LM_HID, 3 * LM_HID, Ov, lane);
+        const __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * STAGE_ELEMS;
+        LfbTile tl;
+        load_x_frags<1>(tl.ax, buf, lane);
+        uint32_t bx[2][4];
+        frag_b_krows(bx[0], buf, LW_PITCH, 0, 0, lane);        // B[k = px][n = c] = xn[px][c]
+        frag_b_krows(bx[1], buf, LW_PITCH, 0, 16, lane);
+        if (PART == 0) {
+            frag_a_rowmajor(tl.ag[0], buf + LFB_TILE, LW_PITCH, 0, 0, lane);
+            frag_a_rowmajor(tl.ag[1], buf + LFB_TILE, LW_PITCH, 0, 16, lane);
+        }
+        __syncwarp();                              // the tile is in registers
+        issue(it + LFB_STAGES);
+        if (PART == 0) {
+            float dq[4][4];
+            lfb_dq(dq, tl, w0, b0, scale);
+            acc_gtx(acc[0], dq, bx);
+        } else {
+            float dk[4][4], dv[4][4];
+            lfb_dkdv(dk, dv, tl.ax, w0, w1, b0, b1, Mc, Zc, cdc, invN);
+            acc_gtx(acc[0], dk, bx);
+            acc_gtx(acc[MATS - 1], dv, bx);
+        }
+    }
+    cp_wait<0>();
+    __syncwarp();                                  // the ring is free: stage the sums there
+    float* S = reinterpret_cast<float*>(ring);
+    const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int m = 0; m < MATS; ++m) {
+#pragma unroll
+        for (int md = 0; md < 2; ++md)
+#pragma unroll
+            for (int nc = 0; nc < 4; ++nc)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) S[(md * 16 + g + 8 * (i >> 1)) * S_PITCH + nc * 8 + 2 * t + (i & 1)] = acc[m][md][nc][i];
+        __syncwarp();
+        // rows of dW: to_qkv output channel (q | k | v block) * 256 + h * 32 + d;  lane = input channel c
+        float* dst = grad_w + (long long)((PART + m) * LM_HID + h * LM_D) * w_stride_n + lane * w_stride_c;
+#pragma unroll 4
+        for (int d = 0; d < LM_D; ++d) atomicAdd(dst + d * w_stride_n, S[d * S_PITCH + lane]);
         __syncwarp();
     }
 }
 
 constexpr size_t LAF_STATS_SMEM = (size_t)LM_HEADS * LFS_STAGES * LW_TILE * 2;
 constexpr size_t LAF_OUT_SMEM = (size_t)LM_HEADS * (LFO_STAGES + 1) * LW_TILE * 2;
-constexpr size_t LAF_BWD_SMEM = (size_t)LM_HEADS * (LFB_STAGES * LFB_STAGE_ELEMS + LFB_OUT_ELEMS) * 2 + (size_t)LM_HEADS * LM_D * 4;
 
 static int laf_attrs() {
     static bool done = false;
@@ -546,6 +748,8 @@ static int laf_attrs() {
         PIDM_CUDA(cudaFuncSetAttribute(laf_ctx_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfcCfg<1>::SMEM));
         PIDM_CUDA(cudaFuncSetAttribute(laf_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_OUT_SMEM));
         PIDM_CUDA(cudaFuncSetAttribute(laf_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_BWD_SMEM));
+        PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<0>::SMEM));
+        PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<1>::SMEM));
         done = true;
     }
     return 0;
@@ -602,9 +806,10 @@ extern "C" int pidm_linattn_fused_fwd(const void* xn, const void* w_qkv, void* o
     return 0;
 }
 
-// dqkv [B,N,768] bf16 is the gradient w.r.t. the (never materialised) qkv = xn W^T; dctx [B,8,32,32] is scratch.
+// dxn [B,N,32] bf16 is the gradient w.r.t. xn (written, not accumulated).  dctx [B,8,32,32] is produced here and read
+// again by pidm_linattn_fused_wgrad.
 extern "C" int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const void* dout, const float* ctx,
-                                      const float* kmax, const float* kzinv, void* dqkv, float* dctx, int B, int N,
+                                      const float* kmax, const float* kzinv, void* dxn, float* dctx, int B, int N,
                                       void* stream) {
     PIDM_REQUIRE(N % 128 == 0, "linattn_fused: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
@@ -618,7 +823,29 @@ extern "C" int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const v
                                                                              nullptr, nullptr, dctx, N, cpx, scale));
     const int bpx = laf_chunk_px(B, N, 1);
     PIDM_CUDA(launch_pdl(laf_bwd_kernel, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), (size_t)(LAF_BWD_SMEM), st, x, w, (const __nv_bfloat16*)dout, ctx, dctx, kmax,
-                                                                          kzinv, (__nv_bfloat16*)dqkv, N, bpx, scale));
+                                                                          kzinv, (__nv_bfloat16*)dxn, N, bpx, scale));
     PIDM_LAUNCH_CHECK("linattn_fused_bwd");
+    return 0;
+}
+
+// Weight gradient of the to_qkv projection, ACCUMULATED into grad_w (fp32; element [n][c] at n * w_stride_n +
+// c * w_stride_c), from the same operands as pidm_linattn_fused_bwd after it has produced dctx.
+extern "C" int pidm_linattn_fused_wgrad(const void* xn, const void* w_qkv, const void* dout, const float* ctx,
+                                        const float* dctx, const float* kmax, const float* kzinv, float* grad_w, int B,
+                                        int N, long long w_stride_n, long long w_stride_c, void* stream) {
+    PIDM_REQUIRE(N % 128 == 0, "linattn_fused: N must be a multiple of 128 (got %d)", N);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int e = laf_attrs()) return e;
+    const float scale = 0.17677669529663687f;
+    const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
+    const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
+    const __nv_bfloat16* g = (const __nv_bfloat16*)dout;
+    const int px = laf_chunk_px(B, N, 1);
+    const dim3 grid((N + px - 1) / px, B);
+    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<0>, grid, dim3(256), LfwCfg<0>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w, N,
+                         px, w_stride_n, w_stride_c, scale));
+    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w, N,
+                         px, w_stride_n, w_stride_c, scale));
+    PIDM_LAUNCH_CHECK("linattn_fused_wgrad");
     return 0;
 }

@@ -466,8 +466,9 @@ class _LinAttn(torch.autograd.Function):
 
 class _LinAttnFused(torch.autograd.Function):
     """to_qkv (1x1, no bias) + linear attention in one op: q, k, v are recomputed per head inside the kernels, the
-    [B, N, 768] qkv tensor is never written (reference unet_model.py:275-297).  Backward produces dqkv once and hands
-    it to the ordinary dgrad / wgrad of the projection."""
+    [B, N, 768] qkv tensor is never written (reference unet_model.py:275-297).  Neither is its gradient: backward
+    writes dxn directly, and a second pass over (xn, dout) on the weight-gradient stream accumulates the projection's
+    weight gradient."""
 
     @staticmethod
     def forward(ctx, xn, weight, spec, heads):
@@ -487,14 +488,16 @@ class _LinAttnFused(torch.autograd.Function):
     def backward(ctx, dout):
         xn, weight, ctxm, kmax, kzinv = ctx.saved_tensors
         spec = ctx.spec
-        B, H, W, C = xn.shape
+        B, H, W, _ = xn.shape
         dout = dout.contiguous()
-        dqkv = torch.empty(B, H, W, 3 * ctx.heads * 32, device=xn.device, dtype=xn.dtype)
+        dx = torch.empty_like(xn)
         dctx = torch.empty_like(ctxm)
-        call('pidm_linattn_fused_bwd', xn, spec.wp_fwd, dout, ctxm, kmax, kzinv, dqkv, dctx, B, H * W, stream())
-        g = (B, H, W, C, H, W, spec.cout, 1, 1, 1, 0)
-        dx, gw_ret, _ = _conv_backward(xn, weight, None, spec, g, dqkv, ctx.needs_input_grad[0])
-        return dx, gw_ret, None, None
+        call('pidm_linattn_fused_bwd', xn, spec.wp_fwd, dout, ctxm, kmax, kzinv, dx, dctx, B, H * W, stream())
+        gw_buf, gw_ret = _grad_buffer(weight)
+        ws = _wgrad_stream(xn, spec.wp_fwd, dout, ctxm, dctx, kmax, kzinv)
+        call('pidm_linattn_fused_wgrad', xn, spec.wp_fwd, dout, ctxm, dctx, kmax, kzinv, gw_buf, B, H * W,
+             spec.w_stride_n, spec.w_stride_c, ws)
+        return (dx if ctx.needs_input_grad[0] else None), gw_ret, None, None
 
 
 def linear_attention_fused_supported(xn, spec, heads):
