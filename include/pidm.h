@@ -131,6 +131,10 @@ int pidm_conv2d_tc_general(const void* x, const void* w_packed, const float* bia
                            int transposed, float* gn_sums, int gn_groups, int gn_sums_zeroed, void* stream);
 int pidm_conv2d_tc_general_supported(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW, int stride,
                                      int pad, int transposed);
+/* plan the tensor-core convolution picks for a supported geometry (test / tuning aid): out[10] = {BN, BK, row-group
+ * staging, resident weights, ring stages, total tiles, grid (persistent CTAs), TN, TH, TW} */
+int pidm_conv2d_tc_plan(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW, int stride, int pad,
+                        int transposed, int* out);
 /* wgrad on the tensor cores (wgmma): D[(tap,cA)][cB] = sum over grid pixels g of a[a_stride*g - pad + tap][cA] * b[g][cB], MN-major
  * (pixel-strided) TMA operands, split over pixel ranges, red.global.add into dw[cA*s_row + cB*s_col + tap] (fp32,
  * ACCUMULATED).  Regular conv: a = x, b = dy.  ConvTranspose: a = dy (a_stride 2), b = x.  Rows cA >= CA_real (channel
@@ -139,6 +143,11 @@ int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int B, int HA,
                          int GW, int CB, int KH, int KW, int a_stride, int pad, long long s_row, long long s_col,
                          void* stream);
 int pidm_conv2d_wgrad_tc_supported(int B, int GH, int GW, int CA, int CB, int KH, int KW, int a_stride);
+/* plan of a pidm_conv2d_wgrad_tc call with the same integer arguments (test / tuning aid): out[12] = {tap-complete 3x3
+ * kernel (1) or generic (0), NP, AA, AB, pixel splits, pixel tiles per split, pixel tiles, CTAs per split, row-group
+ * staging (3x3 kernel), pixel tile TN, TH, TW} */
+int pidm_conv2d_wgrad_tc_plan(int B, int HA, int WA, int CA, int CA_real, int GH, int GW, int CB, int KH, int KW,
+                              int a_stride, int pad, long long s_row, long long s_col, int* out);
 /* out[c] += sum_m x[m][c]: bias gradients (column sums of an NHWC tensor) */
 int pidm_colsum(const void* x, float* out, long long M, int C, int dtype, void* stream);
 
@@ -172,6 +181,8 @@ int pidm_layernorm_c_bwd(const void* x, const void* dy, const float* gamma, void
  * gradient into grad_w (fp32, element [n][c] at n * w_stride_n + c * w_stride_c).  Neither materialises dqkv. */
 int pidm_linattn_fused_supported(int C, int heads, int N, int dtype);
 int pidm_linattn_fused_workspace_floats(int B, int N);
+/* pixel chunking of the fused kernels (test aid): out[5] = {statistics chunks, ctx / out / bwd / wgrad pixels per CTA} */
+int pidm_linattn_fused_plan(int B, int N, int* out);
 int pidm_linattn_fused_fwd(const void* xn, const void* w_qkv, void* out, float* ctx, float* kmax, float* kzinv,
                            float* workspace, int B, int N, void* stream);
 int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const void* dout, const float* ctx, const float* kmax,

@@ -46,8 +46,10 @@ _SIGS = {
     'pidm_debug_set_trace': [P],
     'pidm_conv2d_tc_general': [P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, I, I, P, I, I, P],
     'pidm_conv2d_tc_general_supported': [I, I, I, I, I, I, I, I, I, I, I, I],
+    'pidm_conv2d_tc_plan': [I, I, I, I, I, I, I, I, I, I, I, I, P],
     'pidm_conv2d_wgrad_tc': [P, P, P, I, I, I, I, I, I, I, I, I, I, I, I, L, L, P],
     'pidm_conv2d_wgrad_tc_supported': [I, I, I, I, I, I, I, I],
+    'pidm_conv2d_wgrad_tc_plan': [I, I, I, I, I, I, I, I, I, I, I, I, L, L, P],
     'pidm_colsum': [P, P, L, I, I, P],
     'pidm_groupnorm_silu_fwd': [P, P, P, P, P, P, P, I, I, I, I, I, F, I, P],
     'pidm_groupnorm_silu_bwd': [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, F, I, P],
@@ -56,6 +58,7 @@ _SIGS = {
     'pidm_linattn_workspace_floats': [I, I, I],
     'pidm_linattn_fused_supported': [I, I, I, I],
     'pidm_linattn_fused_workspace_floats': [I, I],
+    'pidm_linattn_fused_plan': [I, I, P],
     'pidm_linattn_fused_fwd': [P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_fused_bwd': [P, P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_fused_wgrad': [P, P, P, P, P, P, P, P, I, I, L, L, P],
@@ -82,7 +85,8 @@ _SIGS = {
 # functions whose int return value is a result, not an error code
 _VALUE_RETURN = {'pidm_pack_entry_size', 'pidm_pack_pair_entry_size', 'pidm_mlp_entry_size', 'pidm_linattn_workspace_floats', 'pidm_version',
                  'pidm_linattn_fused_supported', 'pidm_linattn_fused_workspace_floats',
-                 'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported'}
+                 'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported',
+                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_fused_plan'}
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(f'{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). '

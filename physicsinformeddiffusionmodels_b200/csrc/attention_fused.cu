@@ -780,6 +780,15 @@ extern "C" int pidm_linattn_fused_supported(int C, int heads, int N, int dtype) 
 
 extern "C" int pidm_linattn_fused_workspace_floats(int B, int N) { return B * laf_stat_chunks(N) * LM_HID; }
 
+// pixel chunking of the fused kernels: out[5] = {statistics chunks (kmax), ctx px, out px, bwd px, wgrad px}
+extern "C" int pidm_linattn_fused_plan(int B, int N, int* out) {
+    PIDM_REQUIRE(N % 128 == 0 && B > 0, "linattn_fused_plan: N must be a multiple of 128 (got %d)", N);
+    const int v[5] = {laf_stat_chunks(N), laf_chunk_px(B, N, 2), laf_chunk_px(B, N, 3), laf_chunk_px(B, N, 1),
+                      laf_chunk_px(B, N, 1)};
+    for (int i = 0; i < 5; ++i) out[i] = v[i];
+    return 0;
+}
+
 // xn [B,N,32] bf16 (the PreNorm output), w_qkv [768][32] bf16 (packed to_qkv weights, K-major), out [B,N,256] bf16.
 // ctx [B,8,32,32], kmax / kzinv [B,8,32] are outputs kept for backward; workspace: pidm_linattn_fused_workspace_floats.
 extern "C" int pidm_linattn_fused_fwd(const void* xn, const void* w_qkv, void* out, float* ctx, float* kmax, float* kzinv,

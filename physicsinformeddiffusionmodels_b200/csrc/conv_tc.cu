@@ -561,7 +561,17 @@ static bool tc_geometry(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, 
     p.TW = pl.TW; p.TH = pl.TH; p.TN = pl.TN; p.tiles_h = p.GH / pl.TH; p.tiles_w = p.GW / pl.TW;
     p.rg = pl.rg; p.nb = pl.nb; p.a_bytes = pl.a_bytes; p.stage_bytes = pl.stage_bytes; p.stages = pl.stages;
     p.resident = pl.resident; p.res_bytes = pl.res_bytes; p.operand_bytes = pl.operand_bytes;
+    p.m_tiles = ((B + pl.TN - 1) / pl.TN) * p.tiles_h * p.tiles_w;
+    p.n_tiles = Cout / pl.BN;
+    p.n_classes = classes;
     return true;
+}
+
+// persistent grid: one CTA per SM, or one per tile when there are fewer tiles than SMs
+static int tc_grid(const TcParams& p) {
+    const int total_tiles = p.m_tiles * p.n_tiles * p.n_classes;
+    const int slots = num_sms();
+    return total_tiles < slots ? total_tiles : slots;
 }
 
 static int tc_run(const void* x, const void* w_packed, const float* bias, const void* residual, void* y, int B, int H,
@@ -618,12 +628,7 @@ static int tc_run(const void* x, const void* w_packed, const float* bias, const 
                      "4, 8, 16 or a multiple of 32 channels per group (got %d)", cpg);
         if (!gn_sums_zeroed) PIDM_CUDA(cudaMemsetAsync(gn_sums, 0, (size_t)B * gn_groups * 2 * sizeof(float), st));
     }
-    p.m_tiles = ((B + pl.TN - 1) / pl.TN) * p.tiles_h * p.tiles_w;
-    p.n_tiles = Cout / pl.BN;
-    p.n_classes = classes;
-    const int total_tiles = p.m_tiles * p.n_tiles * p.n_classes;
-    const int slots = num_sms();
-    dim3 grid(total_tiles < slots ? total_tiles : slots);
+    dim3 grid(tc_grid(p));
 #define TC_CASE(bn, bk) if (pl.BN == bn && pl.BK == bk) return launch_tc<bn, bk>(mx, mw, p, grid, st)
     TC_CASE(128, 64); TC_CASE(64, 64); TC_CASE(32, 64);
     TC_CASE(128, 32); TC_CASE(64, 32); TC_CASE(32, 32);
@@ -644,6 +649,17 @@ extern "C" int pidm_conv2d_tc_general_supported(int B, int H, int W, int Cin, in
                                                 int stride, int pad, int transposed) {
     TcParams p; TcPlan pl; int classes;
     return tc_geometry(B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad, transposed, p, pl, classes) ? 1 : 0;
+}
+
+extern "C" int pidm_conv2d_tc_plan(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW, int stride,
+                                   int pad, int transposed, int* out) {
+    TcParams p; TcPlan pl; int classes;
+    PIDM_REQUIRE(tc_geometry(B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad, transposed, p, pl, classes),
+                 "conv2d_tc_plan: unsupported geometry");
+    const int v[10] = {pl.BN, pl.BK, pl.rg, pl.resident, pl.stages, p.m_tiles * p.n_tiles * p.n_classes, tc_grid(p),
+                       pl.TN, pl.TH, pl.TW};
+    for (int i = 0; i < 10; ++i) out[i] = v[i];
+    return 0;
 }
 
 extern "C" int pidm_conv2d_tc_general(const void* x, const void* w_packed, const float* bias, const void* residual,

@@ -238,43 +238,22 @@ static int wg_launch(const CUtensorMap& mx, const CUtensorMap& my, const WgParam
 // tap-complete 3x3 kernel (wgrad_tc3.cu)
 bool wgrad3_supported(int B, int HA, int WA, int CA, int CA_real, int GH, int GW, int CB, int KH, int KW, int a_stride,
                       int pad, long long s_row);
+void wgrad3_geometry(int B, int GH, int GW, int CA, int CB, int* plan);
 int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB,
                long long s_col, cudaStream_t st);
 
-}  // namespace pidm
-using namespace pidm;
-
-extern "C" int pidm_conv2d_wgrad_tc_supported(int B, int GH, int GW, int CA, int CB, int KH, int KW, int a_stride) {
-    WgPlan pl;
-    return (KH == KW && wg_plan(B, GH, GW, CA, CB, a_stride, pl)) ? 1 : 0;
-}
-
-// D[(tap, cA)][cB] = sum over grid pixels g of a[a_stride*g - pad + tap][cA] * b[g][cB], ACCUMULATED into
-// dw[cA*s_row + cB*s_col + tap] (fp32).  a: [B,HA,WA,CA] bf16 (CA may be channel-padded: rows >= CA_real are dropped),
-// b: [B,GH,GW,CB] bf16.
-extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int CA_real,
-                                    int GH, int GW, int CB, int KH, int KW, int a_stride, int pad, long long s_row,
-                                    long long s_col, void* stream) {
+static bool wgrad3_enabled() {
     static int use3 = -1;                       // PIDM_WGRAD3=0 falls back to the generic kernel (A/B testing)
     if (use3 < 0) { const char* ev = getenv("PIDM_WGRAD3"); use3 = (ev && ev[0] == '0') ? 0 : 1; }
-    if (use3 && wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row))
-        return wgrad3_run(a, b, dw, B, HA, WA, CA, GH, GW, CB, s_col, (cudaStream_t)stream);
-    WgPlan pl;
-    PIDM_REQUIRE(KH == KW && wg_plan(B, GH, GW, CA, CB, a_stride, pl), "conv2d_wgrad_tc: unsupported geometry");
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        PIDM_CUDA(cudaFree(0));
-        ctx_bound = true;
-    }
-    cudaStream_t st = (cudaStream_t)stream;
-    CUtensorMap mx, my;
-    if (int e = wg_encode(&mx, a, B, HA, WA, CA, pl.AA, pl.TW, pl.TH, pl.TN, a_stride)) return e;
-    if (int e = wg_encode(&my, b, B, GH, GW, CB, pl.AB, pl.TW, pl.TH, pl.TN, 1)) return e;
-    WgParams p;
-    p.B = B; p.Cin = CA; p.Cout = CB; p.c_real = CA_real; p.KH = KH; p.KW = KW; p.pad = pad; p.a_stride = a_stride;
+    return use3 != 0;
+}
+
+// launch geometry of the generic kernel: M' tiles x n-tiles x pixel splits
+static bool wg_geometry(int B, int GH, int GW, int CA, int CB, int KH, int KW, int a_stride, WgPlan& pl, WgParams& p,
+                        dim3& grid) {
+    if (KH != KW || !wg_plan(B, GH, GW, CA, CB, a_stride, pl)) return false;
     p.TW = pl.TW; p.TH = pl.TH; p.TN = pl.TN; p.tiles_h = GH / pl.TH;
     p.n_pix_tiles = ((B + pl.TN - 1) / pl.TN) * p.tiles_h;
-    p.dw = dw; p.s_row = s_row; p.s_col = s_col;
     const int na = 128 / pl.AA;
     const int n_pairs = KH * KW * (CA / pl.AA);
     const int m_tiles = (n_pairs + na - 1) / na;
@@ -286,7 +265,59 @@ extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int
     if (splits < 1) splits = 1;
     p.tiles_per_split = (p.n_pix_tiles + splits - 1) / splits;
     splits = (p.n_pix_tiles + p.tiles_per_split - 1) / p.tiles_per_split;
-    dim3 grid(m_tiles, n_tiles, splits);
+    grid = dim3(m_tiles, n_tiles, splits);
+    return true;
+}
+
+}  // namespace pidm
+using namespace pidm;
+
+extern "C" int pidm_conv2d_wgrad_tc_supported(int B, int GH, int GW, int CA, int CB, int KH, int KW, int a_stride) {
+    WgPlan pl;
+    return (KH == KW && wg_plan(B, GH, GW, CA, CB, a_stride, pl)) ? 1 : 0;
+}
+
+// plan of one pidm_conv2d_wgrad_tc call: out[12] = {wgrad3, NP, AA, AB, splits, tiles_per_split, n_pix_tiles,
+// CTAs per split, row-group staging (wgrad3 only), TN, TH, TW}
+extern "C" int pidm_conv2d_wgrad_tc_plan(int B, int HA, int WA, int CA, int CA_real, int GH, int GW, int CB, int KH,
+                                         int KW, int a_stride, int pad, long long s_row, long long s_col, int* out) {
+    (void)s_col;
+    if (wgrad3_enabled() && wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row)) {
+        out[0] = 1;
+        wgrad3_geometry(B, GH, GW, CA, CB, out + 1);
+        return 0;
+    }
+    WgPlan pl; WgParams p; dim3 grid;
+    PIDM_REQUIRE(wg_geometry(B, GH, GW, CA, CB, KH, KW, a_stride, pl, p, grid), "conv2d_wgrad_tc_plan: unsupported geometry");
+    const int v[12] = {0, pl.NP, pl.AA, pl.AB, (int)grid.z, p.tiles_per_split, p.n_pix_tiles, (int)(grid.x * grid.y), 0,
+                       pl.TN, pl.TH, pl.TW};
+    for (int i = 0; i < 12; ++i) out[i] = v[i];
+    return 0;
+}
+
+// D[(tap, cA)][cB] = sum over grid pixels g of a[a_stride*g - pad + tap][cA] * b[g][cB], ACCUMULATED into
+// dw[cA*s_row + cB*s_col + tap] (fp32).  a: [B,HA,WA,CA] bf16 (CA may be channel-padded: rows >= CA_real are dropped),
+// b: [B,GH,GW,CB] bf16.
+extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int CA_real,
+                                    int GH, int GW, int CB, int KH, int KW, int a_stride, int pad, long long s_row,
+                                    long long s_col, void* stream) {
+    if (wgrad3_enabled() && wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row))
+        return wgrad3_run(a, b, dw, B, HA, WA, CA, GH, GW, CB, s_col, (cudaStream_t)stream);
+    WgPlan pl;
+    WgParams p;
+    dim3 grid;
+    PIDM_REQUIRE(wg_geometry(B, GH, GW, CA, CB, KH, KW, a_stride, pl, p, grid), "conv2d_wgrad_tc: unsupported geometry");
+    static thread_local bool ctx_bound = false;
+    if (!ctx_bound) {
+        PIDM_CUDA(cudaFree(0));
+        ctx_bound = true;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    CUtensorMap mx, my;
+    if (int e = wg_encode(&mx, a, B, HA, WA, CA, pl.AA, pl.TW, pl.TH, pl.TN, a_stride)) return e;
+    if (int e = wg_encode(&my, b, B, GH, GW, CB, pl.AB, pl.TW, pl.TH, pl.TN, 1)) return e;
+    p.B = B; p.Cin = CA; p.Cout = CB; p.c_real = CA_real; p.KH = KH; p.KW = KW; p.pad = pad; p.a_stride = a_stride;
+    p.dw = dw; p.s_row = s_row; p.s_col = s_col;
 #define WG_CASE(np, aa, ab) if (pl.NP == np && pl.AA == aa && pl.AB == ab) return wg_launch<np, aa, ab>(mx, my, p, grid, st)
     WG_CASE(128, 64, 64); WG_CASE(128, 32, 64); WG_CASE(64, 64, 64); WG_CASE(64, 32, 64);
     WG_CASE(32, 64, 32); WG_CASE(32, 32, 32);

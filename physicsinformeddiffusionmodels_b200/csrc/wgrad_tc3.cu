@@ -222,16 +222,10 @@ bool wgrad3_supported(int B, int HA, int WA, int CA, int CA_real, int GH, int GW
     return GW * GH * tn == 64 && B % tn == 0;
 }
 
-int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB,
-               long long s_col, cudaStream_t st) {
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        PIDM_CUDA(cudaFree(0));
-        ctx_bound = true;
-    }
-    const bool rg = (GW % 8 == 0 && GH % 16 == 0);
-    W3Params p;
-    p.B = B; p.pad = 1; p.dw = dw; p.s_col = s_col;
+// tile plan and launch grid of a supported call
+static void w3_geometry(int B, int GH, int GW, int CA, int CB, W3Params& p, bool& rg, int& NP, int& AB, dim3& grid) {
+    rg = (GW % 8 == 0 && GH % 16 == 0);
+    p.B = B; p.pad = 1;
     if (rg) { p.TW = 8; p.TH = 16; p.TN = 1; }
     else {
         p.TW = GW;
@@ -242,18 +236,42 @@ int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, i
     }
     p.tiles_h = GH / p.TH; p.tiles_w = GW / p.TW;
     p.n_pix_tiles = (B / p.TN) * p.tiles_h * p.tiles_w;
-    const int NP = (CB % 64 == 0) ? 64 : 32;          // 3 x NP / 2 accumulator registers per consumer thread
-    const int AB = (CB % 64 == 0) ? 64 : 32;
-    CUtensorMap mx, my;
-    if (int e = w3_encode(&mx, a, B, HA, WA, CA, 32, p.TW, rg ? p.TH + 3 : p.TH, p.TN)) return e;
-    if (int e = w3_encode(&my, b, B, GH, GW, CB, AB, p.TW, p.TH, p.TN)) return e;
+    NP = (CB % 64 == 0) ? 64 : 32;          // 3 x NP / 2 accumulator registers per consumer thread
+    AB = (CB % 64 == 0) ? 64 : 32;
     const int chunks = CA / 32, n_tiles = CB / NP;
     int splits = num_sms() / (chunks * n_tiles);
     if (splits > p.n_pix_tiles) splits = p.n_pix_tiles;
     if (splits < 1) splits = 1;
     p.tiles_per_split = (p.n_pix_tiles + splits - 1) / splits;
     splits = (p.n_pix_tiles + p.tiles_per_split - 1) / p.tiles_per_split;
-    dim3 grid(chunks, n_tiles, splits);
+    grid = dim3(chunks, n_tiles, splits);
+}
+
+// plan[11] = {NP, AA (= 32), AB, splits, tiles_per_split, n_pix_tiles, CTAs per split, row-group staging, TN, TH, TW}
+void wgrad3_geometry(int B, int GH, int GW, int CA, int CB, int* plan) {
+    W3Params p; bool rg; int NP, AB; dim3 grid;
+    w3_geometry(B, GH, GW, CA, CB, p, rg, NP, AB, grid);
+    const int v[11] = {NP, 32, AB, (int)grid.z, p.tiles_per_split, p.n_pix_tiles, (int)(grid.x * grid.y), rg ? 1 : 0,
+                       p.TN, p.TH, p.TW};
+    for (int i = 0; i < 11; ++i) plan[i] = v[i];
+}
+
+int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB,
+               long long s_col, cudaStream_t st) {
+    static thread_local bool ctx_bound = false;
+    if (!ctx_bound) {
+        PIDM_CUDA(cudaFree(0));
+        ctx_bound = true;
+    }
+    W3Params p;
+    bool rg;
+    int NP, AB;
+    dim3 grid;
+    w3_geometry(B, GH, GW, CA, CB, p, rg, NP, AB, grid);
+    p.dw = dw; p.s_col = s_col;
+    CUtensorMap mx, my;
+    if (int e = w3_encode(&mx, a, B, HA, WA, CA, 32, p.TW, rg ? p.TH + 3 : p.TH, p.TN)) return e;
+    if (int e = w3_encode(&my, b, B, GH, GW, CB, AB, p.TW, p.TH, p.TN)) return e;
 #define W3_CASE(np, ab) \
     if (NP == np && AB == ab) return rg ? w3_launch<np, ab, true>(mx, my, p, grid, st) : w3_launch<np, ab, false>(mx, my, p, grid, st)
     W3_CASE(64, 64); W3_CASE(32, 32);
