@@ -56,14 +56,24 @@ int pidm_toy_pidm_loss(const float* target, const float* output, const float* re
                        int D, void* stream);
 
 /* ---- Darcy residual (src/residuals_darcy.py:134-183 + src/grad_utils.py:64-146) ------------------------- */
+/* The last int argument of the four Darcy entry points below is a flags word:
+ *   PIDM_DARCY_PIXELS_AT_BOUNDARY  h = domain_length / (P-1) (else domain_length / P)
+ *   PIDM_DARCY_PERIODIC            bcs='periodic' (src/grad_utils.py:76-81): every pixel uses the central second-order
+ *                                  stencil and neighbours wrap around the plane; h is unchanged, and the bc_x0 / bc_x1
+ *                                  channels are still written on rows 0 / P-1 and columns 0 / P-1, from the wrapped p_0 / p_1.
+ * 0 and 1 keep their old meaning (pixels_at_boundary false / true); unknown bits are rejected. */
+#define PIDM_DARCY_PIXELS_AT_BOUNDARY 1
+#define PIDM_DARCY_PERIODIC 2
 /* x0hat [B,2,P,P] fp32 NCHW (p, K); f_s [P*P]; residual [B,P*P,3] = (eq_0, bc_x0, bc_x1).  P must be 64. */
 int pidm_darcy_residual_fwd(const float* x0hat, const float* f_s, float* residual, int B, int pixels,
-                            float domain_length, int reverse_d1, int pixels_at_boundary, void* stream);
+                            float domain_length, int reverse_d1, int flags, void* stream);
 /* vector-Jacobian product of the above: grad_x0hat [B,2,P,P] = J^T grad_residual */
 int pidm_darcy_residual_bwd(const float* x0hat, const float* f_s, const float* grad_residual, float* grad_x0hat, int B,
-                            int pixels, float domain_length, int reverse_d1, int pixels_at_boundary, void* stream);
+                            int pixels, float domain_length, int reverse_d1, int flags, void* stream);
 /* one derivative field of u [planes,P,P]: mode 0..4 = d_d0, d_d1, d_d00, d_d11, d_d01 (StencilGradients.forward,
- * src/grad_utils.py:161-175; second-order, one-sided at the boundary) */
+ * src/grad_utils.py:161-175; second-order, one-sided at the boundary), OR PIDM_FD_PERIODIC for the wrapped central
+ * stencil at every pixel (periodic=True, src/grad_utils.py:76-81) */
+#define PIDM_FD_PERIODIC 8
 int pidm_fd_stencil(const float* u, float* out, int planes, int pixels, int mode, float d0, float d1, void* stream);
 /* Fused PIDM loss (src/denoising_utils.py:669-692): sums3 = {c_data*mean_b(p2[t] mse_b), mean(c_res*0.5 r^2/var_t),
  * mean|r|}; optionally the gradient of (sums3[0]+sums3[1]) w.r.t. x0hat (residual operand) and model_out (data
@@ -72,12 +82,12 @@ int pidm_fd_stencil(const float* u, float* out, int planes, int pixels, int mode
 int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, const float* target, const float* f_s,
                          const long long* t, const float* p2_loss_weight, const float* posterior_var_clipped,
                          float c_data, float c_residual, float* sums3, float* grad_x0hat, float* grad_model_out, int B,
-                         int pixels, float domain_length, int reverse_d1, int pixels_at_boundary, void* stream);
+                         int pixels, float domain_length, int reverse_d1, int flags, void* stream);
 /* CoCoGen step size (src/residuals_darcy.py:218-231): max_dr_dp[b] = largest entry (signed, as torch.max) of the Jacobian
  * d residual / d p of sample b -- evaluated analytically from the stencil coefficients and K, the reference materialises
  * the 12288 x 4096 Jacobian per sample with vmap(jacfwd). */
 int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int B, int pixels, float domain_length, int reverse_d1,
-                            int pixels_at_boundary, void* stream);
+                            int flags, void* stream);
 
 /* ---- layout ------------------------------------------------------------------------------------------- */
 /* image_to_b_xy_c / b_xy_c_to_image (src/denoising_utils.py:36-55) fused with the dtype change + channel padding */

@@ -6,6 +6,10 @@
 //   r[b, i*P+j, 1] = (i==0 ? -p_0 : i==P-1 ? +p_0 : 0)
 //   r[b, i*P+j, 2] = (j==0 ? +s p_1 : j==P-1 ? -s p_1 : 0),  s = +1 if reverse_d1 else -1
 //
+// bcs='periodic' (PIDM_DARCY_PERIODIC; reference grad_utils.py:76-81, circular padding + the interior stencil): every
+// kernel has a PER = true instantiation in which every pixel uses the central stencil with wrapped neighbours.  The two
+// BC channels keep their rows / columns and signs.  The PER = false instantiations compile to the same SASS as before.
+//
 // Design: HBM-bound (about 2 flop/byte).  Persistent CTAs; every sample (p-plane + K-plane,
 // 2*P*P*4 = 32 KiB contiguous in NCHW) is staged into shared memory by ONE bulk-async (TMA) copy
 // that completes on an mbarrier, double-buffered so the copy of sample n+1 overlaps the stencil math
@@ -62,31 +66,44 @@ struct DarcyGeom {
 __device__ __forceinline__ float source_fs(int i, int j, const float* __restrict__ fs) { return fs[i * P + j]; }
 
 // ---- pointwise stencil helpers on a PxP plane in shared memory ------------------------------------
+// PER (bcs='periodic', reference grad_utils.py:76-81): the central stencil at every pixel, neighbours wrap around the
+// plane.  PER = false is the one-sided-boundary code.
+__device__ __forceinline__ int wrap(int x) { return x & (P - 1); }   // P is a power of two
+
+template <bool PER>
 __device__ __forceinline__ float d_row(const float* u, int i, int j, float inv_h) {  // d/dx0
+    if constexpr (PER) return (u[wrap(i + 1) * P + j] - u[wrap(i - 1) * P + j]) * (0.5f * inv_h);
     if (i == 0) return (-1.5f * u[j] + 2.f * u[P + j] - 0.5f * u[2 * P + j]) * inv_h;
     if (i == P - 1) return (1.5f * u[(P - 1) * P + j] - 2.f * u[(P - 2) * P + j] + 0.5f * u[(P - 3) * P + j]) * inv_h;
     return (u[(i + 1) * P + j] - u[(i - 1) * P + j]) * (0.5f * inv_h);
 }
+template <bool PER>
 __device__ __forceinline__ float d_col(const float* u, int i, int j, float inv_h) {  // d/dx1
     const float* r = u + i * P;
+    if constexpr (PER) return (r[wrap(j + 1)] - r[wrap(j - 1)]) * (0.5f * inv_h);
     if (j == 0) return (-1.5f * r[0] + 2.f * r[1] - 0.5f * r[2]) * inv_h;
     if (j == P - 1) return (1.5f * r[P - 1] - 2.f * r[P - 2] + 0.5f * r[P - 3]) * inv_h;
     return (r[j + 1] - r[j - 1]) * (0.5f * inv_h);
 }
+template <bool PER>
 __device__ __forceinline__ float d2_row(const float* u, int i, int j, float inv_h2) {
+    if constexpr (PER) return (u[wrap(i + 1) * P + j] - 2.f * u[i * P + j] + u[wrap(i - 1) * P + j]) * inv_h2;
     if (i == 0) return (2.f * u[j] - 5.f * u[P + j] + 4.f * u[2 * P + j] - u[3 * P + j]) * inv_h2;
     if (i == P - 1)
         return (2.f * u[(P - 1) * P + j] - 5.f * u[(P - 2) * P + j] + 4.f * u[(P - 3) * P + j] - u[(P - 4) * P + j]) * inv_h2;
     return (u[(i + 1) * P + j] - 2.f * u[i * P + j] + u[(i - 1) * P + j]) * inv_h2;
 }
+template <bool PER>
 __device__ __forceinline__ float d2_col(const float* u, int i, int j, float inv_h2) {
     const float* r = u + i * P;
+    if constexpr (PER) return (r[wrap(j + 1)] - 2.f * r[j] + r[wrap(j - 1)]) * inv_h2;
     if (j == 0) return (2.f * r[0] - 5.f * r[1] + 4.f * r[2] - r[3]) * inv_h2;
     if (j == P - 1) return (2.f * r[P - 1] - 5.f * r[P - 2] + 4.f * r[P - 3] - r[P - 4]) * inv_h2;
     return (r[j + 1] - 2.f * r[j] + r[j - 1]) * inv_h2;
 }
 
 // Residual triple for the 4 pixels (i, j0..j0+3) from planes p, K in smem.
+template <bool PER>
 __device__ __forceinline__ void residual_quad(const float* sp, const float* sk, const float* __restrict__ fs, int i,
                                               int j0, const DarcyGeom& g, float req[4], float rb0[4], float rb1[4]) {
     // row-direction derivatives are row-uniform across the quad: vectorised float4 rows
@@ -134,9 +151,37 @@ __device__ __forceinline__ void residual_quad(const float* sp, const float* sk, 
     for (int q = 0; q < 4; ++q) {
         int j = j0 + q;
         float kv = sk[i * P + j];
-        float p1 = d_col(sp, i, j, g.inv_h1);
-        float p11 = d2_col(sp, i, j, g.inv_h1sq);
-        float k1 = d_col(sk, i, j, g.inv_h1);
+        float p1 = d_col<PER>(sp, i, j, g.inv_h1);
+        float p11 = d2_col<PER>(sp, i, j, g.inv_h1sq);
+        float k1 = d_col<PER>(sk, i, j, g.inv_h1);
+        req[q] = -kv * (p00[q] + p11) - k0[q] * p0[q] - k1 * p1 - source_fs(i, j, fs);
+        rb0[q] = (i == 0) ? -p0[q] : ((i == P - 1) ? p0[q] : 0.f);
+        rb1[q] = (j == 0) ? g.bc1_sign * p1 : ((j == P - 1) ? -g.bc1_sign * p1 : 0.f);
+    }
+}
+
+// Periodic: rows i-1 and i+1 wrap, so every row takes the central float4 path.
+template <>
+__device__ __forceinline__ void residual_quad<true>(const float* sp, const float* sk, const float* __restrict__ fs, int i,
+                                                    int j0, const DarcyGeom& g, float req[4], float rb0[4], float rb1[4]) {
+    const int im = wrap(i - 1), ip = wrap(i + 1);
+    const float hh = 0.5f * g.inv_h0;
+    float4 a = *reinterpret_cast<const float4*>(sp + im * P + j0);
+    const float4 b = *reinterpret_cast<const float4*>(sp + i * P + j0);
+    float4 c = *reinterpret_cast<const float4*>(sp + ip * P + j0);
+    const float p0[4] = {(c.x - a.x) * hh, (c.y - a.y) * hh, (c.z - a.z) * hh, (c.w - a.w) * hh};
+    const float p00[4] = {(c.x - 2.f * b.x + a.x) * g.inv_h0sq, (c.y - 2.f * b.y + a.y) * g.inv_h0sq,
+                          (c.z - 2.f * b.z + a.z) * g.inv_h0sq, (c.w - 2.f * b.w + a.w) * g.inv_h0sq};
+    a = *reinterpret_cast<const float4*>(sk + im * P + j0);
+    c = *reinterpret_cast<const float4*>(sk + ip * P + j0);
+    const float k0[4] = {(c.x - a.x) * hh, (c.y - a.y) * hh, (c.z - a.z) * hh, (c.w - a.w) * hh};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const int j = j0 + q;
+        const float kv = sk[i * P + j];
+        const float p1 = d_col<true>(sp, i, j, g.inv_h1);
+        const float p11 = d2_col<true>(sp, i, j, g.inv_h1sq);
+        const float k1 = d_col<true>(sk, i, j, g.inv_h1);
         req[q] = -kv * (p00[q] + p11) - k0[q] * p0[q] - k1 * p1 - source_fs(i, j, fs);
         rb0[q] = (i == 0) ? -p0[q] : ((i == P - 1) ? p0[q] : 0.f);
         rb1[q] = (j == 0) ? g.bc1_sign * p1 : ((j == P - 1) ? -g.bc1_sign * p1 : 0.f);
@@ -145,8 +190,10 @@ __device__ __forceinline__ void residual_quad(const float* sp, const float* sk, 
 
 // ---- adjoint (transposed) 1-D operators, gather form ------------------------------------------------
 // (D^T F)[x] for the first-derivative matrix D (central interior rows 1..P-2, one-sided rows 0 and P-1).
-template <typename F>
+// Periodic: D is circulant, D^T F(x) = (F(x-1) - F(x+1)) / 2h and D2^T = D2, indices wrapped.
+template <bool PER, typename F>
 __device__ __forceinline__ float adj_d1(F f, int x, float inv_h) {
+    if constexpr (PER) return (f(wrap(x - 1)) * 0.5f - f(wrap(x + 1)) * 0.5f) * inv_h;
     float acc = 0.f;
     if (x - 1 >= 1) acc += f(x - 1) * 0.5f;           // row x-1 is interior (x-1 <= P-2 always when x<=P-1)
     if (x + 1 <= P - 2) acc -= f(x + 1) * 0.5f;       // row x+1 is interior
@@ -155,8 +202,9 @@ __device__ __forceinline__ float adj_d1(F f, int x, float inv_h) {
     return acc * inv_h;
 }
 // fix-up: interior rows are 1..P-2, so row x-1 is interior iff 1 <= x-1 <= P-2, row x+1 iff 1 <= x+1 <= P-2.
-template <typename F>
+template <bool PER, typename F>
 __device__ __forceinline__ float adj_d2(F f, int x, float inv_h2) {
+    if constexpr (PER) return (f(wrap(x - 1)) - 2.f * f(x) + f(wrap(x + 1))) * inv_h2;
     float acc = 0.f;
     if (x - 1 >= 1 && x - 1 <= P - 2) acc += f(x - 1);
     if (x >= 1 && x <= P - 2) acc -= 2.f * f(x);
@@ -172,6 +220,7 @@ struct DarcySmem {
 };
 
 // Residual, materialised: persistent CTAs, one bulk-async copy per sample, double-buffered.
+template <bool PER>
 __global__ void __launch_bounds__(DARCY_THREADS) darcy_fwd_kernel(const float* __restrict__ x0hat /*[B,2,P,P]*/,
                                                                  const float* __restrict__ fs /*[P*P]*/,
                                                                  float* __restrict__ residual /*[B,P*P,3]*/, int B,
@@ -208,7 +257,7 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_fwd_kernel(const float* _
         for (int q = tid; q < PP / 4; q += DARCY_THREADS) {
             int i = q / (P / 4), j0 = (q % (P / 4)) * 4;
             float req[4], rb0[4], rb1[4];
-            residual_quad(sp, sk, fs, i, j0, geom, req, rb0, rb1);
+            residual_quad<PER>(sp, sk, fs, i, j0, geom, req, rb0, rb1);
             float4* o = reinterpret_cast<float4*>(out + (size_t)(i * P + j0) * 3);
             o[0] = make_float4(req[0], rb0[0], rb1[0], req[1]);
             o[1] = make_float4(rb0[1], rb1[1], req[2], rb0[2]);
@@ -237,6 +286,7 @@ struct DarcyGradSmem {
 };
 
 // residual of a quad + every derivative it is built from
+template <bool PER>
 __device__ __forceinline__ void residual_quad_full(const float* sp, const float* sk, const float* __restrict__ fs, int i,
                                                    int j0, const DarcyGeom& g, float req[4], float rb0[4], float rb1[4],
                                                    float kv[4], float k0[4], float k1[4], float p0[4], float p1[4],
@@ -245,11 +295,11 @@ __device__ __forceinline__ void residual_quad_full(const float* sp, const float*
     for (int q = 0; q < 4; ++q) {
         const int j = j0 + q;
         kv[q] = sk[i * P + j];
-        p0[q] = d_row(sp, i, j, g.inv_h0);
-        k0[q] = d_row(sk, i, j, g.inv_h0);
-        p1[q] = d_col(sp, i, j, g.inv_h1);
-        k1[q] = d_col(sk, i, j, g.inv_h1);
-        lap[q] = d2_row(sp, i, j, g.inv_h0sq) + d2_col(sp, i, j, g.inv_h1sq);
+        p0[q] = d_row<PER>(sp, i, j, g.inv_h0);
+        k0[q] = d_row<PER>(sk, i, j, g.inv_h0);
+        p1[q] = d_col<PER>(sp, i, j, g.inv_h1);
+        k1[q] = d_col<PER>(sk, i, j, g.inv_h1);
+        lap[q] = d2_row<PER>(sp, i, j, g.inv_h0sq) + d2_col<PER>(sp, i, j, g.inv_h1sq);
         // same association as residual_quad: -K (p_00 + p_11) - K_0 p_0 - K_1 p_1 - f_s
         req[q] = -kv[q] * lap[q] - k0[q] * p0[q] - k1[q] * p1[q] - source_fs(i, j, fs);
         rb0[q] = (i == 0) ? -p0[q] : ((i == P - 1) ? p0[q] : 0.f);
@@ -258,8 +308,9 @@ __device__ __forceinline__ void residual_quad_full(const float* sp, const float*
 }
 
 // MODE 1: generic backward (cotangent tensor given).  MODE 2: fused PIDM loss (data MSE + residual NLL sums, |r| sum)
-// and its gradient w.r.t. x0_hat / model_out in one pass.
-template <int MODE>
+// and its gradient w.r.t. x0_hat / model_out in one pass.  PER: periodic stencils; the BC seeds still enter U0 / U1 on
+// rows 0 / P-1 and columns 0 / P-1.
+template <int MODE, bool PER>
 __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
     const float* __restrict__ x0hat,      // [B,2,P,P]
     const float* __restrict__ fs,         // [P*P]
@@ -320,7 +371,7 @@ __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
             const int q = tid + u * DG_THREADS;
             const int i = q / (P / 4), j0 = (q % (P / 4)) * 4;
             float req[4], rb0[4], rb1[4], kv[4], k0[4], k1[4], p0[4], p1[4], lap[4];
-            residual_quad_full(sp, sk, fs, i, j0, geom, req, rb0, rb1, kv, k0, k1, p0, p1, lap);
+            residual_quad_full<PER>(sp, sk, fs, i, j0, geom, req, rb0, rb1, kv, k0, k1, p0, p1, lap);
             float ge[4], g0[4], g1[4];
             if (MODE == 1) {
                 const float4* c = reinterpret_cast<const float4*>(cot + ((size_t)b * PP + i * P + j0) * 3);
@@ -373,9 +424,9 @@ __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
                     auto u1c = [&](int c) { return sU1[i * P + c]; };
                     auto v0r = [&](int r) { return sV0[r * P + j]; };
                     auto v1c = [&](int c) { return sV1[i * P + c]; };
-                    dp[k] = adj_d2(a_row, i, geom.inv_h0sq) + adj_d2(a_col, j, geom.inv_h1sq) + adj_d1(u0r, i, geom.inv_h0) +
-                            adj_d1(u1c, j, geom.inv_h1);
-                    dk[k] = W[u][k] + adj_d1(v0r, i, geom.inv_h0) + adj_d1(v1c, j, geom.inv_h1);
+                    dp[k] = adj_d2<PER>(a_row, i, geom.inv_h0sq) + adj_d2<PER>(a_col, j, geom.inv_h1sq) +
+                            adj_d1<PER>(u0r, i, geom.inv_h0) + adj_d1<PER>(u1c, j, geom.inv_h1);
+                    dk[k] = W[u][k] + adj_d1<PER>(v0r, i, geom.inv_h0) + adj_d1<PER>(v1c, j, geom.inv_h1);
                 }
             }
             if (MODE == 2) {
@@ -436,29 +487,38 @@ __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
 //   d r_eq[i] / d p[i + (dr, 0)] = -K c00_i(dr) - K_0 c0_i(dr),   d r_eq[i] / d p[i + (0, dc)] = -K c11_j(dc) - K_1 c1_j(dc)
 //   (the two centre entries add), d r_bc0 = -/+ c0_i(dr) on rows 0 / P-1, d r_bc1 = +/- s c1_j(dc) on columns 0 / P-1,
 // and every other entry is zero.  One CTA per sample evaluates them from the K plane in shared memory and reduces the
-// (signed, like torch.max) maximum.
+// (signed, like torch.max) maximum.  Periodic: every pixel has the central entries; the neighbours wrap, and since
+// P > 3 the three offsets of a row still name three distinct pixels.
+template <bool PER>
 __device__ __forceinline__ int stencil1(int x, int off[4], float c[4]) {           // first derivative, index x of P
-    if (x == 0) { off[0] = 0; c[0] = -1.5f; off[1] = 1; c[1] = 2.f; off[2] = 2; c[2] = -0.5f; return 3; }
-    if (x == P - 1) { off[0] = 0; c[0] = 1.5f; off[1] = -1; c[1] = -2.f; off[2] = -2; c[2] = 0.5f; return 3; }
+    if (!PER && x == 0) { off[0] = 0; c[0] = -1.5f; off[1] = 1; c[1] = 2.f; off[2] = 2; c[2] = -0.5f; return 3; }
+    if (!PER && x == P - 1) { off[0] = 0; c[0] = 1.5f; off[1] = -1; c[1] = -2.f; off[2] = -2; c[2] = 0.5f; return 3; }
     off[0] = -1; c[0] = -0.5f; off[1] = 1; c[1] = 0.5f; off[2] = 0; c[2] = 0.f;
     return 3;
 }
+template <bool PER>
 __device__ __forceinline__ int stencil2(int x, int off[4], float c[4]) {           // second derivative
+    if (PER) {
+        off[0] = -1; c[0] = 1.f; off[1] = 0; c[1] = -2.f; off[2] = 1; c[2] = 1.f;
+        return 3;
+    }
     if (x == 0) { off[0] = 0; c[0] = 2.f; off[1] = 1; c[1] = -5.f; off[2] = 2; c[2] = 4.f; off[3] = 3; c[3] = -1.f; return 4; }
     if (x == P - 1) { off[0] = 0; c[0] = 2.f; off[1] = -1; c[1] = -5.f; off[2] = -2; c[2] = 4.f; off[3] = -3; c[3] = -1.f; return 4; }
     off[0] = -1; c[0] = 1.f; off[1] = 0; c[1] = -2.f; off[2] = 1; c[2] = 1.f;
     return 3;
 }
 // entries of one direction: e(d) = -K * c2(d) * inv_h2 - Kd * c1(d) * inv_h, merged over the offsets d in [-3, 3]
+template <bool PER>
 __device__ __forceinline__ void dir_entries(int x, float kv, float kd, float inv_h, float inv_h2, float e[7], bool has[7]) {
 #pragma unroll
     for (int d = 0; d < 7; ++d) { e[d] = 0.f; has[d] = false; }
     int off[4]; float c[4];
-    int n = stencil2(x, off, c);
+    int n = stencil2<PER>(x, off, c);
     for (int k = 0; k < n; ++k) { e[off[k] + 3] += -kv * c[k] * inv_h2; has[off[k] + 3] = true; }
-    n = stencil1(x, off, c);
+    n = stencil1<PER>(x, off, c);
     for (int k = 0; k < n; ++k) { e[off[k] + 3] += -kd * c[k] * inv_h; has[off[k] + 3] = true; }
 }
+template <bool PER>
 __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const float* __restrict__ x0hat,
                                                                           float* __restrict__ out, DarcyGeom g) {
     pdl_trigger();
@@ -473,11 +533,11 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const
     for (int q = threadIdx.x; q < PP; q += blockDim.x) {
         const int i = q / P, j = q - i * P;
         const float kv = sk[q];
-        const float k0 = d_row(sk, i, j, g.inv_h0), k1 = d_col(sk, i, j, g.inv_h1);
+        const float k0 = d_row<PER>(sk, i, j, g.inv_h0), k1 = d_col<PER>(sk, i, j, g.inv_h1);
         float er[7], ec[7];
         bool hr[7], hc[7];
-        dir_entries(i, kv, k0, g.inv_h0, g.inv_h0sq, er, hr);
-        dir_entries(j, kv, k1, g.inv_h1, g.inv_h1sq, ec, hc);
+        dir_entries<PER>(i, kv, k0, g.inv_h0, g.inv_h0sq, er, hr);
+        dir_entries<PER>(j, kv, k1, g.inv_h1, g.inv_h1sq, ec, hc);
         m = fmaxf(m, er[3] + ec[3]);                     // both directions touch the pixel itself
 #pragma unroll
         for (int d = 0; d < 7; ++d) {
@@ -487,12 +547,12 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const
         }
         int off[4]; float c[4];
         if (i == 0 || i == P - 1) {                      // bc_x0 = -p_0 (row 0), +p_0 (row P-1)
-            const int n = stencil1(i, off, c);
+            const int n = stencil1<PER>(i, off, c);
             const float sg = (i == 0) ? -g.inv_h0 : g.inv_h0;
             for (int k = 0; k < n; ++k) m = fmaxf(m, sg * c[k]);
         }
         if (j == 0 || j == P - 1) {                      // bc_x1 = +s p_1 (column 0), -s p_1 (column P-1)
-            const int n = stencil1(j, off, c);
+            const int n = stencil1<PER>(j, off, c);
             const float sg = ((j == 0) ? g.bc1_sign : -g.bc1_sign) * g.inv_h1;
             for (int k = 0; k < n; ++k) m = fmaxf(m, sg * c[k]);
         }
@@ -508,6 +568,7 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const
 }
 
 // single derivative field (StencilGradients.forward, grad_utils.py:161-175); global-memory version, forward only
+template <bool PER>
 __global__ void fd_stencil_kernel(const float* __restrict__ u, float* __restrict__ out, int planes, int mode,
                                   float inv_h0, float inv_h1) {
     pdl_trigger();
@@ -519,24 +580,24 @@ __global__ void fd_stencil_kernel(const float* __restrict__ u, float* __restrict
         for (int i = threadIdx.x; i < PP; i += blockDim.x) su[i] = u[(size_t)pl * PP + i];
         __syncthreads();
         if (mode == 4) {   // d_d01 = d/dx0 (d/dx1 u): tensor product of the 1-D stencils
-            for (int i = threadIdx.x; i < PP; i += blockDim.x) st[i] = d_col(su, i / P, i % P, inv_h1);
+            for (int i = threadIdx.x; i < PP; i += blockDim.x) st[i] = d_col<PER>(su, i / P, i % P, inv_h1);
             __syncthreads();
         }
         for (int i = threadIdx.x; i < PP; i += blockDim.x) {
             int r = i / P, c = i % P;
             float v;
-            if (mode == 0) v = d_row(su, r, c, inv_h0);
-            else if (mode == 1) v = d_col(su, r, c, inv_h1);
-            else if (mode == 2) v = d2_row(su, r, c, inv_h0 * inv_h0);
-            else if (mode == 3) v = d2_col(su, r, c, inv_h1 * inv_h1);
-            else v = d_row(st, r, c, inv_h0);
+            if (mode == 0) v = d_row<PER>(su, r, c, inv_h0);
+            else if (mode == 1) v = d_col<PER>(su, r, c, inv_h1);
+            else if (mode == 2) v = d2_row<PER>(su, r, c, inv_h0 * inv_h0);
+            else if (mode == 3) v = d2_col<PER>(su, r, c, inv_h1 * inv_h1);
+            else v = d_row<PER>(st, r, c, inv_h0);
             out[(size_t)pl * PP + i] = v;
         }
     }
 }
 
-static DarcyGeom make_geom(float domain_length, int reverse_d1, int pixels_at_boundary) {
-    float d0 = pixels_at_boundary ? domain_length / (P - 1) : domain_length / P;
+static DarcyGeom make_geom(float domain_length, int reverse_d1, int flags) {
+    float d0 = (flags & PIDM_DARCY_PIXELS_AT_BOUNDARY) ? domain_length / (P - 1) : domain_length / P;
     float d1 = reverse_d1 ? -d0 : d0;
     DarcyGeom g;
     g.inv_h0 = 1.f / d0;
@@ -558,8 +619,15 @@ static int darcy_sm_count(int& sm_count) {
     return 0;
 }
 
+static int check_flags(int flags) {
+    PIDM_REQUIRE((flags & ~(PIDM_DARCY_PIXELS_AT_BOUNDARY | PIDM_DARCY_PERIODIC)) == 0,
+                 "darcy: unknown flag bits 0x%x (PIDM_DARCY_PIXELS_AT_BOUNDARY = 1, PIDM_DARCY_PERIODIC = 2)", flags);
+    return 0;
+}
+
+template <bool PER>
 static int launch_darcy_fwd(const float* x0hat, const float* fs, float* residual, int B, int pixels, float domain_length,
-                            int reverse_d1, int pixels_at_boundary, cudaStream_t stream) {
+                            int reverse_d1, int flags, cudaStream_t stream) {
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
     int sm_count;
@@ -567,40 +635,51 @@ static int launch_darcy_fwd(const float* x0hat, const float* fs, float* residual
     const size_t smem = sizeof(DarcySmem);
     static bool attr_set = false;
     if (!attr_set) {
-        PIDM_CUDA(cudaFuncSetAttribute(darcy_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PIDM_CUDA(cudaFuncSetAttribute(darcy_fwd_kernel<PER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     const int ctas_per_sm = (int)(220 * 1024 / smem);        // smem-limited residency
     int grid = sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 1);
     if (grid > B) grid = B;
-    PIDM_CUDA(launch_pdl(darcy_fwd_kernel, dim3(grid), dim3(DARCY_THREADS), (size_t)(smem), stream, x0hat, fs, residual, B,
-                         make_geom(domain_length, reverse_d1, pixels_at_boundary)));
+    PIDM_CUDA(launch_pdl(darcy_fwd_kernel<PER>, dim3(grid), dim3(DARCY_THREADS), (size_t)(smem), stream, x0hat, fs, residual,
+                         B, make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_fwd_kernel");
     return 0;
 }
 
-template <int MODE>
+template <int MODE, bool PER>
 static int launch_darcy_grad(const float* x0hat, const float* fs, const float* cot, float* grad_x0hat, const float* target,
                              const float* model_out, float* grad_model_out, const long long* t, const float* p2w,
                              const float* pvar, float c_data, float c_res, float* sums, int B, int pixels,
-                             float domain_length, int reverse_d1, int pixels_at_boundary, cudaStream_t stream) {
+                             float domain_length, int reverse_d1, int flags, cudaStream_t stream) {
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
     int sm_count;
     if (int e = darcy_sm_count(sm_count)) return e;
     const size_t smem = sizeof(DarcyGradSmem);
-    static bool attr_set[3] = {false, false, false};
-    if (!attr_set[MODE]) {
-        PIDM_CUDA(cudaFuncSetAttribute(darcy_grad_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[MODE] = true;
+    static bool attr_set = false;                             // one flag per <MODE, PER> instantiation
+    if (!attr_set) {
+        PIDM_CUDA(cudaFuncSetAttribute(darcy_grad_kernel<MODE, PER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem));
+        attr_set = true;
     }
     int grid = sm_count;                                      // 145 KB of shared memory: one CTA of 512 threads per SM
     if (grid > B) grid = B;
-    PIDM_CUDA(launch_pdl(darcy_grad_kernel<MODE>, dim3(grid), dim3(DG_THREADS), (size_t)(smem), stream, x0hat, fs, cot,
-                         grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
-                         make_geom(domain_length, reverse_d1, pixels_at_boundary)));
+    PIDM_CUDA(launch_pdl(darcy_grad_kernel<MODE, PER>, dim3(grid), dim3(DG_THREADS), (size_t)(smem), stream, x0hat, fs,
+                         cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
+                         make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_grad_kernel");
     return 0;
+}
+
+template <int MODE>
+static int launch_darcy_grad_any(const float* x0hat, const float* fs, const float* cot, float* grad_x0hat,
+                                 const float* target, const float* model_out, float* grad_model_out, const long long* t,
+                                 const float* p2w, const float* pvar, float c_data, float c_res, float* sums, int B,
+                                 int pixels, float domain_length, int reverse_d1, int flags, cudaStream_t stream) {
+    auto launch = (flags & PIDM_DARCY_PERIODIC) ? launch_darcy_grad<MODE, true> : launch_darcy_grad<MODE, false>;
+    return launch(x0hat, fs, cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
+                  pixels, domain_length, reverse_d1, flags, stream);
 }
 
 }  // namespace pidm
@@ -610,45 +689,55 @@ using namespace pidm;
 extern "C" int pidm_fd_stencil(const float* u, float* out, int planes, int pixels, int mode, float d0, float d1,
                                void* stream) {
     PIDM_REQUIRE(pixels == P, "fd_stencil is built for %d x %d fields (got %d)", P, P, pixels);
-    PIDM_REQUIRE(mode >= 0 && mode <= 4, "fd_stencil: mode must be 0..4 (d_d0, d_d1, d_d00, d_d11, d_d01)");
+    const bool periodic = (mode & PIDM_FD_PERIODIC) != 0;
+    mode &= ~PIDM_FD_PERIODIC;
+    PIDM_REQUIRE(mode >= 0 && mode <= 4,
+                 "fd_stencil: mode must be 0..4 (d_d0, d_d1, d_d00, d_d11, d_d01), optionally | PIDM_FD_PERIODIC");
     int grid = planes < num_sms() * 4 ? planes : num_sms() * 4;
-    PIDM_CUDA(launch_pdl(fd_stencil_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, u, out, planes, mode, 1.f / d0, 1.f / d1));
+    auto kernel = periodic ? fd_stencil_kernel<true> : fd_stencil_kernel<false>;
+    PIDM_CUDA(launch_pdl(kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, u, out, planes, mode, 1.f / d0,
+                         1.f / d1));
     PIDM_LAUNCH_CHECK("fd_stencil");
     return 0;
 }
 
 extern "C" int pidm_darcy_residual_fwd(const float* x0hat, const float* f_s, float* residual, int B, int pixels,
-                                       float domain_length, int reverse_d1, int pixels_at_boundary, void* stream) {
-    return launch_darcy_fwd(x0hat, f_s, residual, B, pixels, domain_length, reverse_d1, pixels_at_boundary,
-                            (cudaStream_t)stream);
+                                       float domain_length, int reverse_d1, int flags, void* stream) {
+    if (int e = check_flags(flags)) return e;
+    auto launch = (flags & PIDM_DARCY_PERIODIC) ? launch_darcy_fwd<true> : launch_darcy_fwd<false>;
+    return launch(x0hat, f_s, residual, B, pixels, domain_length, reverse_d1, flags, (cudaStream_t)stream);
 }
 
 extern "C" int pidm_darcy_residual_bwd(const float* x0hat, const float* f_s, const float* grad_residual,
                                        float* grad_x0hat, int B, int pixels, float domain_length, int reverse_d1,
-                                       int pixels_at_boundary, void* stream) {
-    return launch_darcy_grad<1>(x0hat, f_s, grad_residual, grad_x0hat, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                nullptr, 0.f, 0.f, nullptr, B, pixels, domain_length, reverse_d1, pixels_at_boundary,
-                                (cudaStream_t)stream);
+                                       int flags, void* stream) {
+    if (int e = check_flags(flags)) return e;
+    return launch_darcy_grad_any<1>(x0hat, f_s, grad_residual, grad_x0hat, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                    nullptr, 0.f, 0.f, nullptr, B, pixels, domain_length, reverse_d1, flags,
+                                    (cudaStream_t)stream);
 }
 
 extern "C" int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, const float* target, const float* f_s,
                                     const long long* t, const float* p2_loss_weight, const float* posterior_var_clipped,
                                     float c_data, float c_residual, float* sums3, float* grad_x0hat,
                                     float* grad_model_out, int B, int pixels, float domain_length, int reverse_d1,
-                                    int pixels_at_boundary, void* stream) {
+                                    int flags, void* stream) {
+    if (int e = check_flags(flags)) return e;
     PIDM_CUDA(cudaMemsetAsync(sums3, 0, 3 * sizeof(float), (cudaStream_t)stream));
-    return launch_darcy_grad<2>(x0hat, f_s, nullptr, grad_x0hat, target, model_out, grad_model_out, t, p2_loss_weight,
-                                posterior_var_clipped, c_data, c_residual, sums3, B, pixels, domain_length, reverse_d1,
-                                pixels_at_boundary, (cudaStream_t)stream);
+    return launch_darcy_grad_any<2>(x0hat, f_s, nullptr, grad_x0hat, target, model_out, grad_model_out, t, p2_loss_weight,
+                                    posterior_var_clipped, c_data, c_residual, sums3, B, pixels, domain_length, reverse_d1,
+                                    flags, (cudaStream_t)stream);
 }
 
 /* max_dr_dp[b] = largest entry of the Jacobian d residual / d p of sample b (CoCoGen step size, residuals_darcy.py:218-231) */
 extern "C" int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int B, int pixels, float domain_length,
-                                       int reverse_d1, int pixels_at_boundary, void* stream) {
+                                       int reverse_d1, int flags, void* stream) {
+    if (int e = check_flags(flags)) return e;
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
-    PIDM_CUDA(launch_pdl(darcy_jacobian_max_kernel, dim3(B), dim3(DARCY_THREADS), (size_t)0, (cudaStream_t)stream, x0hat,
-                         max_dr_dp, make_geom(domain_length, reverse_d1, pixels_at_boundary)));
+    auto kernel = (flags & PIDM_DARCY_PERIODIC) ? darcy_jacobian_max_kernel<true> : darcy_jacobian_max_kernel<false>;
+    PIDM_CUDA(launch_pdl(kernel, dim3(B), dim3(DARCY_THREADS), (size_t)0, (cudaStream_t)stream, x0hat, max_dr_dp,
+                         make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_jacobian_max");
     return 0;
 }

@@ -4,7 +4,8 @@ The training / sampling path never calls these one derivative at a time: `Residu
 derivatives, the PDE residual, the boundary terms and (in training) the loss inside ONE kernel (csrc/darcy.cu).
 `GradientsHelper.stencil_gradients` is kept for callers that want a single derivative field; it is one libpidm
 launch (second-order central stencil in the interior, one-sided 3/4-point stencils on the boundary -- the net
-effect of the reference's 9 conv2d + 9 slice assignments, grad_utils.py:64-146).  Forward only."""
+effect of the reference's 9 conv2d + 9 slice assignments, grad_utils.py:64-146; with periodic=True the central stencil
+with wrapped neighbours at every pixel, grad_utils.py:76-81).  Forward only."""
 import numpy as np
 import torch
 
@@ -28,6 +29,7 @@ def generalized_b_xy_c_to_image(tensor, pixels_x=None, pixels_y=None):
 
 
 _MODES = {'d_d0': 0, 'd_d1': 1, 'd_d00': 2, 'd_d11': 3, 'd_d01': 4}
+_FD_PERIODIC = 8                         # PIDM_FD_PERIODIC (pidm.h)
 
 
 class StencilGradients(torch.nn.Module):
@@ -35,9 +37,8 @@ class StencilGradients(torch.nn.Module):
         super().__init__()
         if fd_acc != 2:
             raise NotImplementedError('only fd_acc = 2 is built (model.yaml: "keep at 2")')
-        if periodic:
-            raise NotImplementedError("periodic boundary stencils are not used by the reference drivers (bcs='none')")
         self.d0, self.d1 = float(d0), float(d1)
+        self.periodic = bool(periodic)          # wrapped central stencil at every pixel (grad_utils.py:76-81)
 
     def forward(self, x, mode):
         from ._lib import call, stream
@@ -51,7 +52,8 @@ class StencilGradients(torch.nn.Module):
         P = shp[-1]
         xf = x.detach().contiguous().float().reshape(-1, P, P)
         out = torch.empty_like(xf)
-        call('pidm_fd_stencil', xf, out, xf.shape[0], P, _MODES[mode], self.d0, self.d1, stream())
+        mode_bits = _MODES[mode] | (_FD_PERIODIC if self.periodic else 0)
+        call('pidm_fd_stencil', xf, out, xf.shape[0], P, mode_bits, self.d0, self.d1, stream())
         return out.reshape(shp)
 
 

@@ -686,12 +686,21 @@ class _DarcyResidual(torch.autograd.Function):
         return gx, None, None
 
 
-def darcy_residual(x0hat, f_s, domain_length=1.0, reverse_d1=True, pixels_at_boundary=True):
+DARCY_PIXELS_AT_BOUNDARY = 1      # flag bits of the Darcy C ABI (pidm.h)
+DARCY_PERIODIC = 2
+
+
+def darcy_flags(pixels_at_boundary, periodic=False):
+    """The flags word of the Darcy entry points: pixels_at_boundary (bit 0) and bcs='periodic' (bit 1)."""
+    return (DARCY_PIXELS_AT_BOUNDARY if pixels_at_boundary else 0) | (DARCY_PERIODIC if periodic else 0)
+
+
+def darcy_residual(x0hat, f_s, domain_length=1.0, reverse_d1=True, pixels_at_boundary=True, periodic=False):
     _need_cuda(x0hat)
     _need_f32(f_s=f_s)
     assert x0hat.shape[1] == 2, 'Darcy fields are (p, K)'
     return _DarcyResidual.apply(x0hat.contiguous().float(), f_s,
-                                (float(domain_length), int(reverse_d1), int(pixels_at_boundary)))
+                                (float(domain_length), int(reverse_d1), darcy_flags(pixels_at_boundary, periodic)))
 
 
 class _DarcyPidmLoss(torch.autograd.Function):
@@ -728,11 +737,11 @@ class _DarcyPidmLoss(torch.autograd.Function):
 
 
 def darcy_pidm_loss(x0hat, model_out, target, t, f_s, p2w, pvar, c_data, c_res, domain_length=1.0, reverse_d1=True,
-                    pixels_at_boundary=True):
+                    pixels_at_boundary=True, periodic=False):
     """Returns (loss, sums) with sums = [data_loss, residual_loss, mean|r|] on the device."""
     _need_cuda(x0hat, target)
     _need_f32(f_s=f_s, p2w=p2w, pvar=pvar)
-    geom = (float(domain_length), int(reverse_d1), int(pixels_at_boundary))
+    geom = (float(domain_length), int(reverse_d1), darcy_flags(pixels_at_boundary, periodic))
     if model_out is not None and model_out is x0hat:
         model_out = None
     return _DarcyPidmLoss.apply(x0hat.contiguous().float(),

@@ -12,15 +12,15 @@ class ResidualsDarcy:
         self.gov_eqs = 'darcy'
         self.model = model
         self.pixels_at_boundary = pixels_at_boundary
+        # bcs='periodic': wrapped central stencils at every pixel (reference grad_utils.py:76-81); h, f_s, the two BC
+        # channels and the trapezoid weights are the same as with 'none'
         self.periodic = bcs == 'periodic'
         self.input_dim = 2
-        if self.periodic:
-            raise NotImplementedError("bcs='periodic' is not used by the reference drivers")
         d0 = domain_length / (pixels_per_dim - 1) if pixels_at_boundary else domain_length / pixels_per_dim
         d1 = -d0 if reverse_d1 else d0
         self.reverse_d1 = reverse_d1
         self.domain_length = domain_length
-        self.grads = GradientsHelper(d0=d0, d1=d1, fd_acc=fd_acc, periodic=False, device=device)
+        self.grads = GradientsHelper(d0=d0, d1=d1, fd_acc=fd_acc, periodic=self.periodic, device=device)
         self.pixels_per_dim = pixels_per_dim
         self.device = device
         # stationary source field on the pixel-centre grid (reference :40-53,95-104)
@@ -39,7 +39,13 @@ class ResidualsDarcy:
         self.residual_grad_guidance = residual_grad_guidance
         self.use_ddim_x0 = use_ddim_x0
         self.ddim_steps = ddim_steps
-        self.geometry = (float(domain_length), bool(reverse_d1), bool(pixels_at_boundary))
+        # (domain_length, reverse_d1, pixels_at_boundary, periodic): trailing arguments of ops.darcy_residual / _pidm_loss
+        self.geometry = (float(domain_length), bool(reverse_d1), bool(pixels_at_boundary), self.periodic)
+
+    def _abi_geometry(self):
+        """(domain_length, reverse_d1, flags) as the Darcy C entry points take them"""
+        dl, rev, pab, per = self.geometry
+        return float(dl), int(rev), ops.darcy_flags(pab, per)
 
     def create_trapezoidal_weights(self):
         P = self.pixels_per_dim
@@ -66,8 +72,7 @@ class ResidualsDarcy:
             r = ops.darcy_residual(img, self.f_s_flat, *self.geometry)
             cot = (torch.sign(r) / r.numel()).contiguous()
             gx = torch.empty_like(img)
-            call('pidm_darcy_residual_bwd', img, self.f_s_flat, cot, gx, B, P, float(self.geometry[0]), int(self.geometry[1]),
-                 int(self.geometry[2]), stream())
+            call('pidm_darcy_residual_bwd', img, self.f_s_flat, cot, gx, B, P, *self._abi_geometry(), stream())
         return generalized_image_to_b_xy_c(gx).contiguous()
 
     def predict_x0(self, model_input, ddim_func=None, sample=False):
@@ -123,11 +128,10 @@ class ResidualsDarcy:
             B, _, P, _ = img.shape
             r = ops.darcy_residual(img, self.f_s_flat, *self.geometry)
             gx = torch.empty_like(img)
-            call('pidm_darcy_residual_bwd', img, self.f_s_flat, (2.0 * r).contiguous(), gx, B, P, float(self.geometry[0]),
-                 int(self.geometry[1]), int(self.geometry[2]), stream())
+            call('pidm_darcy_residual_bwd', img, self.f_s_flat, (2.0 * r).contiguous(), gx, B, P, *self._abi_geometry(),
+                 stream())
             mx = torch.empty(B, device=img.device, dtype=torch.float32)
-            call('pidm_darcy_jacobian_max', img, mx, B, P, float(self.geometry[0]), int(self.geometry[1]),
-                 int(self.geometry[2]), stream())
+            call('pidm_darcy_jacobian_max', img, mx, B, P, *self._abi_geometry(), stream())
             eps = 1.e-6 / torch.clamp(mx, max=1e12)
             x0_pred_in[:, :, 0] -= eps.unsqueeze(1) * gx[:, 0].reshape(B, -1)
             residual_corrected = ops.darcy_residual(generalized_b_xy_c_to_image(x0_pred_in).contiguous().float(),

@@ -126,9 +126,8 @@ class ResidualsMechanics:
         self.model = model
         self.pixels_at_boundary = pixels_at_boundary
         self.E, self.nu = E, nu
+        # the reference only stores the flag (residuals_mechanics_K.py:122-125): 'periodic' computes what 'none' computes
         self.periodic = bcs == 'periodic'
-        if self.periodic:
-            raise NotImplementedError("bcs='periodic' is not used by the reference drivers")
         self.device = device
         self.pixels_per_dim = pixels_per_dim
         self.KE = q4_plane_stress_stiffness(1.0, 0.3).float().to(device).contiguous()

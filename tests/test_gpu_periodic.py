@@ -1,0 +1,455 @@
+"""bcs='periodic' on the GPU: every periodic Darcy kernel per element against the fp64 periodic oracle, edited references
+rejected by the same predicate, and the engine end to end against the fixtures of the unmodified reference
+(scripts/make_golden_periodic.py) at the tolerances of the matching 'none' tests."""
+import os
+import sys
+
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import periodic_oracle as PO  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+DEV = 'cuda'
+P = 64
+U = 2.0 ** -24
+C_BOUND = 16            # |y - r| <= C_BOUND * 2^-24 * A: a handful of fp32 roundings along each stencil / product chain
+GUARD = 1024            # NaN guard floats on each side of every output
+
+
+def rel(a, b):
+    a, b = a.double().cpu(), b.double().cpu()
+    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+
+
+# ---- fp64 reference and its absolute-value operator -----------------------------------------------------------------
+def _d1(u, ax, h, absolute=False):
+    if absolute:
+        return (torch.roll(u, -1, ax) + torch.roll(u, 1, ax)) * (0.5 / abs(h))
+    return PO.fd_first(u, ax, h)
+
+
+def _d2(u, ax, h, absolute=False):
+    if absolute:
+        return (torch.roll(u, -1, ax) + 2.0 * u + torch.roll(u, 1, ax)) / (h * h)
+    return PO.fd_second(u, ax, h)
+
+
+def residual_op(x, absolute=False, edit=None):
+    """the periodic residual in fp64 ([B,P*P,3]); absolute=True evaluates it with |coefficients| on the given
+    (non-negative) fields, which bounds every intermediate of the fp32 evaluation.  `edit` builds the wrong references
+    the predicate has to reject."""
+    d0, d1 = PO.spacing(P)
+    p, K = x[:, 0], x[:, 1]
+    p0, p1, K0, K1 = _d1(p, -2, d0, absolute), _d1(p, -1, d1, absolute), _d1(K, -2, d0, absolute), _d1(K, -1, d1, absolute)
+    p00, p11 = _d2(p, -2, d0, absolute), _d2(p, -1, d1, absolute)
+    if edit == 'one_sided_row0':                 # the wrap dropped at row 0: the one-sided stencils of bcs='none' there
+        from oracle import pidm_oracle as O
+        p0[:, 0], p00[:, 0], K0[:, 0] = (O.fd_first(p, -2, d0)[:, 0], O.fd_second(p, -2, d0)[:, 0],
+                                         O.fd_first(K, -2, d0)[:, 0])
+    fs = PO.O.darcy_source(P, dtype=torch.float64).to(x.device)
+    if absolute:
+        eq0 = K * (p00 + p11) + K0 * p0 + K1 * p1 + fs.abs()
+        bc0 = torch.zeros_like(p)
+        bc1 = torch.zeros_like(p)
+        bc0[:, 0], bc0[:, -1] = p0[:, 0], p0[:, -1]
+        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], p1[:, :, -1]
+    else:
+        eq0 = (-K * p00 - K0 * p0) + (-K * p11 - K1 * p1) - fs
+        bc0 = torch.zeros_like(p)
+        bc1 = torch.zeros_like(p)
+        bc0[:, 0], bc0[:, -1] = -p0[:, 0], p0[:, -1]
+        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], -p1[:, :, -1]          # reverse_d1
+    r = torch.stack([eq0, bc0, bc1], dim=-1).reshape(x.shape[0], P * P, 3)
+    if edit == 'corner_sign':
+        r[:, 0, 1] = -r[:, 0, 1]
+    if edit == 'last_row_zero':
+        r[-1, -P:] = 0
+    return r
+
+
+def vjp(x, cot, absolute=False):
+    """J^T cot in fp64; absolute=True: |J|^T |cot| at |x| (the residual is bilinear in (p, K) with non-negative
+    coefficients in its absolute form, so this gradient bounds every product of the adjoint)"""
+    xa = (x.abs() if absolute else x).clone().requires_grad_(True)
+    r = residual_op(xa, absolute)
+    if absolute:
+        r = r - residual_op(torch.zeros_like(xa), True)           # drop the constant |f_s|
+    return torch.autograd.grad((r * (cot.abs() if absolute else cot)).sum(), xa)[0]
+
+
+def within(y, r, A, c=C_BOUND):
+    return bool(((y.double() - r).abs() <= c * U * A).all())
+
+
+def guarded(n):
+    buf = torch.full((n + 2 * GUARD,), float('nan'), device=DEV)
+    return buf, buf[GUARD:GUARD + n]
+
+
+def guards_intact(buf):
+    return bool(torch.isnan(buf[:GUARD]).all() and torch.isnan(buf[-GUARD:]).all())
+
+
+def fields(B, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(B, 2, P, P, generator=g, dtype=torch.float64)
+    x[:, 1] = torch.exp(0.5 * x[:, 1])
+    return x.float().double()            # fp32-representable inputs
+
+
+FLAGS = 1 | 2             # PIDM_DARCY_PIXELS_AT_BOUNDARY | PIDM_DARCY_PERIODIC
+
+
+def fs_dev():
+    return PO.O.darcy_source(P).to(DEV).contiguous()
+
+
+def launch_fwd(x):
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    B = x.shape[0]
+    buf, out = guarded(B * P * P * 3)
+    call('pidm_darcy_residual_fwd', x.float().to(DEV).contiguous(), fs_dev(), out, B, P, 1.0, 1, FLAGS, stream())
+    torch.cuda.synchronize()
+    return buf, out.reshape(B, P * P, 3).cpu()
+
+
+BATCHES = [1, 3, 32, 400]
+
+
+@pytest.mark.parametrize('B', BATCHES)
+def test_periodic_residual_per_element(B):
+    x = fields(B, 10 + B)
+    buf, y = launch_fwd(x)
+    assert guards_intact(buf) and not torch.isnan(y).any()
+    r, A = residual_op(x), residual_op(x.abs(), absolute=True)
+    err = ((y.double() - r).abs() / (U * A)).max().item()
+    assert within(y, r, A), err
+
+
+@pytest.mark.parametrize('edit', ['one_sided_row0', 'corner_sign', 'last_row_zero'])
+def test_edited_references_are_rejected(edit):
+    x = fields(32, 42)
+    _, y = launch_fwd(x)
+    A = residual_op(x.abs(), absolute=True)
+    assert within(y, residual_op(x), A)
+    assert not within(y, residual_op(x, edit=edit), A), edit
+
+
+@pytest.mark.parametrize('B', BATCHES)
+def test_periodic_vjp_per_element(B):
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    x = fields(B, 20 + B)
+    cot = torch.randn(B, P * P, 3, generator=torch.Generator().manual_seed(B), dtype=torch.float64).float().double()
+    buf, gx = guarded(B * 2 * P * P)
+    call('pidm_darcy_residual_bwd', x.float().to(DEV).contiguous(), fs_dev(), cot.float().to(DEV).contiguous(), gx, B, P,
+         1.0, 1, FLAGS, stream())
+    torch.cuda.synchronize()
+    assert guards_intact(buf) and not torch.isnan(gx).any()
+    gx = gx.reshape(B, 2, P, P).cpu()
+    assert within(gx, vjp(x, cot), vjp(x, cot, absolute=True)), \
+        ((gx.double() - vjp(x, cot)).abs() / (U * vjp(x, cot, absolute=True))).max().item()
+
+
+def _loss_reference(x, m, tgt, t, tab_p2, tab_var, c_data, c_res):
+    """sums and gradients of the fused loss in fp64 with their bounds"""
+    B = x.shape[0]
+    r = residual_op(x)
+    Ar = residual_op(x.abs(), absolute=True)
+    wr = 0.5 * c_res / (tab_var[t] * B * P * P * 3)                     # per sample
+    wd = c_data * tab_p2[t] / (B * 2 * P * P)
+    sums = torch.stack([(wd[:, None, None, None] * (m - tgt) ** 2).sum(), (wr[:, None, None] * r ** 2).sum(),
+                        r.abs().mean()])
+    sums_A = torch.stack([(wd[:, None, None, None] * (m.abs() + tgt.abs()) ** 2).sum(),
+                          (wr[:, None, None] * Ar ** 2).sum(), Ar.mean()])
+    cot = 2 * wr[:, None, None] * r
+    gx = vjp(x, cot)
+    # the fp32 cotangent 2 wr r carries the residual's own error (<= C_BOUND 2^-24 Ar) and that of wr: the adjoint is
+    # bounded with twice 2 wr Ar, which leaves C_BOUND 2^-24 for each of the two
+    A_gx = vjp(x, 4 * wr[:, None, None] * Ar, absolute=True)
+    gm = 2 * wd[:, None, None, None] * (m - tgt)
+    A_gm = 2 * wd[:, None, None, None] * (m.abs() + tgt.abs())
+    return sums, sums_A, gx, A_gx, gm, A_gm
+
+
+@pytest.mark.parametrize('B', BATCHES)
+@pytest.mark.parametrize('variant', ['mean', 'sample', 'loss_only'])
+def test_periodic_fused_loss_per_element(B, variant):
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
+    dd = DenoisingDiffusion(100, DEV).diff_dict
+    p2, var = dd['p2_loss_weight'].float().contiguous(), dd['posterior_variance_clipped'].float().contiguous()
+    x = fields(B, 30 + B)
+    g = torch.Generator().manual_seed(300 + B)
+    tgt = torch.randn(B, 2, P, P, generator=g).double()
+    t = torch.randint(0, 100, (B,), generator=g)
+    m = torch.randn(B, 2, P, P, generator=g).double() if variant == 'sample' else x
+    xd, md = x.float().to(DEV).contiguous(), m.float().to(DEV).contiguous()
+    sums = torch.zeros(3, device=DEV)
+    bx, gx = guarded(B * 2 * P * P)
+    bm, gm = guarded(B * 2 * P * P)
+    c_data, c_res = 1.0, 1e-3
+    call('pidm_darcy_pidm_loss', xd, xd if variant != 'sample' else md, tgt.float().to(DEV).contiguous(), fs_dev(),
+         t.to(DEV), p2, var, c_data, c_res, sums, None if variant == 'loss_only' else gx,
+         gm if variant == 'sample' else None, B, P, 1.0, 1, FLAGS, stream())
+    torch.cuda.synchronize()
+    rs, rA, rgx, A_gx, rgm, A_gm = _loss_reference(x, m, tgt, t, p2.double().cpu(), var.double().cpu(), c_data, c_res)
+    # a sum over N terms: per-term error plus fp32 accumulation (per thread, warp, CTA, one atomic per CTA)
+    depth = 4 * 2 * ((B + 131) // 132) + 5 + 16 + 132
+    assert ((sums.cpu().double() - rs).abs() <= (depth + 2 * C_BOUND) * U * rA).all(), (sums.cpu(), rs)
+    assert guards_intact(bx) and guards_intact(bm)
+    if variant == 'loss_only':
+        assert torch.isnan(gx).all() and torch.isnan(gm).all()           # NULL gradients: nothing written
+        return
+    gxc = gx.reshape(B, 2, P, P).cpu()
+    if variant == 'mean':                                               # data gradient folded into grad_x0hat
+        assert torch.isnan(gm).all()
+        assert within(gxc, rgx + rgm, A_gx + A_gm)
+    else:
+        assert within(gxc, rgx, A_gx)
+        assert within(gm.reshape(B, 2, P, P).cpu(), rgm, A_gm)
+
+
+def _jacobian_max_ref(x):
+    """largest entry (signed, zeros included) of d r / d p per sample in fp64, with an absolute bound per sample"""
+    d0, d1 = PO.spacing(P)
+    K = x[:, 1]
+    K0, K1 = PO.fd_first(K, -2, d0), PO.fd_first(K, -1, d1)
+    e = torch.stack([-K / d0 ** 2 + K0 * 0.5 / d0, -K / d0 ** 2 - K0 * 0.5 / d0,      # rows i-1, i+1
+                     -K / d1 ** 2 + K1 * 0.5 / d1, -K / d1 ** 2 - K1 * 0.5 / d1,      # columns j-1, j+1
+                     2 * K / d0 ** 2 + 2 * K / d1 ** 2], dim=1)                     # the pixel itself
+    bc = torch.tensor(max(0.5 / abs(d0), 0.5 / abs(d1), 0.0), dtype=torch.float64)
+    mx = torch.maximum(e.reshape(x.shape[0], -1).max(dim=1).values, bc)
+    A = (K.abs() * (2 / d0 ** 2 + 2 / d1 ** 2) + (K0.abs() + K1.abs()) / abs(d0)).reshape(x.shape[0], -1).max(dim=1).values
+    return mx, A
+
+
+@pytest.mark.parametrize('B', BATCHES)
+def test_periodic_jacobian_max_per_element(B):
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    x = fields(B, 40 + B)
+    if B == 3:
+        x[1, 1] = -x[1, 1]                        # negative K: the maximum comes from the BC rows / zero entries
+    buf, out = guarded(B)
+    call('pidm_darcy_jacobian_max', x.float().to(DEV).contiguous(), out, B, P, 1.0, 1, FLAGS, stream())
+    torch.cuda.synchronize()
+    assert guards_intact(buf)
+    ref, A = _jacobian_max_ref(x)
+    assert within(out.cpu(), ref, A)
+    if B <= 3:                                    # the closed form above against the oracle's explicit Jacobian
+        assert torch.allclose(PO.jacobian_max(x), ref, rtol=1e-9, atol=0)
+
+
+@pytest.mark.parametrize('B', BATCHES)
+@pytest.mark.parametrize('mode', ['d_d0', 'd_d1', 'd_d00', 'd_d11', 'd_d01'])
+def test_periodic_fd_stencil_per_element(B, mode):
+    from physicsinformeddiffusionmodels_b200.grad_utils import StencilGradients
+    d0, d1 = PO.spacing(P)
+    u = fields(B, 50 + B)[:, 0]
+    y = StencilGradients(d0=d0, d1=d1, periodic=True)(u.float().to(DEV), mode).cpu()
+    r = PO.stencil_gradients(u, mode, d0, d1)
+    ua = u.abs()
+    A = {'d_d0': lambda: _d1(ua, -2, d0, True), 'd_d1': lambda: _d1(ua, -1, d1, True),
+         'd_d00': lambda: _d2(ua, -2, d0, True), 'd_d11': lambda: _d2(ua, -1, d1, True),
+         'd_d01': lambda: _d1(_d1(ua, -1, d1, True), -2, d0, True)}[mode]()
+    assert within(y, r, A)
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    buf, out = guarded(B * P * P)
+    call('pidm_fd_stencil', u.float().to(DEV).contiguous(), out, B, P, ['d_d0', 'd_d1', 'd_d00', 'd_d11', 'd_d01'].index(mode)
+         | 8, float(d0), float(d1), stream())
+    torch.cuda.synchronize()
+    assert guards_intact(buf) and torch.equal(out.reshape(B, P, P).cpu(), y)
+
+
+# ---- end to end ---------------------------------------------------------------------------------------------------
+@pytest.fixture(scope='module')
+def env():
+    from oracle import pidm_oracle as O
+    from physicsinformeddiffusionmodels_b200 import ops
+    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
+    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
+    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
+    cfg = O.unet_config(dim=32, channels=2)
+    sd = O.make_test_state_dict(cfg, 0)
+
+    def build(n_steps=100, **kw):
+        model = Unet3D(dim=32, channels=2).to(DEV)
+        model.load_state_dict(sd)
+        diff = DenoisingDiffusion(n_steps, DEV, kw.get('residual_grad_guidance', False))
+        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
+                             device=DEV, bcs='periodic', domain_length=1., **kw)
+        assert res.periodic
+        return model, diff, res
+    yield dict(O=O, ops=ops, build=build, cfg=cfg, sd=sd)
+    ops.set_precision('bf16')
+
+
+@pytest.mark.parametrize('mode,tol_loss,tol_grad', [('fp32', 5e-5, 1e-3), ('bf16', 3e-2, 8e-2)])
+def test_periodic_training_loss_and_gradients_match_reference(env, golden, mode, tol_loss, tol_grad):
+    env['ops'].set_precision(mode)
+    gd = golden('darcy_loss_periodic.pt')
+    model, diff, res = env['build']()
+    loss, data_l, rabs, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res,
+                                                          1.0, 1e-3)
+    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss
+    assert abs(data_l / gd['data_loss'].item() - 1) < tol_loss
+    assert abs(rabs / gd['residual_abs'].item() - 1) < tol_loss
+    loss.backward()
+    named = dict(model.named_parameters())
+    worst = {k: rel(env['O'].golden_sample(named[k[5:]].grad), v) for k, v in gd.items()
+             if k.startswith('grad_') and k != 'grad_norm'}
+    assert max(worst.values()) < tol_grad, worst
+    gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
+    assert abs(gn / gd['grad_norm'].item() - 1) < tol_grad
+
+
+def test_periodic_graph_replayed_train_step_equals_eager(env):
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
+    env['ops'].set_precision('fp32')
+    B = 32
+    g = torch.Generator().manual_seed(532)
+    x0 = (0.7 * torch.randn(B, 2, 64, 64, generator=g)).to(DEV)
+    t = torch.randint(0, 100, (B,), generator=g).to(DEV)
+    e = torch.randn(B, 2, 64, 64, generator=g).to(DEV)
+    out = {}
+    for use_graph in (False, True):
+        model, diff, res = env['build']()
+        eng = TrainEngine(model, diff, res, use_graph=use_graph, snapshot_grad=True)
+        o1, o2 = torch.randint, torch.randn_like
+        torch.randint, torch.randn_like = (lambda *a, **k: t), (lambda *a, **k: e)
+        try:
+            loss, _, _ = eng.step(x0)
+        finally:
+            torch.randint, torch.randn_like = o1, o2
+        torch.cuda.synchronize()
+        out[use_graph] = (loss.item(), eng.grad_snapshot.clone())
+    (le, ge), (lg, gg) = out[False], out[True]
+    assert abs(lg / le - 1) < 1e-5, (lg, le)
+    assert rel(gg, ge) < 1e-4, rel(gg, ge)
+    assert (ge != 0).float().mean().item() > 0.8
+
+
+def test_periodic_sample_engine_matches_reference_and_graph_replay(env, golden, monkeypatch):
+    env['ops'].set_precision('fp32')
+    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
+    gd = golden('sample_loop_periodic.pt')
+    model, diff, res = env['build'](n_steps=6)
+    model.eval()
+    it = iter(list(gd['noises']))
+    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: next(it).to(DEV))
+    x, r, traj = SampleEngine(model, diff, res, batch=1, use_graph=False).sample(x_init=gd['x_T'].to(DEV), trajectory=True)
+    monkeypatch.undo()
+    assert rel(traj[1], gd['x_after_first']) < 1e-4
+    assert rel(x, gd['x_final']) < 5e-4
+    assert rel(r, gd['residual']) < 5e-3
+    zfix = gd['noises'][0].to(DEV)
+    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: zfix)
+    xe = SampleEngine(model, diff, res, batch=1, use_graph=False).sample(x_init=gd['x_T'].to(DEV))[0].clone()
+    xg = SampleEngine(model, diff, res, batch=1, use_graph=True).sample(x_init=gd['x_T'].to(DEV))[0].clone()
+    monkeypatch.undo()
+    assert rel(xg, xe) < 1e-4, rel(xg, xe)
+
+
+def test_periodic_cocogen_correction_matches_reference(env, golden):
+    gd = golden('cocogen_periodic.pt')
+    _, _, res = env['build']()
+    xin = gd['x0_pred'].permute(0, 2, 3, 1).reshape(2, 4096, 2).clone().to(DEV)
+    x_corr, r_corr = res.residual_correction(xin)
+    assert x_corr is xin
+    img = xin.reshape(2, 64, 64, 2).permute(0, 3, 1, 2).cpu()
+    d_ref = gd['corrected'] - gd['x0_pred']
+    assert rel(img - gd['x0_pred'], d_ref) < 1e-3, rel(img - gd['x0_pred'], d_ref)
+    assert torch.equal(img[:, 1], gd['x0_pred'][:, 1])
+    assert rel(r_corr, gd['residual_corrected']) < 1e-5
+
+
+def test_periodic_residual_gradient_guidance_matches_oracle(env):
+    """guidance branch (cond = d mean|r(x_t)| / d x_t with the periodic residual) through the engine vs the periodic
+    oracle, fp32, with a classifier-free mask that drops one sample"""
+    env['ops'].set_precision('fp32')
+    O = env['O']
+    g = torch.Generator().manual_seed(77)
+    B = 4
+    x0 = torch.randn(B, 2, 64, 64, generator=g)
+    t = torch.randint(0, 100, (B,), generator=g)
+    e = torch.randn(B, 2, 64, 64, generator=g)
+    mask = torch.tensor([False, True, False, False])
+    sdr = {k: v.clone().requires_grad_('freqs' not in k) for k, v in env['sd'].items()}
+    loss_ref, _ = PO.darcy_training_loss(sdr, env['cfg'], x0, t, e, O.diffusion_tables(100), guidance_null_mask=mask)
+    loss_ref.backward()
+    model, diff, res = env['build'](residual_grad_guidance=True)
+    model._null_mask_override = mask.to(DEV)
+    loss, _, _, _, _ = diff.darcy_loss_from_draws(x0.to(DEV), t.to(DEV), e.to(DEV), res, 1.0, 1e-3)
+    model._null_mask_override = None
+    assert abs(loss.item() / loss_ref.item() - 1) < 5e-5, (loss.item(), loss_ref.item())
+    loss.backward()
+    named = dict(model.named_parameters())
+    for k in ('emb_conv.0.weight', 'combine_conv.weight', 'final_conv.1.weight'):
+        assert rel(named[k].grad, sdr[k].grad) < 2e-3, (k, rel(named[k].grad, sdr[k].grad))
+
+
+def test_reference_driver_sequence_runs_with_periodic_bcs(tmp_path):
+    """main.py / sample.py with bcs = 'periodic' on the drop-in modules: training iterations with the reference glue,
+    then the ancestral sampler with the residual evaluated each step (4 diffusion steps, batch 3)."""
+    import numpy as np
+    import torch.optim as optim
+    from src.denoising_utils import DenoisingDiffusion, EMA, device
+    from src.residuals_darcy import ResidualsDarcy
+    from src.unet_model import Unet3D
+    from physicsinformeddiffusionmodels_b200 import ops
+    ops.set_precision('bf16')
+    diffusion_utils = DenoisingDiffusion(4, device, False)
+    model = Unet3D(dim=32, channels=2, sigmoid_last_channel=False).to(device)
+    ema = EMA(0.99)
+    ema.register(model)
+    residuals = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
+                               device=device, bcs='periodic', domain_length=1., residual_grad_guidance=False,
+                               use_ddim_x0=False, ddim_steps=0)
+    optimizer = optim.Adam(model.parameters(), lr=1.e-4)
+    w_before = model.final_conv[1].weight.detach().clone()
+    g = torch.Generator().manual_seed(5)
+    losses = []
+    for iteration in range(3):
+        model.train()
+        cur_batch = torch.randn(3, 2, 64, 64, generator=g).to(device)
+        loss, data_loss, residual_loss, _, _ = diffusion_utils.model_estimation_loss(
+            cur_batch, residual_func=residuals, c_data=1, c_residual=0.001, c_ineq=0, lambda_opt=0)
+        optimizer.zero_grad()
+        loss.backward()
+        torch.nn.utils.clip_grad_norm_(model.parameters(), 1.)
+        optimizer.step()
+        losses.append(loss.item())
+        if iteration > 0:
+            ema.update(model)
+    assert all(np.isfinite(losses)) and not torch.equal(model.final_conv[1].weight.detach(), w_before)
+    model.eval()
+    seqs, aux = diffusion_utils.p_sample_loop(None, (3, 2, 64, 64), save_output=True, surpress_noise=True,
+                                              use_dynamic_threshold=False, residual_func=residuals, eval_residuals=True,
+                                              return_optimizer=False, return_inequality=False, M_correction=1,
+                                              N_correction=1, correction_mode='xt')
+    assert torch.isfinite(aux['residual']).all() and torch.isfinite(seqs[0][-1]).all()
+
+
+def test_mechanics_periodic_equals_none():
+    """ResidualsMechanics only stores the flag in the reference: 'periodic' computes exactly what 'none' computes"""
+    from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
+    g = torch.Generator().manual_seed(4)
+    x = torch.randn(2, 3, 64, 64, generator=g) * 0.1
+    x[:, 2] = torch.sigmoid(torch.randn(2, 64, 64, generator=g))
+    bcs = torch.zeros(2, 4, 65, 65)
+    bcs[:, 0, :, 0] = 1.
+    bcs[:, 1, :, 0] = 1.
+    bcs[:, 3, 20:24, 64] = -1.
+    vf = torch.tensor([0.4, 0.5])
+    outs = {}
+    for b in ('none', 'periodic'):
+        res = ResidualsMechanics(model=None, pixels_per_dim=64, pixels_at_boundary=True, no_BC_folder='', device=DEV,
+                                 bcs=b)
+        assert res.periodic == (b == 'periodic')
+        outs[b] = res.compute_residual((x.to(DEV), bcs.to(DEV), vf.to(DEV), None), reduce='per-batch',
+                                       return_optimizer=True, return_inequality=True, pass_through=True)
+    assert torch.equal(outs['none']['residual'], outs['periodic']['residual'])
+    assert torch.equal(outs['none']['inequality'], outs['periodic']['inequality'])
+    # compliance is a sum of fp32 atomics: equal up to their ordering
+    assert rel(outs['periodic']['optimizer'], outs['none']['optimizer']) < 1e-6

@@ -1,0 +1,140 @@
+"""bcs='periodic' on the CPU: the periodic oracle (tests/periodic_oracle.py) against fixtures produced by the UNMODIFIED
+reference with ResidualsDarcy(bcs='periodic') (scripts/make_golden_periodic.py), an fp64 known answer, and the host
+logic of the flag.  Tolerances are those of the matching 'none' tests in test_oracle_golden.py."""
+import math
+import os
+import sys
+
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import periodic_oracle as PO  # noqa: E402
+from oracle import pidm_oracle as O  # noqa: E402
+
+
+def rel(a, b):
+    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+
+
+def test_periodic_residual_and_vjp_match_reference(golden):
+    gd = golden('darcy_residual_periodic.pt')
+    assert torch.equal(gd['x0_pred'], golden('darcy_residual.pt')['x0_pred'])
+    assert rel(PO.darcy_residual(gd['x0_pred']), gd['residual']) < 1e-5
+    # periodic differs from 'none' (else this file would test nothing new)
+    assert rel(O.darcy_residual(gd['x0_pred']), gd['residual']) > 1e-2
+    x = gd['x0_pred'].clone().requires_grad_(True)
+    (PO.darcy_residual(x) * gd['cotangent']).sum().backward()
+    assert rel(x.grad, gd['grad_x0_pred']) < 1e-5
+
+
+@pytest.mark.parametrize('mode', ['d_d0', 'd_d1', 'd_d00', 'd_d11', 'd_d01'])
+def test_periodic_stencil_modes_match_reference(golden, mode):
+    gd = golden('darcy_residual_periodic.pt')
+    d0, d1 = PO.spacing(64)
+    assert rel(PO.stencil_gradients(gd['x0_pred'][:, 0], mode, d0, d1), gd['stencil_' + mode]) < 1e-5
+
+
+def test_periodic_cocogen_correction_matches_reference(golden):
+    gd = golden('cocogen_periodic.pt')
+    xc, rc = PO.cocogen_correction(gd['x0_pred'])
+    d_ref = gd['corrected'] - gd['x0_pred']
+    assert d_ref.abs().max() > 0
+    assert rel(xc - gd['x0_pred'], d_ref) < 1e-3
+    assert torch.equal(xc[:, 1], gd['x0_pred'][:, 1])
+    assert rel(rc, gd['residual_corrected']) < 1e-5
+
+
+def test_periodic_training_loss_and_grads_match_reference(golden):
+    gd = golden('darcy_loss_periodic.pt')
+    cfg = O.unet_config(dim=32, channels=2)
+    sd = {k: v.clone().requires_grad_(v.is_floating_point() and 'freqs' not in k)
+          for k, v in O.make_test_state_dict(cfg, 0).items()}
+    tables = O.diffusion_tables(100)
+    loss, aux = PO.darcy_training_loss(sd, cfg, gd['x0'], gd['t'], gd['noise'], tables)
+    assert abs(loss.item() / gd['loss'].item() - 1) < 2e-5
+    assert abs(aux['data'].item() / gd['data_loss'].item() - 1) < 2e-5
+    assert abs(aux['residual_abs'].item() / gd['residual_abs'].item() - 1) < 2e-5
+    loss.backward()
+    for k, v in gd.items():
+        if k.startswith('grad_') and k != 'grad_norm':
+            assert rel(O.golden_sample(sd[k[5:]].grad), v) < 5e-4, k
+    gn = math.sqrt(sum((p.grad.double() ** 2).sum().item() for p in sd.values() if p.grad is not None))
+    assert abs(gn / gd['grad_norm'].item() - 1) < 1e-4
+
+
+def test_periodic_sampling_loop_matches_reference(golden):
+    gd = golden('sample_loop_periodic.pt')
+    cfg = O.unet_config(dim=32, channels=2)
+    sd = O.make_test_state_dict(cfg, 0)
+    tables = O.diffusion_tables(6)
+    with torch.no_grad():
+        x, r = PO.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), tables, 6)
+    assert rel(x, gd['x_final']) < 2e-4
+    assert rel(r, gd['residual']) < 2e-3
+
+
+def test_periodic_residual_known_answer_fourier_modes():
+    """p = sin(a i) cos(b j), K = 2 + cos(c i) + sin(e j) with a, b, c, e multiples of 2 pi / 64.  On the periodic grid
+    the wrapped central differences of such modes are exact: D1 sin(t x) = cos(t x) sin t / h and
+    D2 sin(t x) = -4 sin^2(t/2) sin(t x) / h^2 (likewise for cos), so eq_0 and both BC channels are known in closed form."""
+    P = 64
+    h0 = 1.0 / 63
+    h1 = -h0                                                   # reverse_d1
+    a, b, c, e = (2 * math.pi * k / P for k in (1, 2, 3, 1))
+    idx = torch.arange(P, dtype=torch.float64)
+    I, J = torch.meshgrid(idx, idx, indexing='ij')
+    p = torch.sin(a * I) * torch.cos(b * J)
+    K = 2 + torch.cos(c * I) + torch.sin(e * J)
+    r = PO.darcy_residual(torch.stack([p, K])[None]).reshape(P, P, 3)
+    p0 = math.sin(a) / h0 * torch.cos(a * I) * torch.cos(b * J)
+    p1 = torch.sin(a * I) * (-math.sin(b) / h1 * torch.sin(b * J))
+    p00 = -4 * math.sin(a / 2) ** 2 / h0 ** 2 * p
+    p11 = -4 * math.sin(b / 2) ** 2 / h1 ** 2 * p
+    K0 = -math.sin(c) / h0 * torch.sin(c * I)
+    K1 = math.sin(e) / h1 * torch.cos(e * J)
+    fs = O.darcy_source(P, dtype=torch.float64)
+    exact = -(K * p00 + K0 * p0) - (K * p11 + K1 * p1) - fs
+    assert (r[..., 0] - exact).abs().max() < 1e-9
+    assert (r[0, :, 1] + p0[0]).abs().max() < 1e-9 and (r[-1, :, 1] - p0[-1]).abs().max() < 1e-9
+    assert (r[:, 0, 2] - p1[:, 0]).abs().max() < 1e-9 and (r[:, -1, 2] + p1[:, -1]).abs().max() < 1e-9
+    assert r[1:-1, :, 1].abs().max() == 0 and r[:, 1:-1, 2].abs().max() == 0
+
+
+def test_periodic_flag_is_accepted_by_the_host_classes():
+    from physicsinformeddiffusionmodels_b200.grad_utils import StencilGradients
+    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
+    from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
+    res = ResidualsDarcy(model=None, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
+                         device='cpu', bcs='periodic')
+    assert res.periodic and res.geometry == (1.0, True, True, True)
+    assert res.grads.stencil_gradients.periodic
+    none = ResidualsDarcy(model=None, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
+                          device='cpu', bcs='none')
+    assert none.geometry == (1.0, True, True, False)
+    assert torch.equal(res.f_s, none.f_s) and torch.equal(res.trapezoidal_weights, none.trapezoidal_weights)
+    assert StencilGradients(d0=1.0, d1=1.0, periodic=True).periodic
+    with pytest.raises(NotImplementedError):
+        StencilGradients(d0=1.0, d1=1.0, fd_acc=4, periodic=True)
+    assert ResidualsMechanics(model=None, pixels_per_dim=64, pixels_at_boundary=True, no_BC_folder='',
+                              bcs='periodic').periodic
+
+
+def test_darcy_flags_word():
+    from physicsinformeddiffusionmodels_b200 import ops
+    assert ops.darcy_flags(False) == 0 and ops.darcy_flags(True) == 1        # the values callers passed before
+    assert ops.darcy_flags(False, True) == 2 and ops.darcy_flags(True, True) == 3
+
+
+@pytest.mark.parametrize('name', ['pidm_darcy_residual_fwd', 'pidm_darcy_residual_bwd', 'pidm_darcy_pidm_loss',
+                                  'pidm_darcy_jacobian_max', 'pidm_fd_stencil'])
+def test_unknown_flag_bits_are_rejected_by_the_library(name):
+    """The flag check runs before any CUDA call, so it needs no device (null pointers, no stream)."""
+    from physicsinformeddiffusionmodels_b200._lib import call
+    args = {'pidm_darcy_residual_fwd': (None, None, None, 1, 64, 1.0, 1, 4, None),
+            'pidm_darcy_residual_bwd': (None, None, None, None, 1, 64, 1.0, 1, 1 | 8, None),
+            'pidm_darcy_pidm_loss': (None,) * 7 + (1.0, 1e-3) + (None,) * 3 + (1, 64, 1.0, 1, 16, None),
+            'pidm_darcy_jacobian_max': (None, None, 1, 64, 1.0, 1, -1, None),
+            'pidm_fd_stencil': (None, None, 1, 64, 4 | 16, 1.0, 1.0, None)}[name]
+    with pytest.raises(RuntimeError, match='flag|mode'):
+        call(name, *args)
