@@ -200,6 +200,25 @@ int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const void* dout, 
 int pidm_linattn_fused_wgrad(const void* xn, const void* w_qkv, const void* dout, const float* ctx, const float* dctx,
                              const float* kmax, const float* kzinv, float* grad_w, int B, int N, long long w_stride_n,
                              long long w_stride_c, void* stream);
+/* The whole linear-attention block at the 32-channel levels: y = residual + b_out + to_out(attention(to_qkv(xn))), with
+ * to_out a 1x1 256 -> 32 projection (reference unet_model.py:275-297 and the Residual wrapper's `+ x`).  Neither the
+ * attention output nor its gradient [B,N,256] is materialised: forward multiplies each head's output tile by its 32
+ * columns of W_out on chip, backward recomputes dout_h = dy W_out[:, 32h:32h+32] per head from dy.
+ *   xn, residual, y, dy, dxn: [B,N,32] bf16.  w_qkv: packed to_qkv weights [768][32] bf16.  w_out: packed forward to_out
+ *   weights [32][256] bf16 (pidm_pack_weights, row = output channel).  b_out: [32] fp32.
+ *   fwd: y is WRITTEN; ctx / kmax / kzinv / workspace as pidm_linattn_fused_fwd.
+ *   bwd: dxn is WRITTEN (the gradient through to_qkv only: the residual's gradient is dy itself); dctx is filled.
+ *   wgrad: ACCUMULATES the to_qkv weight gradient into grad_w_qkv (element [n][c] at n * qkv_stride_n + c * qkv_stride_c)
+ *   and the to_out weight gradient into grad_w_out (element [c][j] at c * out_stride_n + j * out_stride_c), both fp32.
+ *   The bias gradient (column sums of dy) is left to pidm_colsum. */
+int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const void* w_out, const float* b_out, const void* residual,
+                           void* y, float* ctx, float* kmax, float* kzinv, float* workspace, int B, int N, void* stream);
+int pidm_linattn_block_bwd(const void* xn, const void* w_qkv, const void* w_out, const void* dy, const float* ctx,
+                           const float* kmax, const float* kzinv, void* dxn, float* dctx, int B, int N, void* stream);
+int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const void* w_out, const void* dy, const float* ctx,
+                             const float* dctx, const float* kmax, const float* kzinv, float* grad_w_qkv,
+                             long long qkv_stride_n, long long qkv_stride_c, float* grad_w_out, long long out_stride_n,
+                             long long out_stride_c, int B, int N, void* stream);
 int pidm_linattn_workspace_floats(int B, int N, int heads);
 int pidm_linattn_fwd(const void* qkv, void* out, float* ctx, float* kmax, float* kzinv, float* workspace, int B, int N,
                      int heads, int dtype, void* stream);

@@ -62,6 +62,9 @@ _SIGS = {
     'pidm_linattn_fused_fwd': [P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_fused_bwd': [P, P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_fused_wgrad': [P, P, P, P, P, P, P, P, I, I, L, L, P],
+    'pidm_linattn_block_fwd': [P, P, P, P, P, P, P, P, P, P, I, I, P],
+    'pidm_linattn_block_bwd': [P, P, P, P, P, P, P, P, P, I, I, P],
+    'pidm_linattn_block_wgrad': [P, P, P, P, P, P, P, P, P, L, L, P, L, L, I, I, P],
     'pidm_linattn_fwd': [P, P, P, P, P, P, I, I, I, I, P],
     'pidm_linattn_bwd': [P, P, P, P, P, P, P, I, I, I, I, P],
     'pidm_attn_fwd': [P, P, I, I, I, I, P],

@@ -500,6 +500,58 @@ class _LinAttnFused(torch.autograd.Function):
         return (dx if ctx.needs_input_grad[0] else None), gw_ret, None, None
 
 
+class _LinAttnBlock(torch.autograd.Function):
+    """The whole linear-attention block at the 32-channel levels: y = residual + to_out(attention(to_qkv(xn))) with a 1x1
+    256 -> C to_out (with bias).  The [B, N, 256] attention output and its gradient are never written: forward projects
+    each head's output tile on chip, backward recomputes it and dout per head from dy.  Like the to_out convolution it
+    replaces, it hands dy back as the residual's gradient."""
+
+    @staticmethod
+    def forward(ctx, xn, w_qkv, spec_qkv, w_out, b_out, spec_out, residual, heads):
+        B, H, W, C = xn.shape
+        N = H * W
+        y = torch.empty_like(residual)
+        ctxm = torch.empty(B, heads, 32, 32, device=xn.device, dtype=torch.float32)
+        kmax = torch.empty(B, heads, 32, device=xn.device, dtype=torch.float32)
+        kzinv = torch.empty_like(kmax)
+        ws = torch.empty(call('pidm_linattn_fused_workspace_floats', B, N), device=xn.device, dtype=torch.float32)
+        call('pidm_linattn_block_fwd', xn, spec_qkv.wp_fwd, spec_out.wp_fwd, b_out, residual, y, ctxm, kmax, kzinv, ws,
+             B, N, stream())
+        ctx.save_for_backward(xn, w_qkv, w_out, b_out, ctxm, kmax, kzinv)
+        ctx.specs = (spec_qkv, spec_out)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xn, w_qkv, w_out, b_out, ctxm, kmax, kzinv = ctx.saved_tensors
+        sq, so = ctx.specs
+        B, H, W, _ = xn.shape
+        N = H * W
+        dy = dy.contiguous()
+        dx = torch.empty_like(xn)
+        dctx = torch.empty_like(ctxm)
+        call('pidm_linattn_block_bwd', xn, sq.wp_fwd, so.wp_fwd, dy, ctxm, kmax, kzinv, dx, dctx, B, N, stream())
+        gq_buf, gq_ret = _grad_buffer(w_qkv)
+        go_buf, go_ret = _grad_buffer(w_out)
+        gb_buf, gb_ret = _grad_buffer(b_out)
+        ws = _wgrad_stream(xn, sq.wp_fwd, so.wp_fwd, dy, ctxm, dctx, kmax, kzinv)
+        call('pidm_linattn_block_wgrad', xn, sq.wp_fwd, so.wp_fwd, dy, ctxm, dctx, kmax, kzinv, gq_buf, sq.w_stride_n,
+             sq.w_stride_c, go_buf, so.w_stride_n, so.w_stride_c, B, N, ws)
+        call('pidm_colsum', dy, gb_buf, B * N, dy.shape[-1], _code(dy), ws)
+        return (dx if ctx.needs_input_grad[0] else None), gq_ret, None, go_ret, gb_ret, None, dy, None
+
+
+def linear_attention_block_supported(xn, spec_qkv, spec_out, b_out, heads):
+    return (b_out is not None and spec_out.kh == 1 and spec_out.kw == 1 and not spec_out.transposed
+            and spec_out.cin == heads * 32 and spec_out.cout == xn.shape[-1]
+            and linear_attention_fused_supported(xn, spec_qkv, heads))
+
+
+def linear_attention_block(xn, w_qkv, spec_qkv, w_out, b_out, spec_out, residual, heads):
+    """y = residual + to_out(linear_attention(to_qkv(xn))); to_qkv 1x1 without bias, to_out 1x1 256 -> C with bias."""
+    return _LinAttnBlock.apply(xn.contiguous(), w_qkv, spec_qkv, w_out, b_out, spec_out, residual.contiguous(), heads)
+
+
 def linear_attention_fused_supported(xn, spec, heads):
     B, H, W, C = xn.shape
     return (_STATE['use_tc'] and xn.is_cuda and spec.kh == 1 and spec.kw == 1 and spec.cout == 3 * heads * 32

@@ -316,6 +316,13 @@ class Unet3D(nn.Module):
         xn = ops.layernorm_c(x, pre.norm.gamma, pre.norm.eps, skip_link=sk)
         to_qkv = pre.fn.to_qkv
         spec = self._spec[id(to_qkv)]
+        to_out = pre.fn.to_out
+        b_out = getattr(to_out, 'bias', None)
+        if (getattr(to_qkv, 'bias', None) is None
+                and ops.linear_attention_block_supported(xn, spec, self._spec[id(to_out)], b_out, pre.fn.heads)):
+            # to_qkv, the attention, to_out and the `+ x`: the [B, N, 256] attention output is never materialised
+            return ops.linear_attention_block(xn, to_qkv.weight, spec, to_out.weight, b_out, self._spec[id(to_out)],
+                                              ops.stash_grad(x, sk), pre.fn.heads)
         if getattr(to_qkv, 'bias', None) is None and ops.linear_attention_fused_supported(xn, spec, pre.fn.heads):
             a = ops.linear_attention_fused(xn, to_qkv.weight, spec, pre.fn.heads)   # qkv never materialised
         else:
