@@ -100,6 +100,11 @@ int pidm_gelu_bwd(const void* x, const void* dy, void* dx, long long n, int dtyp
 /* torch.cat((x, skip), dim=1) on NHWC rows and its backward (src/unet_model.py:606,612) */
 int pidm_concat_channels(const void* a, const void* b, void* out, long long rows, int Ca, int Cb, int dtype, void* stream);
 int pidm_split_channels(const void* g, void* ga, void* gb, long long rows, int Ca, int Cb, int dtype, void* stream);
+/* circular padding (Unet3D(padding_mode='circular'), src/unet_model.py:161-199): y [B, H+2h, W+2h, C] is x [B,H,W,C]
+ * with a halo of h = 1..3 pixels wrapped around both spatial axes, y[b,i,j] = x[b, (i-h) mod H, (j-h) mod W], copied
+ * bit for bit in 16-byte units (C * sizeof(dtype) % 16 == 0, 16-byte aligned pointers).  A circular convolution is the
+ * valid (pad 0) convolution of this copy; see pidm_conv2d_tc_general for the transposed gather. */
+int pidm_wrap_pad_nhwc(const void* x, void* y, int B, int H, int W, int C, int halo, int dtype, void* stream);
 
 /* ---- convolutions as implicit GEMM (src/unet_model.py:163,197,227,253,275,279,453,517) ------------------- */
 /* Packed weights: Wp[n][tap*Cin + c] in the activation dtype, built by pidm_pack_weights from the framework
@@ -132,7 +137,9 @@ int pidm_conv2d_wgrad_simt(const void* x, const void* dy, float* dw, float* dbia
 int pidm_debug_set_trace(void* buf);
 /* wgmma + TMA implicit-GEMM convolution, bf16 operands, fp32 register accumulation; same contract as pidm_conv2d_simt
  * (requires Cin % 32 == 0, Cout % 32 == 0): stride-1/2 regular convolution (input sampled through TMA elementStrides) and the
- * stride-2 transposed gather (ConvTranspose forward / dgrad of the stride-2 conv) as 4 output-parity classes.
+ * stride-2 transposed gather (ConvTranspose forward / dgrad of the stride-2 conv) as 4 output-parity classes over the
+ * Ho/2 x Wo/2 grid, Ho = 2(H-1) - 2 pad + KH.  pad = KH/2 - 1 is the zero-padded layer (Ho = 2H); an input with a wrapped
+ * 1-pixel halo (pidm_wrap_pad_nhwc, H = Ho/2 + 2) and pad = KH/2 + 1 is the circular one.
  * gn_sums (optional, [B, gn_groups, 2]): per-(sample, group) sum and sum of squares of the fp32 output, accumulated in
  * the epilogue so that the following GroupNorm needs no statistics pass.  It is zeroed here (one memset node) unless
  * gn_sums_zeroed != 0, i.e. the caller hands in a slice of a buffer it has already cleared. */
@@ -148,7 +155,8 @@ int pidm_conv2d_tc_plan(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, 
 /* wgrad on the tensor cores (wgmma): D[(tap,cA)][cB] = sum over grid pixels g of a[a_stride*g - pad + tap][cA] * b[g][cB], MN-major
  * (pixel-strided) TMA operands, split over pixel ranges, red.global.add into dw[cA*s_row + cB*s_col + tap] (fp32,
  * ACCUMULATED).  Regular conv: a = x, b = dy.  ConvTranspose: a = dy (a_stride 2), b = x.  Rows cA >= CA_real (channel
- * padding) are dropped. */
+ * padding) are dropped.  Circular layers pass the halo'd copy of a (pidm_wrap_pad_nhwc) with pad 0; the 3x3 stride-1
+ * case takes the tap-complete kernel both with (HA = GH, pad 1) and with (HA = GH + 2, pad 0). */
 int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int CA_real, int GH,
                          int GW, int CB, int KH, int KW, int a_stride, int pad, long long s_row, long long s_col,
                          void* stream);

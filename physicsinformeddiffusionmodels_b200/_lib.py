@@ -37,6 +37,7 @@ _SIGS = {
     'pidm_gelu_bwd': [P, P, P, L, I, P],
     'pidm_concat_channels': [P, P, P, L, I, I, I, P],
     'pidm_split_channels': [P, P, P, L, I, I, I, P],
+    'pidm_wrap_pad_nhwc': [P, P, I, I, I, I, I, I, P],
     'pidm_pack_entry_size': [],
     'pidm_pack_weights': [P, I, I, P],
     'pidm_pack_pair_entry_size': [],

@@ -538,8 +538,12 @@ static bool tc_geometry(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, 
         if ((H + 2 * pad - KH) / stride + 1 != Ho || (W + 2 * pad - KW) / stride + 1 != Wo) return false;
         p.mode = 0; p.GH = Ho; p.GW = Wo; p.in_stride = stride; p.out_scale = 1; classes = 1;
     } else {
-        if (stride != 2 || (KH & 1) || Ho != 2 * H || Wo != 2 * W) return false;     // 4x4/s2/p1 style up-sampling
-        p.mode = 1; p.GH = H; p.GW = W; p.in_stride = 1; p.out_scale = 2; classes = 4;
+        // 4x4/s2/p1 style up-sampling: GEMM grid = output / 2 (= the input grid when pad = KH/2 - 1).  An input that
+        // carries a wrapped 1-pixel halo (circular padding) is the same gather with pad + 2: the grid stays the
+        // unpadded one and every class offset dh shifts by +1
+        if (stride != 2 || (KH & 1) || (KW & 1) || (Ho & 1) || (Wo & 1)) return false;
+        if (Ho != 2 * (H - 1) - 2 * pad + KH || Wo != 2 * (W - 1) - 2 * pad + KW) return false;
+        p.mode = 1; p.GH = Ho / 2; p.GW = Wo / 2; p.in_stride = 1; p.out_scale = 2; classes = 4;
         for (int pa = 0; pa < 2; ++pa)
             for (int pb = 0; pb < 2; ++pb) {
                 TcClass& c = p.cls[pa * 2 + pb];

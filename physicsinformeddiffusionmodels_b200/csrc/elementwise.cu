@@ -156,6 +156,28 @@ __global__ void split_kernel(const T* __restrict__ g, T* __restrict__ ga, T* __r
     }
 }
 
+// y[b, oh, ow] = x[b, (oh - halo) mod H, (ow - halo) mod W]: one 16-byte unit of a pixel row per thread iteration, copied
+// as raw bits (dtype-agnostic, exact).  The output is [B, H + 2 halo, W + 2 halo, U * 16 bytes].
+__global__ void wrap_pad_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int H, int W, int halo, int U,
+                                long long total) {
+    pdl_trigger();
+    pdl_wait();
+    const int Hp = H + 2 * halo, Wp = W + 2 * halo;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int u = (int)(i % U);
+        const long long pix = i / U;
+        const int ow = (int)(pix % Wp);
+        const long long r = pix / Wp;
+        const int oh = (int)(r % Hp);
+        const long long b = r / Hp;
+        int ih = oh - halo, iw = ow - halo;
+        ih += ih < 0 ? H : (ih >= H ? -H : 0);
+        iw += iw < 0 ? W : (iw >= W ? -W : 0);
+        y[i] = __ldg(x + ((b * H + ih) * W + iw) * U + u);
+    }
+}
+
 // out = a_b x + b_b y + c_b z with per-sample coefficients (DDIM jump inside ddim_sample_x0, denoising_utils.py:771-785)
 __global__ void axpby_ps_kernel(const float* __restrict__ a, const float4* __restrict__ x, const float* __restrict__ b,
                                 const float4* __restrict__ y, const float* __restrict__ c, const float4* __restrict__ z,
@@ -532,6 +554,23 @@ extern "C" int pidm_split_channels(const void* g, void* ga, void* gb, long long 
     long long total = rows * (Ca + Cb) / 8;
     PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(split_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)g, (T*)ga, (T*)gb, Ca / 8, Cb / 8, rows)));
     PIDM_LAUNCH_CHECK("split");
+    return 0;
+}
+
+extern "C" int pidm_wrap_pad_nhwc(const void* x, void* y, int B, int H, int W, int C, int halo, int dtype,
+                                  void* stream) {
+    PIDM_REQUIRE(dtype == 0 || dtype == 1, "wrap_pad: unknown dtype %d", dtype);
+    const int esize = dtype == 0 ? 4 : 2;
+    PIDM_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && ((long long)C * esize) % 16 == 0,
+                 "wrap_pad: a pixel row must be a whole number of 16-byte units (C=%d)", C);
+    PIDM_REQUIRE(halo >= 1 && halo <= 3 && halo <= H && halo <= W, "wrap_pad: halo must be 1..3 and <= H, W (got %d)",
+                 halo);
+    PIDM_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 15) == 0, "wrap_pad: operands must be 16-byte aligned");
+    const int U = C * esize / 16;
+    const long long total = (long long)B * (H + 2 * halo) * (W + 2 * halo) * U;
+    PIDM_CUDA(launch_pdl(wrap_pad_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
+                         (const uint4*)x, (uint4*)y, H, W, halo, U, total));
+    PIDM_LAUNCH_CHECK("wrap_pad");
     return 0;
 }
 

@@ -239,7 +239,7 @@ static int wg_launch(const CUtensorMap& mx, const CUtensorMap& my, const WgParam
 bool wgrad3_supported(int B, int HA, int WA, int CA, int CA_real, int GH, int GW, int CB, int KH, int KW, int a_stride,
                       int pad, long long s_row);
 void wgrad3_geometry(int B, int GH, int GW, int CA, int CB, int* plan);
-int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB,
+int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB, int pad,
                long long s_col, cudaStream_t st);
 
 static bool wgrad3_enabled() {
@@ -302,7 +302,7 @@ extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int
                                     int GH, int GW, int CB, int KH, int KW, int a_stride, int pad, long long s_row,
                                     long long s_col, void* stream) {
     if (wgrad3_enabled() && wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row))
-        return wgrad3_run(a, b, dw, B, HA, WA, CA, GH, GW, CB, s_col, (cudaStream_t)stream);
+        return wgrad3_run(a, b, dw, B, HA, WA, CA, GH, GW, CB, pad, s_col, (cudaStream_t)stream);
     WgPlan pl;
     WgParams p;
     dim3 grid;

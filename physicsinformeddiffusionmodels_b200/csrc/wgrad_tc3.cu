@@ -208,12 +208,15 @@ static int w3_launch(const CUtensorMap& mx, const CUtensorMap& my, const W3Param
     return 0;
 }
 
-// Is this call covered?  a = x [B,HA,WA,CA], b = dy [B,GH,GW,CB], stride 1, 3x3, "same" padding, framework layout
-// dw[cB][cA][tap] (s_row == 9), no channel padding.
+// Is this call covered?  a = x [B,HA,WA,CA], b = dy [B,GH,GW,CB], stride 1, 3x3, framework layout dw[cB][cA][tap]
+// (s_row == 9), no channel padding.  a is either the unpadded input ("same" padding, pad 1, TMA zero fill) or a copy
+// that already carries a 1-pixel halo (circular padding: HA = GH + 2, pad 0).
 bool wgrad3_supported(int B, int HA, int WA, int CA, int CA_real, int GH, int GW, int CB, int KH, int KW, int a_stride,
                       int pad, long long s_row) {
-    if (KH != 3 || KW != 3 || a_stride != 1 || pad != 1 || s_row != 9) return false;
-    if (CA % 32 != 0 || CA_real != CA || CB % 32 != 0 || HA != GH || WA != GW) return false;
+    if (KH != 3 || KW != 3 || a_stride != 1 || s_row != 9) return false;
+    const bool same = pad == 1 && HA == GH && WA == GW;
+    const bool halo = pad == 0 && HA == GH + 2 && WA == GW + 2;
+    if (CA % 32 != 0 || CA_real != CA || CB % 32 != 0 || !(same || halo)) return false;
     if (GW % 8 == 0 && GH % 16 == 0) return true;                       // RG
     if (GW > 64 || 64 % GW != 0) return false;
     const int th = 64 / GW;
@@ -225,7 +228,7 @@ bool wgrad3_supported(int B, int HA, int WA, int CA, int CA_real, int GH, int GW
 // tile plan and launch grid of a supported call
 static void w3_geometry(int B, int GH, int GW, int CA, int CB, W3Params& p, bool& rg, int& NP, int& AB, dim3& grid) {
     rg = (GW % 8 == 0 && GH % 16 == 0);
-    p.B = B; p.pad = 1;
+    p.B = B;
     if (rg) { p.TW = 8; p.TH = 16; p.TN = 1; }
     else {
         p.TW = GW;
@@ -256,7 +259,7 @@ void wgrad3_geometry(int B, int GH, int GW, int CA, int CB, int* plan) {
     for (int i = 0; i < 11; ++i) plan[i] = v[i];
 }
 
-int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB,
+int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB, int pad,
                long long s_col, cudaStream_t st) {
     static thread_local bool ctx_bound = false;
     if (!ctx_bound) {
@@ -268,6 +271,7 @@ int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, i
     int NP, AB;
     dim3 grid;
     w3_geometry(B, GH, GW, CA, CB, p, rg, NP, AB, grid);
+    p.pad = pad;
     p.dw = dw; p.s_col = s_col;
     CUtensorMap mx, my;
     if (int e = w3_encode(&mx, a, B, HA, WA, CA, 32, p.TW, rg ? p.TH + 3 : p.TH, p.TN)) return e;

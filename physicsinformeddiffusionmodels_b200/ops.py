@@ -225,6 +225,28 @@ def _conv_launch(x, wp, bias, residual, y, g, transposed, gn_sums=None, gn_group
         return False
 
 
+def wrap_pad(x, halo):
+    """[B,H,W,C] -> [B,H+2h,W+2h,C] with the halo wrapped around both spatial axes (circular padding)."""
+    B, H, W, C = x.shape
+    y = torch.empty(B, H + 2 * halo, W + 2 * halo, C, device=x.device, dtype=x.dtype)
+    call('pidm_wrap_pad_nhwc', x, y, B, H, W, C, halo, _code(x), stream())
+    return y
+
+
+def _halo_geometry(g, halo, transposed):
+    """geometry g = (B,H,W,Cin,Ho,Wo,Cout,KH,KW,stride,pad) of a circular layer restated over its input with a wrapped
+    halo: a valid (pad 0) convolution, or for the transposed gather (halo 1) every tap one pixel further in (pad + 2)"""
+    B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad = g
+    return (B, H + 2 * halo, W + 2 * halo, Cin, Ho, Wo, Cout, KH, KW, stride, pad + 2 if transposed else 0)
+
+
+def _convT_wgrad_tc(dtype, g):
+    """does the weight gradient of a transposed layer with forward geometry g run on the tensor cores?"""
+    B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad = g
+    return (_STATE['use_tc'] and dtype == torch.bfloat16
+            and call('pidm_conv2d_wgrad_tc_supported', B, H, W, Cout, Cin, KH, KW, stride) == 1)
+
+
 class _Conv2d(torch.autograd.Function):
     """`link` (optional dict) couples this convolution to the GroupNorm that consumes its output: forward leaves the
     fused statistics in link['sums']; the GroupNorm backward leaves this conv's bias gradient in link['dbias']."""
@@ -237,18 +259,27 @@ class _Conv2d(torch.autograd.Function):
         Ho, Wo = spec.out_hw(H, W)
         y = torch.empty(B, Ho, Wo, spec.cout, device=x.device, dtype=x.dtype)
         g = (B, H, W, Cin, Ho, Wo, spec.cout, spec.kh, spec.kw, spec.stride, spec.pad)
+        xin, gin = x, g
+        if spec.circular:
+            xin, gin = wrap_pad(x, spec.halo), _halo_geometry(g, spec.halo, spec.transposed)
         sums, zeroed = None, False
         if link is not None:
             sums = _zero_take(B, link['groups'], 2)
             zeroed = sums is not None
             if sums is None:
                 sums = torch.empty(B, link['groups'], 2, device=x.device, dtype=torch.float32)
-        fused = _conv_launch(x, spec.wp_fwd, bias, residual, y, g, spec.transposed, sums, link['groups'] if link else 0,
-                             zeroed)
+        fused = _conv_launch(xin, spec.wp_fwd, bias, residual, y, gin, spec.transposed, sums,
+                             link['groups'] if link else 0, zeroed)
         if link is not None:
             link['sums'] = sums if fused else None
             link['bias'] = bias
-        ctx.save_for_backward(x, weight, bias)
+        # a circular conv keeps the halo'd copy: its weight gradient reads it as the forward did and backward never pads
+        # x again.  Exception: the tensor-core weight gradient of the transposed layer gathers from dy and reads x on
+        # its own (unpadded) grid.
+        keep = xin
+        if spec.transposed and (not spec.circular or _convT_wgrad_tc(x.dtype, g)):
+            keep = x
+        ctx.save_for_backward(keep, weight, bias)
         ctx.spec, ctx.g, ctx.has_res, ctx.link, ctx.skip = spec, g, residual is not None, link, skip
         if skip is not None and skip[0] == 'park':
             skip[1]['expect_skip'] = True
@@ -321,39 +352,62 @@ def _conv_backward(x, weight, bias, spec, g, dy, need_dx, link=None, dgrad_resid
     dgrad_residual (same shape as x) is added to dx in the dgrad epilogue."""
     B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad = g
     dx = None
-    if need_dx or dgrad_residual is not None:
-        dx = torch.empty_like(x)
+    # circular layer: x is the halo'd input copy (regular conv) and dy gets its own wrapped halo for the dgrad (and for
+    # the transposed layer's weight gradient, which gathers from dy)
+    need_dgrad = need_dx or dgrad_residual is not None
+    dyh = wrap_pad(dy, spec.dgrad_halo) if spec.circular and (need_dgrad or spec.transposed) else None
+    if need_dgrad:
+        dx = torch.empty(B, H, W, Cin, device=x.device, dtype=x.dtype)
         # dgrad: roles of input/output swap; regular conv -> transposed gather and vice versa.
         # For stride 1 the transposed gather equals a regular conv with the flipped kernel, which the
         # dgrad packing already encodes (pad' = K-1-pad), so the tensor-core kernel can take it.
         if stride == 1 and not spec.transposed:
             gd = (B, Ho, Wo, Cout, H, W, Cin, KH, KW, 1, KH - 1 - pad)
-            _conv_launch(dy, spec.wp_dgrad, None, dgrad_residual, dx, gd, False)
         else:
             gd = (B, Ho, Wo, Cout, H, W, Cin, KH, KW, stride, pad)
-            _conv_launch(dy, spec.wp_dgrad, None, dgrad_residual, dx, gd, not spec.transposed)
+        tr_d = not spec.transposed and stride != 1
+        dy_d = dy
+        if dyh is not None:
+            dy_d, gd = dyh, _halo_geometry(gd, spec.dgrad_halo, tr_d)
+        _conv_launch(dy_d, spec.wp_dgrad, None, dgrad_residual, dx, gd, tr_d)
     gw_buf, gw_ret = _grad_buffer(weight)
     gb_buf, gb_ret = (None, None) if bias is None else _grad_buffer(bias)
     if link is not None and 'dbias' in link:
         # the consuming GroupNorm's backward already reduced dy over pixels (= this conv's bias gradient)
         gb_buf, gb_ret = None, link.pop('dbias')
     use_tc = _STATE['use_tc'] and x.dtype == torch.bfloat16
-    ws = _wgrad_stream(x, dy)
-    if use_tc and not spec.transposed and call('pidm_conv2d_wgrad_tc_supported', B, Ho, Wo, Cin, Cout, KH, KW, stride):
+    tc_conv = (use_tc and not spec.transposed
+               and call('pidm_conv2d_wgrad_tc_supported', B, Ho, Wo, Cin, Cout, KH, KW, stride))
+    # the forward of a circular layer saved either its halo'd input (read as the forward read it) or, for the
+    # tensor-core weight gradient of the transposed layer, x itself
+    x_halo = spec.circular and x.shape[1] != H
+    if spec.circular and spec.transposed:
+        tc_convT = not x_halo
+    else:
+        tc_convT = spec.transposed and use_tc and call('pidm_conv2d_wgrad_tc_supported', B, H, W, Cout, Cin, KH, KW,
+                                                       stride)
+    # gathered operands as the kernels read them: (tensor, H, W, pad)
+    xa, dya = (x, H, W, pad), (dy, Ho, Wo, pad)
+    if x_halo:
+        xa = (x, x.shape[1], x.shape[2], pad + 2 if spec.transposed else 0)
+    elif spec.circular:
+        dya = (dyh, Ho + 2, Wo + 2, 0)
+    ws = _wgrad_stream(xa[0], dy, dya[0])
+    if tc_conv:
         # D[(tap, ci)][co]: gathered operand = x, reduction grid = output pixels
-        call('pidm_conv2d_wgrad_tc', x, dy, gw_buf, B, H, W, Cin, spec.cin_real, Ho, Wo, Cout, KH, KW, stride, pad,
-             spec.w_stride_c, spec.w_stride_n, ws)
+        call('pidm_conv2d_wgrad_tc', xa[0], dy, gw_buf, B, xa[1], xa[2], Cin, spec.cin_real, Ho, Wo, Cout, KH, KW,
+             stride, xa[3], spec.w_stride_c, spec.w_stride_n, ws)
         if gb_buf is not None:
             call('pidm_colsum', dy, gb_buf, B * Ho * Wo, Cout, _code(dy), ws)
-    elif use_tc and spec.transposed and call('pidm_conv2d_wgrad_tc_supported', B, H, W, Cout, Cin, KH, KW, stride):
+    elif tc_convT:
         # ConvTranspose: D[(tap, co)][ci]: gathered operand = dy (sampled with the stride), grid = input pixels
-        call('pidm_conv2d_wgrad_tc', dy, x, gw_buf, B, Ho, Wo, Cout, Cout, H, W, Cin, KH, KW, stride, pad,
-             spec.w_stride_n, spec.w_stride_c, ws)
+        call('pidm_conv2d_wgrad_tc', dya[0], x, gw_buf, B, dya[1], dya[2], Cout, Cout, H, W, Cin, KH, KW, stride,
+             dya[3], spec.w_stride_n, spec.w_stride_c, ws)
         if gb_buf is not None:
             call('pidm_colsum', dy, gb_buf, B * Ho * Wo, Cout, _code(dy), ws)
     else:
-        call('pidm_conv2d_wgrad_simt', x, dy, gw_buf, gb_buf, B, H, W, Cin, spec.cin_real, Ho, Wo, Cout, KH, KW,
-             stride, pad, 1 if spec.transposed else 0, spec.w_stride_n, spec.w_stride_c, _code(x), ws)
+        call('pidm_conv2d_wgrad_simt', xa[0], dy, gw_buf, gb_buf, B, xa[1], xa[2], Cin, spec.cin_real, Ho, Wo, Cout,
+             KH, KW, stride, xa[3], 1 if spec.transposed else 0, spec.w_stride_n, spec.w_stride_c, _code(x), ws)
     return dx, gw_ret, gb_ret
 
 

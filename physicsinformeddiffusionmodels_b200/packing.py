@@ -32,14 +32,26 @@ class ConvSpec:
 
     kind 'conv'  : weight [Cout, Cin, (1,) kh, kw]   (nn.Conv3d/Conv2d/Linear layout)
     kind 'convT' : weight [Cin, Cout, (1,) kh, kw]   (nn.ConvTranspose3d layout), forward = transposed gather
+
+    circular=True: the layer pads periodically (padding_mode='circular').  It then runs on a copy of its input with a
+    wrapped halo of `halo` pixels: a valid convolution for 'conv', the transposed gather with pad + 2 for 'convT'.
+    `dgrad_halo` is the halo its input gradient needs on dy.  A layer without padding is never circular.
     """
 
-    def __init__(self, weight, kind, kh, kw, stride, pad, cin_pad=None, need_dgrad=True):
+    def __init__(self, weight, kind, kh, kw, stride, pad, cin_pad=None, need_dgrad=True, circular=False):
         self.weight = weight
         self.kind = kind
         self.kh, self.kw, self.stride, self.pad = kh, kw, stride, pad
         self.taps = kh * kw
         self.transposed = kind == 'convT'
+        self.circular = bool(circular) and pad > 0
+        self.halo = self.dgrad_halo = 0
+        if self.circular:
+            if kh != kw or not ((stride == 1 and kh == 2 * pad + 1) or (stride == 2 and kh == 2 * pad + 2)):
+                raise ValueError(f'circular padding needs a "same" stride-1 or a k = 2 pad + 2 stride-2 layer '
+                                 f'(got {kh}x{kw}, stride {stride}, pad {pad})')
+            self.halo = 1 if self.transposed else pad
+            self.dgrad_halo = pad if stride == 1 else 1
         if kind == 'conv':
             self.cout, self.cin_real = weight.shape[0], weight.shape[1]
             self.w_stride_n, self.w_stride_c = self.cin_real * self.taps, self.taps

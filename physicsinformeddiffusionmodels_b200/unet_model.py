@@ -119,6 +119,21 @@ class ResnetBlock(nn.Module):
         self.groups = groups
 
 
+class CircularUpsample(nn.Module):
+    """Holder for the circular up-sampling layer (unet_model.py:161-194): the reference pads by 2 circularly and runs a
+    ConvTranspose3d with padding 5; its state_dict keys are `conv_transpose.weight|bias`.  The engine runs it as the
+    periodic 4x4/stride-2 transposed convolution over a 1-pixel wrapped halo (ops._halo_geometry)."""
+
+    def __init__(self, in_channels, out_channels):
+        super().__init__()
+        self.conv_transpose = nn.ConvTranspose3d(in_channels, out_channels, (1, 4, 4), (1, 2, 2), padding=(0, 5, 5))
+
+
+def _up_conv(up):
+    """the ConvTranspose3d that holds an up-sampling layer's parameters"""
+    return up.conv_transpose if isinstance(up, CircularUpsample) else up
+
+
 class SignalEmbedding(nn.Module):
     """Holder for sign_emb_CNN (unet_model.py:370-404, only used by an ablation that forward never reaches)."""
 
@@ -137,8 +152,8 @@ class Unet3D(nn.Module):
                  cond_bias=False, cond_attention='none', cond_attention_tokens=6, cond_to_time='add',
                  padding_mode='zeros', sigmoid_last_channel=False):
         super().__init__()
-        if padding_mode != 'zeros':
-            raise NotImplementedError("only padding_mode='zeros' (the reference default) is implemented")
+        if padding_mode not in ('zeros', 'circular'):
+            raise ValueError('Unknown padding mode: {}'.format(padding_mode))
         if not use_sparse_linear_attn:
             raise NotImplementedError('use_sparse_linear_attn=False is not used by the reference drivers')
         if attn_dim_head != 32:
@@ -193,11 +208,14 @@ class Unet3D(nn.Module):
         self.mid_spatial_attn = Residual(PreNorm(mid, spatial_attn))
         self.mid_temporal_attn = Residual(PreNorm(mid, temporal_attn(mid)))
         self.mid_block2 = rb(mid, mid)
+        def upsample(d):
+            if padding_mode == 'circular':
+                return CircularUpsample(d, d)
+            return nn.ConvTranspose3d(d, d, (1, 4, 4), (1, 2, 2), (0, 1, 1))
         for ind, (di, do) in enumerate(reversed(in_out)):
             is_last = ind >= (n_res - 1)
             self.ups.append(nn.ModuleList([
-                rb(do * 2, di), rb(di, di), lin_attn(di),
-                nn.ConvTranspose3d(di, di, (1, 4, 4), (1, 2, 2), (0, 1, 1)) if not is_last else nn.Identity()]))
+                rb(do * 2, di), rb(di, di), lin_attn(di), upsample(di) if not is_last else nn.Identity()]))
         out_dim = default(out_dim, channels)
         self.out_dim = out_dim
         self.final_conv = nn.Sequential(rb(dim * 2, dim, time=False), nn.Conv3d(dim, out_dim, 1))
@@ -218,8 +236,13 @@ class Unet3D(nn.Module):
         k = self.init_kernel_size
         self._spec = {}
 
-        def conv(mod, kh, stride, pad, kind='conv', cin_pad=None, need_dgrad=True):
-            s = pk.add(ConvSpec(mod.weight, kind, kh, kh, stride, pad, cin_pad=cin_pad, need_dgrad=need_dgrad))
+        # padding_mode='circular' reaches every padded spatial convolution except emb_conv[2], which the reference
+        # hard-codes to zero padding (unet_model.py:524)
+        circ = self.padding_mode == 'circular'
+
+        def conv(mod, kh, stride, pad, kind='conv', cin_pad=None, need_dgrad=True, circular=circ):
+            s = pk.add(ConvSpec(mod.weight, kind, kh, kh, stride, pad, cin_pad=cin_pad, need_dgrad=need_dgrad,
+                                circular=circular))
             self._spec[id(mod)] = s
             return s
         conv(self.init_conv, k, 1, k // 2, cin_pad=self._cin_pad, need_dgrad=False)
@@ -252,11 +275,11 @@ class Unet3D(nn.Module):
         for b1, b2, la, up in self.ups:
             plan_rb(b1); plan_rb(b2); plan_la(la)
             if not isinstance(up, nn.Identity):
-                conv(up, 4, 2, 1, kind='convT')
+                conv(_up_conv(up), 4, 2, 1, kind='convT')
         plan_rb(self.final_conv[0])
         # residual-gradient guidance branch (only executed when forward() is given cond=..., reference :585-603)
         conv(self.emb_conv[0], 1, 1, 0, cin_pad=self._cin_pad, need_dgrad=False)
-        conv(self.emb_conv[2], 3, 1, 1)
+        conv(self.emb_conv[2], 3, 1, 1, circular=False)
         conv(self.combine_conv, 1, 1, 0)
         self._mlp_table = MlpTable(mlps)
 
@@ -447,7 +470,7 @@ class Unet3D(nn.Module):
             h = self._resblock(b2, h, ss)
             h = self._linear_attention(la, h)
             if not isinstance(up, nn.Identity):
-                h = self._conv(up, h)
+                h = self._conv(_up_conv(up), h)
         h = ops.concat(h, r)
         h = self._resblock(self.final_conv[0], h, None)
         fc = self.final_conv[1]
