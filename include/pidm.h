@@ -191,34 +191,26 @@ int pidm_layernorm_c_bwd(const void* x, const void* dy, const float* gamma, void
 /* ---- attention ------------------------------------------------------------------------------------------ */
 /* SpatialLinearAttention core between to_qkv and to_out (src/unet_model.py:286-297), dim_head = 32.
  * qkv [B,N,3*heads*32]; out [B,N,heads*32]; ctx [B,heads,32,32], kmax/kzinv [B,heads,32] kept for backward. */
-/* Linear attention fused with its to_qkv 1x1 projection (C = 32 input channels, 8 heads, bf16): q, k, v are recomputed
- * per head on the tensor cores from xn = PreNorm(x) instead of being materialised (reference unet_model.py:275-297 --
- * `qkv = self.to_qkv(x)` and everything after it).  w_qkv = packed to_qkv weights [768][32] bf16 (pidm_pack_weights).
- * Forward keeps ctx / kmax / kzinv for backward.  Backward writes dxn [B,N,32] bf16 (gradient w.r.t. xn through
- * qkv = xn W^T) and fills dctx [B,8,32,32]; the weight-gradient pass then reads dctx and ACCUMULATES the to_qkv weight
- * gradient into grad_w (fp32, element [n][c] at n * w_stride_n + c * w_stride_c).  Neither materialises dqkv. */
-int pidm_linattn_fused_supported(int C, int heads, int N, int dtype);
-int pidm_linattn_fused_workspace_floats(int B, int N);
-/* pixel chunking of the fused kernels (test aid): out[5] = {statistics chunks, ctx / out / bwd / wgrad pixels per CTA} */
-int pidm_linattn_fused_plan(int B, int N, int* out);
-int pidm_linattn_fused_fwd(const void* xn, const void* w_qkv, void* out, float* ctx, float* kmax, float* kzinv,
-                           float* workspace, int B, int N, void* stream);
-int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const void* dout, const float* ctx, const float* kmax,
-                           const float* kzinv, void* dxn, float* dctx, int B, int N, void* stream);
-int pidm_linattn_fused_wgrad(const void* xn, const void* w_qkv, const void* dout, const float* ctx, const float* dctx,
-                             const float* kmax, const float* kzinv, float* grad_w, int B, int N, long long w_stride_n,
-                             long long w_stride_c, void* stream);
-/* The whole linear-attention block at the 32-channel levels: y = residual + b_out + to_out(attention(to_qkv(xn))), with
- * to_out a 1x1 256 -> 32 projection (reference unet_model.py:275-297 and the Residual wrapper's `+ x`).  Neither the
- * attention output nor its gradient [B,N,256] is materialised: forward multiplies each head's output tile by its 32
- * columns of W_out on chip, backward recomputes dout_h = dy W_out[:, 32h:32h+32] per head from dy.
- *   xn, residual, y, dy, dxn: [B,N,32] bf16.  w_qkv: packed to_qkv weights [768][32] bf16.  w_out: packed forward to_out
- *   weights [32][256] bf16 (pidm_pack_weights, row = output channel).  b_out: [32] fp32.
- *   fwd: y is WRITTEN; ctx / kmax / kzinv / workspace as pidm_linattn_fused_fwd.
- *   bwd: dxn is WRITTEN (the gradient through to_qkv only: the residual's gradient is dy itself); dctx is filled.
+/* The whole linear-attention block at the 32-channel levels (C = 32, 8 heads, bf16):
+ * y = residual + b_out + to_out(attention(to_qkv(xn))), with to_qkv a 1x1 32 -> 768 projection without bias and to_out
+ * a 1x1 256 -> 32 projection (reference unet_model.py:275-297 and the Residual wrapper's `+ x`).  q, k, v are recomputed
+ * per head on the tensor cores from xn = PreNorm(x), and neither the attention output nor its gradient [B,N,256] is
+ * materialised: forward multiplies each head's output tile by its 32 columns of W_out on chip, backward recomputes
+ * dout_h = dy W_out[:, 32h:32h+32] per head from dy.  Neither qkv nor dqkv [B,N,768] is materialised either.
+ *   xn, residual, y, dy, dxn: [B,N,32] bf16.  w_qkv: packed to_qkv weights [768][32] bf16 (pidm_pack_weights).
+ *   w_out: packed forward to_out weights [32][256] bf16 (pidm_pack_weights, row = output channel).  b_out: [32] fp32.
+ *   fwd: y is WRITTEN; ctx [B,8,32,32] and kmax / kzinv [B,8,32] are WRITTEN and kept for backward; workspace holds
+ *   pidm_linattn_block_workspace_floats(B, N) floats of scratch.
+ *   bwd: dxn is WRITTEN (the gradient w.r.t. xn through to_qkv only: the residual's gradient is dy itself); dctx
+ *   [B,8,32,32] is WRITTEN and read again by wgrad.
  *   wgrad: ACCUMULATES the to_qkv weight gradient into grad_w_qkv (element [n][c] at n * qkv_stride_n + c * qkv_stride_c)
  *   and the to_out weight gradient into grad_w_out (element [c][j] at c * out_stride_n + j * out_stride_c), both fp32.
  *   The bias gradient (column sums of dy) is left to pidm_colsum. */
+int pidm_linattn_block_supported(int C, int heads, int N, int dtype);
+int pidm_linattn_block_workspace_floats(int B, int N);
+/* pixel chunking of the block's launches (test aid): out[5] = {statistics chunks, ctx / fwd / bwd / wgrad pixels per
+ * CTA} */
+int pidm_linattn_block_plan(int B, int N, int* out);
 int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const void* w_out, const float* b_out, const void* residual,
                            void* y, float* ctx, float* kmax, float* kzinv, float* workspace, int B, int N, void* stream);
 int pidm_linattn_block_bwd(const void* xn, const void* w_qkv, const void* w_out, const void* dy, const float* ctx,

@@ -57,12 +57,9 @@ _SIGS = {
     'pidm_layernorm_c_fwd': [P, P, P, L, I, F, I, P],
     'pidm_layernorm_c_bwd': [P, P, P, P, P, P, L, I, F, I, P],
     'pidm_linattn_workspace_floats': [I, I, I],
-    'pidm_linattn_fused_supported': [I, I, I, I],
-    'pidm_linattn_fused_workspace_floats': [I, I],
-    'pidm_linattn_fused_plan': [I, I, P],
-    'pidm_linattn_fused_fwd': [P, P, P, P, P, P, P, I, I, P],
-    'pidm_linattn_fused_bwd': [P, P, P, P, P, P, P, P, I, I, P],
-    'pidm_linattn_fused_wgrad': [P, P, P, P, P, P, P, P, I, I, L, L, P],
+    'pidm_linattn_block_supported': [I, I, I, I],
+    'pidm_linattn_block_workspace_floats': [I, I],
+    'pidm_linattn_block_plan': [I, I, P],
     'pidm_linattn_block_fwd': [P, P, P, P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_block_bwd': [P, P, P, P, P, P, P, P, P, I, I, P],
     'pidm_linattn_block_wgrad': [P, P, P, P, P, P, P, P, P, L, L, P, L, L, I, I, P],
@@ -88,9 +85,9 @@ _SIGS = {
 }
 # functions whose int return value is a result, not an error code
 _VALUE_RETURN = {'pidm_pack_entry_size', 'pidm_pack_pair_entry_size', 'pidm_mlp_entry_size', 'pidm_linattn_workspace_floats', 'pidm_version',
-                 'pidm_linattn_fused_supported', 'pidm_linattn_fused_workspace_floats',
+                 'pidm_linattn_block_supported', 'pidm_linattn_block_workspace_floats',
                  'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported',
-                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_fused_plan'}
+                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_block_plan'}
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(f'{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). '

@@ -1,16 +1,19 @@
-// Linear attention FUSED with its to_qkv 1x1 projection, for the full-resolution level of the U-Net (C = 32 input
-// channels, 8 heads x 32; reference unet_model.py:275-297).
+// The whole linear-attention block at the full-resolution levels of the U-Net (C = 32 channels, 8 heads x 32;
+// reference unet_model.py:275-297 and the Residual wrapper's `+ x`):
+//   y = x + b_out + to_out(attention(to_qkv(xn))),  to_qkv 1x1 32 -> 768 without bias, to_out 1x1 256 -> 32 with bias.
 //
-// At 64x64 the qkv tensor is 24x larger than the tensor it is projected from (768 vs 32 channels): writing it and
-// streaming it back through the statistics / context / output / backward kernels was ~1.2 GB of HBM traffic per layer.
-// Here every warp (one head) recomputes its q / k / v slices on the tensor cores from the 64-byte pixel rows of the
-// normalised input xn -- a 32x32x32 mma.sync product per 32 pixels -- so that forward reads xn (8 MB) and writes
-// `out` only.  Backward recomputes them the same way in two passes over (xn, dout): one multiplies dq | dk | dv by W
-// and writes dxn (8 MB), the other multiplies them by xn into the to_qkv weight gradient; the [B, N, 768] dqkv is
-// never written either.
+// At 64x64 the qkv tensor is 24x larger than the tensor it is projected from (768 vs 32 channels) and the attention
+// output 8x (256): writing them and streaming them back through the statistics / context / output / backward kernels
+// was ~1.2 GB of HBM traffic per layer.  Here every warp (one head) recomputes its q / k / v slices on the tensor cores
+// from the 64-byte pixel rows of the normalised input xn -- a 32x32x32 mma.sync product per 32 pixels -- and multiplies
+// its output tile by its 32 columns of W_out on chip, so that forward reads xn and x and writes y only.  Backward
+// recomputes dout_h = dy W_out[:, 32h:32h+32] per head from the 32-channel dy, in two passes over (xn, dy): one
+// multiplies dq | dk | dv by W and writes dxn, the other multiplies them by xn into the to_qkv weight gradient and
+// accumulates the to_out weight gradient; neither the [B, N, 768] dqkv nor the [B, N, 256] dout is written.
 // All intermediate tiles stay in registers: accumulator fragments are converted to A fragments directly and to
-// transposed (K-major) fragments with movmatrix; only xn / dout tiles and the output staging touch shared memory.
-// The two paths differ only by the bf16 rounding of the (here never materialised) q, k, v.
+// transposed (K-major) fragments with movmatrix; only xn / dy tiles, the W_out slices and the cross-head partial sums
+// touch shared memory.  The unfused path differs by the bf16 rounding of the q, k, v and attention output it
+// materialises.
 #define PIDM_PDL_GROUP 1
 #include "common.cuh"
 #include "mma_util.cuh"
@@ -166,10 +169,10 @@ __global__ void laf_finalize_kernel(float* __restrict__ ctx, float* __restrict__
     if (lane == 0) kzinv[row] = zi;
 }
 
-// ---- to_out projection (PROJ): the block output y = x + b + sum_h out_h W_out[:, 32h:32h+32]^T --------------------------
-// With PROJ the kernels below never see `out` or `dout` [B, N, 256]: the forward multiplies each head's out tile by its
-// 32-column slice of W_out and sums the eight partials, and backward recomputes dout_h = dy W_out[:, 32h:32h+32] from
-// the 32-channel dy tile.  Every warp keeps its slice Wo_h[c][e] = W_out[c][32h + e] (packed forward to_out weights
+// ---- to_out projection: the block output y = x + b + sum_h out_h W_out[:, 32h:32h+32]^T -------------------------------
+// The kernels below never see `out` or `dout` [B, N, 256]: the forward multiplies each head's out tile by its 32-column
+// slice of W_out and sums the eight partials, and backward recomputes dout_h = dy W_out[:, 32h:32h+32] from the
+// 32-channel dy tile.  Every warp keeps its slice Wo_h[c][e] = W_out[c][32h + e] (packed forward to_out weights
 // [32][256]) in shared memory; ldmatrix reads it in both orientations.
 constexpr int LFP_WO_TILE = LF_C * LW_PITCH;                        // one head's W_out slice [32 c][LW_PITCH]
 
@@ -201,22 +204,21 @@ __device__ __forceinline__ void lfp_dout(uint32_t (&ag)[2][4], const __nv_bfloat
 
 // ---- context (MODE 0) / dcontext (MODE 1) --------------------------------------------------------------------------
 //   MODE 0: ctx[h][d][e]  += sum_n exp(k[n,d] - M_d) v[n,e]          k, v projected from xn
-//   MODE 1: dctx[h][d][e] += sum_n softmax_d(q[n,:])[d] s dout[n,e]  q projected from xn, dout streamed (PROJ: dout
-//           recomputed from the streamed dy)
-template <int MODE, bool PROJ = false>
+//   MODE 1: dctx[h][d][e] += sum_n softmax_d(q[n,:])[d] s dout[n,e]  q projected from xn, dout recomputed from the
+//           streamed dy
+template <int MODE>
 struct LfcCfg {
     static constexpr int STAGES = MODE == 0 ? 4 : 2;                       // tiles are consumed into registers at once
-    static constexpr int STAGE_ELEMS = MODE == 0 ? LW_TILE : 2 * LW_TILE;  // xn tile (| dout / dy tile)
-    static constexpr size_t SMEM = (size_t)LM_HEADS * STAGES * STAGE_ELEMS * 2 + (size_t)LM_HEADS * 2 * LM_D * 4 +
-                                   (PROJ ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
+    static constexpr int STAGE_ELEMS = MODE == 0 ? LW_TILE : 2 * LW_TILE;  // xn tile (| dy tile)
+    static constexpr size_t SMEM_BASE = (size_t)LM_HEADS * STAGES * STAGE_ELEMS * 2 + (size_t)LM_HEADS * 2 * LM_D * 4;
+    static constexpr size_t SMEM = SMEM_BASE + (MODE == 1 ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
 };
-template <int MODE, bool PROJ = false>
+template <int MODE>
 __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
-                                                      const __nv_bfloat16* __restrict__ dout, const float* __restrict__ part,
+                                                      const __nv_bfloat16* __restrict__ dy, const float* __restrict__ part,
                                                       int n_stat_chunks, float* __restrict__ kmax, float* __restrict__ kzinv,
                                                       float* __restrict__ ctx, int N, int chunk_px, float scale,
                                                       const __nv_bfloat16* __restrict__ w_out) {
-    static_assert(!PROJ || MODE == 1, "PROJ applies to the dcontext pass");
     pdl_trigger();
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
@@ -225,14 +227,13 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
     __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFC_STAGES * LFC_STAGE_ELEMS);
     float* sM = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFC_STAGES * LFC_STAGE_ELEMS * 2) + h * 2 * LM_D;
     float* sZi = sM + LM_D;
-    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + LfcCfg<MODE>::SMEM) + h * LFP_WO_TILE;   // PROJ only
+    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + LfcCfg<MODE>::SMEM_BASE) + h * LFP_WO_TILE;   // MODE 1
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / 32;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
-    const __nv_bfloat16* gsrc = (MODE == 1) ? (PROJ ? dout + pix0 * LF_C : dout + pix0 * LM_HID + h * LM_D) : nullptr;
-    constexpr int G_STRIDE = PROJ ? LF_C : LM_HID;
-    if (PROJ) {                                    // this head's W_out slice: the oldest copy group
+    const __nv_bfloat16* gsrc = (MODE == 1) ? dy + pix0 * LF_C : nullptr;
+    if (MODE == 1) {                               // this head's W_out slice: the oldest copy group
         lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
         cp_commit();
     }
@@ -240,7 +241,7 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
         if (it < n_tiles) {
             __nv_bfloat16* buf = ring + (size_t)(it % LFC_STAGES) * LFC_STAGE_ELEMS;
             lw_issue<32>(buf, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
-            if (MODE == 1) lw_issue<32>(buf + LW_TILE, gsrc + (size_t)it * 32 * G_STRIDE, G_STRIDE, lane);
+            if (MODE == 1) lw_issue<32>(buf + LW_TILE, gsrc + (size_t)it * 32 * LF_C, LF_C, lane);
         }
         cp_commit();
     };
@@ -276,7 +277,7 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
         uint32_t ax[2][2][4];
         load_x_frags<2>(ax, buf, lane);
         uint32_t bv[2][4][2];                         // B fragments [k = px][n = e] per 16-pixel step
-        if (PROJ) {                                   // accumulator [px][e] -> transposed 8x8 blocks, as v in MODE 0
+        if (MODE == 1) {                              // dout accumulator [px][e] -> transposed 8x8 blocks, as v in MODE 0
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
                 uint32_t ady[2][4];
@@ -289,15 +290,6 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
                     bv[mt][nt][0] = movm_t(pack_bf16(cd[nt][0], cd[nt][1]));
                     bv[mt][nt][1] = movm_t(pack_bf16(cd[nt][2], cd[nt][3]));
                 }
-            }
-        } else if (MODE == 1) {
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                uint32_t b01[4], b23[4];
-                frag_b_krows(b01, buf + LW_TILE, LW_PITCH, ks * 16, 0, lane);
-                frag_b_krows(b23, buf + LW_TILE, LW_PITCH, ks * 16, 16, lane);
-                bv[ks][0][0] = b01[0]; bv[ks][0][1] = b01[1]; bv[ks][1][0] = b01[2]; bv[ks][1][1] = b01[3];
-                bv[ks][2][0] = b23[0]; bv[ks][2][1] = b23[1]; bv[ks][3][0] = b23[2]; bv[ks][3][1] = b23[3];
             }
         }
         __syncwarp();                              // the tile is in registers
@@ -372,47 +364,39 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
         }
 }
 
-// ---- out[n,h,e] = sum_d softmax_d(q[n,:])[d] * s * ctx[h][d][e],  q projected from xn --------------------------------
-// PROJ: out is y [B, N, 32] = x + b + sum_h out_h Wo_h^T.  The warps then share one xn ring (three stages) and step
-// through the tiles together; each leaves its fp32 [32 px][32] partial in shared memory, and after a CTA barrier every
-// thread sums two columns of two rows over the eight heads, adds the bias and the residual and writes y once.
-constexpr int LFO_STAGES = 2;      // 61 KB per CTA: three CTAs (24 warps) per SM
-constexpr int LFOP_STAGES = 3;     // PROJ: 68 KB per CTA; 110 registers: two CTAs per SM
+// ---- y = x + b + sum_h out_h Wo_h^T,  out[n,h,e] = sum_d softmax_d(q[n,:])[d] * s * ctx[h][d][e],  q projected from xn
+// The warps share one xn ring and step through the tiles together; each leaves its fp32 [32 px][32] partial in shared
+// memory, and after a CTA barrier every thread sums two columns of two rows over the eight heads, adds the bias and the
+// residual and writes y once.
+constexpr int LFO_STAGES = 3;      // 68 KB per CTA; 110 registers: two CTAs per SM
 constexpr int LFO_R_PITCH = LF_C + 8;                              // fp32 partial rows: conflict-free float2 stores
-constexpr size_t LAF_OUT_PROJ_SMEM = (size_t)LFOP_STAGES * LW_TILE * 2 + (size_t)LM_HEADS * LFP_WO_TILE * 2 +
-                                     (size_t)LM_HEADS * 32 * LFO_R_PITCH * 4;
-template <bool PROJ = false>
+constexpr size_t LAF_OUT_SMEM = (size_t)LFO_STAGES * LW_TILE * 2 + (size_t)LM_HEADS * LFP_WO_TILE * 2 +
+                                (size_t)LM_HEADS * 32 * LFO_R_PITCH * 4;
 __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
-                                                      const float* __restrict__ ctx, __nv_bfloat16* __restrict__ out, int N,
+                                                      const float* __restrict__ ctx, __nv_bfloat16* __restrict__ y, int N,
                                                       int chunk_px, float scale, const __nv_bfloat16* __restrict__ w_out,
                                                       const float* __restrict__ b_out,
                                                       const __nv_bfloat16* __restrict__ residual) {
     pdl_trigger();
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
-    constexpr int STAGES = PROJ ? LFOP_STAGES : LFO_STAGES;
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (PROJ ? 0 : (size_t)h * ((LFO_STAGES + 1) * LW_TILE));
-    __nv_bfloat16* Os = ring + LFO_STAGES * LW_TILE;
-    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw) + LFOP_STAGES * LW_TILE + h * LFP_WO_TILE;     // PROJ only
-    float* R = reinterpret_cast<float*>(reinterpret_cast<__nv_bfloat16*>(raw) + LFOP_STAGES * LW_TILE +
-                                        LM_HEADS * LFP_WO_TILE);                                      // PROJ only
+    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw);
+    __nv_bfloat16* Wo = ring + LFO_STAGES * LW_TILE + h * LFP_WO_TILE;
+    float* R = reinterpret_cast<float*>(ring + LFO_STAGES * LW_TILE + LM_HEADS * LFP_WO_TILE);
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / 32;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
-    __nv_bfloat16* odst = out + pix0 * LM_HID + h * LM_D;
-    if (PROJ) {                                    // this head's W_out slice: the oldest copy group
-        lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
-        cp_commit();
-    }
+    lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);   // this head's W_out slice: the oldest copy group
+    cp_commit();
     auto issue = [&](int it) {
-        if (it < n_tiles && (!PROJ || h == 0))
-            lw_issue<32>(ring + (size_t)(it % STAGES) * LW_TILE, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
+        if (it < n_tiles && h == 0)
+            lw_issue<32>(ring + (size_t)(it % LFO_STAGES) * LW_TILE, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
         cp_commit();
     };
 #pragma unroll
-    for (int s = 0; s < (PROJ ? STAGES - 1 : STAGES); ++s) issue(s);
+    for (int s = 0; s < LFO_STAGES - 1; ++s) issue(s);
     uint32_t wq[2][4][2];
     load_w_frags(wq, W + (size_t)(h * LM_D) * LF_C, lane);
     const float* ch = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
@@ -422,29 +406,19 @@ __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __res
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) frag_b_global<true>(bf[ks][nt], ch, ks * 16, nt * 8, lane);
     const int g = lane >> 2, t = lane & 3;
-    const int rrow = threadIdx.x >> 4, rcol = (threadIdx.x & 15) * 2;     // PROJ: the y elements this thread sums
-    float2 bias = make_float2(0.f, 0.f);
-    if (PROJ) bias = make_float2(b_out[rcol], b_out[rcol + 1]);
+    const int rrow = threadIdx.x >> 4, rcol = (threadIdx.x & 15) * 2;     // the y elements this thread sums
+    const float2 bias = make_float2(b_out[rcol], b_out[rcol + 1]);
     float* Rw = R + h * 32 * LFO_R_PITCH;
     for (int it = 0; it < n_tiles; ++it) {
         uint32_t ax[2][2][4];
-        if (PROJ) {
-            cp_wait<STAGES - 2>();
-            __syncthreads();                       // tile `it` is visible to every warp; slot (it - 1) and R are free
-            issue(it + STAGES - 1);
-            load_x_frags<2>(ax, ring + (size_t)(it % STAGES) * LW_TILE, lane);
-        } else {
-            cp_wait<LFO_STAGES - 1>();
-            __syncwarp();
-            load_x_frags<2>(ax, ring + (size_t)(it % LFO_STAGES) * LW_TILE, lane);
-            __syncwarp();
-            issue(it + LFO_STAGES);
-        }
-        __nv_bfloat162 res[2];                     // PROJ: the residual elements this thread adds, loaded early
-        if (PROJ)
+        cp_wait<LFO_STAGES - 2>();
+        __syncthreads();                           // tile `it` is visible to every warp; slot (it - 1) and R are free
+        issue(it + LFO_STAGES - 1);
+        load_x_frags<2>(ax, ring + (size_t)(it % LFO_STAGES) * LW_TILE, lane);
+        __nv_bfloat162 res[2];                     // the residual elements this thread adds, loaded early
 #pragma unroll
-            for (int rh = 0; rh < 2; ++rh)
-                res[rh] = *reinterpret_cast<const __nv_bfloat162*>(residual + (pix0 + (size_t)it * 32 + rrow + rh * 16) * LF_C + rcol);
+        for (int rh = 0; rh < 2; ++rh)
+            res[rh] = *reinterpret_cast<const __nv_bfloat162*>(residual + (pix0 + (size_t)it * 32 + rrow + rh * 16) * LF_C + rcol);
         float cq[2][4][4];
         project<2>(cq, ax, wq);
 #pragma unroll
@@ -461,57 +435,42 @@ __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __res
             for (int ks = 0; ks < 2; ++ks)
 #pragma unroll
                 for (int nt = 0; nt < 4; ++nt) mma_bf16(c[nt], a[ks], bf[ks][nt][0], bf[ks][nt][1]);
-            if (PROJ) {                            // y_h[16 px][32 c] = out_h Wo_h^T: B[k = e][n = c] = Wo_h[c][e]
-                c_to_a(a, c);
-                float y[4][4];
+            c_to_a(a, c);                          // yh[16 px][32 c] = out_h Wo_h^T: B[k = e][n = c] = Wo_h[c][e]
+            float yh[4][4];
 #pragma unroll
-                for (int i = 0; i < 4; ++i)
+            for (int i = 0; i < 4; ++i)
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) y[i][k] = 0.f;
+                for (int k = 0; k < 4; ++k) yh[i][k] = 0.f;
 #pragma unroll
-                for (int ke = 0; ke < 2; ++ke)
+            for (int ke = 0; ke < 2; ++ke)
 #pragma unroll
-                    for (int np = 0; np < 2; ++np) {
-                        uint32_t bw[4];
-                        frag_b_nrows(bw, Wo, LW_PITCH, np * 16, ke * 16, lane);
-                        mma_bf16(y[2 * np], a[ke], bw[0], bw[1]);
-                        mma_bf16(y[2 * np + 1], a[ke], bw[2], bw[3]);
-                    }
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                    for (int half = 0; half < 2; ++half)
-                        *reinterpret_cast<float2*>(Rw + (mt * 16 + g + half * 8) * LFO_R_PITCH + nt * 8 + 2 * t) =
-                            make_float2(y[nt][half * 2], y[nt][half * 2 + 1]);
-            } else {
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    __nv_bfloat16* o = Os + (size_t)(mt * 16 + g) * LW_PITCH + nt * 8 + 2 * t;
-                    *reinterpret_cast<uint32_t*>(o) = pack_bf16(c[nt][0], c[nt][1]);
-                    *reinterpret_cast<uint32_t*>(o + 8 * LW_PITCH) = pack_bf16(c[nt][2], c[nt][3]);
+                for (int np = 0; np < 2; ++np) {
+                    uint32_t bw[4];
+                    frag_b_nrows(bw, Wo, LW_PITCH, np * 16, ke * 16, lane);
+                    mma_bf16(yh[2 * np], a[ke], bw[0], bw[1]);
+                    mma_bf16(yh[2 * np + 1], a[ke], bw[2], bw[3]);
                 }
-            }
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                for (int half = 0; half < 2; ++half)
+                    *reinterpret_cast<float2*>(Rw + (mt * 16 + g + half * 8) * LFO_R_PITCH + nt * 8 + 2 * t) =
+                        make_float2(yh[nt][half * 2], yh[nt][half * 2 + 1]);
         }
-        if (PROJ) {
-            __syncthreads();                       // the eight head partials of this tile are in R
+        __syncthreads();                           // the eight head partials of this tile are in R
 #pragma unroll
-            for (int rh = 0; rh < 2; ++rh) {
-                const int row = rrow + rh * 16;
-                const size_t pix = pix0 + (size_t)it * 32 + row;
-                const float2 x = __bfloat1622float2(res[rh]);
-                float sx = x.x + bias.x, sy = x.y + bias.y;
+        for (int rh = 0; rh < 2; ++rh) {
+            const int row = rrow + rh * 16;
+            const size_t pix = pix0 + (size_t)it * 32 + row;
+            const float2 x = __bfloat1622float2(res[rh]);
+            float sx = x.x + bias.x, sy = x.y + bias.y;
 #pragma unroll
-                for (int w = 0; w < LM_HEADS; ++w) {
-                    const float2 v = *reinterpret_cast<const float2*>(R + (w * 32 + row) * LFO_R_PITCH + rcol);
-                    sx += v.x;
-                    sy += v.y;
-                }
-                *reinterpret_cast<uint32_t*>(out + pix * LF_C + rcol) = pack_bf16(sx, sy);
+            for (int w = 0; w < LM_HEADS; ++w) {
+                const float2 v = *reinterpret_cast<const float2*>(R + (w * 32 + row) * LFO_R_PITCH + rcol);
+                sx += v.x;
+                sy += v.y;
             }
-        } else {
-            __syncwarp();
-            lw_store<32>(odst + (size_t)it * 32 * LM_HID, LM_HID, Os, lane);
-            __syncwarp();
+            *reinterpret_cast<uint32_t*>(y + pix * LF_C + rcol) = pack_bf16(sx, sy);
         }
     }
 }
@@ -611,15 +570,14 @@ __device__ __forceinline__ void lfb_cd(float (&cdc)[8], float* scd, const float*
 // head's dq | dk | dv by its 32-row slices of W at once (B fragments [k = d][n = c] by ldmatrix.trans from a shared
 // copy of W), leaving a [16 px][32] fp32 partial; the eight partials are summed through shared memory and dxn is
 // written once, in bf16.  The nine loop-invariant 32x32 B-operand fragment sets stay in registers: one CTA per SM.
-// PROJ: a stage holds the xn tile and the one dy tile all heads share; each warp recomputes its dout tile from dy.
+// A stage holds the xn tile and the one dy tile all heads share; each warp recomputes its dout tile from dy.
 constexpr int LFB_W_PITCH = LF_C + 8;                              // W copy [768][40] bf16: conflict-free ldmatrix
 constexpr int LFB_R_PITCH = LF_C + 8;                              // fp32 partial rows: conflict-free float2 stores
-template <bool PROJ>
 struct LfbCfg {
-    static constexpr int STAGE_ELEMS = (PROJ ? 2 : 1 + LM_HEADS) * LFB_TILE;   // xn tile | dy tile or 8 dout tiles
+    static constexpr int STAGE_ELEMS = 2 * LFB_TILE;                            // xn tile | dy tile
     static constexpr size_t SMEM_BASE = (size_t)LFB_STAGES * STAGE_ELEMS * 2 + (size_t)3 * LM_HID * LFB_W_PITCH * 2 +
                                         (size_t)LM_HEADS * LFB_ROWS * LFB_R_PITCH * 4 + (size_t)LM_HEADS * LM_D * 4;
-    static constexpr size_t SMEM = SMEM_BASE + (PROJ ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
+    static constexpr size_t SMEM = SMEM_BASE + (size_t)LM_HEADS * LFP_WO_TILE * 2;
 };
 
 // c[16 px][32 c] += g[16 px][32 d] Wh[d][c]   (g as A fragments; Wh = one head's 32 rows of the shared W copy)
@@ -635,37 +593,35 @@ __device__ __forceinline__ void mma_w(float (&c)[4][4], const uint32_t (&g)[2][4
         }
 }
 
-template <bool PROJ = false>
 __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
-                                                      const __nv_bfloat16* __restrict__ dout, const float* __restrict__ ctx,
+                                                      const __nv_bfloat16* __restrict__ dy, const float* __restrict__ ctx,
                                                       const float* __restrict__ dctx, const float* __restrict__ kmax,
                                                       const float* __restrict__ kzinv, __nv_bfloat16* __restrict__ dxn,
                                                       int N, int chunk_px, float scale, const __nv_bfloat16* __restrict__ w_out) {
     pdl_trigger();
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
-    constexpr int LFB_STAGE_ELEMS = LfbCfg<PROJ>::STAGE_ELEMS;
+    constexpr int LFB_STAGE_ELEMS = LfbCfg::STAGE_ELEMS;
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
     __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw);
     __nv_bfloat16* Ws = ring + LFB_STAGES * LFB_STAGE_ELEMS;
-    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + LfbCfg<PROJ>::SMEM_BASE) + h * LFP_WO_TILE;   // PROJ only
+    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + LfbCfg::SMEM_BASE) + h * LFP_WO_TILE;
     float* R = reinterpret_cast<float*>(Ws + 3 * LM_HID * LFB_W_PITCH);
     float* scd = R + LM_HEADS * LFB_ROWS * LFB_R_PITCH + h * LM_D;
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / LFB_ROWS;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
-    const __nv_bfloat16* gsrc = PROJ ? dout + pix0 * LF_C : dout + pix0 * LM_HID + h * LM_D;
+    const __nv_bfloat16* gsrc = dy + pix0 * LF_C;
     for (int i = threadIdx.x; i < 3 * LM_HID * (LF_C / 8); i += blockDim.x)      // W -> smem: the oldest copy group
         cp_async16(Ws + (i >> 2) * LFB_W_PITCH + (i & 3) * 8, W + (size_t)(i >> 2) * LF_C + (i & 3) * 8);
-    if (PROJ) lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
+    lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
     cp_commit();
     auto issue = [&](int it) {
         if (it < n_tiles) {
             __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * LFB_STAGE_ELEMS;
             if (h == 0) lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-            if (!PROJ) lw_issue<LFB_ROWS>(buf + (1 + h) * LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LM_HID, LM_HID, lane);
-            else if (h == 1) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
+            if (h == 1) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
         }
         cp_commit();
     };
@@ -704,12 +660,7 @@ __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __res
         const __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * LFB_STAGE_ELEMS;
         LfbTile tl;
         load_x_frags<1>(tl.ax, buf, lane);
-        if (PROJ) {
-            lfp_dout(tl.ag, buf + LFB_TILE, Wo, lane);
-        } else {
-            frag_a_rowmajor(tl.ag[0], buf + (1 + h) * LFB_TILE, LW_PITCH, 0, 0, lane);      // dout [px][e]
-            frag_a_rowmajor(tl.ag[1], buf + (1 + h) * LFB_TILE, LW_PITCH, 0, 16, lane);
-        }
+        lfp_dout(tl.ag, buf + LFB_TILE, Wo, lane);
         float dx[4][4];
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
@@ -749,20 +700,18 @@ __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __res
 }
 
 // ---- pass B (weight gradient): dW_h = [dq | dk | dv]_h^T xn over the CTA's pixels, one reduction per CTA ---------------
-// PART 0 accumulates dWq (reads xn and dout), PART 1 dWk and dWv (reads xn only): split so that neither instantiation
-// holds more than 64 accumulators next to its operand fragments.  Warps are independent (one head each, own tiles).
-// The [32 d][32 c] sums leave through shared memory as coalesced 128-byte red.global.add rows of the fp32 gradient.
-// PART 0 with PROJ streams dy in place of dout, recomputes dout_h from it, and also accumulates the to_out weight
-// gradient dW_out[c][32h + e] = sum_n dy[n][c] out_h[n][e], with out_h recomputed exactly as the forward forms it.
-template <int PART, bool PROJ = false>
+// PART 0 streams xn and dy, recomputes dout_h from dy and accumulates dWq and the to_out weight gradient
+// dW_out[c][32h + e] = sum_n dy[n][c] out_h[n][e], with out_h recomputed exactly as the forward forms it; PART 1
+// accumulates dWk and dWv (reads xn only): split so that neither instantiation holds more than 64 accumulators next to
+// its operand fragments.  Warps are independent (one head each, own tiles).  The [32][32] sums leave through shared
+// memory as coalesced 128-byte red.global.add rows of the fp32 gradient.
+template <int PART>
 struct LfwCfg {
-    static_assert(!PROJ || PART == 0, "PROJ applies to part 0");
-    static constexpr int MATS = (PART == 0 && !PROJ) ? 1 : 2;
-    static constexpr int STAGE_ELEMS = (PART == 0 ? 2 : 1) * LFB_TILE;     // xn tile (| dout / dy tile)
+    static constexpr int STAGE_ELEMS = (PART == 0 ? 2 : 1) * LFB_TILE;     // xn tile (| dy tile)
     static constexpr int S_PITCH = LM_D + 1;                                 // epilogue staging [32 d][33] fp32
     static_assert(LFB_STAGES * STAGE_ELEMS * 2 >= LM_D * S_PITCH * 4, "the epilogue staging reuses the tile ring");
     static constexpr size_t SMEM_BASE = (size_t)LM_HEADS * (LFB_STAGES * STAGE_ELEMS * 2 + LM_D * 4);
-    static constexpr size_t SMEM = SMEM_BASE + (PROJ ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
+    static constexpr size_t SMEM = SMEM_BASE + (PART == 0 ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
 };
 
 // acc[32 d][32 c] += gf^T x over one 16-pixel tile: gf = accumulator fragment [16 px][32 d], bx = B fragments
@@ -783,9 +732,9 @@ __device__ __forceinline__ void acc_gtx(float (&acc)[2][4][4], const float (&gf)
     }
 }
 
-template <int PART, bool PROJ = false>
+template <int PART>
 __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __restrict__ xn, const __nv_bfloat16* __restrict__ W,
-                                                        const __nv_bfloat16* __restrict__ dout, const float* __restrict__ ctx,
+                                                        const __nv_bfloat16* __restrict__ dy, const float* __restrict__ ctx,
                                                         const float* __restrict__ dctx, const float* __restrict__ kmax,
                                                         const float* __restrict__ kzinv, float* __restrict__ grad_w, int N,
                                                         int chunk_px, long long w_stride_n, long long w_stride_c, float scale,
@@ -794,19 +743,18 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
     pdl_trigger();
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
-    using Cfg = LfwCfg<PART, PROJ>;
-    constexpr int MATS = Cfg::MATS, STAGE_ELEMS = Cfg::STAGE_ELEMS, S_PITCH = Cfg::S_PITCH;
+    using Cfg = LfwCfg<PART>;
+    constexpr int STAGE_ELEMS = Cfg::STAGE_ELEMS, S_PITCH = Cfg::S_PITCH;
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
     __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFB_STAGES * STAGE_ELEMS);
     float* scd = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFB_STAGES * STAGE_ELEMS * 2) + h * LM_D;
-    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + Cfg::SMEM_BASE) + h * LFP_WO_TILE;        // PROJ only
+    __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + Cfg::SMEM_BASE) + h * LFP_WO_TILE;        // PART 0
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / LFB_ROWS;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
-    const __nv_bfloat16* gsrc = PROJ ? dout + pix0 * LF_C : dout + pix0 * LM_HID + h * LM_D;
-    constexpr int G_STRIDE = PROJ ? LF_C : LM_HID;
-    if (PROJ) {                                    // this head's W_out slice: the oldest copy group
+    const __nv_bfloat16* gsrc = dy + pix0 * LF_C;
+    if (PART == 0) {                               // this head's W_out slice: the oldest copy group
         lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
         cp_commit();
     }
@@ -814,7 +762,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
         if (it < n_tiles) {
             __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * STAGE_ELEMS;
             lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-            if (PART == 0) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * G_STRIDE, G_STRIDE, lane);
+            if (PART == 0) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
         }
         cp_commit();
     };
@@ -824,7 +772,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
     const float* dg = dctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
     float Mc[8], Zc[8], cdc[8];
     uint32_t w0[2][4][2], w1[2][4][2];             // PART 0: Wq, (unused)   PART 1: Wk, Wv
-    uint32_t b0[2][4][2], b1[2][4][2];             // PART 0: ctx^T, (PROJ: ctx)   PART 1: dctx^T, dctx
+    uint32_t b0[2][4][2], b1[2][4][2];             // PART 0: ctx^T, ctx   PART 1: dctx^T, dctx
     if (PART == 0) {
         load_w_frags(w0, W + (size_t)(h * LM_D) * LF_C, lane);
     } else {
@@ -839,12 +787,12 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
             frag_b_global<false>(b0[ks][nt], PART == 0 ? cg : dg, ks * 16, nt * 8, lane);
-            if (PART == 1 || PROJ) frag_b_global<true>(b1[ks][nt], PART == 1 ? dg : cg, ks * 16, nt * 8, lane);
+            frag_b_global<true>(b1[ks][nt], PART == 1 ? dg : cg, ks * 16, nt * 8, lane);
         }
     const float invN = 1.f / (float)N;
-    float acc[MATS][2][4][4];
+    float acc[2][2][4][4];
 #pragma unroll
-    for (int m = 0; m < MATS; ++m)
+    for (int m = 0; m < 2; ++m)
 #pragma unroll
         for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -860,20 +808,17 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
         uint32_t bx[2][4];
         frag_b_krows(bx[0], buf, LW_PITCH, 0, 0, lane);        // B[k = px][n = c] = xn[px][c]
         frag_b_krows(bx[1], buf, LW_PITCH, 0, 16, lane);
-        uint32_t ady[2][4], bdy[2][4];             // PROJ: A fragments [px][c] and B fragments [k = px][n = c] of dy
-        if (PROJ) {
+        uint32_t ady[2][4], bdy[2][4];             // PART 0: A fragments [px][c] and B fragments [k = px][n = c] of dy
+        if (PART == 0) {
             frag_a_rowmajor(ady[0], buf + LFB_TILE, LW_PITCH, 0, 0, lane);
             frag_a_rowmajor(ady[1], buf + LFB_TILE, LW_PITCH, 0, 16, lane);
             frag_b_krows(bdy[0], buf + LFB_TILE, LW_PITCH, 0, 0, lane);
             frag_b_krows(bdy[1], buf + LFB_TILE, LW_PITCH, 0, 16, lane);
-        } else if (PART == 0) {
-            frag_a_rowmajor(tl.ag[0], buf + LFB_TILE, LW_PITCH, 0, 0, lane);
-            frag_a_rowmajor(tl.ag[1], buf + LFB_TILE, LW_PITCH, 0, 16, lane);
         }
         __syncwarp();                              // the tile is in registers
         issue(it + LFB_STAGES);
         if (PART == 0) {
-            if (PROJ) {
+            {
                 float c[4][4];
                 lfp_dout_acc(c, ady, Wo, lane);
                 c_to_a(tl.ag, c);
@@ -881,26 +826,25 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
             float dq[4][4];
             lfb_dq(dq, tl, w0, b0, scale);
             acc_gtx(acc[0], dq, bx);
-            if (PROJ) {                            // out_h as laf_out_kernel forms it, then dW_out^T += out_h^T dy
-                float cq[1][4][4], o[4][4];
-                project<1>(cq, tl.ax, w0);
-                frag_softmax(cq[0], scale);
-                uint32_t a[2][4];
-                c_to_a(a, cq[0]);
+            // out_h as laf_out_kernel forms it, then dW_out^T += out_h^T dy
+            float cq[1][4][4], o[4][4];
+            project<1>(cq, tl.ax, w0);
+            frag_softmax(cq[0], scale);
+            uint32_t a[2][4];
+            c_to_a(a, cq[0]);
 #pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
+            for (int nt = 0; nt < 4; ++nt) {
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) o[nt][i] = 0.f;
+                for (int i = 0; i < 4; ++i) o[nt][i] = 0.f;
 #pragma unroll
-                    for (int ks = 0; ks < 2; ++ks) mma_bf16(o[nt], a[ks], b1[ks][nt][0], b1[ks][nt][1]);
-                }
-                acc_gtx(acc[MATS - 1], o, bdy);
+                for (int ks = 0; ks < 2; ++ks) mma_bf16(o[nt], a[ks], b1[ks][nt][0], b1[ks][nt][1]);
             }
+            acc_gtx(acc[1], o, bdy);
         } else {
             float dk[4][4], dv[4][4];
             lfb_dkdv(dk, dv, tl.ax, w0, w1, b0, b1, Mc, Zc, cdc, invN);
             acc_gtx(acc[0], dk, bx);
-            acc_gtx(acc[MATS - 1], dv, bx);
+            acc_gtx(acc[1], dv, bx);
         }
     }
     cp_wait<0>();
@@ -908,7 +852,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
     float* S = reinterpret_cast<float*>(ring);
     const int g = lane >> 2, t = lane & 3;
 #pragma unroll
-    for (int m = 0; m < MATS; ++m) {
+    for (int m = 0; m < 2; ++m) {
 #pragma unroll
         for (int md = 0; md < 2; ++md)
 #pragma unroll
@@ -916,7 +860,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
 #pragma unroll
                 for (int i = 0; i < 4; ++i) S[(md * 16 + g + 8 * (i >> 1)) * S_PITCH + nc * 8 + 2 * t + (i & 1)] = acc[m][md][nc][i];
         __syncwarp();
-        if (PROJ && m == 1) {                      // S[e][c] = dW_out[c][32h + e]: lane = e, one row c at a time
+        if (PART == 0 && m == 1) {                    // S[e][c] = dW_out[c][32h + e]: lane = e, one row c at a time
             float* dst = grad_wo + (long long)(h * LM_D + lane) * wo_stride_c;
 #pragma unroll 4
             for (int c = 0; c < LF_C; ++c) atomicAdd(dst + c * wo_stride_n, S[lane * S_PITCH + c]);
@@ -931,7 +875,6 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
 }
 
 constexpr size_t LAF_STATS_SMEM = (size_t)LM_HEADS * LFS_STAGES * LW_TILE * 2;
-constexpr size_t LAF_OUT_SMEM = (size_t)LM_HEADS * (LFO_STAGES + 1) * LW_TILE * 2;
 
 static int laf_attrs() {
     static bool done = false;
@@ -939,13 +882,9 @@ static int laf_attrs() {
         PIDM_CUDA(cudaFuncSetAttribute(laf_kmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_STATS_SMEM));
         PIDM_CUDA(cudaFuncSetAttribute(laf_ctx_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfcCfg<0>::SMEM));
         PIDM_CUDA(cudaFuncSetAttribute(laf_ctx_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfcCfg<1>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_ctx_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfcCfg<1, true>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_out_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_OUT_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_out_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_OUT_PROJ_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfbCfg<false>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfbCfg<true>::SMEM));
+        PIDM_CUDA(cudaFuncSetAttribute(laf_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_OUT_SMEM));
+        PIDM_CUDA(cudaFuncSetAttribute(laf_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfbCfg::SMEM));
         PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<0>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<0, true>::SMEM));
         PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<1>::SMEM));
         done = true;
     }
@@ -968,12 +907,30 @@ static int laf_stat_chunks(int N) {
     return c;
 }
 
-// The three phases below are shared by pidm_linattn_fused_* (PROJ = false: `out` / `dout` are [B, N, 256]) and
-// pidm_linattn_block_* (PROJ = true: `out` / `dout` are y / dy [B, N, 32], w_out the packed to_out weights).
-template <bool PROJ>
-static int laf_fwd(const void* xn, const void* w_qkv, const void* w_out, const float* b_out, const void* residual, void* out,
-                   float* ctx, float* kmax, float* kzinv, float* workspace, int B, int N, void* stream) {
-    PIDM_REQUIRE(N % 128 == 0, "linattn_fused: N must be a multiple of 128 (got %d)", N);
+}  // namespace pidm
+using namespace pidm;
+
+extern "C" int pidm_linattn_block_supported(int C, int heads, int N, int dtype) {
+    return (C == LF_C && heads == LM_HEADS && dtype == PIDM_BF16 && N % 128 == 0) ? 1 : 0;
+}
+
+extern "C" int pidm_linattn_block_workspace_floats(int B, int N) { return B * laf_stat_chunks(N) * LM_HID; }
+
+// pixel chunking of the block's kernels: out[5] = {statistics chunks (kmax), ctx px, fwd (y) px, bwd px, wgrad px}
+extern "C" int pidm_linattn_block_plan(int B, int N, int* out) {
+    PIDM_REQUIRE(N % 128 == 0 && B > 0, "linattn_block_plan: N must be a multiple of 128 (got %d)", N);
+    const int v[5] = {laf_stat_chunks(N), laf_chunk_px(B, N, 2), laf_chunk_px(B, N, 2), laf_chunk_px(B, N, 1),
+                      laf_chunk_px(B, N, 1)};
+    for (int i = 0; i < 5; ++i) out[i] = v[i];
+    return 0;
+}
+
+// The whole linear-attention block: y = residual + b_out + to_out(attention(to_qkv(xn))), see pidm.h.
+extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const void* w_out, const float* b_out,
+                                      const void* residual, void* y, float* ctx, float* kmax, float* kzinv,
+                                      float* workspace, int B, int N, void* stream) {
+    PIDM_REQUIRE(w_out && b_out && residual, "linattn_block_fwd: w_out, b_out and residual are required");
+    PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
     if (int e = laf_attrs()) return e;
     const float scale = 0.17677669529663687f;   // 32^-0.5
@@ -983,118 +940,39 @@ static int laf_fwd(const void* xn, const void* w_qkv, const void* w_out, const f
     PIDM_CUDA(cudaMemsetAsync(kzinv, 0, (size_t)B * LM_HID * sizeof(float), st));
     const int chunks = laf_stat_chunks(N);
     const int rpc = N / chunks;
-    PIDM_REQUIRE(rpc % 32 == 0 && rpc * chunks == N, "linattn_fused: bad statistics chunking for N=%d", N);
+    PIDM_REQUIRE(rpc % 32 == 0 && rpc * chunks == N, "linattn_block: bad statistics chunking for N=%d", N);
     PIDM_CUDA(launch_pdl(laf_kmax_kernel, dim3(dim3(chunks, B)), dim3(256), (size_t)(LAF_STATS_SMEM), st, x, w, workspace, N, rpc));
-    const int cpx = laf_chunk_px(B, N, 2);
-    PIDM_CUDA(launch_pdl(laf_ctx_kernel<0>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), (size_t)(LfcCfg<0>::SMEM), st, x, w, nullptr, workspace, chunks, kmax, kzinv,
-                                                                             ctx, N, cpx, scale, nullptr));
-    PIDM_CUDA(launch_pdl(laf_finalize_kernel, dim3((B * LM_HID + 7) / 8), dim3(256), (size_t)(0), st, ctx, kzinv, B * LM_HID));
-    const int opx = laf_chunk_px(B, N, PROJ ? 2 : 3);
-    PIDM_CUDA(launch_pdl(laf_out_kernel<PROJ>, dim3(dim3((N + opx - 1) / opx, B)), dim3(256),
-                         PROJ ? LAF_OUT_PROJ_SMEM : LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)out, N, opx, scale,
-                         (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
-    PIDM_LAUNCH_CHECK("linattn_fused_fwd");
-    return 0;
-}
-
-template <bool PROJ>
-static int laf_bwd(const void* xn, const void* w_qkv, const void* w_out, const void* dout, const float* ctx,
-                   const float* kmax, const float* kzinv, void* dxn, float* dctx, int B, int N, void* stream) {
-    PIDM_REQUIRE(N % 128 == 0, "linattn_fused: N must be a multiple of 128 (got %d)", N);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (int e = laf_attrs()) return e;
-    const float scale = 0.17677669529663687f;
-    const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
-    const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
-    const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
-    PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * LM_HEADS * LM_D * LM_D * sizeof(float), st));
-    const int cpx = laf_chunk_px(B, N, 2);
-    PIDM_CUDA(launch_pdl(laf_ctx_kernel<1, PROJ>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), LfcCfg<1, PROJ>::SMEM, st, x, w,
-                         (const __nv_bfloat16*)dout, nullptr, 0, nullptr, nullptr, dctx, N, cpx, scale, wo));
-    const int bpx = laf_chunk_px(B, N, 1);
-    PIDM_CUDA(launch_pdl(laf_bwd_kernel<PROJ>, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), LfbCfg<PROJ>::SMEM, st, x, w,
-                         (const __nv_bfloat16*)dout, ctx, dctx, kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, scale, wo));
-    PIDM_LAUNCH_CHECK("linattn_fused_bwd");
-    return 0;
-}
-
-template <bool PROJ>
-static int laf_wgrad(const void* xn, const void* w_qkv, const void* w_out, const void* dout, const float* ctx,
-                     const float* dctx, const float* kmax, const float* kzinv, float* grad_w, long long w_stride_n,
-                     long long w_stride_c, float* grad_wo, long long wo_stride_n, long long wo_stride_c, int B, int N,
-                     void* stream) {
-    PIDM_REQUIRE(N % 128 == 0, "linattn_fused: N must be a multiple of 128 (got %d)", N);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (int e = laf_attrs()) return e;
-    const float scale = 0.17677669529663687f;
-    const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
-    const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
-    const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
-    const __nv_bfloat16* g = (const __nv_bfloat16*)dout;
-    const int px = laf_chunk_px(B, N, 1);
+    const int px = laf_chunk_px(B, N, 2);         // the context and output kernels: two CTAs per SM
     const dim3 grid((N + px - 1) / px, B);
-    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<0, PROJ>, grid, dim3(256), LfwCfg<0, PROJ>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv,
-                         grad_w, N, px, w_stride_n, w_stride_c, scale, wo, grad_wo, wo_stride_n, wo_stride_c));
-    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w, N,
-                         px, w_stride_n, w_stride_c, scale, nullptr, nullptr, 0LL, 0LL));
-    PIDM_LAUNCH_CHECK("linattn_fused_wgrad");
+    PIDM_CUDA(launch_pdl(laf_ctx_kernel<0>, grid, dim3(256), LfcCfg<0>::SMEM, st, x, w, nullptr, workspace, chunks, kmax, kzinv,
+                         ctx, N, px, scale, nullptr));
+    PIDM_CUDA(launch_pdl(laf_finalize_kernel, dim3((B * LM_HID + 7) / 8), dim3(256), (size_t)(0), st, ctx, kzinv, B * LM_HID));
+    PIDM_CUDA(launch_pdl(laf_out_kernel, grid, dim3(256), LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)y, N, px, scale,
+                         (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
+    PIDM_LAUNCH_CHECK("linattn_block_fwd");
     return 0;
-}
-
-}  // namespace pidm
-using namespace pidm;
-
-extern "C" int pidm_linattn_fused_supported(int C, int heads, int N, int dtype) {
-    return (C == LF_C && heads == LM_HEADS && dtype == PIDM_BF16 && N % 128 == 0) ? 1 : 0;
-}
-
-extern "C" int pidm_linattn_fused_workspace_floats(int B, int N) { return B * laf_stat_chunks(N) * LM_HID; }
-
-// pixel chunking of the fused kernels: out[5] = {statistics chunks (kmax), ctx px, out px, bwd px, wgrad px}
-extern "C" int pidm_linattn_fused_plan(int B, int N, int* out) {
-    PIDM_REQUIRE(N % 128 == 0 && B > 0, "linattn_fused_plan: N must be a multiple of 128 (got %d)", N);
-    const int v[5] = {laf_stat_chunks(N), laf_chunk_px(B, N, 2), laf_chunk_px(B, N, 3), laf_chunk_px(B, N, 1),
-                      laf_chunk_px(B, N, 1)};
-    for (int i = 0; i < 5; ++i) out[i] = v[i];
-    return 0;
-}
-
-// xn [B,N,32] bf16 (the PreNorm output), w_qkv [768][32] bf16 (packed to_qkv weights, K-major), out [B,N,256] bf16.
-// ctx [B,8,32,32], kmax / kzinv [B,8,32] are outputs kept for backward; workspace: pidm_linattn_fused_workspace_floats.
-extern "C" int pidm_linattn_fused_fwd(const void* xn, const void* w_qkv, void* out, float* ctx, float* kmax, float* kzinv,
-                                      float* workspace, int B, int N, void* stream) {
-    return laf_fwd<false>(xn, w_qkv, nullptr, nullptr, nullptr, out, ctx, kmax, kzinv, workspace, B, N, stream);
-}
-
-// dxn [B,N,32] bf16 is the gradient w.r.t. xn (written, not accumulated).  dctx [B,8,32,32] is produced here and read
-// again by pidm_linattn_fused_wgrad.
-extern "C" int pidm_linattn_fused_bwd(const void* xn, const void* w_qkv, const void* dout, const float* ctx,
-                                      const float* kmax, const float* kzinv, void* dxn, float* dctx, int B, int N,
-                                      void* stream) {
-    return laf_bwd<false>(xn, w_qkv, nullptr, dout, ctx, kmax, kzinv, dxn, dctx, B, N, stream);
-}
-
-// Weight gradient of the to_qkv projection, ACCUMULATED into grad_w (fp32; element [n][c] at n * w_stride_n +
-// c * w_stride_c), from the same operands as pidm_linattn_fused_bwd after it has produced dctx.
-extern "C" int pidm_linattn_fused_wgrad(const void* xn, const void* w_qkv, const void* dout, const float* ctx,
-                                        const float* dctx, const float* kmax, const float* kzinv, float* grad_w, int B,
-                                        int N, long long w_stride_n, long long w_stride_c, void* stream) {
-    return laf_wgrad<false>(xn, w_qkv, nullptr, dout, ctx, dctx, kmax, kzinv, grad_w, w_stride_n, w_stride_c, nullptr, 0, 0,
-                            B, N, stream);
-}
-
-// The whole linear-attention block: y = residual + b_out + to_out(attention(to_qkv(xn))), see pidm.h.
-extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const void* w_out, const float* b_out,
-                                      const void* residual, void* y, float* ctx, float* kmax, float* kzinv,
-                                      float* workspace, int B, int N, void* stream) {
-    PIDM_REQUIRE(w_out && b_out && residual, "linattn_block_fwd: w_out, b_out and residual are required");
-    return laf_fwd<true>(xn, w_qkv, w_out, b_out, residual, y, ctx, kmax, kzinv, workspace, B, N, stream);
 }
 
 extern "C" int pidm_linattn_block_bwd(const void* xn, const void* w_qkv, const void* w_out, const void* dy, const float* ctx,
                                       const float* kmax, const float* kzinv, void* dxn, float* dctx, int B, int N,
                                       void* stream) {
-    return laf_bwd<true>(xn, w_qkv, w_out, dy, ctx, kmax, kzinv, dxn, dctx, B, N, stream);
+    PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int e = laf_attrs()) return e;
+    const float scale = 0.17677669529663687f;
+    const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
+    const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
+    const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
+    const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
+    PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * LM_HEADS * LM_D * LM_D * sizeof(float), st));
+    const int cpx = laf_chunk_px(B, N, 2);
+    PIDM_CUDA(launch_pdl(laf_ctx_kernel<1>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), LfcCfg<1>::SMEM, st, x, w, g,
+                         nullptr, 0, nullptr, nullptr, dctx, N, cpx, scale, wo));
+    const int bpx = laf_chunk_px(B, N, 1);
+    PIDM_CUDA(launch_pdl(laf_bwd_kernel, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), LfbCfg::SMEM, st, x, w, g, ctx, dctx,
+                         kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, scale, wo));
+    PIDM_LAUNCH_CHECK("linattn_block_bwd");
+    return 0;
 }
 
 extern "C" int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const void* w_out, const void* dy,
@@ -1102,6 +980,20 @@ extern "C" int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const
                                         float* grad_w_qkv, long long qkv_stride_n, long long qkv_stride_c,
                                         float* grad_w_out, long long out_stride_n, long long out_stride_c, int B, int N,
                                         void* stream) {
-    return laf_wgrad<true>(xn, w_qkv, w_out, dy, ctx, dctx, kmax, kzinv, grad_w_qkv, qkv_stride_n, qkv_stride_c,
-                           grad_w_out, out_stride_n, out_stride_c, B, N, stream);
+    PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int e = laf_attrs()) return e;
+    const float scale = 0.17677669529663687f;
+    const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
+    const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
+    const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
+    const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
+    const int px = laf_chunk_px(B, N, 1);
+    const dim3 grid((N + px - 1) / px, B);
+    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<0>, grid, dim3(256), LfwCfg<0>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
+                         N, px, qkv_stride_n, qkv_stride_c, scale, wo, grad_w_out, out_stride_n, out_stride_c));
+    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
+                         N, px, qkv_stride_n, qkv_stride_c, scale, nullptr, nullptr, 0LL, 0LL));
+    PIDM_LAUNCH_CHECK("linattn_block_wgrad");
+    return 0;
 }

@@ -518,47 +518,13 @@ class _LinAttn(torch.autograd.Function):
         return dqkv, None
 
 
-class _LinAttnFused(torch.autograd.Function):
-    """to_qkv (1x1, no bias) + linear attention in one op: q, k, v are recomputed per head inside the kernels, the
-    [B, N, 768] qkv tensor is never written (reference unet_model.py:275-297).  Neither is its gradient: backward
-    writes dxn directly, and a second pass over (xn, dout) on the weight-gradient stream accumulates the projection's
-    weight gradient."""
-
-    @staticmethod
-    def forward(ctx, xn, weight, spec, heads):
-        B, H, W, C = xn.shape
-        N = H * W
-        out = torch.empty(B, H, W, heads * 32, device=xn.device, dtype=xn.dtype)
-        ctxm = torch.empty(B, heads, 32, 32, device=xn.device, dtype=torch.float32)
-        kmax = torch.empty(B, heads, 32, device=xn.device, dtype=torch.float32)
-        kzinv = torch.empty_like(kmax)
-        ws = torch.empty(call('pidm_linattn_fused_workspace_floats', B, N), device=xn.device, dtype=torch.float32)
-        call('pidm_linattn_fused_fwd', xn, spec.wp_fwd, out, ctxm, kmax, kzinv, ws, B, N, stream())
-        ctx.save_for_backward(xn, weight, ctxm, kmax, kzinv)
-        ctx.spec, ctx.heads = spec, heads
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        xn, weight, ctxm, kmax, kzinv = ctx.saved_tensors
-        spec = ctx.spec
-        B, H, W, _ = xn.shape
-        dout = dout.contiguous()
-        dx = torch.empty_like(xn)
-        dctx = torch.empty_like(ctxm)
-        call('pidm_linattn_fused_bwd', xn, spec.wp_fwd, dout, ctxm, kmax, kzinv, dx, dctx, B, H * W, stream())
-        gw_buf, gw_ret = _grad_buffer(weight)
-        ws = _wgrad_stream(xn, spec.wp_fwd, dout, ctxm, dctx, kmax, kzinv)
-        call('pidm_linattn_fused_wgrad', xn, spec.wp_fwd, dout, ctxm, dctx, kmax, kzinv, gw_buf, B, H * W,
-             spec.w_stride_n, spec.w_stride_c, ws)
-        return (dx if ctx.needs_input_grad[0] else None), gw_ret, None, None
-
-
 class _LinAttnBlock(torch.autograd.Function):
     """The whole linear-attention block at the 32-channel levels: y = residual + to_out(attention(to_qkv(xn))) with a 1x1
-    256 -> C to_out (with bias).  The [B, N, 256] attention output and its gradient are never written: forward projects
-    each head's output tile on chip, backward recomputes it and dout per head from dy.  Like the to_out convolution it
-    replaces, it hands dy back as the residual's gradient."""
+    32 -> 768 to_qkv (no bias) and a 1x1 256 -> C to_out (with bias) (reference unet_model.py:275-297).  Neither the
+    [B, N, 768] qkv nor the [B, N, 256] attention output, nor their gradients, are written: the kernels recompute q, k, v
+    per head from xn, forward projects each head's output tile on chip, and backward recomputes it and dout per head
+    from dy; a second pass over (xn, dy) on the weight-gradient stream accumulates both projections' weight gradients.
+    Like the to_out convolution it replaces, it hands dy back as the residual's gradient."""
 
     @staticmethod
     def forward(ctx, xn, w_qkv, spec_qkv, w_out, b_out, spec_out, residual, heads):
@@ -568,7 +534,7 @@ class _LinAttnBlock(torch.autograd.Function):
         ctxm = torch.empty(B, heads, 32, 32, device=xn.device, dtype=torch.float32)
         kmax = torch.empty(B, heads, 32, device=xn.device, dtype=torch.float32)
         kzinv = torch.empty_like(kmax)
-        ws = torch.empty(call('pidm_linattn_fused_workspace_floats', B, N), device=xn.device, dtype=torch.float32)
+        ws = torch.empty(call('pidm_linattn_block_workspace_floats', B, N), device=xn.device, dtype=torch.float32)
         call('pidm_linattn_block_fwd', xn, spec_qkv.wp_fwd, spec_out.wp_fwd, b_out, residual, y, ctxm, kmax, kzinv, ws,
              B, N, stream())
         ctx.save_for_backward(xn, w_qkv, w_out, b_out, ctxm, kmax, kzinv)
@@ -596,24 +562,17 @@ class _LinAttnBlock(torch.autograd.Function):
 
 
 def linear_attention_block_supported(xn, spec_qkv, spec_out, b_out, heads):
-    return (b_out is not None and spec_out.kh == 1 and spec_out.kw == 1 and not spec_out.transposed
-            and spec_out.cin == heads * 32 and spec_out.cout == xn.shape[-1]
-            and linear_attention_fused_supported(xn, spec_qkv, heads))
+    B, H, W, C = xn.shape
+    return (_STATE['use_tc'] and xn.is_cuda and b_out is not None
+            and spec_qkv.kh == 1 and spec_qkv.kw == 1 and spec_qkv.cout == 3 * heads * 32
+            and spec_out.kh == 1 and spec_out.kw == 1 and not spec_out.transposed
+            and spec_out.cin == heads * 32 and spec_out.cout == C
+            and bool(call('pidm_linattn_block_supported', C, heads, H * W, _code(xn))))
 
 
 def linear_attention_block(xn, w_qkv, spec_qkv, w_out, b_out, spec_out, residual, heads):
     """y = residual + to_out(linear_attention(to_qkv(xn))); to_qkv 1x1 without bias, to_out 1x1 256 -> C with bias."""
     return _LinAttnBlock.apply(xn.contiguous(), w_qkv, spec_qkv, w_out, b_out, spec_out, residual.contiguous(), heads)
-
-
-def linear_attention_fused_supported(xn, spec, heads):
-    B, H, W, C = xn.shape
-    return (_STATE['use_tc'] and xn.is_cuda and spec.kh == 1 and spec.kw == 1 and spec.cout == 3 * heads * 32
-            and bool(call('pidm_linattn_fused_supported', C, heads, H * W, _code(xn))))
-
-
-def linear_attention_fused(xn, weight, spec, heads):
-    return _LinAttnFused.apply(xn.contiguous(), weight, spec, heads)
 
 
 def linear_attention(qkv, heads):

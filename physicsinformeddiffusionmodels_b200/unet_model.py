@@ -346,12 +346,9 @@ class Unet3D(nn.Module):
             # to_qkv, the attention, to_out and the `+ x`: the [B, N, 256] attention output is never materialised
             return ops.linear_attention_block(xn, to_qkv.weight, spec, to_out.weight, b_out, self._spec[id(to_out)],
                                               ops.stash_grad(x, sk), pre.fn.heads)
-        if getattr(to_qkv, 'bias', None) is None and ops.linear_attention_fused_supported(xn, spec, pre.fn.heads):
-            a = ops.linear_attention_fused(xn, to_qkv.weight, spec, pre.fn.heads)   # qkv never materialised
-        else:
-            qkv = self._conv(to_qkv, xn)
-            a = ops.linear_attention(qkv, pre.fn.heads)
-        return self._conv(pre.fn.to_out, a, residual=ops.stash_grad(x, sk))
+        qkv = self._conv(to_qkv, xn)
+        a = ops.linear_attention(qkv, pre.fn.heads)
+        return self._conv(to_out, a, residual=ops.stash_grad(x, sk))
 
     def _mid_attention(self, res, x):
         pre = res.fn

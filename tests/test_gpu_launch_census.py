@@ -1,21 +1,23 @@
 """Every tensor-core launch of the benchmarked steps, replayed element by element against an fp64 reference.
 
-The convolution (conv_tc.cu), the two weight-gradient kernels (wgrad_tc.cu, wgrad_tc3.cu) and the fused linear attention
+The convolution (conv_tc.cu), the two weight-gradient kernels (wgrad_tc.cu, wgrad_tc3.cu) and the linear-attention block
 (attention_fused.cu) choose their plan -- tile widths, persistent-grid waves, pixel splits, pixel chunks -- from the batch
 size and the SM count.  The per-op tests in test_gpu_ops.py run small batches, so they see few of the plans the
 benchmark runs, and they compare whole tensors by a norm ratio, which a bug confined to one tile row cannot move.  Here:
 
   1. census: one eager step of every workload bench.py times (Darcy training at batch 32, mechanics training at batch 32
      with Unet3D(dim=128), one Darcy sampling step at batch 16 / 64 / 256) is run with `ops.call` swapped for a recorder,
-     and the distinct integer arguments of every tensor-core call are kept.  They must be a subset of the tables below
+     and the distinct integer arguments of every tensor-core call are kept.  They must equal the tables below
      (`python tests/test_gpu_launch_census.py --print-table` regenerates them);
   2. replay: every table row (plus a few synthetic rows that reach the planner choices the workloads do not) is run
      directly through the C ABI on fresh seeded bf16-exact operands and compared with an fp64 reference of the contract
      in include/pidm.h, per element:
         conv (bf16 out)         |y - r| <= 2^-8 |r| + C_ACC sqrt(K) 2^-24 A      A = the same op on |x|, |W|, |bias|, |res|
         wgrad, gn_sums (fp32)   |y - r| <=              C_ACC sqrt(K) 2^-24 A      K = summed pixels (elements)
-        fused attention         |y - r| <= A_ATT |r| + B_ATT rms(r over the (sample, head) slice)
-     Output buffers sit between sentinel guard regions that must survive the launch; accumulating outputs are prefilled;
+        attention block         |y - r| <= A_ATT |r| + B_ATT rms(r over a slice)  (+ 2^-14 |prefill| when accumulated)
+     The block's residual and bias are scaled to the rms of its attention term, so that each of the three terms of y is
+     visible to the bound.  Output buffers sit between sentinel guard regions that must survive the launch;
+     accumulating outputs are prefilled;
   3. mutants: the same predicates reject the fp64 reference edited the way a subtle kernel bug would change it;
   4. plan coverage: the C-ABI plan queries show that the table plus the synthetic rows reach every tile instantiation and
      every planner branch (ragged persistent waves, short last splits, ragged last chunks, odd batch with TN = 2).
@@ -35,23 +37,25 @@ DEV = 'cuda'
 
 # Error-bound constants.  Products of bf16 operands are exact in fp32, so the only kernel-side errors are the fp32
 # accumulation (bounded by C_ACC sqrt(K) 2^-24 times the absolute-value reference) and, for bf16 outputs, one rounding.
-# The fused attention keeps q / k / v / ctx as bf16 tensor-core operands, hence the relative + slice-rms form.
-# C_ACC, A_ATT and B_ATT were set from H100 80GB HBM3 runs of this file; the worst |err| / bound observed per kernel
-# family is recorded in DESIGN.md section 2.
+# The attention block keeps q / k / v / ctx / out / dout as bf16 tensor-core operands, hence the relative + slice-rms
+# form.  C_ACC, A_ATT and B_ATT were set from H100 80GB HBM3 runs of this file; the worst |err| / bound observed per
+# kernel family is recorded in DESIGN.md section 2.
 C_ACC = 1.0
 A_ATT = 2.0 ** -7
-B_ATT = {'fwd': 2.0 ** -3, 'bwd': 2.0 ** -2, 'wgrad': 2.0 ** -4}     # out, dxn, grad_w
+# y and dxn: slice = sample; dW_qkv: slice = (q | k | v, head); dW_out: slice = one head's 32 columns; db: whole vector
+B_ATT = {'fwd': 2.0 ** -3, 'bwd': 2.0 ** -2, 'wgrad': 2.0 ** -4}     # y, dxn, dW_qkv / dW_out / db
+PREFILL = 2.0 ** -14     # fp32 accumulation into a prefilled gradient: one rounding of the prefill
 GUARD_BF16 = 0x7FBF            # a NaN bit pattern: an unwritten output element fails every bound
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # the committed census table (regenerate with --print-table); distinct keys per workload:
-#   darcy_train_b32: conv 85, wgrad 36, laf 6
-#   darcy_sample_b16: conv 40, wgrad 0, laf 2
-#   darcy_sample_b64: conv 40, wgrad 0, laf 2
-#   darcy_sample_b256: conv 40, wgrad 0, laf 2
+#   darcy_train_b32: conv 81, wgrad 34, laf 6
+#   darcy_sample_b16: conv 38, wgrad 0, laf 2
+#   darcy_sample_b64: conv 38, wgrad 0, laf 2
+#   darcy_sample_b256: conv 38, wgrad 0, laf 2
 #   mech_train_b32: conv 87, wgrad 37, laf 0
-#   distinct: conv 292, wgrad 73, laf 12
+#   distinct: conv 282, wgrad 71, laf 12
 # ----------------------------------------------------------------------------------------------------------------------
 # conv: B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad, transposed, bias, residual, gn_sums, gn_groups, gn_sums_zeroed
 CONV_TABLE = [
@@ -87,14 +91,12 @@ CONV_TABLE = [
     (16, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16
     (16, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
     (16, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 32, 32, 256, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
     (16, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
     (16, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16
     (16, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
     (16, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16
     (16, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
     (16, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 64, 64, 256, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 0, 1, 0, 0, 0),  # darcy_train_b32
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_train_b32
@@ -200,7 +202,6 @@ CONV_TABLE = [
     (32, 32, 32, 32, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_train_b32
     (32, 32, 32, 32, 32, 32, 128, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 32, 32, 32, 32, 32, 128, 3, 3, 1, 1, 0, 0, 1, 0, 0, 0),  # darcy_train_b32
-    (32, 32, 32, 32, 32, 32, 256, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 32, 32, 32, 64, 64, 32, 4, 4, 2, 1, 1, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 32, 32, 32, 64, 64, 32, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_train_b32
     (32, 32, 32, 64, 16, 16, 64, 4, 4, 2, 1, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
@@ -227,7 +228,6 @@ CONV_TABLE = [
     (32, 32, 32, 128, 64, 64, 128, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # mech_train_b32
     (32, 32, 32, 256, 16, 16, 256, 4, 4, 2, 1, 0, 0, 0, 0, 0, 0),  # mech_train_b32
     (32, 32, 32, 256, 16, 16, 256, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # mech_train_b32
-    (32, 32, 32, 256, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_train_b32
     (32, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_train_b32
     (32, 32, 32, 256, 32, 32, 128, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # mech_train_b32
     (32, 32, 32, 256, 32, 32, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # mech_train_b32
@@ -252,7 +252,6 @@ CONV_TABLE = [
     (32, 64, 64, 32, 64, 64, 64, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 64, 64, 32, 64, 64, 64, 3, 3, 1, 1, 0, 0, 1, 0, 0, 0),  # darcy_train_b32
     (32, 64, 64, 32, 64, 64, 128, 7, 7, 1, 3, 0, 1, 0, 0, 0, 0),  # mech_train_b32
-    (32, 64, 64, 32, 64, 64, 256, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_train_b32
     (32, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_train_b32
     (32, 64, 64, 128, 32, 32, 128, 4, 4, 2, 1, 0, 0, 0, 0, 0, 0),  # mech_train_b32
@@ -263,7 +262,6 @@ CONV_TABLE = [
     (32, 64, 64, 128, 64, 64, 256, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # mech_train_b32
     (32, 64, 64, 128, 64, 64, 256, 3, 3, 1, 1, 0, 0, 1, 0, 0, 0),  # mech_train_b32
     (32, 64, 64, 128, 64, 64, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # mech_train_b32
-    (32, 64, 64, 256, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_train_b32
     (32, 64, 64, 256, 64, 64, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # mech_train_b32
     (32, 64, 64, 256, 64, 64, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # mech_train_b32
     (32, 64, 64, 768, 64, 64, 128, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # mech_train_b32
@@ -299,14 +297,12 @@ CONV_TABLE = [
     (64, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b64
     (64, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b64
     (64, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b64
-    (64, 32, 32, 256, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b64
     (64, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b64
     (64, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b64
     (64, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b64
     (64, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0, 0, 0, 0),  # darcy_sample_b64
     (64, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b64
     (64, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b64
-    (64, 64, 64, 256, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b64
     (256, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b256
     (256, 8, 8, 128, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b256
     (256, 8, 8, 128, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b256
@@ -339,14 +335,12 @@ CONV_TABLE = [
     (256, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b256
     (256, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b256
     (256, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b256
-    (256, 32, 32, 256, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b256
     (256, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b256
     (256, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b256
     (256, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b256
     (256, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0, 0, 0, 0),  # darcy_sample_b256
     (256, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b256
     (256, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b256
-    (256, 64, 64, 256, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b256
 ]
 # wgrad: B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row, s_col
 WGRAD_TABLE = [
@@ -403,7 +397,6 @@ WGRAD_TABLE = [
     (32, 32, 32, 128, 128, 32, 32, 256, 3, 3, 1, 1, 9, 1152),  # mech_train_b32
     (32, 32, 32, 128, 128, 32, 32, 768, 1, 1, 1, 0, 1, 128),  # mech_train_b32
     (32, 32, 32, 256, 256, 16, 16, 256, 4, 4, 2, 1, 16, 4096),  # mech_train_b32
-    (32, 32, 32, 256, 256, 32, 32, 32, 1, 1, 1, 0, 1, 256),  # darcy_train_b32
     (32, 32, 32, 256, 256, 32, 32, 64, 1, 1, 1, 0, 1, 256),  # darcy_train_b32
     (32, 32, 32, 256, 256, 32, 32, 128, 1, 1, 1, 0, 1, 256),  # mech_train_b32
     (32, 32, 32, 256, 256, 32, 32, 256, 1, 1, 1, 0, 1, 256),  # mech_train_b32
@@ -420,24 +413,23 @@ WGRAD_TABLE = [
     (32, 64, 64, 128, 128, 32, 32, 128, 4, 4, 2, 1, 16, 2048),  # mech_train_b32
     (32, 64, 64, 128, 128, 64, 64, 128, 3, 3, 1, 1, 9, 1152),  # mech_train_b32
     (32, 64, 64, 128, 128, 64, 64, 768, 1, 1, 1, 0, 1, 128),  # mech_train_b32
-    (32, 64, 64, 256, 256, 64, 64, 32, 1, 1, 1, 0, 1, 256),  # darcy_train_b32
     (32, 64, 64, 256, 256, 64, 64, 128, 1, 1, 1, 0, 1, 256),  # mech_train_b32
     (32, 64, 64, 256, 256, 64, 64, 128, 3, 3, 1, 1, 9, 2304),  # mech_train_b32
 ]
-# fused linear attention: kernel, B, N, w_stride_n, w_stride_c
+# linear-attention block: kernel, B, N, qkv_stride_n, qkv_stride_c, out_stride_n, out_stride_c
 LAF_TABLE = [
-    ('bwd', 32, 1024, 0, 0),  # darcy_train_b32
-    ('bwd', 32, 4096, 0, 0),  # darcy_train_b32
-    ('fwd', 16, 1024, 0, 0),  # darcy_sample_b16
-    ('fwd', 16, 4096, 0, 0),  # darcy_sample_b16
-    ('fwd', 32, 1024, 0, 0),  # darcy_train_b32
-    ('fwd', 32, 4096, 0, 0),  # darcy_train_b32
-    ('fwd', 64, 1024, 0, 0),  # darcy_sample_b64
-    ('fwd', 64, 4096, 0, 0),  # darcy_sample_b64
-    ('fwd', 256, 1024, 0, 0),  # darcy_sample_b256
-    ('fwd', 256, 4096, 0, 0),  # darcy_sample_b256
-    ('wgrad', 32, 1024, 32, 1),  # darcy_train_b32
-    ('wgrad', 32, 4096, 32, 1),  # darcy_train_b32
+    ('bwd', 32, 1024, 0, 0, 0, 0),  # darcy_train_b32
+    ('bwd', 32, 4096, 0, 0, 0, 0),  # darcy_train_b32
+    ('fwd', 16, 1024, 0, 0, 0, 0),  # darcy_sample_b16
+    ('fwd', 16, 4096, 0, 0, 0, 0),  # darcy_sample_b16
+    ('fwd', 32, 1024, 0, 0, 0, 0),  # darcy_train_b32
+    ('fwd', 32, 4096, 0, 0, 0, 0),  # darcy_train_b32
+    ('fwd', 64, 1024, 0, 0, 0, 0),  # darcy_sample_b64
+    ('fwd', 64, 4096, 0, 0, 0, 0),  # darcy_sample_b64
+    ('fwd', 256, 1024, 0, 0, 0, 0),  # darcy_sample_b256
+    ('fwd', 256, 4096, 0, 0, 0, 0),  # darcy_sample_b256
+    ('wgrad', 32, 1024, 32, 1, 256, 1),  # darcy_train_b32
+    ('wgrad', 32, 4096, 32, 1, 256, 1),  # darcy_train_b32
 ]
 
 # rows no benchmarked step produces, for planner branches the workloads do not reach (see test_plan_coverage)
@@ -447,8 +439,8 @@ CONV_SYNTHETIC = [
 WGRAD_SYNTHETIC = [
 ]
 LAF_SYNTHETIC = [
-    ('fwd', 5, 4096, 0, 0), ('bwd', 5, 4096, 0, 0), ('wgrad', 5, 4096, 32, 1),
-    ('fwd', 24, 4096, 0, 0), ('bwd', 24, 4096, 0, 0), ('wgrad', 24, 4096, 32, 1),
+    ('fwd', 5, 4096, 0, 0, 0, 0), ('bwd', 5, 4096, 0, 0, 0, 0), ('wgrad', 5, 4096, 32, 1, 256, 1),
+    ('fwd', 24, 4096, 0, 0, 0, 0), ('bwd', 24, 4096, 0, 0, 0, 0), ('wgrad', 24, 4096, 32, 1, 256, 1),
 ]
 
 
@@ -464,15 +456,15 @@ def wgrad_id(k):
 
 
 def laf_id(k):
-    kind, B, N, sn, sc = k
-    return f'{kind}_B{B}_N{N}' + (f'_w{sn}.{sc}' if kind == 'wgrad' else '')
+    kind, B, N, sn, sc, osn, osc = k
+    return f'{kind}_B{B}_N{N}' + (f'_w{sn}.{sc}_o{osn}.{osc}' if kind == 'wgrad' else '')
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # census
 # ----------------------------------------------------------------------------------------------------------------------
-_NAMES = {'pidm_conv2d_tc_general': 'conv', 'pidm_conv2d_wgrad_tc': 'wgrad', 'pidm_linattn_fused_fwd': 'fwd',
-          'pidm_linattn_fused_bwd': 'bwd', 'pidm_linattn_fused_wgrad': 'wgrad_laf'}
+_NAMES = {'pidm_conv2d_tc_general': 'conv', 'pidm_conv2d_wgrad_tc': 'wgrad', 'pidm_linattn_block_fwd': 'fwd',
+          'pidm_linattn_block_bwd': 'bwd', 'pidm_linattn_block_wgrad': 'wgrad_laf'}
 
 
 def _key_of(name, a):
@@ -484,10 +476,10 @@ def _key_of(name, a):
     if kind == 'wgrad':
         return 'wgrad', tuple(int(v) for v in a[3:17])
     if kind == 'fwd':
-        return 'laf', ('fwd', int(a[7]), int(a[8]), 0, 0)
+        return 'laf', ('fwd', int(a[10]), int(a[11]), 0, 0, 0, 0)
     if kind == 'bwd':
-        return 'laf', ('bwd', int(a[8]), int(a[9]), 0, 0)
-    return 'laf', ('wgrad', int(a[8]), int(a[9]), int(a[10]), int(a[11]))
+        return 'laf', ('bwd', int(a[9]), int(a[10]), 0, 0, 0, 0)
+    return 'laf', ('wgrad', int(a[14]), int(a[15]), int(a[9]), int(a[10]), int(a[12]), int(a[13]))
 
 
 def _record(fn):
@@ -604,6 +596,18 @@ def test_census_is_covered_by_the_table():
                          '`python tests/test_gpu_launch_census.py --print-table`):\n' + '\n'.join(missing))
 
 
+def test_every_table_row_is_produced_by_the_census():
+    produced = {'conv': set(), 'wgrad': set(), 'laf': set()}
+    for keys in census().values():
+        for fam, k in keys:
+            produced[fam].add(k)
+    stale = [f'{fam} {k!r}' for fam, table in (('conv', CONV_TABLE), ('wgrad', WGRAD_TABLE), ('laf', LAF_TABLE))
+             for k in table if k not in produced[fam]]
+    assert not stale, ('table rows that no benchmarked step launches (drop them, or move a row kept for planner coverage '
+                       'to the synthetic rows; `python tests/test_gpu_launch_census.py --print-table`):\n'
+                       + '\n'.join(stale))
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # operands, references, predicates
 # ----------------------------------------------------------------------------------------------------------------------
@@ -656,7 +660,7 @@ def plan_wgrad(k):
 def plan_laf(B, N):
     from physicsinformeddiffusionmodels_b200._lib import call
     out = torch.zeros(5, dtype=torch.int32)
-    assert call('pidm_linattn_fused_plan', B, N, out.data_ptr()) == 0
+    assert call('pidm_linattn_block_plan', B, N, out.data_ptr()) == 0
     v = out.tolist()
     return dict(stat=v[0], ctx=v[1], fwd=v[2], bwd=v[3], wgrad=v[4])
 
@@ -796,103 +800,139 @@ class WgradCase:
         return dw, untouched_ok
 
 
-# ---- fused linear attention -------------------------------------------------------------------------------------------
-def _laf_ref(xn, w, dout, need_grad, chunk=8):
-    """fp64 autograd of qkv = xn W^T followed by the linear attention core (reference unet_model.py:275-297), computed
-    per group of samples; returns out [B,N,256], dxn [B,N,32], grad_w [768,32] (the latter two None without need_grad)"""
+# ---- linear-attention block -------------------------------------------------------------------------------------------
+def _ref(xn, wq, wo, bo, res, dy, need_grad, chunk=8):
+    """fp64: y = res + bo + attention(xn Wq^T) Wo^T (reference unet_model.py:275-297 and the Residual wrapper's `+ x`),
+    computed per group of samples, and with need_grad the gradients for the cotangent dy.
+    Returns y, dxn, dWq [768,32], dWo [32,256], db [32], and the attention output out [B,N,256]."""
     B, N, _ = xn.shape
-    outs, dxs = [], []
-    gw = torch.zeros(768, 32, dtype=torch.float64, device=DEV) if need_grad else None
+    ys, dxs, outs = [], [], []
+    gq = torch.zeros(768, 32, dtype=torch.float64, device=DEV)
+    go = torch.zeros(32, 256, dtype=torch.float64, device=DEV)
     for b0 in range(0, B, chunk):
         with torch.set_grad_enabled(need_grad):
             xr = xn[b0:b0 + chunk].double().requires_grad_(need_grad)
-            wr = w.double().requires_grad_(need_grad)
+            wqr = wq.double().requires_grad_(need_grad)
+            wor = wo.double().requires_grad_(need_grad)
             nb = xr.shape[0]
-            q, k, v = (xr @ wr.t()).view(nb, N, 3, 8, 32).permute(2, 0, 3, 4, 1)      # [nb, heads, 32, N]
+            q, k, v = (xr @ wqr.t()).view(nb, N, 3, 8, 32).permute(2, 0, 3, 4, 1)      # [nb, heads, 32, N]
             q = q.softmax(dim=-2) * 32 ** -0.5
             k = k.softmax(dim=-1)
             v = v / N
             ctx = torch.einsum('bhdn,bhen->bhde', k, v)
             out = torch.einsum('bhde,bhdn->bhen', ctx, q).permute(0, 3, 1, 2).reshape(nb, N, 256)
+            y = res[b0:b0 + chunk].double() + bo.double() + out @ wor.t()
             if need_grad:
-                (out * dout[b0:b0 + chunk].double()).sum().backward()
+                (y * dy[b0:b0 + chunk].double()).sum().backward()
                 dxs.append(xr.grad)
-                gw += wr.grad
+                gq += wqr.grad
+                go += wor.grad
+        ys.append(y.detach())
         outs.append(out.detach())
-    return torch.cat(outs), (torch.cat(dxs) if need_grad else None), gw
+    db = dy.double().sum(dim=(0, 1)) if need_grad else None
+    return (torch.cat(ys), torch.cat(dxs) if need_grad else None, gq, go, db, torch.cat(outs))
 
 
-def laf_out_bound(r):            # [B, N, 256]: slice = (sample, head)
-    B, N, _ = r.shape
-    rh = r.view(B, N, 8, 32)
-    rms = rh.pow(2).mean(dim=(1, 3), keepdim=True).sqrt()
-    return (A_ATT * rh.abs() + B_ATT['fwd'] * rms).view(B, N, 256)
+def y_bound(r):                       # [B, N, 32]: slice = sample
+    rms = r.pow(2).mean(dim=(1, 2), keepdim=True).sqrt()
+    return A_ATT * r.abs() + B_ATT['fwd'] * rms
 
 
-def laf_dx_bound(r):             # [B, N, 32]: slice = sample
+def dx_bound(r):                      # [B, N, 32]: slice = sample
     rms = r.pow(2).mean(dim=(1, 2), keepdim=True).sqrt()
     return A_ATT * r.abs() + B_ATT['bwd'] * rms
 
 
-def laf_gw_bound(r, prefill):    # [768, 32]: slice = the 32 rows of one (q/k/v, head)
+def gq_bound(r, prefill):             # [768, 32]: slice = the 32 rows of one (q | k | v, head)
     rh = r.view(24, 32, 32)
     rms = rh.pow(2).mean(dim=(1, 2), keepdim=True).sqrt()
-    return (A_ATT * rh.abs() + B_ATT['wgrad'] * rms).view(768, 32) + 2.0 ** -14 * prefill.abs()
+    return (A_ATT * rh.abs() + B_ATT['wgrad'] * rms).view(768, 32) + PREFILL * prefill.abs()
 
 
-class LafCase:
+def go_bound(r, prefill):             # [32, 256]: slice = one head's 32 columns
+    rh = r.view(32, 8, 32)
+    rms = rh.pow(2).mean(dim=(0, 2), keepdim=True).sqrt()
+    return (A_ATT * rh.abs() + B_ATT['wgrad'] * rms).view(32, 256) + PREFILL * prefill.abs()
+
+
+def db_bound(r, prefill):             # [32]: slice = the whole vector
+    return A_ATT * r.abs() + B_ATT['wgrad'] * r.pow(2).mean().sqrt() + PREFILL * prefill.abs()
+
+
+class BlockCase:
+    """operands + fp64 reference of one attention row: a fwd row checks y, a bwd row dxn, a wgrad row dW_qkv, dW_out and
+    the bias gradient"""
+
     def __init__(self, k):
-        kind, B, N, sn, sc = k
+        kind, B, N = k[:3]
         self.k = k
-        g = _gen(('laf', B, N))                             # same operands for the fwd / bwd / wgrad rows of a shape
+        g = _gen(('linattn-block', B, N))                   # same operands for the fwd / bwd / wgrad rows of a shape
         self.xn = _randn(g, B, N, 32)
-        self.w = _randn(g, 768, 32, scale=1.5 / math.sqrt(32))
-        self.dout = _randn(g, B, N, 256)
-        self.out_r, self.dx_r, self.gw_r = _laf_ref(self.xn, self.w, self.dout, kind != 'fwd')
+        self.wq = _randn(g, 768, 32, scale=1.5 / math.sqrt(32))
+        self.wo = _randn(g, 32, 256, scale=1.0 / math.sqrt(256))
+        # the attention term of y is ~1/N of its inputs (v / N): residual and bias at its rms
+        _, _, _, _, _, out = _ref(self.xn[:1], self.wq, self.wo, torch.zeros(32, device=DEV),
+                                  torch.zeros(1, N, 32, device=DEV), None, False)
+        s = (out @ self.wo.double().t()).pow(2).mean().sqrt().item()
+        self.res = _randn(g, B, N, 32, scale=s)
+        self.bo = _randn(g, 32, scale=s, dtype=torch.float32).bfloat16().float()
+        self.dy = _randn(g, B, N, 32)
+        self.y_r, self.dx_r, self.gq_r, self.go_r, self.db_r, self.out_r = _ref(
+            self.xn, self.wq, self.wo, self.bo, self.res, self.dy, kind != 'fwd')
 
     def run(self):
-        """launches fwd (and bwd / wgrad as the row asks); returns the checked output and whether the guards held"""
+        """launches fwd (and bwd / wgrad as the row asks); returns {output: worst |err| / bound} and whether every
+        element outside the outputs (guard regions, the rest of the gradient buffer) survived"""
         from physicsinformeddiffusionmodels_b200._lib import call, stream
-        kind, B, N, sn, sc = self.k
+        kind, B, N, sn, sc, osn, osc = self.k
         ctx = torch.empty(B, 8, 32, 32, device=DEV)
         kmax, kzinv = torch.empty(B, 8, 32, device=DEV), torch.empty(B, 8, 32, device=DEV)
-        ws = torch.empty(call('pidm_linattn_fused_workspace_floats', B, N), device=DEV)
-        n = B * N * 256
-        buf, out, guard = _guarded(n, GUARD_BF16)
-        call('pidm_linattn_fused_fwd', self.xn, self.w, out, ctx, kmax, kzinv, ws, B, N, stream())
+        ws = torch.empty(call('pidm_linattn_block_workspace_floats', B, N), device=DEV)
+        n = B * N * 32
+        buf, y, guard = _guarded(n, GUARD_BF16)
+        call('pidm_linattn_block_fwd', self.xn, self.wq, self.wo, self.bo, self.res, y, ctx, kmax, kzinv, ws, B, N,
+             stream())
         if kind == 'fwd':
             torch.cuda.synchronize()
-            return out.view(B, N, 256), _guards_intact(buf, guard, n, GUARD_BF16)
-        n = B * N * 32
+            return {'y': self.y_ratio(y.view(B, N, 32))}, _guards_intact(buf, guard, n, GUARD_BF16)
         buf, dx, guard = _guarded(n, GUARD_BF16)
         dctx = torch.empty_like(ctx)
-        call('pidm_linattn_fused_bwd', self.xn, self.w, self.dout, ctx, kmax, kzinv, dx, dctx, B, N, stream())
+        call('pidm_linattn_block_bwd', self.xn, self.wq, self.wo, self.dy, ctx, kmax, kzinv, dx, dctx, B, N, stream())
         if kind == 'bwd':
             torch.cuda.synchronize()
-            return dx.view(B, N, 32), _guards_intact(buf, guard, n, GUARD_BF16)
-        # grad_w: a strided view into a prefilled buffer (the flat gradient buffer of the engine), accumulated into
-        g = _gen(('laf-gw', B, N))
-        span = 767 * sn + 31 * sc + 1
+            r = _ratio((dx.view(B, N, 32).double() - self.dx_r).abs(), dx_bound(self.dx_r))
+            return {'dxn': r}, _guards_intact(buf, guard, n, GUARD_BF16)
+        # both weight gradients accumulate into strided views of one prefilled flat buffer (as the engine's flat
+        # gradient buffer), and pidm_colsum the bias gradient into the same buffer
+        g = _gen(('linattn-block-gw', B, N))
         guard = 1024
-        gbuf = torch.randn(span + 2 * guard, generator=g, device=DEV)
+        nq, no = 767 * sn + 31 * sc + 1, 31 * osn + 255 * osc + 1
+        oq, oo, ob = guard, 2 * guard + nq, 3 * guard + nq + no
+        gbuf = torch.randn(ob + 32 + guard, generator=g, device=DEV)
         keep = gbuf.clone()
-        gview = torch.as_strided(gbuf, (768, 32), (sn, sc), guard)
-        call('pidm_linattn_fused_wgrad', self.xn, self.w, self.dout, ctx, dctx, kmax, kzinv, gview, B, N, sn, sc,
-             stream())
+
+        def views(t):
+            return (torch.as_strided(t, (768, 32), (sn, sc), oq), torch.as_strided(t, (32, 256), (osn, osc), oo),
+                    t[ob:ob + 32])
+        gq, go, gb = views(gbuf)
+        call('pidm_linattn_block_wgrad', self.xn, self.wq, self.wo, self.dy, ctx, dctx, kmax, kzinv, gq, sn, sc, go, osn,
+             osc, B, N, stream())
+        call('pidm_colsum', self.dy, gb, B * N, 32, 1, stream())
         torch.cuda.synchronize()
         touched = torch.zeros_like(gbuf, dtype=torch.bool)
-        torch.as_strided(touched, (768, 32), (sn, sc), guard).fill_(True)
+        for v in views(touched):
+            v.fill_(True)
         ok = bool((gbuf[~touched] == keep[~touched]).all())
-        self.gw_prefill = torch.as_strided(keep, (768, 32), (sn, sc), guard).double()
-        return gview.double() - self.gw_prefill, ok
+        pq, po, pb = (v.double() for v in views(keep))
+        return {'dWqkv': _ratio((gq.double() - pq - self.gq_r).abs(), gq_bound(self.gq_r, pq)),
+                'dWout': self.go_ratio(go.double() - po, po),
+                'db': _ratio((gb.double() - pb - self.db_r).abs(), db_bound(self.db_r, pb))}, ok
 
-    def ratio(self, y):
-        kind = self.k[0]
-        if kind == 'fwd':
-            return _ratio((y.double() - self.out_r).abs(), laf_out_bound(self.out_r))
-        if kind == 'bwd':
-            return _ratio((y.double() - self.dx_r).abs(), laf_dx_bound(self.dx_r))
-        return _ratio((y.double() - self.gw_r).abs(), laf_gw_bound(self.gw_r, self.gw_prefill))
+    def y_ratio(self, y):
+        return _ratio((y.double() - self.y_r).abs(), y_bound(self.y_r))
+
+    def go_ratio(self, go, prefill):
+        return _ratio((go.double() - self.go_r).abs(), go_bound(self.go_r, prefill))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -945,13 +985,12 @@ def test_wgrad_replay(k):
 
 
 @pytest.mark.parametrize('k', LAF_ROWS, ids=[laf_id(k) for k in LAF_ROWS])
-def test_fused_attention_replay(k):
-    c = LafCase(k)
-    y, ok = c.run()
-    assert ok, f'{laf_id(k)}: a store landed outside the output'
-    r = c.ratio(y)
-    _note('laf_' + k[0], r)
-    assert r <= 1.0, f'{laf_id(k)}: worst |err| / bound = {r:.3g} (plan {plan_laf(k[1], k[2])})'
+def test_attention_block_replay(k):
+    ratios, ok = BlockCase(k).run()
+    assert ok, f'{laf_id(k)}: a store landed outside the outputs'
+    for name, r in ratios.items():
+        _note('laf_' + name, r)
+    assert max(ratios.values()) <= 1.0, f'{laf_id(k)}: worst |err| / bound = {ratios} (plan {plan_laf(k[1], k[2])})'
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -1042,16 +1081,39 @@ def test_mutant_wgrad_split_partial_missing():
         assert c.ratio(mut.float()) > 1.0, (wgrad_id(k), p)
 
 
-def test_mutant_fused_attention_last_chunk_from_previous_chunk():
-    k = _row(lambda k: k[0] == 'fwd' and k[2] % plan_laf(k[1], k[2])['fwd'] != 0, LAF_ROWS)
-    c = LafCase(k)
+def _ragged_fwd_row():
+    return _row(lambda k: k[0] == 'fwd' and k[2] % plan_laf(k[1], k[2])['fwd'] != 0, LAF_ROWS)
+
+
+def test_mutant_attention_block_last_chunk_from_previous_chunk():
+    k = _ragged_fwd_row()
+    c = BlockCase(k)
     N, px = k[2], plan_laf(k[1], k[2])['fwd']
     last = (N - 1) // px * px
     L = N - last
-    y = c.out_r.clone()
-    y[:, last:] = c.out_r[:, last - px:last - px + L]
-    assert c.ratio(_bf16(c.out_r)) <= 1.0
-    assert c.ratio(_bf16(y)) > 1.0, laf_id(k)
+    y = c.y_r.clone()
+    y[:, last:] = c.y_r[:, last - px:last - px + L]
+    assert c.y_ratio(_bf16(c.y_r)) <= 1.0
+    assert c.y_ratio(_bf16(y)) > 1.0, laf_id(k)
+
+
+def test_mutant_attention_block_term_missing():
+    """one head's partial, the bias or the residual missing from y"""
+    k = _ragged_fwd_row()
+    c = BlockCase(k)
+    head = c.out_r[..., 3 * 32:4 * 32] @ c.wo.double()[:, 3 * 32:4 * 32].t()
+    for name, term in (('one head partial', head), ('bias', c.bo.double()), ('residual', c.res.double())):
+        assert c.y_ratio(_bf16(c.y_r - term)) > 1.0, (laf_id(k), name)
+
+
+def test_mutant_attention_block_dw_out_head_transposed():
+    k = _row(lambda k: k[0] == 'wgrad', LAF_ROWS)
+    c = BlockCase(k)
+    zero = torch.zeros(32, 256, dtype=torch.float64, device=DEV)
+    assert c.go_ratio(c.go_r.float(), zero) <= 1.0
+    go = c.go_r.clone()
+    go[:, 32 * 5:32 * 6] = c.go_r[:, 32 * 5:32 * 6].t()
+    assert c.go_ratio(go.float(), zero) > 1.0, laf_id(k)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -1095,13 +1157,17 @@ def laf_coverage():
 
 
 def test_plan_coverage():
-    cv, wg, la = conv_coverage(), wgrad_coverage(), laf_coverage()
+    cv, wg = conv_coverage(), wgrad_coverage()
     assert cv['BN x BK'] == TC_CASES, cv
     assert cv['row-group'] == {0, 1} and cv['resident'] == {0, 1} and cv['transposed'] == {0, 1}, cv
     assert cv['ragged persistent wave'] and cv['odd B with TN=2'], cv
     assert wg['generic NP x AA x AB'] == WG_CASES, wg
     assert wg['wgrad3 NP x AB'] == W3_CASES and wg['wgrad3 row-group'] == {0, 1}, wg
     assert wg['short last split'] and wg['CA_real < CA'], wg
+
+
+def test_attention_block_plan_coverage():
+    la = laf_coverage()
     assert all(la.values()), la
 
 

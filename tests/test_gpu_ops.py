@@ -302,40 +302,57 @@ def test_linear_attention(pk, H, dtype, tol):
     assert rel(nchw(qd.grad), qr.grad) < 2 * tol
 
 
-@pytest.mark.parametrize('B,H', [(2, 64), (3, 16), (1, 32)])
-def test_linear_attention_fused_with_qkv_projection(pk, B, H):
-    """to_qkv 1x1 projection + linear attention in one op (qkv recomputed per head from the 32-channel input, never
-    written) vs an fp32 torch reference of conv + attention on bf16-representable operands, and vs the unfused
-    libpidm path (conv2d + linear_attention).  bf16 activations: 3e-2 like the other bf16 attention tests; the two
-    libpidm paths differ only by the bf16 rounding of the (never materialised) q, k, v: 1e-2 / 2e-2."""
+@pytest.mark.parametrize('B,H', [(2, 64), (3, 16), (1, 32), (4, 64), (3, 32)])
+def test_block_op_matches_unfused_composition(pk, B, H):
+    """The linear-attention block op (to_qkv 1x1, linear attention, to_out 1x1 with bias and the residual add in one op;
+    neither qkv nor the attention output is written) vs an fp32 torch reference on bf16-representable operands, and vs
+    the unfused libpidm composition conv2d(to_qkv) -> linear_attention -> conv2d(to_out, bias, residual=x).  The
+    residual and the bias are scaled to the rms of the attention term, so that all three terms of y count.  bf16
+    activations: 3e-2 on y and 6e-2 on the gradients against fp32, like the other bf16 attention tests; the two libpidm
+    compositions differ by the bf16 rounding of q, k, v, the attention output and its gradient, which only the unfused
+    one materialises: 1e-2 / 2e-2.  The per-element bounds of every launch the benchmark runs are checked against fp64
+    in test_gpu_launch_census.py."""
     ops, packing = pk
     ops.set_precision('bf16')
+    ops.set_tensor_core_conv(True)
     g = torch.Generator().manual_seed(66)
     heads, C = 8, 32
-    x = (torch.randn(B, C, H, H, generator=g)).bfloat16().float()
-    w = (torch.randn(3 * heads * 32, C, 1, 1, 1, generator=g) * (1.5 / math.sqrt(C))).bfloat16().float()
-    xr, wr = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
-    yr = _linattn_ref(F.conv2d(xr, wr[:, :, 0]), heads)
-    cot = torch.randn(yr.shape, generator=g)
-    (yr * cot).sum().backward()
+    bf = lambda t: t.bfloat16().float()
+    xn = bf(torch.randn(B, C, H, H, generator=g))
+    wq = bf(torch.randn(3 * heads * 32, C, 1, 1, 1, generator=g) * (1.5 / math.sqrt(C)))
+    wo = bf(torch.randn(C, heads * 32, 1, 1, 1, generator=g) / math.sqrt(heads * 32))
+    s = F.conv2d(_linattn_ref(F.conv2d(xn, wq[:, :, 0]), heads), wo[:, :, 0]).pow(2).mean().sqrt().item()
+    x = bf(torch.randn(B, C, H, H, generator=g) * s)
+    bo = torch.randn(C, generator=g) * s
+    dy = bf(torch.randn(B, C, H, H, generator=g))
+    ref = [t.clone().requires_grad_(True) for t in (xn, x, wq, wo, bo)]
+    xnr, xr, wqr, wor, bor = ref
+    yr = xr + F.conv2d(_linattn_ref(F.conv2d(xnr, wqr[:, :, 0]), heads), wor[:, :, 0], bor)
+    (yr * dy).sum().backward()
+    ref = [yr.detach()] + [t.grad for t in ref]
 
-    def run(fused):
-        wd = torch.nn.Parameter(w.to(DEV))
-        spec = packing.ConvSpec(wd, 'conv', 1, 1, 1, 0)
-        pkr = packing.WeightPacker(); pkr.add(spec); pkr.refresh(torch.bfloat16)
+    def run(block):
+        wqd, wod, bod = (torch.nn.Parameter(t.to(DEV)) for t in (wq, wo, bo))
+        sq, so = packing.ConvSpec(wqd, 'conv', 1, 1, 1, 0), packing.ConvSpec(wod, 'conv', 1, 1, 1, 0)
+        pkr = packing.WeightPacker(); pkr.add(sq); pkr.add(so); pkr.refresh(torch.bfloat16)
+        xnd = nhwc(xn, torch.bfloat16).to(DEV).requires_grad_(True)
         xd = nhwc(x, torch.bfloat16).to(DEV).requires_grad_(True)
-        if fused:
-            assert ops.linear_attention_fused_supported(xd, spec, heads)
-            y = ops.linear_attention_fused(xd, wd, spec, heads)
+        if block:
+            assert ops.linear_attention_block_supported(xnd, sq, so, bod, heads)
+            y = ops.linear_attention_block(xnd, wqd, sq, wod, bod, so, xd, heads)
         else:
-            y = ops.linear_attention(ops.conv2d(xd, wd, None, spec), heads)
-        y.backward(nhwc(cot, torch.bfloat16).to(DEV))
-        return nchw(y), nchw(xd.grad), wd.grad.float().cpu()
-    yf, dxf, dwf = run(True)
-    yu, dxu, dwu = run(False)
-    assert rel(yf, yr) < 3e-2 and rel(dxf, xr.grad) < 6e-2 and rel(dwf, wr.grad) < 6e-2, \
-        (rel(yf, yr), rel(dxf, xr.grad), rel(dwf, wr.grad))
-    assert rel(yf, yu) < 1e-2 and rel(dxf, dxu) < 2e-2 and rel(dwf, dwu) < 2e-2, (rel(yf, yu), rel(dxf, dxu), rel(dwf, dwu))
+            y = ops.conv2d(ops.linear_attention(ops.conv2d(xnd, wqd, None, sq), heads), wod, bod, so, residual=xd)
+        y.backward(nhwc(dy, torch.bfloat16).to(DEV))
+        torch.cuda.synchronize()
+        return [nchw(y), nchw(xnd.grad), nchw(xd.grad), wqd.grad.float().cpu(), wod.grad.float().cpu(),
+                bod.grad.float().cpu()]
+    got, unf = run(True), run(False)
+    names = ('y', 'dxn', 'dx', 'dWqkv', 'dWout', 'db')
+    for name, a, u, r in zip(names, got, unf, ref):
+        tol_ref, tol_unf = (3e-2, 1e-2) if name == 'y' else (6e-2, 2e-2)
+        print(f'[block] B={B} H={H} {name}: rel vs fp32 {rel(a, r):.3g}, vs unfused {rel(a, u):.3g}')
+        assert rel(a, r) < tol_ref and rel(a, u) < tol_unf, (name, rel(a, r), rel(a, u))
+    assert torch.equal(got[2].cpu(), dy), 'the residual gradient is dy'
 
 
 @pytest.mark.parametrize('dtype,tol', DTYPES)
