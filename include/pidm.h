@@ -88,15 +88,27 @@ int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, const float
  * the 12288 x 4096 Jacobian per sample with vmap(jacfwd). */
 int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int B, int pixels, float domain_length, int reverse_d1,
                             int flags, void* stream);
+/* Residual-gradient guidance (src/residuals_darcy.py:116-120): cond = d (sum|r(x_t)|) / n_norm / d x_t, the residual
+ * evaluated on x_t [B,2,P,P] itself, written in the b_xy_c layout [B,P*P,2] fp32 the network takes.  sign(0) = 0.  n_norm
+ * is the count the mean divides by: B*P*P*3, or world*B*P*P*3 for a shard of a global batch. */
+int pidm_darcy_abs_residual_grad(const float* x_t, const float* f_s, float* cond, int B, long long n_norm, int pixels,
+                                 float domain_length, int reverse_d1, int flags, void* stream);
 
 /* ---- layout ------------------------------------------------------------------------------------------- */
 /* image_to_b_xy_c / b_xy_c_to_image (src/denoising_utils.py:36-55) fused with the dtype change + channel padding */
 int pidm_nchw_to_nhwc(const float* src, void* dst, int B, int C, int HW, int Cpad, int dtype, void* stream);
 int pidm_nhwc_to_nchw(const void* src, float* dst, int B, int C, int HW, int Cpad, int dtype, void* stream);
 int pidm_add(const void* a, const void* b, void* out, long long n, int dtype, void* stream);
-/* exact (erf) GELU on activations, n % 8 == 0: emb_conv of the residual-gradient guidance branch (src/unet_model.py:520-524) */
-int pidm_gelu_fwd(const void* x, void* y, long long n, int dtype, void* stream);
-int pidm_gelu_bwd(const void* x, const void* dy, void* dx, long long n, int dtype, void* stream);
+/* emb_conv[0] + GELU of the residual-gradient guidance branch (src/unet_model.py:520-524,585-603):
+ * out[b,hw,:] = GELU_erf(W0 cond[b,hw,:] + b0) as NHWC activations [B,HW,C] (dtype), cond [B,HW,2] fp32, W0 [C,2], b0 [C]
+ * fp32.  null_mask [B] (bool bytes, may be NULL = none): those samples take cond = 0 (cond is not read), i.e. GELU(b0).
+ * C % 8 == 0 and C / 8 divides 32. */
+int pidm_cond_embed_fwd(const float* cond, const unsigned char* null_mask, const float* w0, const float* b0, void* out,
+                        int B, int HW, int C, int dtype, void* stream);
+/* its weight gradient from dg = d loss / d out [B,HW,C] (dtype): the pre-activation is recomputed;
+ * dW0 [C,2] += sum dz * cond, db0 [C] += sum dz (fp32, accumulated: block partials + global reductions) */
+int pidm_cond_embed_wgrad(const float* cond, const unsigned char* null_mask, const float* w0, const float* b0,
+                          const void* dg, float* dw0, float* db0, int B, int HW, int C, int dtype, void* stream);
 /* torch.cat((x, skip), dim=1) on NHWC rows and its backward (src/unet_model.py:606,612) */
 int pidm_concat_channels(const void* a, const void* b, void* out, long long rows, int Ca, int Cb, int dtype, void* stream);
 int pidm_split_channels(const void* g, void* ga, void* gb, long long rows, int Ca, int Cb, int dtype, void* stream);

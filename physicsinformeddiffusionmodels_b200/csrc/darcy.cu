@@ -307,15 +307,21 @@ __device__ __forceinline__ void residual_quad_full(const float* sp, const float*
     }
 }
 
+// sign(x) * s for s > 0, with sign(0) = 0
+__device__ __forceinline__ float scaled_sign(float x, float s) { return x > 0.f ? s : (x < 0.f ? -s : 0.f); }
+
 // MODE 1: generic backward (cotangent tensor given).  MODE 2: fused PIDM loss (data MSE + residual NLL sums, |r| sum)
-// and its gradient w.r.t. x0_hat / model_out in one pass.  PER: periodic stencils; the BC seeds still enter U0 / U1 on
-// rows 0 / P-1 and columns 0 / P-1.
+// and its gradient w.r.t. x0_hat / model_out in one pass.  MODE 3: gradient of sum|r| / n_norm (the cotangent sign(r) *
+// inv_norm is formed in registers), written in the b_xy_c layout [B,P*P,2] (residual-gradient guidance).  PER: periodic
+// stencils; the BC seeds still enter U0 / U1 on rows 0 / P-1 and columns 0 / P-1.
+// MODE 3 declares one resident CTA per SM (what its 145 KB of shared memory allows anyway): without it ptxas squeezes
+// that instantiation into 64 registers and spills.  0 leaves MODE 1 / 2 exactly as they were compiled before.
 template <int MODE, bool PER>
-__global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
+__global__ void __launch_bounds__(DG_THREADS, MODE == 3 ? 1 : 0) darcy_grad_kernel(
     const float* __restrict__ x0hat,      // [B,2,P,P]
     const float* __restrict__ fs,         // [P*P]
     const float* __restrict__ cot,        // MODE 1: [B,P*P,3]
-    float* __restrict__ grad_x0hat,       // [B,2,P,P]  (may be null in MODE 2 = loss only)
+    float* __restrict__ grad_x0hat,       // [B,2,P,P] (may be null in MODE 2 = loss only); MODE 3: [B,P*P,2]
     const float* __restrict__ target,     // MODE 2: x0 [B,2,P,P]
     const float* __restrict__ model_out,  // MODE 2: [B,2,P,P] (data-loss operand; == x0hat in mean mode)
     float* __restrict__ grad_model_out,   // MODE 2: gradient of data term (== grad_x0hat when same tensor)
@@ -323,7 +329,8 @@ __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
     const float* __restrict__ p2w,        // MODE 2: p2_loss_weight table
     const float* __restrict__ pvar,       // MODE 2: posterior_variance_clipped table
     float c_data, float c_res, float* __restrict__ sums,  // MODE 2: sums[0]=data loss, [1]=residual loss, [2]=mean|r|
-    int B, DarcyGeom geom) {
+    int B, DarcyGeom geom,
+    float inv_norm) {                     // MODE 3: 1 / n_norm
     extern __shared__ __align__(128) unsigned char smem_raw[];
     DarcyGradSmem& S = *reinterpret_cast<DarcyGradSmem*>(smem_raw);
     const int tid = threadIdx.x;
@@ -379,6 +386,11 @@ __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
                 ge[0] = c0.x; g0[0] = c0.y; g1[0] = c0.z; ge[1] = c0.w;
                 g0[1] = c1.x; g1[1] = c1.y; ge[2] = c1.z; g0[2] = c1.w;
                 g1[2] = c2.x; ge[3] = c2.y; g0[3] = c2.z; g1[3] = c2.w;
+            } else if (MODE == 3) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    ge[k] = scaled_sign(req[k], inv_norm); g0[k] = scaled_sign(rb0[k], inv_norm); g1[k] = scaled_sign(rb1[k], inv_norm);
+                }
             } else {
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
@@ -457,7 +469,11 @@ __global__ void __launch_bounds__(DG_THREADS) darcy_grad_kernel(
                     }
                 }
             }
-            if (want_grad) {
+            if (MODE == 3) {                // (p, K) interleaved per pixel: 32 contiguous bytes per thread
+                float4* o = reinterpret_cast<float4*>(grad_x0hat + ((size_t)b * PP + i * P + j0) * 2);
+                o[0] = make_float4(dp[0], dk[0], dp[1], dk[1]);
+                o[1] = make_float4(dp[2], dk[2], dp[3], dk[3]);
+            } else if (want_grad) {
                 const size_t off = (size_t)b * 2 * PP + i * P + j0;
                 *reinterpret_cast<float4*>(grad_x0hat + off) = make_float4(dp[0], dp[1], dp[2], dp[3]);
                 *reinterpret_cast<float4*>(grad_x0hat + off + PP) = make_float4(dk[0], dk[1], dk[2], dk[3]);
@@ -651,7 +667,7 @@ template <int MODE, bool PER>
 static int launch_darcy_grad(const float* x0hat, const float* fs, const float* cot, float* grad_x0hat, const float* target,
                              const float* model_out, float* grad_model_out, const long long* t, const float* p2w,
                              const float* pvar, float c_data, float c_res, float* sums, int B, int pixels,
-                             float domain_length, int reverse_d1, int flags, cudaStream_t stream) {
+                             float domain_length, int reverse_d1, int flags, cudaStream_t stream, float inv_norm = 0.f) {
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
     int sm_count;
@@ -667,7 +683,7 @@ static int launch_darcy_grad(const float* x0hat, const float* fs, const float* c
     if (grid > B) grid = B;
     PIDM_CUDA(launch_pdl(darcy_grad_kernel<MODE, PER>, dim3(grid), dim3(DG_THREADS), (size_t)(smem), stream, x0hat, fs,
                          cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
-                         make_geom(domain_length, reverse_d1, flags)));
+                         make_geom(domain_length, reverse_d1, flags), inv_norm));
     PIDM_LAUNCH_CHECK("darcy_grad_kernel");
     return 0;
 }
@@ -676,10 +692,11 @@ template <int MODE>
 static int launch_darcy_grad_any(const float* x0hat, const float* fs, const float* cot, float* grad_x0hat,
                                  const float* target, const float* model_out, float* grad_model_out, const long long* t,
                                  const float* p2w, const float* pvar, float c_data, float c_res, float* sums, int B,
-                                 int pixels, float domain_length, int reverse_d1, int flags, cudaStream_t stream) {
+                                 int pixels, float domain_length, int reverse_d1, int flags, cudaStream_t stream,
+                                 float inv_norm = 0.f) {
     auto launch = (flags & PIDM_DARCY_PERIODIC) ? launch_darcy_grad<MODE, true> : launch_darcy_grad<MODE, false>;
     return launch(x0hat, fs, cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
-                  pixels, domain_length, reverse_d1, flags, stream);
+                  pixels, domain_length, reverse_d1, flags, stream, inv_norm);
 }
 
 }  // namespace pidm
@@ -727,6 +744,19 @@ extern "C" int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, 
     return launch_darcy_grad_any<2>(x0hat, f_s, nullptr, grad_x0hat, target, model_out, grad_model_out, t, p2_loss_weight,
                                     posterior_var_clipped, c_data, c_residual, sums3, B, pixels, domain_length, reverse_d1,
                                     flags, (cudaStream_t)stream);
+}
+
+extern "C" int pidm_darcy_abs_residual_grad(const float* x_t, const float* f_s, float* cond, int B, long long n_norm,
+                                            int pixels, float domain_length, int reverse_d1, int flags, void* stream) {
+    if (int e = check_flags(flags)) return e;
+    PIDM_REQUIRE(cond != nullptr, "darcy_abs_residual_grad: cond must not be NULL");
+    PIDM_REQUIRE(n_norm >= (long long)B * pixels * pixels * 3 && (long long)(float)n_norm == n_norm,
+                 "darcy_abs_residual_grad: n_norm = %lld must be at least B*P*P*3 and exact in fp32", n_norm);
+    // the reference's mean backward: a float 1 / numel (exact numel), times sign(r)
+    const float inv_norm = 1.f / (float)n_norm;
+    return launch_darcy_grad_any<3>(x_t, f_s, nullptr, cond, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f,
+                                    0.f, nullptr, B, pixels, domain_length, reverse_d1, flags, (cudaStream_t)stream,
+                                    inv_norm);
 }
 
 /* max_dr_dp[b] = largest entry of the Jacobian d residual / d p of sample b (CoCoGen step size, residuals_darcy.py:218-231) */

@@ -278,23 +278,86 @@ __global__ void ddim_coefs_kernel(const long long* __restrict__ t, const long lo
     coef_x[b] = c * (sra[tt] - c2[tt]) / nmc[tt];
 }
 
-// ---- GELU (exact erf form, nn.GELU()) on activations: the residual-gradient embedding emb_conv of the guidance branch
-//      (reference unet_model.py:520-524).  n8 = number of 8-element vectors.
-template <typename T, bool BWD>
-__global__ void gelu_kernel(const T* __restrict__ x, const T* __restrict__ dy, T* __restrict__ out, long long n8) {
+// ---- residual-gradient guidance embedding: emb_conv[0] (1x1, 2 -> C) + GELU (exact erf form, nn.GELU()) ---------------
+//      (reference unet_model.py:520-524,585-603).  The 2-channel 1x1 convolution is two FMAs per output channel, so it is
+//      evaluated from the fp32 cond [B,HW,2] directly instead of as a channel-padded GEMM.  Thread layout: (pixel row,
+//      channel octet); a thread writes 8 channels of one pixel (16 bytes in bf16).  Samples in null_mask take cond = 0:
+//      their pre-activation is b0 exactly.
+__device__ __forceinline__ float gelu_erf_f(float z) { return z * 0.5f * (1.f + erff(z * 0.70710678118654752f)); }
+__device__ __forceinline__ float gelu_erf_grad_f(float z) {
+    return 0.5f * (1.f + erff(z * 0.70710678118654752f)) + z * 0.3989422804014327f * expf(-0.5f * z * z);
+}
+
+__device__ __forceinline__ float2 cond_at(const float* __restrict__ cond, const unsigned char* __restrict__ null_mask,
+                                          int m, int HW) {
+    if (null_mask != nullptr && null_mask[m / HW]) return make_float2(0.f, 0.f);
+    return reinterpret_cast<const float2*>(cond)[m];
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) cond_embed_fwd_kernel(const float* __restrict__ cond,
+                                                             const unsigned char* __restrict__ null_mask,
+                                                             const float* __restrict__ w0, const float* __restrict__ b0,
+                                                             T* __restrict__ out, int HW, int C, int M) {
     pdl_trigger();
+    const int oct = C >> 3;
+    const int rows = blockDim.x / oct;
+    const int c0 = (threadIdx.x % oct) * 8;
+    float wa[8], wb[8], bb[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { wa[k] = w0[2 * (c0 + k)]; wb[k] = w0[2 * (c0 + k) + 1]; bb[k] = b0[c0 + k]; }
     pdl_wait();
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
-        float v[8], d[8];
-        ld8(x + i * 8, v);
-        if (BWD) ld8(dy + i * 8, d);
+    for (int m = blockIdx.x * rows + threadIdx.x / oct; m < M; m += gridDim.x * rows) {
+        const float2 x = cond_at(cond, null_mask, m, HW);
+        float v[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = gelu_erf_f(fmaf(wb[k], x.y, fmaf(wa[k], x.x, bb[k])));
+        st8(out + (size_t)m * C + c0, v);
+    }
+}
+
+// dz = dg * GELU'(z) with z recomputed; per-thread sums over its pixels, lanes of the same octet reduced by shuffles, the
+// warps of a block through shared memory, then one global reduction per (block, output value).
+template <typename T>
+__global__ void __launch_bounds__(256) cond_embed_wgrad_kernel(const float* __restrict__ cond,
+                                                               const unsigned char* __restrict__ null_mask,
+                                                               const float* __restrict__ w0, const float* __restrict__ b0,
+                                                               const T* __restrict__ dg, float* __restrict__ dw0,
+                                                               float* __restrict__ db0, int HW, int C, int M) {
+    pdl_trigger();
+    __shared__ float red[3 * 256];                     // [C][3]: dW0[c,0], dW0[c,1], db0[c]
+    const int oct = C >> 3;
+    const int rows = blockDim.x / oct;
+    const int c0 = (threadIdx.x % oct) * 8;
+    for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) red[i] = 0.f;
+    float wa[8], wb[8], bb[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { wa[k] = w0[2 * (c0 + k)]; wb[k] = w0[2 * (c0 + k) + 1]; bb[k] = b0[c0 + k]; }
+    float acc[24];
+#pragma unroll
+    for (int k = 0; k < 24; ++k) acc[k] = 0.f;
+    pdl_wait();
+    for (int m = blockIdx.x * rows + threadIdx.x / oct; m < M; m += gridDim.x * rows) {
+        const float2 x = cond_at(cond, null_mask, m, HW);
+        float d[8];
+        ld8(dg + (size_t)m * C + c0, d);
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
-            const float cdf = 0.5f * (1.f + erff(v[k] * 0.70710678118654752f));
-            if (BWD) v[k] = d[k] * (cdf + v[k] * 0.3989422804014327f * expf(-0.5f * v[k] * v[k]));
-            else v[k] = v[k] * cdf;
+            const float dz = d[k] * gelu_erf_grad_f(fmaf(wb[k], x.y, fmaf(wa[k], x.x, bb[k])));
+            acc[3 * k] += dz * x.x;
+            acc[3 * k + 1] += dz * x.y;
+            acc[3 * k + 2] += dz;
         }
-        st8(out + i * 8, v);
+    }
+    __syncthreads();                                   // red[] is zeroed
+    if (reduce_same_octet<24>(acc, oct)) {
+#pragma unroll
+        for (int k = 0; k < 24; ++k) atomicAdd(&red[3 * c0 + k], acc[k]);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) {
+        const int c = i / 3, r = i - 3 * c;
+        atomicAdd(r == 2 ? &db0[c] : &dw0[2 * c + r], red[i]);
     }
 }
 
@@ -605,19 +668,34 @@ extern "C" int pidm_ddim_coefs(const long long* t, const long long* t_next, cons
     return 0;
 }
 
-extern "C" int pidm_gelu_fwd(const void* x, void* y, long long n, int dtype, void* stream) {
-    PIDM_REQUIRE(n % 8 == 0, "gelu: element count must be a multiple of 8");
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(gelu_kernel<T, false>, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)0,
-                                                    (cudaStream_t)stream, (const T*)x, (const T*)nullptr, (T*)y, n / 8)));
-    PIDM_LAUNCH_CHECK("gelu_fwd");
+static int check_cond_embed(const float* cond, const void* act, int B, int HW, int C) {
+    PIDM_REQUIRE(B > 0 && HW > 0 && (long long)B * HW < (1LL << 31), "cond_embed: B*HW out of range");
+    PIDM_REQUIRE(C % 8 == 0 && C <= 256 && 32 % (C / 8) == 0, "cond_embed: C = %d must be 8, 16, 32, 64, 128 or 256", C);
+    PIDM_REQUIRE(((uintptr_t)cond & 7) == 0 && ((uintptr_t)act & 15) == 0, "cond_embed: misaligned cond / activation");
     return 0;
 }
 
-extern "C" int pidm_gelu_bwd(const void* x, const void* dy, void* dx, long long n, int dtype, void* stream) {
-    PIDM_REQUIRE(n % 8 == 0, "gelu: element count must be a multiple of 8");
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(gelu_kernel<T, true>, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)0,
-                                                    (cudaStream_t)stream, (const T*)x, (const T*)dy, (T*)dx, n / 8)));
-    PIDM_LAUNCH_CHECK("gelu_bwd");
+extern "C" int pidm_cond_embed_fwd(const float* cond, const unsigned char* null_mask, const float* w0, const float* b0,
+                                   void* out, int B, int HW, int C, int dtype, void* stream) {
+    if (int e = check_cond_embed(cond, out, B, HW, C)) return e;
+    const int M = B * HW, rows = 256 / (C / 8);
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(cond_embed_fwd_kernel<T>, dim3(grid_for(M, rows)), dim3(256),
+                                                    (size_t)0, (cudaStream_t)stream, cond, null_mask, w0, b0, (T*)out, HW,
+                                                    C, M)));
+    PIDM_LAUNCH_CHECK("cond_embed_fwd");
+    return 0;
+}
+
+extern "C" int pidm_cond_embed_wgrad(const float* cond, const unsigned char* null_mask, const float* w0, const float* b0,
+                                     const void* dg, float* dw0, float* db0, int B, int HW, int C, int dtype,
+                                     void* stream) {
+    if (int e = check_cond_embed(cond, dg, B, HW, C)) return e;
+    const int M = B * HW, rows = 256 / (C / 8);
+    // 4 CTAs per SM: every thread sums several pixels before the block reduction
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(cond_embed_wgrad_kernel<T>, dim3(grid_for(M, rows, num_sms() * 4)),
+                                                    dim3(256), (size_t)0, (cudaStream_t)stream, cond, null_mask, w0, b0,
+                                                    (const T*)dg, dw0, db0, HW, C, M)));
+    PIDM_LAUNCH_CHECK("cond_embed_wgrad");
     return 0;
 }
 

@@ -239,18 +239,22 @@ class DenoisingDiffusion(nn.Module):
         sync = self.sync_scalars if sync_scalars is None else sync_scalars
         if residual_func.gov_eqs == 'darcy':
             t, e = draw_t_and_noise(self.n_steps, input, draw_shard)
-            return self.darcy_loss_from_draws(input, t, e, residual_func, c_data, c_residual, sync_scalars=sync)
+            return self.darcy_loss_from_draws(input, t, e, residual_func, c_data, c_residual, sync_scalars=sync,
+                                              draw_shard=draw_shard)
         if residual_func.gov_eqs == 'mechanics':
             return residual_func.training_loss(self, input, None, c_data, c_residual, c_ineq, lambda_opt,
                                                sync_scalars=sync, draw_shard=draw_shard)
         raise ValueError('Unknown governing equations.')
 
-    def darcy_loss_from_draws(self, x_0, t, e, residual_func, c_data=1., c_residual=0., sync_scalars=None):
-        """The RNG-free body of model_estimation_loss for Darcy: q_sample -> U-Net (-> DDIM walk) -> fused
-        residual + loss kernel.  Returns (loss, data_loss, mean|r|, 0., 0.)."""
+    def darcy_loss_from_draws(self, x_0, t, e, residual_func, c_data=1., c_residual=0., sync_scalars=None,
+                              draw_shard=None):
+        """The body of model_estimation_loss for Darcy after the t / eps draws: q_sample -> U-Net (-> DDIM walk) ->
+        fused residual + loss kernel.  Returns (loss, data_loss, mean|r|, 0., 0.).  With residual-gradient guidance the
+        network draws the classifier-free mask (for the global batch under draw_shard)."""
         dd = self.diff_dict
         x = ops.q_sample(x_0, e, t, dd['alphas_bar_sqrt'], dd['one_minus_alphas_bar_sqrt'])
-        x0_hat, model_out = residual_func.predict_x0((image_to_b_xy_c(x), t), ddim_func=self.ddim_sample_x0)
+        kw = {} if draw_shard is None else {'draw_shard': draw_shard}
+        x0_hat, model_out = residual_func.predict_x0((image_to_b_xy_c(x), t), ddim_func=self.ddim_sample_x0, **kw)
         loss, sums = ops.darcy_pidm_loss(x0_hat, model_out, x_0, t, residual_func.f_s_flat, dd['p2_loss_weight'],
                                          dd['posterior_variance_clipped'], c_data, c_residual, *residual_func.geometry)
         if self.sync_scalars if sync_scalars is None else sync_scalars:

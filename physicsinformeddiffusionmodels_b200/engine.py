@@ -23,14 +23,15 @@ _ALIGN = 64     # elements: every parameter starts on a 256-byte boundary (float
 class FlatParams:
     """Re-homes the trainable parameters of `model` into one flat fp32 buffer (plus grad / moment / EMA twins)."""
 
-    def __init__(self, model, with_optimizer_state=True, group_of=None):
+    def __init__(self, model, with_optimizer_state=True, group_of=None, guidance=False):
         """group_of(name) -> int (optional): parameters are laid out group by group (stable within a group), and
         `group_bounds[g] = (lo, hi)` is the flat range of group g -- the engine all-reduces ranges separately.
         Parameters the forward pass never uses (model.unused_parameter_names(), 1.46 M elements for the Darcy U-Net)
         are laid out LAST: `live_total` is the length of the prefix that can carry a gradient, and only that prefix
-        is exchanged between the ranks (their gradient is identically zero on every rank)."""
+        is exchanged between the ranks (their gradient is identically zero on every rank).  guidance: the model runs the
+        residual-gradient guidance branch, whose layers (emb_conv, combine_conv) are then live."""
         named = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
-        dead = set(model.unused_parameter_names()) if hasattr(model, 'unused_parameter_names') else set()
+        dead = set(model.unused_parameter_names(guidance=guidance)) if hasattr(model, 'unused_parameter_names') else set()
         order = {n: i for i, (n, _) in enumerate(named)}
         named.sort(key=lambda np_: (np_[0] in dead, group_of(np_[0]) if group_of is not None else 0, order[np_[0]]))
         params = [p for _, p in named]
@@ -110,10 +111,11 @@ class TrainEngine:
         CUDA-graph safe.  global_draws (world > 1): t and eps are drawn for the GLOBAL batch from a generator that is
         identical on every rank and sliced to this rank's rows (SURVEY 8e: seed parity with the one-process run).
         snapshot_grad: keep a copy of the (all-reduced, unclipped) flat gradient of the last step in `grad_snapshot`
-        (parity tests; the Adam kernel zeroes the live buffer)."""
-        if getattr(residuals, 'residual_grad_guidance', False):
-            raise NotImplementedError('TrainEngine lays the guidance-only parameters (emb_conv, combine_conv) out as unused; '
-                                      'train residual-gradient guidance through the eager reference loop (main.py)')
+        (parity tests; the Adam kernel zeroes the live buffer).
+        Residual-gradient guidance (residuals.residual_grad_guidance): the guidance front end runs inside the step, the
+        classifier-free mask is drawn inside the captured graph (a fresh draw every replay; the last one is left in
+        model._null_mask_last) and, with global_draws, drawn for the global batch and normalised by the global count."""
+        self.guidance = bool(getattr(residuals, 'residual_grad_guidance', False))
         self.model, self.diffusion, self.residuals = model, diffusion, residuals
         self.lr, self.betas, self.eps, self.max_norm, self.ema_mu = lr, betas, eps, max_norm, ema_mu
         self.c_data, self.c_residual, self.c_ineq, self.lambda_opt = c_data, c_residual, c_ineq, lambda_opt
@@ -129,7 +131,7 @@ class TrainEngine:
             import os
             bucketed_allreduce = world > 1 and os.environ.get('PIDM_BUCKET_AR', '1') != '0'
         self.bucketed = bool(bucketed_allreduce) and hasattr(model, '_boundary_cb')
-        self.fp = FlatParams(model, group_of=_unet_grad_group if self.bucketed else None)
+        self.fp = FlatParams(model, group_of=_unet_grad_group if self.bucketed else None, guidance=self.guidance)
         self._ar_stream = None
         self._reduced = set()
         if self.bucketed:

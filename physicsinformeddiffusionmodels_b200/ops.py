@@ -102,24 +102,42 @@ def add(a, b):
     return _Add.apply(a.contiguous(), b.contiguous())
 
 
-class _Gelu(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x):
-        y = torch.empty_like(x)
-        call('pidm_gelu_fwd', x, y, x.numel(), _code(x), stream())
-        ctx.save_for_backward(x)
-        return y
+class _CondEmbed(torch.autograd.Function):
+    """GELU(emb_conv[0](cond)) of the residual-gradient guidance branch (reference unet_model.py:520-524,585-603) as NHWC
+    activations, from cond [B, HW, 2] fp32 (data: no gradient) with the samples in null_mask [B] (bool) taking cond = 0.
+    Backward only produces the weight and bias gradients, on the weight-gradient stream."""
 
     @staticmethod
-    def backward(ctx, dy):
-        (x,) = ctx.saved_tensors
-        dx = torch.empty_like(x)
-        call('pidm_gelu_bwd', x, dy.contiguous(), dx, x.numel(), _code(x), stream())
-        return dx
+    def forward(ctx, cond, null_mask, weight, bias, dtype):
+        B, HW, _ = cond.shape
+        C = weight.shape[0]
+        out = torch.empty(B, HW, C, device=cond.device, dtype=dtype)
+        call('pidm_cond_embed_fwd', cond, null_mask, weight, bias, out, B, HW, C, _lib.DTYPE_CODE[dtype], stream())
+        ctx.save_for_backward(cond, null_mask, weight, bias)
+        return out
+
+    @staticmethod
+    def backward(ctx, dg):
+        cond, null_mask, weight, bias = ctx.saved_tensors
+        B, HW, _ = cond.shape
+        C = weight.shape[0]
+        dg = dg.contiguous()
+        gw_buf, gw_ret = _grad_buffer(weight)
+        gb_buf, gb_ret = _grad_buffer(bias)
+        call('pidm_cond_embed_wgrad', cond, null_mask, weight, bias, dg, gw_buf, gb_buf, B, HW, C, _code(dg),
+             _wgrad_stream(cond, null_mask, dg))
+        return None, None, gw_ret, gb_ret, None
 
 
-def gelu(x):
-    return _Gelu.apply(x.contiguous())
+def cond_embed(cond, null_mask, weight, bias, P, dtype=None):
+    """[B, P*P, 2] fp32 cond, [B] bool null mask -> [B, P, P, C] activations GELU(W0 cond + b0)"""
+    _need_cuda(cond, null_mask)
+    if cond.shape[-1] != 2 or weight.shape[1] != 2:
+        raise NotImplementedError('the guidance embedding is built for the 2-channel Darcy residual gradient')
+    B = cond.shape[0]
+    out = _CondEmbed.apply(cond.detach().contiguous().float(), null_mask.contiguous(), weight, bias,
+                           dtype or act_dtype())
+    return out.view(B, P, P, -1)
 
 
 class _Stash(torch.autograd.Function):

@@ -110,7 +110,7 @@ class WeightPacker:
                 s.wp_dgrad = take(s.dgrad_elems())
             flip = 1 if (s.stride == 1 and not s.transposed) else 0
             # layers with whole 32-channel blocks and <= 16 taps: both operands from one read (pidm_pack_weights_pairs);
-            # the rest (channel-padded stem / emb_conv, 7x7) through the generic strided kernel
+            # the rest (channel-padded 7x7 stem) through the generic strided kernel
             if (s.cin == s.cin_real and s.cin % 32 == 0 and s.cout % 32 == 0 and s.taps <= 16
                     and s.taps in (s.w_stride_n, s.w_stride_c)):
                 pairs.append((s.weight.data_ptr(), s.wp_fwd.data_ptr(), s.wp_dgrad.data_ptr() if s.need_dgrad else 0,

@@ -61,28 +61,33 @@ class ResidualsDarcy:
         return w.reshape(1, -1).to(self.device)
 
     # (x0_pred, model_out) for the residual / loss kernels
-    def residual_gradient(self, noisy_in):
-        """d mean|r(x_t)| / d x_t for x_t [B, P*P, 2] (reference :117-120): one residual launch, the cotangent sign(r) / N
-        and one adjoint-stencil launch.  Returned in the b_xy_c layout of the input; it is data for the network (no
-        graph is attached, as in the reference's torch.autograd.grad call)."""
+    def residual_gradient(self, noisy_in, world=1):
+        """d mean|r(x_t)| / d x_t for x_t [B, P*P, 2] (reference :117-120), the residual evaluated on x_t itself: one
+        kernel forms the cotangent sign(r) / n in registers and applies the adjoint stencils.  Returned in the b_xy_c
+        layout of the input; it is data for the network (no graph is attached, as in the reference's
+        torch.autograd.grad call).  world > 1: x_t is one of `world` equal shards of a global batch and the mean runs over
+        the global batch (n = world * B * P*P * 3), as in the one-process run on that batch."""
         from ._lib import call, stream
         with torch.no_grad():
             img = generalized_b_xy_c_to_image(noisy_in.detach()).contiguous().float()
             B, _, P, _ = img.shape
-            r = ops.darcy_residual(img, self.f_s_flat, *self.geometry)
-            cot = (torch.sign(r) / r.numel()).contiguous()
-            gx = torch.empty_like(img)
-            call('pidm_darcy_residual_bwd', img, self.f_s_flat, cot, gx, B, P, *self._abi_geometry(), stream())
-        return generalized_image_to_b_xy_c(gx).contiguous()
+            cond = torch.empty(B, P * P, 2, device=img.device, dtype=torch.float32)
+            call('pidm_darcy_abs_residual_grad', img, self.f_s_flat, cond, B, world * B * P * P * 3, P,
+                 *self._abi_geometry(), stream())
+        return cond
 
-    def predict_x0(self, model_input, ddim_func=None, sample=False):
+    def predict_x0(self, model_input, ddim_func=None, sample=False, draw_shard=None):
+        """draw_shard=(rank, world) (training only): the batch is this rank's shard of a global batch; the guidance
+        gradient is normalised by the global count and the classifier-free mask is drawn for the global batch."""
         noisy_in, time = model_input
         if self.residual_grad_guidance:
             assert not self.use_ddim_x0, 'Residual gradient guidance is not implemented with sample estimation for residual.'
-            dr_dx = self.residual_gradient(noisy_in)
+            dr_dx = self.residual_gradient(noisy_in, 1 if draw_shard is None else draw_shard[1])
             if sample:
                 # NOTE (reference): "There is no mentioning of value for the guidance scale in the paper and repo"
                 out = self.model.forward_with_guidance_scale(noisy_in, time, cond=dr_dx, guidance_scale=3.)
+            elif draw_shard is not None:
+                out = self.model(noisy_in, time, cond=dr_dx, null_cond_prob=0.1, draw_shard=draw_shard)
             else:
                 out = self.model(noisy_in, time, cond=dr_dx, null_cond_prob=0.1)
             return out, out

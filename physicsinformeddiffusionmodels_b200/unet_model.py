@@ -30,6 +30,18 @@ def _round_up(x, m):
     return (x + m - 1) // m * m
 
 
+def draw_null_mask(B, prob, device, draw_shard=None):
+    """The classifier-free mask of the reference's prob_mask_like (unet_model.py:63-69): [B] bool, True = the sample's
+    conditioning is dropped.  draw_shard=(rank, world): drawn for the global batch of world * B samples and this rank's
+    rows sliced out, so ranks with identical generator states consume the draw of the one-process run."""
+    if prob == 1:
+        return torch.ones(B, device=device, dtype=torch.bool)
+    if prob == 0:
+        return torch.zeros(B, device=device, dtype=torch.bool)
+    rank, world = draw_shard if draw_shard is not None else (0, 1)
+    return (torch.zeros(B * world, device=device).float().uniform_(0, 1) < prob)[rank * B:(rank + 1) * B]
+
+
 # ---- parameter holders (names = reference attribute names) ---------------------------------------------
 class RotaryEmbedding(nn.Module):
     """Holder for the frozen `freqs` of rotary_embedding_torch.RotaryEmbedding (unet_model.py:439); the
@@ -277,26 +289,28 @@ class Unet3D(nn.Module):
             if not isinstance(up, nn.Identity):
                 conv(_up_conv(up), 4, 2, 1, kind='convT')
         plan_rb(self.final_conv[0])
-        # residual-gradient guidance branch (only executed when forward() is given cond=..., reference :585-603)
-        conv(self.emb_conv[0], 1, 1, 0, cin_pad=self._cin_pad, need_dgrad=False)
+        # residual-gradient guidance branch (only executed when forward() is given cond=..., reference :585-603);
+        # emb_conv[0] (1x1, 2 channels in) runs fused with its GELU in ops.cond_embed, from the fp32 cond
         conv(self.emb_conv[2], 3, 1, 1, circular=False)
         conv(self.combine_conv, 1, 1, 0)
         self._mlp_table = MlpTable(mlps)
 
-    def unused_parameter_names(self):
-        """Trainable parameters that Unet3D.forward never touches WITHOUT residual-gradient guidance (cond=None: the
-        configuration of model.yaml; with cond=... emb_conv / combine_conv are live) (they exist for state_dict parity with the reference:
-        temporal attentions, relative position bias, signal embedding, the to_q / to_k / to_v side projections, emb_conv,
-        combine_conv).  They never receive a gradient -- in the reference their .grad stays None (checked against the
-        reference-generated tests/golden/params_without_grad.txt) -- so a data-parallel step need not exchange them."""
+    def unused_parameter_names(self, guidance=False):
+        """Trainable parameters that Unet3D.forward never touches (they exist for state_dict parity with the reference:
+        temporal attentions, relative position bias, signal embedding, the to_q / to_k / to_v side projections and,
+        without residual-gradient guidance (cond=None: the configuration of model.yaml), emb_conv and combine_conv).
+        They never receive a gradient -- in the reference their .grad stays None (checked against the reference-generated
+        tests/golden/params_without_grad.txt and, guidance=True, params_without_grad_guidance.txt) -- so a data-parallel
+        step need not exchange them."""
         dead = []
+        prefixes = ('time_rel_pos_bias.', 'sign_emb_CNN.', 'init_temporal_attn.', 'mid_temporal_attn.')
+        if not guidance:
+            prefixes += ('emb_conv.', 'combine_conv.')
         for name, p in self.named_parameters():
             if not p.requires_grad:
                 continue
             parts = name.split('.')
-            if (name.startswith(('time_rel_pos_bias.', 'sign_emb_CNN.', 'emb_conv.', 'combine_conv.', 'init_temporal_attn.',
-                                 'mid_temporal_attn.'))
-                    or parts[-2] in ('to_q', 'to_k', 'to_v')):
+            if name.startswith(prefixes) or parts[-2] in ('to_q', 'to_k', 'to_v'):
                 dead.append(name)
         return dead
 
@@ -371,35 +385,32 @@ class Unet3D(nn.Module):
         full = lambda v: torch.full((B,), float(v), device=logits.device, dtype=torch.float32)   # noqa: E731
         return _axpby(full(guidance_scale), logits, full(1. - guidance_scale), null_logits, full(0.), null_logits)
 
-    def _cond_embedding(self, h, cond, null_cond_prob):
+    # the classifier-free mask of the last guided forward, [B] bool, written in place (a CUDA-graph replay leaves the mask
+    # it drew there)
+    _null_mask_last = None
+
+    def _cond_embedding(self, h, cond, null_cond_prob, draw_shard=None):
         """x <- combine_conv(cat(x, emb_conv(cond))) with cond zeroed for the samples drawn as "unconditional"
-        (classifier-free guidance, reference :585-603).  cond [B, P*P, C] is data (the residual gradient): no gradient."""
-        from .denoising_utils import _axpby
+        (classifier-free guidance, reference :585-603).  cond [B, P*P, 2] is data (the residual gradient): no gradient."""
         if cond.dim() != 3:
             raise ValueError('Input must be [BxP*PxC].')
-        B, N, C = cond.shape
+        B, N, _ = cond.shape
         P = int(math.isqrt(N))
         mask = getattr(self, '_null_mask_override', None)          # tests inject the reference's draw
         if mask is None:
-            if null_cond_prob == 1:
-                mask = torch.ones(B, device=cond.device, dtype=torch.bool)
-            elif null_cond_prob == 0:
-                mask = torch.zeros(B, device=cond.device, dtype=torch.bool)
-            else:                                                   # same draw as the reference's prob_mask_like (:63-69)
-                mask = torch.zeros(B, device=cond.device).float().uniform_(0, 1) < null_cond_prob
-        cimg = cond.detach().reshape(B, P, P, C).permute(0, 3, 1, 2).contiguous().float()
-        keep = (~mask).float().contiguous()
-        zero = torch.zeros_like(keep)
-        cimg = _axpby(keep, cimg, zero, cimg, zero, cimg)
-        e = ops.nchw_to_nhwc(cimg, self._cin_pad, ops.act_dtype())
-        e = self._conv(self.emb_conv[0], e)
-        e = ops.gelu(e)
+            mask = draw_null_mask(B, null_cond_prob, cond.device, draw_shard)
+        last = self._null_mask_last
+        if last is None or last.shape != mask.shape or last.device != mask.device:
+            last = self._null_mask_last = torch.empty(B, device=cond.device, dtype=torch.bool)
+        last.copy_(mask)
+        e = ops.cond_embed(cond, last, self.emb_conv[0].weight, self.emb_conv[0].bias, P)
         e = self._conv(self.emb_conv[2], e)
         return self._conv(self.combine_conv, ops.concat(h, e))
 
-    def forward(self, x, time, x_self_cond=None, cond=None, null_cond_prob=0.):
+    def forward(self, x, time, x_self_cond=None, cond=None, null_cond_prob=0., draw_shard=None):
         """x: [B, P*P, C] (as handed over by the residual operators), [B, C, P, P] or [B, C, 1, P, P].
-        Returns fp32 [B, out_dim, P, P] ([B, out_dim, 1, P, P] for 5-D input), reference :542-623."""
+        Returns fp32 [B, out_dim, P, P] ([B, out_dim, 1, P, P] for 5-D input), reference :542-623.
+        draw_shard=(rank, world): the classifier-free mask is drawn for the global batch and sliced (draw_null_mask)."""
         if exists(x_self_cond):
             raise NotImplementedError('self-conditioning is not used by the reference drivers')
         video = False
@@ -443,7 +454,7 @@ class Unet3D(nn.Module):
             torch.cuda.current_stream().wait_stream(pack_stream)
         h = self._conv(self.init_conv, h)
         if exists(cond):
-            h = self._cond_embedding(h, cond, null_cond_prob)
+            h = self._cond_embedding(h, cond, null_cond_prob, draw_shard)
         r = h
         skips = []
         for lvl, (b1, b2, la, down) in enumerate(self.downs):

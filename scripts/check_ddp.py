@@ -1,6 +1,9 @@
 """Multi-GPU consistency checks of the data-parallel training step (run with torchrun on >= 2 GPUs):
 
-  torchrun --nnodes=1 --nproc-per-node=2 --master-addr 127.0.0.1 scripts/check_ddp.py
+  torchrun --nnodes=1 --nproc-per-node=2 --master-addr 127.0.0.1 scripts/check_ddp.py [--guidance]
+
+--guidance runs every check with residual-gradient guidance: the classifier-free mask is drawn for the global batch
+and sliced, and the guidance gradient is normalised by the global count, so part 1 holds with guidance too.
 
  1. the 2-rank step on row shards of a global batch, with t / eps drawn for the global batch and sliced, produces the
     same (all-reduced, averaged) flat gradient as the ONE-process step on the whole batch             (fp32, 1e-4)
@@ -27,6 +30,7 @@ dev = torch.device('cuda', local)
 dist.init_process_group('nccl', device_id=dev)
 ops.set_precision(os.environ.get('PIDM_CHECK_PRECISION', 'fp32'))
 PER = 8
+GUIDANCE = '--guidance' in sys.argv[1:]
 
 
 def rel(a, b):
@@ -36,8 +40,9 @@ def rel(a, b):
 def build(world_, rank_, use_graph, bucketed, global_draws=True):
     torch.manual_seed(0)
     model = Unet3D(dim=32, channels=2).to(dev)
-    diff = DenoisingDiffusion(100, dev)
-    res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True, device=dev)
+    diff = DenoisingDiffusion(100, dev, residual_grad_guidance=GUIDANCE)
+    res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True, device=dev,
+                         residual_grad_guidance=GUIDANCE)
     return model, TrainEngine(model, diff, res, use_graph=use_graph, world=world_, rank=rank_, bucketed_allreduce=bucketed,
                               global_draws=global_draws, snapshot_grad=True)
 
@@ -60,7 +65,7 @@ g_one = eng1.grad_snapshot
 r1 = rel(g_ddp, g_one)
 tail = eng.grad_snapshot[eng.fp.live_total:].abs().max().item()
 if rank == 0:
-    print(f'[1] {world}-rank step vs one process on the global batch of {world * PER}: rel diff of the flat gradient {r1:.3e}; '
+    print(f'[1] (guidance={GUIDANCE}) {world}-rank step vs one process on the global batch of {world * PER}: rel diff of the flat gradient {r1:.3e}; '
           f'unused-parameter tail max |g| = {tail:.1e} ({eng.fp.total - eng.fp.live_total} elements not exchanged)', flush=True)
 ok = ok and r1 < 1e-4 and tail == 0.0
 eng.close(); eng1.close()

@@ -1,0 +1,419 @@
+"""Residual-gradient guidance on the GPU: the guidance kernels per element against fp64 references (edited references
+rejected by the same bounds), and the engine end to end: graph replay against the eager step, the eager step against
+one training iteration of the unmodified reference (scripts/make_golden_guidance.py), the optimizer update of the
+guidance layers, the in-graph mask draw, the sharded draw and the guided sampler."""
+import math
+import os
+import sys
+
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import circular_oracle as CO  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+DEV = 'cuda'
+P = 64
+U = 2.0 ** -24
+C_BOUND = 16            # |y - r| <= C_BOUND * 2^-24 * A, as for the other Darcy kernels
+GUARD = 1024            # NaN guard elements on each side of every output
+
+
+def rel(a, b):
+    a, b = a.double().cpu(), b.double().cpu()
+    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+
+
+def guarded(n, dtype=torch.float32):
+    buf = torch.full((n + 2 * GUARD,), float('nan'), device=DEV, dtype=dtype)
+    return buf, buf[GUARD:GUARD + n]
+
+
+def guards_intact(buf):
+    return bool(torch.isnan(buf[:GUARD]).all() and torch.isnan(buf[-GUARD:]).all())
+
+
+# ---- fp64 Darcy residual from explicit stencil matrices (|matrices| give the absolute operator) ---------------------
+def _mats(h, periodic):
+    D1 = torch.zeros(P, P, dtype=torch.float64)
+    D2 = torch.zeros(P, P, dtype=torch.float64)
+    for i in range(P):
+        if periodic or 0 < i < P - 1:
+            D1[i, (i - 1) % P] -= 0.5
+            D1[i, (i + 1) % P] += 0.5
+            D2[i, (i - 1) % P] += 1.
+            D2[i, i] -= 2.
+            D2[i, (i + 1) % P] += 1.
+        elif i == 0:
+            D1[0, :3] = torch.tensor([-1.5, 2., -0.5], dtype=torch.float64)
+            D2[0, :4] = torch.tensor([2., -5., 4., -1.], dtype=torch.float64)
+        else:
+            D1[-1, -3:] = torch.tensor([0.5, -2., 1.5], dtype=torch.float64)
+            D2[-1, -4:] = torch.tensor([-1., 4., -5., 2.], dtype=torch.float64)
+    return D1 / h, D2 / (h * h)
+
+
+def residual_op(x, periodic, absolute=False):
+    """[B,2,P,P] fp64 -> [B,P*P,3] (pixels_at_boundary, reverse_d1, domain 1); absolute=True: |stencils|, |fields|, |f_s|"""
+    from oracle import pidm_oracle as O
+    d0 = 1.0 / (P - 1)
+    D1a, D2a = _mats(d0, periodic)
+    D1b, D2b = _mats(-d0, periodic)
+    if absolute:
+        D1a, D2a, D1b, D2b, x = D1a.abs(), D2a.abs(), D1b.abs(), D2b.abs(), x.abs()
+    D1a, D2a, D1b, D2b = (m.to(x.device) for m in (D1a, D2a, D1b, D2b))
+    p, K = x[:, 0], x[:, 1]
+
+    def row(M, u):
+        return torch.einsum('ij,bjk->bik', M, u)
+
+    def col(M, u):
+        return torch.einsum('kj,bij->bik', M, u)
+    p0, p1, K0, K1 = row(D1a, p), col(D1b, p), row(D1a, K), col(D1b, K)
+    lap = row(D2a, p) + col(D2b, p)
+    fs = O.darcy_source(P, dtype=torch.float64).to(x.device)
+    bc0, bc1 = torch.zeros_like(p), torch.zeros_like(p)
+    if absolute:
+        eq0 = K * lap + K0 * p0 + K1 * p1 + fs.abs()
+        bc0[:, 0], bc0[:, -1] = p0[:, 0], p0[:, -1]
+        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], p1[:, :, -1]
+    else:
+        eq0 = -K * lap - K0 * p0 - K1 * p1 - fs
+        bc0[:, 0], bc0[:, -1] = -p0[:, 0], p0[:, -1]
+        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], -p1[:, :, -1]
+    return torch.stack([eq0, bc0, bc1], dim=-1).reshape(x.shape[0], P * P, 3)
+
+
+def cond_reference(x, periodic, n_norm, edit=None):
+    """(cond, bound A) in fp64, [B,P*P,2]: cond = J^T sign(r) / n_norm, A = |J|^T |sign(r)| / n_norm at |x|"""
+    B = x.shape[0]
+    xr = x.clone().requires_grad_(True)
+    r = residual_op(xr, periodic)
+    cot = torch.sign(r.detach()) / n_norm
+    if edit == 'bc_row_sign':                 # the bc_x0 seeds of row 0 with the wrong sign
+        cot[:, :P, 1] = -cot[:, :P, 1]
+    g = torch.autograd.grad((r * cot).sum(), xr)[0]
+    xa = x.abs().clone().requires_grad_(True)
+    ra = residual_op(xa, periodic, True) - residual_op(torch.zeros_like(x), periodic, True)
+    A = torch.autograd.grad((ra * cot.abs()).sum(), xa)[0]
+    to_rows = lambda t: t.permute(0, 2, 3, 1).reshape(B, P * P, 2)      # noqa: E731
+    return to_rows(g), to_rows(A)
+
+
+def fields(B, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(B, 2, P, P, generator=g, dtype=torch.float64)
+    x[:, 1] = torch.exp(0.5 * x[:, 1])
+    return x.float().double().to(DEV)         # fp32-representable inputs
+
+
+def launch_abs_residual_grad(x, periodic, n_norm):
+    from oracle import pidm_oracle as O
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    B = x.shape[0]
+    buf, out = guarded(B * P * P * 2)
+    call('pidm_darcy_abs_residual_grad', x.float().contiguous(), O.darcy_source(P).to(DEV).contiguous(), out, B, n_norm,
+         P, 1.0, 1, 1 | (2 if periodic else 0), stream())
+    torch.cuda.synchronize()
+    return buf, out.reshape(B, P * P, 2)
+
+
+def within(y, r, A, c=C_BOUND):
+    return bool(((y.double() - r).abs() <= c * U * A).all())
+
+
+@pytest.mark.parametrize('bcs', ['none', 'periodic'])
+@pytest.mark.parametrize('B', [1, 3, 32, 400])
+def test_abs_residual_grad_per_element(B, bcs):
+    periodic = bcs == 'periodic'
+    x = fields(B, 1008 if B == 400 else 600 + B + (7 if periodic else 0))     # seeds without sign-ambiguous entries
+    # the stencil matrices restate the oracles' residuals
+    from oracle import pidm_oracle as O
+    import periodic_oracle as PO
+    r = residual_op(x, periodic)
+    ref_r = (PO if periodic else O).darcy_residual(x[:2].cpu())
+    assert rel(r[:2], ref_r) < 1e-12
+    # no sign-ambiguous entry: every entry that is not structurally zero lies outside the residual's rounding bound
+    Ar = residual_op(x, periodic, absolute=True)
+    live = r != 0
+    assert bool((r.abs()[live] > C_BOUND * U * Ar[live]).all())
+    assert bool((r[:, :, 1:][~live[:, :, 1:]] == 0).all()) and bool(live[:, :, 0].all())
+    n = B * P * P * 3
+    buf, y = launch_abs_residual_grad(x, periodic, n)
+    assert guards_intact(buf) and not torch.isnan(y).any()
+    g, A = cond_reference(x, periodic, n)
+    assert within(y, g, A), ((y.double() - g).abs() / (U * A)).max().item()
+
+
+@pytest.mark.parametrize('bcs', ['none', 'periodic'])
+@pytest.mark.parametrize('edit', ['local_norm', 'bc_row_sign'])
+def test_abs_residual_grad_rejects_edited_references(bcs, edit):
+    periodic = bcs == 'periodic'
+    x = fields(32, 77)
+    n = 32 * P * P * 3
+    if edit == 'local_norm':              # a shard of a 2-rank global batch normalised by its local count
+        _, y = launch_abs_residual_grad(x, periodic, 2 * n)
+        g, A = cond_reference(x, periodic, 2 * n)
+        assert within(y, g, A)
+        g_bad, _ = cond_reference(x, periodic, n)
+    else:
+        _, y = launch_abs_residual_grad(x, periodic, n)
+        g, A = cond_reference(x, periodic, n)
+        assert within(y, g, A)
+        g_bad, _ = cond_reference(x, periodic, n, edit='bc_row_sign')
+    assert not within(y, g_bad, A), edit
+
+
+# ---- guidance embedding: emb_conv[0] + GELU, and its weight gradient -------------------------------------------------
+def _embed_inputs(B, seed, C=32):
+    g = torch.Generator().manual_seed(seed)
+    cond = (torch.randn(B, P * P, 2, generator=g) * 3e-4).to(DEV)          # the scale of d mean|r| / d x_t
+    w0 = (torch.randn(C, 2, 1, 1, generator=g) * 2e3).to(DEV)
+    b0 = (torch.randn(C, generator=g) * 0.5).to(DEV)
+    mask = torch.zeros(B, dtype=torch.bool)
+    if B > 1:
+        mask[1::3] = True
+    return cond, mask.to(DEV), w0, b0
+
+
+def _gelu64(z, tanh=False):
+    if tanh:
+        return 0.5 * z * (1 + torch.tanh(math.sqrt(2 / math.pi) * (z + 0.044715 * z ** 3)))
+    return 0.5 * z * (1 + torch.erf(z / math.sqrt(2)))
+
+
+def _pre64(cond, mask, w0, b0, unmask=None):
+    c = cond.double().clone()
+    keep_masked = mask.clone()
+    if unmask is not None:
+        keep_masked[unmask] = False
+    c[keep_masked] = 0
+    W = w0.double().reshape(-1, 2)
+    z = c @ W.T + b0.double()
+    A = c.abs() @ W.abs().T + b0.double().abs()
+    return z, A, c
+
+
+def launch_embed(cond, mask, w0, b0, dtype):
+    from physicsinformeddiffusionmodels_b200 import _lib
+    B, C = cond.shape[0], w0.shape[0]
+    buf, out = guarded(B * P * P * C, dtype)
+    _lib.call('pidm_cond_embed_fwd', cond, mask, w0, b0, out, B, P * P, C, _lib.DTYPE_CODE[dtype], _lib.stream())
+    torch.cuda.synchronize()
+    return buf, out.reshape(B, P * P, C)
+
+
+@pytest.mark.parametrize('dtype', [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize('B', [1, 3, 32])
+def test_cond_embed_per_element(B, dtype):
+    cond, mask, w0, b0 = _embed_inputs(B, 900 + B)
+    buf, e = launch_embed(cond, mask, w0, b0, dtype)
+    assert guards_intact(buf) and not torch.isnan(e).any()
+    z, A, _ = _pre64(cond, mask, w0, b0)
+    ref = _gelu64(z)
+    bound = 2.0 ** -20 * A + (2.0 ** -8 * ref.abs() if dtype == torch.bfloat16 else 0)
+    err = (e.double() - ref).abs()
+    assert bool((err <= bound).all()), (err / bound).max().item()
+    null = torch.nn.functional.gelu(b0.float()).to(dtype)
+    for b in range(B):
+        if mask[b]:
+            assert torch.equal(e[b], null.expand(P * P, -1)), b
+
+
+@pytest.mark.parametrize('edit', ['unmasked_sample', 'tanh_gelu'])
+def test_cond_embed_rejects_edited_references(edit):
+    cond, mask, w0, b0 = _embed_inputs(32, 950)
+    _, e = launch_embed(cond, mask, w0, b0, torch.float32)
+    z, A, _ = _pre64(cond, mask, w0, b0)
+    assert bool(((e.double() - _gelu64(z)).abs() <= 2.0 ** -20 * A).all())
+    if edit == 'unmasked_sample':
+        z_bad, _, _ = _pre64(cond, mask, w0, b0, unmask=int(mask.nonzero()[0]))
+        bad = _gelu64(z_bad)
+    else:
+        bad = _gelu64(z, tanh=True)
+    assert not bool(((e.double() - bad).abs() <= 2.0 ** -20 * A).all()), edit
+
+
+@pytest.mark.parametrize('dtype', [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize('B', [1, 3, 32])
+def test_cond_embed_wgrad_per_element(B, dtype):
+    from physicsinformeddiffusionmodels_b200 import _lib
+    cond, mask, w0, b0 = _embed_inputs(B, 970 + B)
+    C = w0.shape[0]
+    g = torch.Generator().manual_seed(B)
+    dg = torch.randn(B, P * P, C, generator=g).to(DEV).to(dtype)
+    pre_w, pre_b = torch.full((C, 2), 0.25, device=DEV), torch.full((C,), -0.5, device=DEV)   # accumulated into
+    dw, db = pre_w.clone(), pre_b.clone()
+    _lib.call('pidm_cond_embed_wgrad', cond, mask, w0, b0, dg, dw, db, B, P * P, C, _lib.DTYPE_CODE[dtype], _lib.stream())
+    torch.cuda.synchronize()
+    z, _, c = _pre64(cond, mask, w0, b0)
+    cdf, pdf = 0.5 * (1 + torch.erf(z / math.sqrt(2))), torch.exp(-0.5 * z * z) / math.sqrt(2 * math.pi)
+    d = dg.double()
+    dz, dz_abs = d * (cdf + z * pdf), d.abs() * (cdf + z.abs() * pdf)
+    M = B * P * P
+    ref_w = torch.einsum('bmo,bmk->ok', dz, c)
+    ref_b = dz.sum((0, 1))
+    A_w = torch.einsum('bmo,bmk->ok', dz_abs, c.abs())
+    A_b = dz_abs.sum((0, 1))
+    k = 16 * math.sqrt(M) * U
+    assert bool(((dw.double() - pre_w.double() - ref_w).abs() <= k * A_w + U).all())
+    assert bool(((db.double() - pre_b.double() - ref_b).abs() <= k * A_b + U).all())
+
+
+# ---- engine ------------------------------------------------------------------------------------------------------------
+@pytest.fixture(scope='module')
+def env():
+    from oracle import pidm_oracle as O
+    from physicsinformeddiffusionmodels_b200 import ops
+    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
+    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
+    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
+    cfg = O.unet_config(dim=32, channels=2)
+    sd = O.make_test_state_dict(cfg, 0)
+
+    def build(n_steps=100, bcs='none', padding_mode='zeros'):
+        model = Unet3D(dim=32, channels=2, padding_mode=padding_mode).to(DEV)
+        model.load_state_dict(CO.circular_state_dict(sd) if padding_mode == 'circular' else sd)
+        diff = DenoisingDiffusion(n_steps, DEV, residual_grad_guidance=True)
+        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
+                             device=DEV, bcs=bcs, domain_length=1., residual_grad_guidance=True)
+        return model, diff, res
+    yield dict(O=O, ops=ops, build=build)
+    ops.set_precision('bf16')
+
+
+def _offset(eng, p):
+    return eng.fp.offsets[next(i for i, q in enumerate(eng.fp.params) if q is p)]
+
+
+def _inject(t, e):
+    o1, o2 = torch.randint, torch.randn_like
+    torch.randint, torch.randn_like = (lambda *a, **k: t), (lambda *a, **k: e)
+    return lambda: setattr(torch, 'randint', o1) or setattr(torch, 'randn_like', o2)
+
+
+@pytest.mark.parametrize('B,bcs,padding_mode', [(32, 'none', 'zeros'), (5, 'none', 'zeros'),
+                                                (8, 'periodic', 'circular')])
+def test_graph_replayed_guidance_step_equals_eager(env, B, bcs, padding_mode):
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
+    env['ops'].set_precision('fp32')
+    g = torch.Generator().manual_seed(700 + B)
+    x0 = (0.7 * torch.randn(B, 2, 64, 64, generator=g)).to(DEV)
+    t = torch.randint(0, 100, (B,), generator=g).to(DEV)
+    e = torch.randn(B, 2, 64, 64, generator=g).to(DEV)
+    mask = (torch.arange(B) % 3 == 1).to(DEV)
+    out = {}
+    for use_graph in (False, True):
+        model, diff, res = env['build'](bcs=bcs, padding_mode=padding_mode)
+        model._null_mask_override = mask
+        eng = TrainEngine(model, diff, res, use_graph=use_graph, snapshot_grad=True)
+        restore = _inject(t, e)
+        try:
+            loss, _, _ = eng.step(x0)
+        finally:
+            restore()
+        torch.cuda.synchronize()
+        assert torch.equal(model._null_mask_last, mask)
+        out[use_graph] = (loss.item(), eng.grad_snapshot.clone())
+        named = dict(model.named_parameters())
+        for n in ('emb_conv.0.weight', 'emb_conv.2.weight', 'combine_conv.weight'):     # in the exchanged prefix
+            assert _offset(eng, named[n]) < eng.fp.live_total, n
+    (le, ge), (lg, gg) = out[False], out[True]
+    assert abs(lg / le - 1) < 1e-5, (lg, le)
+    assert rel(gg, ge) < 1e-4, rel(gg, ge)
+
+
+@pytest.mark.parametrize('mode,tol_loss,tol_grad,tol_norm', [('fp32', 5e-5, 2e-3, 1e-3), ('bf16', 3e-2, 1e-1, 8e-2)])
+def test_guidance_step_matches_reference(env, golden, mode, tol_loss, tol_grad, tol_norm):
+    env['ops'].set_precision(mode)
+    gd = golden('darcy_guidance_step.pt')
+    model, diff, res = env['build']()
+    model._null_mask_override = gd['null_mask'].to(DEV)
+    loss, data_l, rabs, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res,
+                                                          1.0, 1e-3)
+    model._null_mask_override = None
+    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss, (loss.item(), gd['loss'].item())
+    assert abs(float(data_l) / gd['data_loss'].item() - 1) < tol_loss
+    assert abs(float(rabs) / gd['residual_abs'].item() - 1) < tol_loss
+    loss.backward()
+    named = dict(model.named_parameters())
+    n = int(gd['grad_sample'])
+    worst = {k: rel(env['O'].golden_sample(named[k[5:]].grad, n), v) for k, v in gd.items()
+             if k.startswith('grad_') and k not in ('grad_norm', 'grad_sample')}
+    assert max(worst.values()) < tol_grad, sorted(worst.items(), key=lambda kv: -kv[1])[:5]
+    gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
+    assert abs(gn / gd['grad_norm'].item() - 1) < tol_norm
+    dead = sorted(k for k, p in named.items() if p.requires_grad and p.grad is None)
+    assert dead == sorted(model.unused_parameter_names(guidance=True))
+
+
+def test_guidance_layers_take_clip_and_adam_of_the_snapshot(env):
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
+    env['ops'].set_precision('fp32')
+    model, diff, res = env['build']()
+    eng = TrainEngine(model, diff, res, use_graph=True, snapshot_grad=True)
+    g = torch.Generator().manual_seed(11)
+    x0 = (0.7 * torch.randn(8, 2, 64, 64, generator=g)).to(DEV)
+    p0 = eng.fp.flat.clone()
+    eng.step(x0)
+    torch.cuda.synchronize()
+    gs = eng.grad_snapshot.double()
+    coef = min(eng.max_norm / (gs.norm().item() + 1e-6), 1.0)
+    gc = gs * coef
+    upd = eng.lr * gc / (gc.abs() + eng.eps)              # Adam step 1 with bias correction
+    for name, p in model.named_parameters():
+        if not name.startswith(('emb_conv.', 'combine_conv.')):
+            continue
+        o = _offset(eng, p)
+        sl = slice(o, o + p.numel())
+        assert gs[sl].abs().sum() > 0, name
+        err = (eng.fp.flat[sl].double() - (p0[sl].double() - upd[sl])).abs()
+        assert bool((err <= 4 * U * p0[sl].double().abs() + 1e-4 * eng.lr).all()), (name, err.max().item())
+
+
+def test_in_graph_mask_is_redrawn_every_replay(env):
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
+    env['ops'].set_precision('bf16')
+    model, diff, res = env['build']()
+    eng = TrainEngine(model, diff, res, use_graph=True)
+    g = torch.Generator().manual_seed(12)
+    x0 = (0.7 * torch.randn(32, 2, 64, 64, generator=g)).to(DEV)
+    masks = []
+    for _ in range(50):
+        eng.step(x0)
+        masks.append(model._null_mask_last.clone())
+    m = torch.stack(masks).float()
+    assert sum(not torch.equal(a, b) for a, b in zip(masks[:-1], masks[1:])) >= 40
+    assert 0.07 <= m.mean().item() <= 0.13, m.mean().item()
+
+
+def test_sharded_cond_and_mask_are_slices_of_the_global_batch(env):
+    from physicsinformeddiffusionmodels_b200.unet_model import draw_null_mask
+    _, _, res = env['build']()
+    world, B = 4, 6
+    x = fields(world * B, 31).float().permute(0, 2, 3, 1).reshape(world * B, P * P, 2).contiguous()
+    full = res.residual_gradient(x)
+    torch.manual_seed(9)
+    mfull = draw_null_mask(world * B, 0.1, DEV)
+    for rank in range(world):
+        lo, hi = rank * B, (rank + 1) * B
+        assert torch.equal(res.residual_gradient(x[lo:hi].contiguous(), world), full[lo:hi])
+        torch.manual_seed(9)
+        assert torch.equal(draw_null_mask(B, 0.1, DEV, (rank, world)), mfull[lo:hi])
+
+
+def test_guidance_sample_engine_graph_equals_eager(env, monkeypatch):
+    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
+    env['ops'].set_precision('fp32')
+    model, diff, res = env['build'](n_steps=6)
+    model.eval()
+    g = torch.Generator().manual_seed(13)
+    x_T = torch.randn(2, 2, 64, 64, generator=g).to(DEV)
+    zfix = torch.randn(2, 2, 64, 64, generator=g).to(DEV)
+    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: zfix)
+    xe = SampleEngine(model, diff, res, batch=2, use_graph=False).sample(x_init=x_T)[0].clone()
+    xg = SampleEngine(model, diff, res, batch=2, use_graph=True).sample(x_init=x_T)[0].clone()
+    monkeypatch.undo()
+    assert torch.isfinite(xe).all()
+    assert rel(xg, xe) < 1e-4, rel(xg, xe)
