@@ -94,6 +94,27 @@ int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int B, int pix
 int pidm_darcy_abs_residual_grad(const float* x_t, const float* f_s, float* cond, int B, long long n_norm, int pixels,
                                  float domain_length, int reverse_d1, int flags, void* stream);
 
+/* ---- Darcy training-data generation (src/darcy_data_generation.py), fp64, P = 64 --------------------------- */
+/* KLE permeability (:63-78, :131-133): K[b] = exp(phi_s z[b]); phi_s [q, P*P] = [sqrt(lambda_k) phi_k], z [B, q],
+ * K [B, P*P].  The sum runs over k in ascending order, one sample per column of the grid: K[b] depends on z[b] only. */
+int pidm_darcy_gen_kle(const double* phi_s, const double* z, double* K, int B, int q, int pixels, void* stream);
+/* bytes of workspace pidm_darcy_gen_solve needs for B samples (about 6.5 MB per sample); -1 on bad arguments */
+long long pidm_darcy_gen_workspace_bytes(int B, int pixels);
+/* pressure for given K [B, P*P] (:135-165): p = lstsq([A; BC; w^T], [f_s; 0; 0]) computed as the normal equations with
+ * node 0 pinned (banded fp64 Cholesky, half-bandwidth 3P+3) followed by p -= (w^T p) / (w^T 1).  f_s [P*P] fp64.
+ * Outputs (each may be NULL): p [B, P*P] fp64; res [B] = mean |M p - b| over the P*P + 4P + 1 rows (:163-165, fp64);
+ * batch [B, 2, P, P] fp32 = (p, K).  h = domain_length / (P-1) with PIDM_DARCY_PIXELS_AT_BOUNDARY in flags (trapezoid
+ * weights {1,2,4} h^2/4), else domain_length / P (plain mean); reverse_dy: h1 = -h and the y BC rows +D1 | -D1 (:149-152).
+ * stages: PIDM_DARCY_GEN_ASSEMBLE | _FACTOR | _POST, run in that order (PIDM_DARCY_GEN_ALL for a solve); the workspace
+ * carries the band and right-hand side between them. */
+#define PIDM_DARCY_GEN_ASSEMBLE 1
+#define PIDM_DARCY_GEN_FACTOR 2
+#define PIDM_DARCY_GEN_POST 4
+#define PIDM_DARCY_GEN_ALL 7
+int pidm_darcy_gen_solve(const double* K, const double* f_s, double* p, double* res, float* batch, void* workspace,
+                         long long workspace_bytes, int B, int pixels, double domain_length, int reverse_dy, int flags,
+                         int stages, void* stream);
+
 /* ---- layout ------------------------------------------------------------------------------------------- */
 /* image_to_b_xy_c / b_xy_c_to_image (src/denoising_utils.py:36-55) fused with the dtype change + channel padding */
 int pidm_nchw_to_nhwc(const float* src, void* dst, int B, int C, int HW, int Cpad, int dtype, void* stream);

@@ -82,13 +82,18 @@ _SIGS = {
     'pidm_mech_pidm_loss': [P, P, P, P, P, P, P, P, P, F, F, F, F, P, P, P, P, P, I, I, P],
     'pidm_bilinear_resize_fwd': [P, P, I, I, I, P],
     'pidm_bilinear_resize_bwd': [P, P, I, I, I, P],
+    'pidm_darcy_gen_kle': [P, P, P, I, I, I, P],
+    'pidm_darcy_gen_workspace_bytes': [I, I],
+    'pidm_darcy_gen_solve': [P, P, P, P, P, P, L, I, I, D, I, I, I, P],
     'pidm_version': [],
 }
+_RESTYPES = {'pidm_darcy_gen_workspace_bytes': ctypes.c_longlong}
 # functions whose int return value is a result, not an error code
 _VALUE_RETURN = {'pidm_pack_entry_size', 'pidm_pack_pair_entry_size', 'pidm_mlp_entry_size', 'pidm_linattn_workspace_floats', 'pidm_version',
                  'pidm_linattn_block_supported', 'pidm_linattn_block_workspace_floats',
                  'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported',
-                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_block_plan'}
+                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_block_plan',
+                 'pidm_darcy_gen_workspace_bytes'}
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(f'{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). '
@@ -100,7 +105,7 @@ _lib.pidm_last_error.argtypes = []
 for _n, _a in _SIGS.items():
     _f = getattr(_lib, _n)          # AttributeError here == header/library mismatch
     _f.argtypes = _a
-    _f.restype = ctypes.c_int
+    _f.restype = _RESTYPES.get(_n, ctypes.c_int)
 
 launch_count = 0     # number of libpidm entry-point calls (each issues >= 1 kernel); read by bench.py
 
