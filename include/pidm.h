@@ -317,6 +317,20 @@ int pidm_mech_pidm_loss(const float* u, const float* rho, const float* x0, const
 /* bilinear resize, align_corners=False, antialias=False (resize_image, src/residuals_mechanics_K.py:10-21) */
 int pidm_bilinear_resize_fwd(const float* x, float* y, int planes, int in, int out, void* stream);
 int pidm_bilinear_resize_bwd(const float* dy, float* dx, int planes, int in, int out, void* stream);
+/* conditional sampling of the topology-optimisation model, the two per-step pieces around the network call:
+ * U-Net input out [B,3+nc,P,P] = (bilinear resize of x [B,3,P+1,P+1] to P, the nc constant planes [B,nc,P,P]) */
+int pidm_mech_sample_input(const float* x, const float* planes, float* out, int B, int nc, int P, void* stream);
+/* x_out [B,3,P+1,P+1] = c1[t_b] model_out + c2[t_b] x + sigma[t_b] z, model_out = (bilinear P -> P+1 of y[:, :2],
+ * y[:, 2] zero-padded), y [B,3,P,P]; t [B] on the device indexes the tables.  x_out may alias x. */
+int pidm_mech_posterior_step(const float* y, const float* x, const float* z, const long long* t, const float* coef1,
+                             const float* coef2, const float* sigma, float* x_out, int B, int P, void* stream);
+/* Jacobi-PCG of K(rho) u = f on the free dofs (u = 0 on the Dirichlet dofs), one CTA per sample, one launch for the
+ * whole solve: rho [B,nel,nel], bcs [B,4,nel+1,nel+1], KE [8,8].  Stops at ||r||/||f|| < tol (fp64) or max_iter.
+ * Writes u [B,2,nel+1,nel+1], iters [B] and the final relative residual relres [B].  (nel+1)^2 <= 4608. */
+int pidm_mech_fem_pcg(const float* rho, const float* bcs, const float* KE, float* u, int* iters, double* relres,
+                      double tol, int max_iter, int B, int nel, void* stream);
+/* fm [B] = 1 unless the pixels rho > 0.5 form exactly one 8-connected component (reference :369-380) */
+int pidm_mech_floating_material(const float* rho, long long* fm, int B, int nel, void* stream);
 
 #ifdef __cplusplus
 }

@@ -82,6 +82,10 @@ _SIGS = {
     'pidm_mech_pidm_loss': [P, P, P, P, P, P, P, P, P, F, F, F, F, P, P, P, P, P, I, I, P],
     'pidm_bilinear_resize_fwd': [P, P, I, I, I, P],
     'pidm_bilinear_resize_bwd': [P, P, I, I, I, P],
+    'pidm_mech_sample_input': [P, P, P, I, I, I, P],
+    'pidm_mech_posterior_step': [P, P, P, P, P, P, P, P, I, I, P],
+    'pidm_mech_fem_pcg': [P, P, P, P, P, P, D, I, I, I, P],
+    'pidm_mech_floating_material': [P, P, I, I, P],
     'pidm_darcy_gen_kle': [P, P, P, I, I, I, P],
     'pidm_darcy_gen_workspace_bytes': [I, I],
     'pidm_darcy_gen_solve': [P, P, P, P, P, P, L, I, I, D, I, I, I, P],

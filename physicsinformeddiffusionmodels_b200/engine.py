@@ -271,7 +271,15 @@ class SampleEngine:
     trajectory); this is the throughput path.
 
     external_noise=True: the per-step noise z is read from a static buffer that `sample(noises=...)` refreshes before
-    every replay (parity tests inject the reference's draws); otherwise z is drawn by torch's Philox inside the graph."""
+    every replay (parity tests inject the reference's draws); otherwise z is drawn by torch's Philox inside the graph.
+
+    Topology optimisation (residuals.gov_eqs == 'mechanics', image_shape=(3, 65, 65); reference sample.py:136-150,
+    244-342): `sample(conditioning_input=(conditioning, bcs, solution))` copies the resized conditioning and boundary
+    conditions into a static buffer, so a new test batch needs no recapture.  A step is the input kernel
+    (pidm_mech_sample_input) -> U-Net (or the DDIM walk) -> the posterior kernel (pidm_mech_posterior_step).  The
+    residual, compliance and inequality are needed at t = 0 only and are evaluated once, on the last step's x0
+    prediction; with residuals.topopt_eval and a solution the evaluation metrics use the fused solver.  A batch
+    smaller than `batch` is padded with copies of its last sample and the results are sliced."""
 
     def __init__(self, model, diffusion, residuals, batch, image_shape=(2, 64, 64), surpress_noise=True, use_graph=True,
                  steps_per_graph=None, external_noise=False):
@@ -287,6 +295,13 @@ class SampleEngine:
         assert self.n_steps % steps_per_graph == 0, 'steps_per_graph must divide n_steps'
         self.k = steps_per_graph if use_graph else 1
         self.external_noise = external_noise
+        self.mechanics = getattr(residuals, 'gov_eqs', 'darcy') == 'mechanics'
+        if self.mechanics:
+            assert tuple(image_shape) == (3, 65, 65), 'the topology-optimisation model samples [B, 3, 65, 65]'
+            self.batch = batch
+            self.planes = torch.zeros(batch, 7, 64, 64, device=dev)      # resized conditioning (3) and bcs (4)
+            self.net_in = torch.zeros(batch, 10, 64, 64, device=dev)
+            self.x0_pred = None
         self.x = torch.zeros(batch, *image_shape, device=dev)
         self.z = torch.zeros(self.k, batch, *image_shape, device=dev) if external_noise else None
         self.t = torch.zeros(batch, device=dev, dtype=torch.long)
@@ -301,6 +316,8 @@ class SampleEngine:
         self._graph = None
 
     def _step_body(self, j=0):
+        if self.mechanics:
+            return self._mech_step_body(j)
         with torch.no_grad():
             x, t = self.x, self.t
             out = self.residuals.compute_residual(((self._to_rows(x), t),), reduce='per-batch', return_model_out=True,
@@ -317,6 +334,50 @@ class SampleEngine:
             self.x.copy_(new_x)
             self.t.sub_(1)
 
+    def _mech_step_body(self, j=0):
+        with torch.no_grad():
+            x, t = self.x, self.t
+            ops.mech_sample_input(x, self.planes, self.net_in)
+            res = self.residuals
+            if res.use_ddim_x0:
+                x0_pred, y = self.diffusion.ddim_sample_x0(self.net_in, t, res.model, x.shape, res.ddim_steps, 0.,
+                                                           gov_eqs='mechanics')
+            else:
+                x0_pred = y = res.model(self.net_in, t)
+            z = self.z[j] if self.external_noise else torch.randn_like(x)   # drawn at every step, t == 0 included
+            ops.mech_posterior_step(y.float().contiguous(), x, z, t, self.c1, self.c2, self.sigma, x)
+            self.x0_pred = x0_pred                  # the last step's tensor: after the loop it holds the x0 of t = 0
+            self.t.sub_(1)
+
+    def _mech_condition(self, conditioning_input):
+        """Resize the conditioning and boundary conditions into the static planes (padded to `batch` rows)."""
+        from .residuals_mechanics_K import resize_image
+        conditioning, bcs, _ = conditioning_input
+        n = conditioning.shape[0]
+        assert 0 < n <= self.batch and bcs.shape[0] == n, f'conditioning of {n} samples for an engine of batch {self.batch}'
+        planes = torch.cat((resize_image(conditioning, 64), resize_image(bcs, 64)), dim=1)
+        self.planes[:n].copy_(planes)
+        if n < self.batch:
+            self.planes[n:].copy_(planes[n - 1:n].expand(self.batch - n, -1, -1, -1))
+        return n
+
+    def _mech_aux(self, conditioning_input, n):
+        """Residual, compliance and inequality of the last x0 prediction (reference aux keys), and the evaluation metrics
+        (fused solver) when residuals.topopt_eval is set and a solution is given; device tensors, no host sync."""
+        from .residuals_mechanics_K import _MechResidual, resize_image
+        conditioning, bcs, solution = conditioning_input
+        res = self.residuals
+        bcs = bcs.contiguous().float()
+        x0 = self.x0_pred[:n].float()
+        u = resize_image(x0[:, :-1], x0.shape[-1] + 1)
+        rho = x0[:, -1].contiguous()
+        residual, compliance = _MechResidual.apply(u, rho, bcs, res.KE)
+        vf = conditioning[:, 0, 0, 0]
+        aux = {'residual': residual, 'optimized_quant': compliance, 'inequality_quant': rho.reshape(n, -1).mean(1) - vf}
+        if res.topopt_eval and solution is not None:
+            aux.update(res.topopt_metrics(rho, bcs, vf, solution, solver='fused'))
+        return aux
+
     def _capture(self):
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
@@ -332,29 +393,40 @@ class SampleEngine:
             for j in range(self.k):
                 self._step_body(j)
 
-    def sample(self, x_init=None, trajectory=False, noises=None):
+    def sample(self, x_init=None, trajectory=False, noises=None, conditioning_input=None):
         """Runs the whole loop; returns (x_0 [B,C,P,P], residual of the last step [B,P*P,3]) as device tensors and,
         if asked, the trajectory [n_steps+1,B,C,P,P] (device; recorded per replay, so it needs steps_per_graph=1).
-        noises [n_steps,B,C,P,P]: the z of every step (external_noise engines only)."""
+        noises [n_steps,B,C,P,P]: the z of every step (external_noise engines only).
+        Topology optimisation: conditioning_input=(conditioning [n,3,65,65], bcs [n,4,65,65], solution or None) with
+        n <= batch is required, x_init / noises have n rows, and the second value returned is the dict of the
+        reference's aux keys (residual, optimized_quant, inequality_quant and, with topopt_eval and a solution,
+        rel_CE_error_full_batch, vf_error_full_batch, fm_error_full_batch)."""
         assert (noises is not None) == self.external_noise, 'noises= goes with external_noise=True'
         assert not (trajectory and self.k != 1), 'trajectory=True needs steps_per_graph=1'
+        assert (conditioning_input is not None) == self.mechanics, 'conditioning_input= goes with the mechanics study'
+        n = self._mech_condition(conditioning_input) if self.mechanics else self.x.shape[0]
         packer = getattr(self.model, '_packer', None)
         if packer is not None:
             packer.refresh_if_stale(ops.act_dtype())       # the captured steps do not re-pack the weights
         if self.use_graph and self._graph is None:
             self._capture()
         if x_init is None:
-            x_init = torch.randn_like(self.x)
-        self.x.copy_(x_init)
+            x_init = torch.randn_like(self.x[:n])
+        self.x[:n].copy_(x_init)
+        if n < self.x.shape[0]:
+            self.x[n:].copy_(x_init[n - 1:n].expand(self.x.shape[0] - n, *x_init.shape[1:]))
         self.t.fill_(self.n_steps - 1)
-        traj = [self.x.clone()] if trajectory else None
+        traj = [self.x[:n].clone()] if trajectory else None
         for it in range(self.n_steps // self.k):
             if self.external_noise:
-                self.z.copy_(noises[it * self.k:(it + 1) * self.k])
+                self.z[:, :n].copy_(noises[it * self.k:(it + 1) * self.k])
             if self.use_graph:
                 self._graph.replay()
             else:
                 self._step_body()
             if trajectory:
-                traj.append(self.x.clone())
-        return self.x, self.residual, (torch.stack(traj) if trajectory else None)
+                traj.append(self.x[:n].clone())
+        traj = torch.stack(traj) if trajectory else None
+        if self.mechanics:
+            return self.x[:n], self._mech_aux(conditioning_input, n), traj
+        return self.x, self.residual, traj

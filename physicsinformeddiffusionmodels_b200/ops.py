@@ -750,6 +750,29 @@ def posterior_step(x_t, x0_pred, z, c1, c2, sigma):
     return out
 
 
+def mech_sample_input(x, planes, out):
+    """U-Net input of a conditional sampling step of the topology-optimisation model, written into `out`
+    [B,3+nc,P,P]: the sample x [B,3,P+1,P+1] resized to P x P, then the constant planes [B,nc,P,P]."""
+    _need_cuda(x, planes, out)
+    _need_f32(x=x, planes=planes, out=out)
+    B, nc, P, _ = planes.shape
+    assert x.shape == (B, 3, P + 1, P + 1) and out.shape == (B, 3 + nc, P, P), (x.shape, planes.shape, out.shape)
+    call('pidm_mech_sample_input', x.contiguous(), planes.contiguous(), out, B, nc, P, stream())
+    return out
+
+
+def mech_posterior_step(y, x, z, t, c1, c2, sigma, out):
+    """Posterior step of the topology-optimisation sampler from the network output y [B,3,P,P], written into `out`
+    [B,3,P+1,P+1] (may be x): c1[t] model_out + c2[t] x + sigma[t] z, model_out = (u_x, u_y resized to P+1, rho
+    zero-padded); t [B] int64 stays on the device."""
+    _need_cuda(y, x, z, t, out)
+    _need_f32(y=y, x=x, z=z, c1=c1, c2=c2, sigma=sigma)
+    B, _, P, _ = y.shape
+    assert x.shape == out.shape == z.shape == (B, 3, P + 1, P + 1) and t.dtype == torch.int64, (x.shape, y.shape, t.dtype)
+    call('pidm_mech_posterior_step', y.contiguous(), x.contiguous(), z.contiguous(), t, c1, c2, sigma, out, B, P, stream())
+    return out
+
+
 class _DarcyResidual(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x0hat, f_s, geom):
