@@ -166,8 +166,6 @@ int pidm_conv2d_simt(const void* x, const void* w_packed, const float* bias, con
 int pidm_conv2d_wgrad_simt(const void* x, const void* dy, float* dw, float* dbias, int B, int H, int W, int Cin,
                            int Cin_real, int Ho, int Wo, int Cout, int KH, int KW, int stride, int pad, int transposed,
                            long long w_stride_n, long long w_stride_c, int dtype, void* stream);
-/* debugging aid: device buffer (>= 4096 int64) receiving a clock64 timeline of CTA 0 of every tensor-core conv launch */
-int pidm_debug_set_trace(void* buf);
 /* wgmma + TMA implicit-GEMM convolution, bf16 operands, fp32 register accumulation; same contract as pidm_conv2d_simt
  * (requires Cin % 32 == 0, Cout % 32 == 0): stride-1/2 regular convolution (input sampled through TMA elementStrides) and the
  * stride-2 transposed gather (ConvTranspose forward / dgrad of the stride-2 conv) as 4 output-parity classes over the

@@ -45,7 +45,6 @@ _SIGS = {
     'pidm_pack_weights_pairs': [P, P, I, I, I, I, P],
     'pidm_conv2d_simt': [P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, I, I, I, P],
     'pidm_conv2d_wgrad_simt': [P, P, P, P, I, I, I, I, I, I, I, I, I, I, I, I, I, L, L, I, P],
-    'pidm_debug_set_trace': [P],
     'pidm_conv2d_tc_general': [P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, I, I, P, I, I, P],
     'pidm_conv2d_tc_general_supported': [I, I, I, I, I, I, I, I, I, I, I, I],
     'pidm_conv2d_tc_plan': [I, I, I, I, I, I, I, I, I, I, I, I, P],

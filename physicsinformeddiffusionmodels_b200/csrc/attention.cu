@@ -11,7 +11,6 @@
 //     so no extra pass over N is needed for the k-softmax Jacobian.
 // (2) Mid-block softmax attention over <= 64 tokens (Attention.forward, unet_model.py:341-367): one CTA per
 //     (sample, head), everything in shared memory.
-#define PIDM_PDL_GROUP 1
 #include "common.cuh"
 #include "pidm.h"
 
@@ -477,7 +476,7 @@ extern "C" int pidm_linattn_fwd(const void* qkv, void* out, float* ctx, float* k
         return la_small_fwd(qkv, out, ctx, kmax, kzinv, B, N, heads, scale, st);
     PIDM_CUDA(cudaMemsetAsync(ctx, 0, (size_t)B * heads * DH * DH * sizeof(float), st));
     if (dtype == PIDM_BF16 && heads == 8 && N % 64 == 0) {
-        PIDM_CUDA(launch_pdl(la_kstats_kernel<__nv_bfloat16>, dim3(dim3(chunks, B)), dim3(256), (size_t)(la_kstats_smem(HID)), st, (const __nv_bfloat16*)qkv, workspace, N, HID, rpc));
+        PIDM_CUDA(launch_plain(la_kstats_kernel<__nv_bfloat16>, dim3(dim3(chunks, B)), dim3(256), (size_t)(la_kstats_smem(HID)), st, (const __nv_bfloat16*)qkv, workspace, N, HID, rpc));
         if (int e = la_mma_ctx(0, qkv, nullptr, workspace, chunks, kmax, kzinv, ctx, B, N, scale, st)) return e;
         if (int e = la_mma_out(qkv, ctx, out, B, N, scale, st)) return e;
         PIDM_LAUNCH_CHECK("linattn_fwd");
@@ -486,9 +485,9 @@ extern "C" int pidm_linattn_fwd(const void* qkv, void* out, float* ctx, float* k
     const int cchunks = (N + 255) / 256 > 16 ? 16 : (N + 255) / 256;
     const int crpc = ((N + cchunks - 1) / cchunks + LA_TN - 1) / LA_TN * LA_TN;
     PIDM_DISPATCH_DTYPE(dtype, {
-        PIDM_CUDA(launch_pdl(la_kstats_kernel<T>, dim3(dim3(chunks, B)), dim3(la_kstats_block(HID)), (size_t)(la_kstats_smem(HID)), st, (const T*)qkv, workspace, N, HID, rpc));
-        PIDM_CUDA(launch_pdl(la_context_kernel<T, 0>, dim3(dim3((N + crpc - 1) / crpc, heads, B)), dim3(256), (size_t)(0), st, (const T*)qkv, nullptr, workspace, chunks, kmax, kzinv, ctx, N, heads, crpc, scale));
-        PIDM_CUDA(launch_pdl(la_out_kernel<T>, dim3((unsigned)((long long)B * N / 32)), dim3(32 * heads), (size_t)(heads * DH * DH * sizeof(float)), st, (const T*)qkv, ctx, (T*)out, N, heads, scale));
+        PIDM_CUDA(launch_plain(la_kstats_kernel<T>, dim3(dim3(chunks, B)), dim3(la_kstats_block(HID)), (size_t)(la_kstats_smem(HID)), st, (const T*)qkv, workspace, N, HID, rpc));
+        PIDM_CUDA(launch_plain(la_context_kernel<T, 0>, dim3(dim3((N + crpc - 1) / crpc, heads, B)), dim3(256), (size_t)(0), st, (const T*)qkv, nullptr, workspace, chunks, kmax, kzinv, ctx, N, heads, crpc, scale));
+        PIDM_CUDA(launch_plain(la_out_kernel<T>, dim3((unsigned)((long long)B * N / 32)), dim3(32 * heads), (size_t)(heads * DH * DH * sizeof(float)), st, (const T*)qkv, ctx, (T*)out, N, heads, scale));
     });
     PIDM_LAUNCH_CHECK("linattn_fwd");
     return 0;
@@ -513,8 +512,8 @@ extern "C" int pidm_linattn_bwd(const void* qkv, const void* dout, const float* 
     const int cchunks = (N + 255) / 256 > 16 ? 16 : (N + 255) / 256;
     const int crpc = ((N + cchunks - 1) / cchunks + LA_TN - 1) / LA_TN * LA_TN;
     PIDM_DISPATCH_DTYPE(dtype, {
-        PIDM_CUDA(launch_pdl(la_context_kernel<T, 1>, dim3(dim3((N + crpc - 1) / crpc, heads, B)), dim3(256), (size_t)(0), st, (const T*)qkv, (const T*)dout, nullptr, 0, nullptr, nullptr, dctx, N, heads, crpc, scale));
-        PIDM_CUDA(launch_pdl(la_bwd_pixel_kernel<T>, dim3(dim3((unsigned)((long long)B * N / 32), heads / LA_HB)), dim3(32 * LA_HB), (size_t)(0), st, (const T*)qkv, (const T*)dout, ctx, dctx, kmax, kzinv, (T*)dqkv, N, heads, scale));
+        PIDM_CUDA(launch_plain(la_context_kernel<T, 1>, dim3(dim3((N + crpc - 1) / crpc, heads, B)), dim3(256), (size_t)(0), st, (const T*)qkv, (const T*)dout, nullptr, 0, nullptr, nullptr, dctx, N, heads, crpc, scale));
+        PIDM_CUDA(launch_plain(la_bwd_pixel_kernel<T>, dim3(dim3((unsigned)((long long)B * N / 32), heads / LA_HB)), dim3(32 * LA_HB), (size_t)(0), st, (const T*)qkv, (const T*)dout, ctx, dctx, kmax, kzinv, (T*)dqkv, N, heads, scale));
     });
     PIDM_LAUNCH_CHECK("linattn_bwd");
     return 0;
@@ -532,8 +531,8 @@ extern "C" int pidm_attn_fwd(const void* qkv, void* out, int B, int n_tokens, in
                                            (int)sizeof(AttnSmemF)));
             flag = true;
         }
-        PIDM_CUDA(launch_pdl(attn_fwd_kernel<T>, dim3(dim3(heads, B)), dim3(256), (size_t)(sizeof(AttnSmemF)), (cudaStream_t)stream, (const T*)qkv, (T*)out,
-                                                                                            n_tokens, heads, scale));
+        PIDM_CUDA(launch_plain(attn_fwd_kernel<T>, dim3(dim3(heads, B)), dim3(256), (size_t)(sizeof(AttnSmemF)), (cudaStream_t)stream, (const T*)qkv, (T*)out,
+                                                                                              n_tokens, heads, scale));
     });
     PIDM_LAUNCH_CHECK("attn_fwd");
     return 0;
@@ -552,7 +551,7 @@ extern "C" int pidm_attn_bwd(const void* qkv, const void* dout, void* dqkv, int 
                                            (int)sizeof(AttnSmemB)));
             flag = true;
         }
-        PIDM_CUDA(launch_pdl(attn_bwd_kernel<T>, dim3(dim3(heads, B)), dim3(256), (size_t)(sizeof(AttnSmemB)), (cudaStream_t)stream, (const T*)qkv, (const T*)dout, (T*)dqkv, n_tokens, heads, scale));
+        PIDM_CUDA(launch_plain(attn_bwd_kernel<T>, dim3(dim3(heads, B)), dim3(256), (size_t)(sizeof(AttnSmemB)), (cudaStream_t)stream, (const T*)qkv, (const T*)dout, (T*)dqkv, n_tokens, heads, scale));
     });
     PIDM_LAUNCH_CHECK("attn_bwd");
     return 0;

@@ -14,7 +14,6 @@
 // transposed (K-major) fragments with movmatrix; only xn / dy tiles, the W_out slices and the cross-head partial sums
 // touch shared memory.  The unfused path differs by the bf16 rounding of the q, k, v and attention output it
 // materialises.
-#define PIDM_PDL_GROUP 1
 #include "common.cuh"
 #include "mma_util.cuh"
 #include "pidm.h"
@@ -941,14 +940,14 @@ extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const v
     const int chunks = laf_stat_chunks(N);
     const int rpc = N / chunks;
     PIDM_REQUIRE(rpc % 32 == 0 && rpc * chunks == N, "linattn_block: bad statistics chunking for N=%d", N);
-    PIDM_CUDA(launch_pdl(laf_kmax_kernel, dim3(dim3(chunks, B)), dim3(256), (size_t)(LAF_STATS_SMEM), st, x, w, workspace, N, rpc));
+    PIDM_CUDA(launch_plain(laf_kmax_kernel, dim3(dim3(chunks, B)), dim3(256), (size_t)(LAF_STATS_SMEM), st, x, w, workspace, N, rpc));
     const int px = laf_chunk_px(B, N, 2);         // the context and output kernels: two CTAs per SM
     const dim3 grid((N + px - 1) / px, B);
-    PIDM_CUDA(launch_pdl(laf_ctx_kernel<0>, grid, dim3(256), LfcCfg<0>::SMEM, st, x, w, nullptr, workspace, chunks, kmax, kzinv,
-                         ctx, N, px, scale, nullptr));
-    PIDM_CUDA(launch_pdl(laf_finalize_kernel, dim3((B * LM_HID + 7) / 8), dim3(256), (size_t)(0), st, ctx, kzinv, B * LM_HID));
-    PIDM_CUDA(launch_pdl(laf_out_kernel, grid, dim3(256), LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)y, N, px, scale,
-                         (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
+    PIDM_CUDA(launch_plain(laf_ctx_kernel<0>, grid, dim3(256), LfcCfg<0>::SMEM, st, x, w, nullptr, workspace, chunks, kmax, kzinv,
+                           ctx, N, px, scale, nullptr));
+    PIDM_CUDA(launch_plain(laf_finalize_kernel, dim3((B * LM_HID + 7) / 8), dim3(256), (size_t)(0), st, ctx, kzinv, B * LM_HID));
+    PIDM_CUDA(launch_plain(laf_out_kernel, grid, dim3(256), LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)y, N, px, scale,
+                           (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
     PIDM_LAUNCH_CHECK("linattn_block_fwd");
     return 0;
 }
@@ -966,11 +965,11 @@ extern "C" int pidm_linattn_block_bwd(const void* xn, const void* w_qkv, const v
     const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
     PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * LM_HEADS * LM_D * LM_D * sizeof(float), st));
     const int cpx = laf_chunk_px(B, N, 2);
-    PIDM_CUDA(launch_pdl(laf_ctx_kernel<1>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), LfcCfg<1>::SMEM, st, x, w, g,
-                         nullptr, 0, nullptr, nullptr, dctx, N, cpx, scale, wo));
+    PIDM_CUDA(launch_plain(laf_ctx_kernel<1>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), LfcCfg<1>::SMEM, st, x, w, g,
+                           nullptr, 0, nullptr, nullptr, dctx, N, cpx, scale, wo));
     const int bpx = laf_chunk_px(B, N, 1);
-    PIDM_CUDA(launch_pdl(laf_bwd_kernel, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), LfbCfg::SMEM, st, x, w, g, ctx, dctx,
-                         kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, scale, wo));
+    PIDM_CUDA(launch_plain(laf_bwd_kernel, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), LfbCfg::SMEM, st, x, w, g, ctx, dctx,
+                           kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, scale, wo));
     PIDM_LAUNCH_CHECK("linattn_block_bwd");
     return 0;
 }
@@ -990,10 +989,10 @@ extern "C" int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const
     const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
     const int px = laf_chunk_px(B, N, 1);
     const dim3 grid((N + px - 1) / px, B);
-    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<0>, grid, dim3(256), LfwCfg<0>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
-                         N, px, qkv_stride_n, qkv_stride_c, scale, wo, grad_w_out, out_stride_n, out_stride_c));
-    PIDM_CUDA(launch_pdl(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
-                         N, px, qkv_stride_n, qkv_stride_c, scale, nullptr, nullptr, 0LL, 0LL));
+    PIDM_CUDA(launch_plain(laf_wgrad_kernel<0>, grid, dim3(256), LfwCfg<0>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
+                           N, px, qkv_stride_n, qkv_stride_c, scale, wo, grad_w_out, out_stride_n, out_stride_c));
+    PIDM_CUDA(launch_plain(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
+                           N, px, qkv_stride_n, qkv_stride_c, scale, nullptr, nullptr, 0LL, 0LL));
     PIDM_LAUNCH_CHECK("linattn_block_wgrad");
     return 0;
 }

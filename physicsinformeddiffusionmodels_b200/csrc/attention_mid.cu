@@ -9,7 +9,6 @@
 // activations and for fewer than 64 tokens) spends ~3.8 k shared-memory loads per thread on five 64x64x32 products;
 // here the five products are 40 MMAs per warp, the probabilities
 // never leave the registers in forward, and backward stages P and dS once (bf16) for the two key-side products.
-#define PIDM_PDL_GROUP 1
 #include "common.cuh"
 #include "mma_util.cuh"
 #include "pidm.h"
@@ -219,15 +218,15 @@ __global__ void __launch_bounds__(AM_THREADS) attn_mid_bwd_kernel(const __nv_bfl
 bool attn_mid_supported(int n_tokens, int dtype) { return dtype == PIDM_BF16 && n_tokens == AM_N; }
 
 int attn_mid_fwd(const void* qkv, void* out, int B, int heads, float scale, cudaStream_t st) {
-    PIDM_CUDA(launch_pdl(attn_mid_fwd_kernel, dim3(heads, B), dim3(AM_THREADS), (size_t)0, st, (const __nv_bfloat16*)qkv,
-                         (__nv_bfloat16*)out, heads, scale));
+    PIDM_CUDA(launch_plain(attn_mid_fwd_kernel, dim3(heads, B), dim3(AM_THREADS), (size_t)0, st, (const __nv_bfloat16*)qkv,
+                           (__nv_bfloat16*)out, heads, scale));
     PIDM_LAUNCH_CHECK("attn_mid_fwd");
     return 0;
 }
 
 int attn_mid_bwd(const void* qkv, const void* dout, void* dqkv, int B, int heads, float scale, cudaStream_t st) {
-    PIDM_CUDA(launch_pdl(attn_mid_bwd_kernel, dim3(heads, B), dim3(AM_THREADS), (size_t)0, st, (const __nv_bfloat16*)qkv,
-                         (const __nv_bfloat16*)dout, (__nv_bfloat16*)dqkv, heads, scale));
+    PIDM_CUDA(launch_plain(attn_mid_bwd_kernel, dim3(heads, B), dim3(AM_THREADS), (size_t)0, st, (const __nv_bfloat16*)qkv,
+                           (const __nv_bfloat16*)dout, (__nv_bfloat16*)dqkv, heads, scale));
     PIDM_LAUNCH_CHECK("attn_mid_bwd");
     return 0;
 }

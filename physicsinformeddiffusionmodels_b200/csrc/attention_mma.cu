@@ -11,7 +11,6 @@
 //   la_ctx_mma<1>: dctx[h][d][e] += sum_n softmax_d(q[n,:])[d]*s * dout[n,e]
 //   la_out_mma   : out[n,h,e]     = sum_d softmax_d(q[n,:])[d]*s * ctx[h][d][e]
 //   la_bwd_mma   : dq, dk, dv per pixel from dout, ctx, dctx and the saved column statistics
-#define PIDM_PDL_GROUP 1
 #include "common.cuh"
 #include "mma_util.cuh"
 #include "pidm.h"
@@ -373,11 +372,11 @@ int la_mma_ctx(int mode, const void* qkv, const void* dout, const float* part, i
     const int cpx = la_chunk_px(B, N, 2);
     dim3 grid((N + cpx - 1) / cpx, B);
     if (mode == 0)
-        PIDM_CUDA(launch_pdl(la_ctx_mma_kernel<0>, dim3(grid), dim3(256), (size_t)(LA_CTX_SMEM), st, (const __nv_bfloat16*)qkv, nullptr, part, n_stat_chunks, kmax,
-                                                            kzinv, ctx, N, cpx, scale));
+        PIDM_CUDA(launch_plain(la_ctx_mma_kernel<0>, dim3(grid), dim3(256), (size_t)(LA_CTX_SMEM), st, (const __nv_bfloat16*)qkv, nullptr, part, n_stat_chunks, kmax,
+                                                              kzinv, ctx, N, cpx, scale));
     else
-        PIDM_CUDA(launch_pdl(la_ctx_mma_kernel<1>, dim3(grid), dim3(256), (size_t)(LA_CTX_SMEM), st, (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)dout, nullptr,
-                                                            0, nullptr, nullptr, ctx, N, cpx, scale));
+        PIDM_CUDA(launch_plain(la_ctx_mma_kernel<1>, dim3(grid), dim3(256), (size_t)(LA_CTX_SMEM), st, (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)dout, nullptr,
+                                                              0, nullptr, nullptr, ctx, N, cpx, scale));
     PIDM_LAUNCH_CHECK("la_ctx_mma");
     return 0;
 }
@@ -385,7 +384,7 @@ int la_mma_out(const void* qkv, const float* ctx, void* out, int B, int N, float
     if (int e = la_mma_attrs()) return e;
     const int cpx = la_chunk_px(B, N, 2);
     dim3 grid((N + cpx - 1) / cpx, B);
-    PIDM_CUDA(launch_pdl(la_out_mma_kernel, dim3(grid), dim3(256), (size_t)(LA_OUT_SMEM), st, (const __nv_bfloat16*)qkv, ctx, (__nv_bfloat16*)out, N, cpx, scale));
+    PIDM_CUDA(launch_plain(la_out_mma_kernel, dim3(grid), dim3(256), (size_t)(LA_OUT_SMEM), st, (const __nv_bfloat16*)qkv, ctx, (__nv_bfloat16*)out, N, cpx, scale));
     PIDM_LAUNCH_CHECK("la_out_mma");
     return 0;
 }
@@ -394,8 +393,8 @@ int la_mma_bwd(const void* qkv, const void* dout, const float* ctx, const float*
     if (int e = la_mma_attrs()) return e;
     const int cpx = la_chunk_px(B, N, 2);
     dim3 grid((N + cpx - 1) / cpx, B);
-    PIDM_CUDA(launch_pdl(la_bwd_mma_kernel, dim3(grid), dim3(256), (size_t)(LA_BWD_SMEM), st, (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)dout, ctx, dctx, kmax,
-                                                     kzinv, (__nv_bfloat16*)dqkv, N, cpx, scale));
+    PIDM_CUDA(launch_plain(la_bwd_mma_kernel, dim3(grid), dim3(256), (size_t)(LA_BWD_SMEM), st, (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)dout, ctx, dctx, kmax,
+                                                       kzinv, (__nv_bfloat16*)dqkv, N, cpx, scale));
     PIDM_LAUNCH_CHECK("la_bwd_mma");
     return 0;
 }

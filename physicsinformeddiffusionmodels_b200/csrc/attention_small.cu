@@ -12,7 +12,6 @@
 // traffic.  Here the whole chain runs inside one CTA on
 // CUDA cores (the products are 32-wide: 2 MFLOP per CTA), 256 CTAs = one wave.
 // (A one-CTA backward was built and measured too: no faster than the streaming backward at 64 tokens, slower at 256.)
-#define PIDM_PDL_GROUP 1
 #include "common.cuh"
 #include "pidm.h"
 
@@ -188,8 +187,8 @@ int la_small_fwd(const void* qkv, void* out, float* ctx, float* kmax, float* kzi
         PIDM_CUDA(cudaFuncSetAttribute(la_small_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ls_smem(LS_MAXN, false)));
         attr = true;
     }
-    PIDM_CUDA(launch_pdl(la_small_fwd_kernel, dim3(heads, B), dim3(LS_THREADS), ls_smem(N, false), st, (const __nv_bfloat16*)qkv,
-                         (__nv_bfloat16*)out, ctx, kmax, kzinv, N, heads, scale));
+    PIDM_CUDA(launch_plain(la_small_fwd_kernel, dim3(heads, B), dim3(LS_THREADS), ls_smem(N, false), st, (const __nv_bfloat16*)qkv,
+                           (__nv_bfloat16*)out, ctx, kmax, kzinv, N, heads, scale));
     PIDM_LAUNCH_CHECK("la_small_fwd");
     return 0;
 }

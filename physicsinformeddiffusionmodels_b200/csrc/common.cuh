@@ -126,18 +126,14 @@ int num_sms();
 // draining: they run their prologue (barrier init, tensor-map prefetch, parameter loads that do not
 // depend on the predecessor) and then block in pdl_wait() until the predecessor grid has completed and flushed.
 // Every kernel calls pdl_trigger() first so that ITS successor can be scheduled as early as possible.  Both
-// instructions are no-ops for kernels launched without the attribute.  PIDM_PDL=0 disables the attribute.
+// instructions are no-ops for kernels launched without the attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// PIDM_PDL = bit mask of kernel groups launched with the attribute: 0 conv / wgrad / norm, 1 attention,
-// 2 element-wise, 3 linear / optimizer / residual.  Default 1: group 0 only (kernels whose first instruction is the
-// wait gain nothing and their early-scheduled CTAs only take SM slots from the forked weight-gradient stream).
-#ifndef PIDM_PDL_GROUP
-#define PIDM_PDL_GROUP 0
-#endif
-bool pdl_enabled(int group);
-
+// Only the prologue-heavy persistent kernels (convolutions, weight gradients, normalisations) are launched with the
+// attribute.  The attention, element-wise, linear, optimizer and residual kernels go through launch_plain(): a kernel
+// whose first instruction is the wait gains nothing, and its early-scheduled CTAs only take SM slots from the forked
+// weight-gradient stream.
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                                      Args... args) {
@@ -150,7 +146,18 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled(PIDM_PDL_GROUP) ? 1 : 0;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_plain(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                       Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 

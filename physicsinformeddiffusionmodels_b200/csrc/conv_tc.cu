@@ -29,7 +29,6 @@
 //                the next tile
 #include "hopper.cuh"
 #include "pidm.h"
-#include <stdlib.h>
 
 namespace pidm {
 
@@ -65,7 +64,6 @@ struct TcParams {
     const float* bias;
     const __nv_bfloat16* residual;
     __nv_bfloat16* y;
-    long long* trace;        // optional debug timeline of CTA 0 (pidm_debug_set_trace): [role][event] = clock64
     float* gn_sums;          // optional [B, G, 2]: GroupNorm sum / sum-of-squares of the output, fused into the epilogue
     int gn_cpg, gn_groups;   // channels per group, groups
     TcClass cls[4];
@@ -136,7 +134,6 @@ struct TcCfg {
 // persistent kernel, one CTA per SM: the operand ring takes most of the shared memory so that the TMA producers run
 // many K-steps (and tiles) ahead of the tensor cores; latency is hidden by the ring, not by co-resident CTAs
 constexpr int TC_MAX_STAGES = 12;
-constexpr int TC_RING_STAGES = 12;      // default ring depth (PIDM_TC_STAGES overrides)
 
 // Persistent, warp-specialised implicit-GEMM convolution.  Tiles (m_tile, n_tile, class) are walked with a static
 // stride of gridDim.x by all three roles in lock step:
@@ -185,7 +182,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     pdl_wait();                 // prologue done; everything below reads what the previous kernel wrote
 
     if (warp < 4) {
-        // ===== TMA producers: four warps, one elected lane each, K-step `git` belongs to producer git % 4 ============
+        // ===== TMA producers: four warps, one elected lane each, K-step i belongs to producer i % 4 ================
         // (a single thread can only issue a K-step every ~600 cycles -- wait + expect_tx + 2 TMA -- which starves the
         //  tensor cores on the small-channel layers; the issue streams are independent)
         const uint32_t pidx = (uint32_t)warp;
@@ -197,14 +194,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 for (int i = 0; i < n_k; ++i) tma_load_2d(wres + (size_t)i * Cfg::B_BYTES, &map_w, wfull, i * BK, 0);
             }
             // ring position (stage, phase, whose turn) is carried incrementally: no integer divisions in the loop
-            uint32_t st = 0, ph = 0, turn = 0, git = 0;
+            uint32_t st = 0, ph = 0, turn = 0;
             unsigned char* a_dst = ring;
-            const bool tracing = p.trace != nullptr && blockIdx.x == 0;
             const int groups_m0 = p.rg ? p.KW : p.KH * p.KW;
             int tile_m = blockIdx.x % p.m_tiles, rest = blockIdx.x / p.m_tiles;      // tile = rest * m_tiles + tile_m
             const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
-            int lt = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int n0 = (rest % p.n_tiles) * BN;
                 const TcClass& cl = p.cls[rest / p.n_tiles];
                 const int tw_idx = tile_m % p.tiles_w;
@@ -212,7 +207,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 const int tb = t2 / p.tiles_h, th_idx = t2 - tb * p.tiles_h;
                 const int b0 = tb * p.TN, hh0 = p.in_stride * th_idx * p.TH, ww0 = p.in_stride * tw_idx * p.TW;
                 const int n_groups = (p.mode == 0) ? groups_m0 : cl.n_taps;
-                if (tracing && pidx == 0 && lt < 500) p.trace[lt * 2] = clock64();
                 int r = 0, q = 0;                              // mode 0, plain: tap (r, q) walked incrementally
                 for (int g = 0; g < n_groups; ++g) {
                     int dh, dw, ktap;
@@ -227,7 +221,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     for (int kc = 0; kc < kc_per_tap; ++kc, kcol += BK) {
                         if (turn == pidx) {
                             mbar_wait(&empty[st], ph ^ 1);
-                            if (tracing && git < 1000) p.trace[6144 + git] = clock64();
                             mbar_expect_tx(&full[st], (uint32_t)p.stage_bytes);
                             tma_load_4d(a_dst, &map_x, &full[st], kc * BK, ww0 + dw, hh0 + dh, b0);
                             if (!p.resident) {
@@ -237,7 +230,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                                     tma_load_2d(b_dst, &map_w, &full[st], kj, n0);   // row-group mode: tap (r = j, q = g)
                             }
                         }
-                        ++git;
                         if (++turn == 4u) turn = 0;
                         if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_dst = ring; } else a_dst += p.stage_bytes;
                     }
@@ -252,7 +244,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         // to their low word (16-byte units).  One wgmma group is kept in flight: the stage of K-step i - 1 is released
         // once the group of K-step i has been issued and the older one has retired.
         const int cg = (warp - 4) >> 2;
-        const bool tracing = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 128;
         constexpr uint32_t desc_hi = gmma_desc_hi<Cfg::SW>();
         const uint32_t row_half_lo = (uint32_t)(64 * BK * 2) >> 4;           // 64 pixel rows of the A tile
         const uint32_t ring_lo = gmma_desc_lo(smem_u32(ring), 16) + (uint32_t)cg * row_half_lo;
@@ -267,21 +258,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         const bool resident = p.resident != 0;
         // fragment -> staging tile: this thread's rows 64 cg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
         float* acc_row = acc_tile + (size_t)(64 * cg + 16 * (warp & 3) + (lane >> 2)) * Cfg::ACC_PITCH + 2 * (lane & 3);
-        uint32_t st = 0, ph = 0, a_lo = ring_lo, git = 0;
+        uint32_t st = 0, ph = 0, a_lo = ring_lo;
         int rest = blockIdx.x / p.m_tiles, tile_m = blockIdx.x % p.m_tiles;
         const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
         int lt = 0;
         float acc[BN / 2];
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
             const int n_iters = ((p.mode == 0) ? groups_m0 : p.cls[rest / p.n_tiles].n_taps) * kc_per_tap;
-            if (tracing && lt < 64) p.trace[1024 + lt * 4] = clock64();
             if (lt == 0 && resident) mbar_wait(wfull, 0);
             uint32_t accum = 0;
             uint32_t res_lo = wres_lo;                           // resident weights: tile (it) of kernel row 0
             uint32_t prev_st = 0;
             for (int it = 0; it < n_iters; ++it, res_lo += b_tile_lo) {
                 mbar_wait(&full[st], ph);
-                if (tracing && git < 1000) p.trace[4096 + git * 2] = clock64();
                 uint32_t aj = a_lo;
                 uint32_t bj = resident ? res_lo : a_lo + b_off_lo;
                 const uint32_t bj_step = resident ? res_j_lo : b_tile_lo;
@@ -296,14 +285,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 wgmma_commit();
                 wgmma_wait<1>();
                 if (it > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
-                if (tracing && git < 1000) p.trace[4096 + git * 2 + 1] = clock64();
                 prev_st = st;
-                ++git;
                 if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_lo = ring_lo; } else a_lo += stage_lo;
             }
             wgmma_wait<0>();
             if (n_iters > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
-            if (tracing && lt < 64) p.trace[1024 + lt * 4 + 1] = clock64();
             mbar_wait(acc_empty, (lt & 1) ^ 1);                 // the epilogue has read the previous tile back
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
@@ -311,7 +297,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 *reinterpret_cast<float2*>(acc_row + 8 * Cfg::ACC_PITCH + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
             }
             mbar_arrive(acc_full);
-            if (tracing && lt < 64) p.trace[1024 + lt * 4 + 3] = clock64();
             tile_m += step_m; rest += step_r;
             if (tile_m >= p.m_tiles) { tile_m -= p.m_tiles; ++rest; }
         }
@@ -334,7 +319,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         const int th = rem / p.TW, tw = rem - th * p.TW;
         const int my_sw = (LPR == 8) ? (lane & 7) : ((lane >> 1) & 3);
         const int sr = lane / LPR, su = lane % LPR;   // store phase: row within the group of RPI rows, 16-byte unit
-        const bool tracing = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 384;
         int tile_m = blockIdx.x % p.m_tiles, rest = blockIdx.x / p.m_tiles;
         const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
         int lt = 0;
@@ -352,9 +336,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             long long st_off[LPR];
 #pragma unroll
             for (int it = 0; it < LPR; ++it) st_off[it] = __shfl_sync(0xffffffffu, row_off, it * RPI + sr);
-            if (tracing && lt < 64) p.trace[2048 + lt * 4] = clock64();
             mbar_wait(acc_full, lt & 1);
-            if (tracing && lt < 64) p.trace[2048 + lt * 4 + 1] = clock64();
 #pragma unroll 1
             for (int c = 0; c < BN; c += CH) {
                 float f[CH];
@@ -364,7 +346,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     f[j] = row_ok ? v.x : 0.f; f[j + 1] = row_ok ? v.y : 0.f;
                     f[j + 2] = row_ok ? v.z : 0.f; f[j + 3] = row_ok ? v.w : 0.f;
                 }
-                if (tracing && lt < 64 && c == 0) p.trace[3072 + lt * 4] = clock64();
                 // the last columns of the parked tile are in registers: hand the staging tile back to the consumers
                 if (c + CH >= BN) mbar_arrive(acc_empty);
                 if (p.bias && row_ok) {
@@ -413,7 +394,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     if (st_off[it] >= 0)
                         *reinterpret_cast<uint4*>(p.y + st_off[it] + c + su * 8) = stage[r * LPR + (su ^ sw)];
                 }
-                if (tracing && lt < 64 && c == 0) p.trace[3072 + lt * 4 + 1] = clock64();
                 if (p.gn_sums != nullptr && b < p.B) {        // warp-uniform: the 32 rows of a warp lie in one sample
                     float* sums_b = p.gn_sums + (size_t)b * p.gn_groups * 2;
 #pragma unroll
@@ -427,9 +407,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     }
                 }
                 __syncwarp();                                   // staging tile is reused by the next pass
-                if (tracing && lt < 64 && c == 0) p.trace[3072 + lt * 4 + 2] = clock64();
             }
-            if (tracing && lt < 64) p.trace[2048 + lt * 4 + 2] = clock64();
             tile_m += step_m; rest += step_r;
             if (tile_m >= p.m_tiles) { tile_m -= p.m_tiles; ++rest; }
         }
@@ -483,13 +461,10 @@ static bool tc_plan(int B, int GH, int GW, int Cin, int Cout, int KH, int KW, in
     const long long m_tiles = (long long)((B + pl.TN - 1) / pl.TN) * (GH / pl.TH) * (GW / pl.TW) * classes;
     // n-tile widths: a consumer warpgroup holds 64 x BN fp32 accumulators in registers, BN / 2 per thread
     const int cands[3] = {128, 64, 32};
-    static int force_bn = -1;                       // debugging aid: PIDM_TC_BN pins the n-tile width
-    if (force_bn < 0) { const char* ev = getenv("PIDM_TC_BN"); force_bn = ev ? atoi(ev) : 0; }
     pl.BN = 0;
     for (int i = 0; i < 3; ++i) {
         const int bn = cands[i];
         if (Cout % bn != 0) continue;
-        if (force_bn > 0 && bn != force_bn && Cout % force_bn == 0) continue;
         // weights resident in shared memory when the CTA only ever sees one n-tile and they leave room for the ring
         const long long wbytes = (long long)bn * K * 2;
         int resident = (mode == 0 && Cout == bn && wbytes <= 100 * 1024) ? 1 : 0;
@@ -497,9 +472,6 @@ static bool tc_plan(int B, int GH, int GW, int Cin, int Cout, int KH, int KW, in
         int stages = (int)((tc_operand_bytes(bn) - (resident ? wbytes : 0)) / stage);
         if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
         if (stages < 3) continue;
-        static int stage_cap = -1;                  // tuning aid: PIDM_TC_STAGES caps the ring depth
-        if (stage_cap < 0) { const char* ev = getenv("PIDM_TC_STAGES"); stage_cap = ev ? atoi(ev) : TC_RING_STAGES; }
-        if (stage_cap >= 3 && stages > stage_cap) stages = stage_cap;
         pl.BN = bn; pl.resident = resident; pl.res_bytes = resident ? (int)wbytes : 0;
         pl.stage_bytes = stage; pl.stages = stages;
         pl.operand_bytes = (int)(((resident ? wbytes : 0) + (long long)stages * stage + 1023) / 1024 * 1024);
@@ -526,8 +498,6 @@ static int launch_tc(const CUtensorMap& mx, const CUtensorMap& mw, const TcParam
 }
 
 // geometry of one call -> (pixel grid, classes).  Returns false when the tensor-core kernel does not cover it.
-static long long* g_tc_trace = nullptr;
-
 static bool tc_geometry(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW, int stride, int pad,
                         int transposed, TcParams& p, TcPlan& pl, int& classes) {
     if (KH != KW) return false;
@@ -623,7 +593,6 @@ static int tc_run(const void* x, const void* w_packed, const float* bias, const 
         PIDM_REQUIRE(r == CUDA_SUCCESS, "conv2d_tc: cuTensorMapEncodeTiled(w) failed with %d", (int)r);
     }
     p.bias = bias; p.residual = (const __nv_bfloat16*)residual; p.y = (__nv_bfloat16*)y;
-    p.trace = g_tc_trace;
     p.gn_sums = gn_sums; p.gn_groups = gn_groups; p.gn_cpg = gn_groups > 0 ? Cout / gn_groups : 0;
     if (gn_sums) {
         PIDM_REQUIRE(gn_groups > 0 && Cout % gn_groups == 0, "conv2d_tc: bad GroupNorm group count %d", gn_groups);
@@ -642,12 +611,6 @@ static int tc_run(const void* x, const void* w_packed, const float* bias, const 
 
 }  // namespace pidm
 using namespace pidm;
-
-// debugging aid: device buffer of >= 8192 int64 that receives a clock64 timeline of CTA 0 of every conv_tc launch
-extern "C" int pidm_debug_set_trace(void* buf) {
-    g_tc_trace = (long long*)buf;
-    return 0;
-}
 
 extern "C" int pidm_conv2d_tc_general_supported(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW,
                                                 int stride, int pad, int transposed) {

@@ -18,7 +18,6 @@
 // written with 128-bit coalesced stores (48 contiguous bytes per thread, 1536 per warp).
 // Loss-fused variants never materialise r: warp-shuffle + one atomic per CTA for the sums, and the
 // gradient is produced in the same pass (transposed stencils gathered from five product planes in smem).
-#define PIDM_PDL_GROUP 3
 #include "common.cuh"
 #include "pidm.h"
 #include <stddef.h>
@@ -657,8 +656,8 @@ static int launch_darcy_fwd(const float* x0hat, const float* fs, float* residual
     const int ctas_per_sm = (int)(220 * 1024 / smem);        // smem-limited residency
     int grid = sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 1);
     if (grid > B) grid = B;
-    PIDM_CUDA(launch_pdl(darcy_fwd_kernel<PER>, dim3(grid), dim3(DARCY_THREADS), (size_t)(smem), stream, x0hat, fs, residual,
-                         B, make_geom(domain_length, reverse_d1, flags)));
+    PIDM_CUDA(launch_plain(darcy_fwd_kernel<PER>, dim3(grid), dim3(DARCY_THREADS), (size_t)(smem), stream, x0hat, fs, residual,
+                           B, make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_fwd_kernel");
     return 0;
 }
@@ -681,9 +680,9 @@ static int launch_darcy_grad(const float* x0hat, const float* fs, const float* c
     }
     int grid = sm_count;                                      // 145 KB of shared memory: one CTA of 512 threads per SM
     if (grid > B) grid = B;
-    PIDM_CUDA(launch_pdl(darcy_grad_kernel<MODE, PER>, dim3(grid), dim3(DG_THREADS), (size_t)(smem), stream, x0hat, fs,
-                         cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
-                         make_geom(domain_length, reverse_d1, flags), inv_norm));
+    PIDM_CUDA(launch_plain(darcy_grad_kernel<MODE, PER>, dim3(grid), dim3(DG_THREADS), (size_t)(smem), stream, x0hat, fs,
+                           cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
+                           make_geom(domain_length, reverse_d1, flags), inv_norm));
     PIDM_LAUNCH_CHECK("darcy_grad_kernel");
     return 0;
 }
@@ -712,8 +711,8 @@ extern "C" int pidm_fd_stencil(const float* u, float* out, int planes, int pixel
                  "fd_stencil: mode must be 0..4 (d_d0, d_d1, d_d00, d_d11, d_d01), optionally | PIDM_FD_PERIODIC");
     int grid = planes < num_sms() * 4 ? planes : num_sms() * 4;
     auto kernel = periodic ? fd_stencil_kernel<true> : fd_stencil_kernel<false>;
-    PIDM_CUDA(launch_pdl(kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, u, out, planes, mode, 1.f / d0,
-                         1.f / d1));
+    PIDM_CUDA(launch_plain(kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, u, out, planes, mode, 1.f / d0,
+                           1.f / d1));
     PIDM_LAUNCH_CHECK("fd_stencil");
     return 0;
 }
@@ -766,8 +765,8 @@ extern "C" int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
     auto kernel = (flags & PIDM_DARCY_PERIODIC) ? darcy_jacobian_max_kernel<true> : darcy_jacobian_max_kernel<false>;
-    PIDM_CUDA(launch_pdl(kernel, dim3(B), dim3(DARCY_THREADS), (size_t)0, (cudaStream_t)stream, x0hat, max_dr_dp,
-                         make_geom(domain_length, reverse_d1, flags)));
+    PIDM_CUDA(launch_plain(kernel, dim3(B), dim3(DARCY_THREADS), (size_t)0, (cudaStream_t)stream, x0hat, max_dr_dp,
+                           make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_jacobian_max");
     return 0;
 }

@@ -1,7 +1,6 @@
 // HBM-bound element-wise pieces of the PIDM step: q_sample, ancestral posterior step, layout changes
 // (NCHW fp32 <-> NHWC activations), channel concat/split, residual add, and the tiny-N output head
 // (final 1x1 conv -> NCHW fp32, optional sigmoid on the last channel).  128-bit vectorised accesses.
-#define PIDM_PDL_GROUP 2
 #include "common.cuh"
 #include "pidm.h"
 
@@ -556,13 +555,13 @@ extern "C" int pidm_qsample(const float* x0, const float* noise, const long long
                             const float* sqrt_1mab, float* xt, int B, int per_sample, void* stream) {
     if (per_sample % 4 != 0) {
         const long long total = (long long)B * per_sample;
-        PIDM_CUDA(launch_pdl(qsample_scalar_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream, x0,
-                             noise, t, sqrt_ab, sqrt_1mab, xt, per_sample, total));
+        PIDM_CUDA(launch_plain(qsample_scalar_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream, x0,
+                               noise, t, sqrt_ab, sqrt_1mab, xt, per_sample, total));
         PIDM_LAUNCH_CHECK("qsample");
         return 0;
     }
     long long total4 = (long long)B * per_sample / 4;
-    PIDM_CUDA(launch_pdl(qsample_kernel, dim3(grid_for(total4, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const float4*)x0, (const float4*)noise, t, sqrt_ab, sqrt_1mab, (float4*)xt, per_sample / 4, total4));
+    PIDM_CUDA(launch_plain(qsample_kernel, dim3(grid_for(total4, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const float4*)x0, (const float4*)noise, t, sqrt_ab, sqrt_1mab, (float4*)xt, per_sample / 4, total4));
     PIDM_LAUNCH_CHECK("qsample");
     return 0;
 }
@@ -570,12 +569,12 @@ extern "C" int pidm_qsample(const float* x0, const float* noise, const long long
 extern "C" int pidm_posterior_step(const float* x_t, const float* x0_pred, const float* z, float* out, float coef1,
                                    float coef2, float sigma, long long n, void* stream) {
     if (n % 4 != 0) {
-        PIDM_CUDA(launch_pdl(posterior_scalar_kernel, dim3(grid_for(n, 256)), dim3(256), (size_t)0, (cudaStream_t)stream, x_t,
-                             x0_pred, z, out, coef1, coef2, sigma, n));
+        PIDM_CUDA(launch_plain(posterior_scalar_kernel, dim3(grid_for(n, 256)), dim3(256), (size_t)0, (cudaStream_t)stream, x_t,
+                               x0_pred, z, out, coef1, coef2, sigma, n));
         PIDM_LAUNCH_CHECK("posterior_step");
         return 0;
     }
-    PIDM_CUDA(launch_pdl(posterior_kernel, dim3(grid_for(n / 4, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const float4*)x_t, (const float4*)x0_pred, (const float4*)z, (float4*)out, coef1, coef2, sigma, n / 4));
+    PIDM_CUDA(launch_plain(posterior_kernel, dim3(grid_for(n / 4, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const float4*)x_t, (const float4*)x0_pred, (const float4*)z, (float4*)out, coef1, coef2, sigma, n / 4));
     PIDM_LAUNCH_CHECK("posterior_step");
     return 0;
 }
@@ -583,21 +582,21 @@ extern "C" int pidm_posterior_step(const float* x_t, const float* x0_pred, const
 extern "C" int pidm_nchw_to_nhwc(const float* src, void* dst, int B, int C, int HW, int Cpad, int dtype, void* stream) {
     PIDM_REQUIRE(Cpad % 8 == 0 && Cpad >= C, "nchw_to_nhwc: padded channel count must be a multiple of 8, >= C");
     long long n_pix = (long long)B * HW;
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(nchw_to_nhwc_kernel<T>, dim3(grid_for(n_pix, 128)), dim3(128), (size_t)(0), (cudaStream_t)stream, src, (T*)dst, C, HW, Cpad, n_pix)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(nchw_to_nhwc_kernel<T>, dim3(grid_for(n_pix, 128)), dim3(128), (size_t)(0), (cudaStream_t)stream, src, (T*)dst, C, HW, Cpad, n_pix)));
     PIDM_LAUNCH_CHECK("nchw_to_nhwc");
     return 0;
 }
 
 extern "C" int pidm_nhwc_to_nchw(const void* src, float* dst, int B, int C, int HW, int Cpad, int dtype, void* stream) {
     long long total = (long long)B * HW * C;
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(nhwc_to_nchw_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)src, dst, C, HW, Cpad, total)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(nhwc_to_nchw_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)src, dst, C, HW, Cpad, total)));
     PIDM_LAUNCH_CHECK("nhwc_to_nchw");
     return 0;
 }
 
 extern "C" int pidm_add(const void* a, const void* b, void* out, long long n, int dtype, void* stream) {
     PIDM_REQUIRE(n % 8 == 0, "add: size must be a multiple of 8");
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(add_kernel<T>, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)a, (const T*)b, (T*)out, n / 8)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(add_kernel<T>, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)a, (const T*)b, (T*)out, n / 8)));
     PIDM_LAUNCH_CHECK("add");
     return 0;
 }
@@ -606,7 +605,7 @@ extern "C" int pidm_concat_channels(const void* a, const void* b, void* out, lon
                                     void* stream) {
     PIDM_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "concat: channel counts must be multiples of 8");
     long long total = rows * (Ca + Cb) / 8;
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(concat_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)a, (const T*)b, (T*)out, Ca / 8, Cb / 8, rows)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(concat_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)a, (const T*)b, (T*)out, Ca / 8, Cb / 8, rows)));
     PIDM_LAUNCH_CHECK("concat");
     return 0;
 }
@@ -615,7 +614,7 @@ extern "C" int pidm_split_channels(const void* g, void* ga, void* gb, long long 
                                    void* stream) {
     PIDM_REQUIRE(Ca % 8 == 0 && Cb % 8 == 0, "split: channel counts must be multiples of 8");
     long long total = rows * (Ca + Cb) / 8;
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(split_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)g, (T*)ga, (T*)gb, Ca / 8, Cb / 8, rows)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(split_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)g, (T*)ga, (T*)gb, Ca / 8, Cb / 8, rows)));
     PIDM_LAUNCH_CHECK("split");
     return 0;
 }
@@ -631,8 +630,8 @@ extern "C" int pidm_wrap_pad_nhwc(const void* x, void* y, int B, int H, int W, i
     PIDM_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 15) == 0, "wrap_pad: operands must be 16-byte aligned");
     const int U = C * esize / 16;
     const long long total = (long long)B * (H + 2 * halo) * (W + 2 * halo) * U;
-    PIDM_CUDA(launch_pdl(wrap_pad_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
-                         (const uint4*)x, (uint4*)y, H, W, halo, U, total));
+    PIDM_CUDA(launch_plain(wrap_pad_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream,
+                           (const uint4*)x, (uint4*)y, H, W, halo, U, total));
     PIDM_LAUNCH_CHECK("wrap_pad");
     return 0;
 }
@@ -641,19 +640,19 @@ extern "C" int pidm_axpby_per_sample(const float* a, const float* x, const float
                                      const float* z, float* out, int B, int per_sample, void* stream) {
     if (per_sample % 4 != 0) {
         const long long total = (long long)B * per_sample;
-        PIDM_CUDA(launch_pdl(axpby_ps_scalar_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream, a, x,
-                             b, y, c, z, out, per_sample, total));
+        PIDM_CUDA(launch_plain(axpby_ps_scalar_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)0, (cudaStream_t)stream, a, x,
+                               b, y, c, z, out, per_sample, total));
         PIDM_LAUNCH_CHECK("axpby_per_sample");
         return 0;
     }
     long long total4 = (long long)B * per_sample / 4;
-    PIDM_CUDA(launch_pdl(axpby_ps_kernel, dim3(grid_for(total4, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, a, (const float4*)x, b, (const float4*)y, c, (const float4*)z, (float4*)out, per_sample / 4, total4));
+    PIDM_CUDA(launch_plain(axpby_ps_kernel, dim3(grid_for(total4, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, a, (const float4*)x, b, (const float4*)y, c, (const float4*)z, (float4*)out, per_sample / 4, total4));
     PIDM_LAUNCH_CHECK("axpby_per_sample");
     return 0;
 }
 
 extern "C" int pidm_scale(const float* x, const float* alpha_dev, float* out, long long n, void* stream) {
-    PIDM_CUDA(launch_pdl(scale_kernel, dim3(grid_for(n, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, x, alpha_dev, out, n));
+    PIDM_CUDA(launch_plain(scale_kernel, dim3(grid_for(n, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, x, alpha_dev, out, n));
     PIDM_LAUNCH_CHECK("scale");
     return 0;
 }
@@ -661,9 +660,9 @@ extern "C" int pidm_scale(const float* x, const float* alpha_dev, float* out, lo
 extern "C" int pidm_ddim_coefs(const long long* t, const long long* t_next, const float* posterior_mean_coef1,
                                const float* posterior_mean_coef2, const float* sqrt_recip_alphas, const float* noise_mean_coeff,
                                const float* alphas_prod, float* coef_x0, float* coef_x, int B, void* stream) {
-    PIDM_CUDA(launch_pdl(ddim_coefs_kernel, dim3(grid_for(B, 128)), dim3(128), (size_t)0, (cudaStream_t)stream, t, t_next,
-                         posterior_mean_coef1, posterior_mean_coef2, sqrt_recip_alphas, noise_mean_coeff, alphas_prod, coef_x0,
-                         coef_x, B));
+    PIDM_CUDA(launch_plain(ddim_coefs_kernel, dim3(grid_for(B, 128)), dim3(128), (size_t)0, (cudaStream_t)stream, t, t_next,
+                           posterior_mean_coef1, posterior_mean_coef2, sqrt_recip_alphas, noise_mean_coeff, alphas_prod, coef_x0,
+                           coef_x, B));
     PIDM_LAUNCH_CHECK("ddim_coefs");
     return 0;
 }
@@ -679,9 +678,9 @@ extern "C" int pidm_cond_embed_fwd(const float* cond, const unsigned char* null_
                                    void* out, int B, int HW, int C, int dtype, void* stream) {
     if (int e = check_cond_embed(cond, out, B, HW, C)) return e;
     const int M = B * HW, rows = 256 / (C / 8);
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(cond_embed_fwd_kernel<T>, dim3(grid_for(M, rows)), dim3(256),
-                                                    (size_t)0, (cudaStream_t)stream, cond, null_mask, w0, b0, (T*)out, HW,
-                                                    C, M)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(cond_embed_fwd_kernel<T>, dim3(grid_for(M, rows)), dim3(256),
+                                                      (size_t)0, (cudaStream_t)stream, cond, null_mask, w0, b0, (T*)out, HW,
+                                                      C, M)));
     PIDM_LAUNCH_CHECK("cond_embed_fwd");
     return 0;
 }
@@ -692,9 +691,9 @@ extern "C" int pidm_cond_embed_wgrad(const float* cond, const unsigned char* nul
     if (int e = check_cond_embed(cond, dg, B, HW, C)) return e;
     const int M = B * HW, rows = 256 / (C / 8);
     // 4 CTAs per SM: every thread sums several pixels before the block reduction
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(cond_embed_wgrad_kernel<T>, dim3(grid_for(M, rows, num_sms() * 4)),
-                                                    dim3(256), (size_t)0, (cudaStream_t)stream, cond, null_mask, w0, b0,
-                                                    (const T*)dg, dw0, db0, HW, C, M)));
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(cond_embed_wgrad_kernel<T>, dim3(grid_for(M, rows, num_sms() * 4)),
+                                                      dim3(256), (size_t)0, (cudaStream_t)stream, cond, null_mask, w0, b0,
+                                                      (const T*)dg, dw0, db0, HW, C, M)));
     PIDM_LAUNCH_CHECK("cond_embed_wgrad");
     return 0;
 }
@@ -705,9 +704,9 @@ extern "C" int pidm_toy_pidm_loss(const float* target, const float* output, cons
                                   float lambda_opt, float* sums7, float* grad_output, float* grad_residual, float* grad_ineq,
                                   float* grad_opt, int B, int D, void* stream) {
     PIDM_REQUIRE(B > 0 && D > 0, "toy_pidm_loss: bad sizes B=%d D=%d", B, D);
-    PIDM_CUDA(launch_pdl(toy_loss_kernel, dim3(1), dim3(256), (size_t)0, (cudaStream_t)stream, target, output, residual, ineq, opt,
-                         t, p2_loss_weight, posterior_var_clipped, c_data, c_residual, c_ineq, lambda_opt, sums7, grad_output,
-                         grad_residual, grad_ineq, grad_opt, B, D));
+    PIDM_CUDA(launch_plain(toy_loss_kernel, dim3(1), dim3(256), (size_t)0, (cudaStream_t)stream, target, output, residual, ineq, opt,
+                           t, p2_loss_weight, posterior_var_clipped, c_data, c_residual, c_ineq, lambda_opt, sums7, grad_output,
+                           grad_residual, grad_ineq, grad_opt, B, D));
     PIDM_LAUNCH_CHECK("toy_pidm_loss");
     return 0;
 }
@@ -718,7 +717,7 @@ extern "C" int pidm_head_fwd(const void* x, const float* w, const float* bias, f
     long long M = (long long)B * HW;
     size_t smem = (size_t)O * C * sizeof(float);
 #define HEAD_F(OO)                                                                                     \
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_fwd_kernel<T, OO>, dim3(grid_for(M, 256)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(head_fwd_kernel<T, OO>, dim3(grid_for(M, 256)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
                                    (const T*)x, w, bias, y, C, HW, M, sigmoid_last)))
     switch (O) { case 1: HEAD_F(1); break; case 2: HEAD_F(2); break; case 3: HEAD_F(3); break; default: HEAD_F(4); }
 #undef HEAD_F
@@ -735,7 +734,7 @@ extern "C" int pidm_head_bwd(const void* x, const float* w, const float* y, cons
     if (lpp <= 32 && (lpp & (lpp - 1)) == 0) {
         const long long items = M * lpp;
 #define HEAD_BO(OO)                                                                                    \
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_bwd_octet_kernel<T, OO>, dim3(grid_for(items, 256, num_sms() * 4)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(head_bwd_octet_kernel<T, OO>, dim3(grid_for(items, 256, num_sms() * 4)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
                                    (const T*)x, w, y, dy, (T*)dx, dw, db, C, HW, M, sigmoid_last)))
         switch (O) { case 1: HEAD_BO(1); break; case 2: HEAD_BO(2); break; case 3: HEAD_BO(3); break; default: HEAD_BO(4); }
 #undef HEAD_BO
@@ -743,7 +742,7 @@ extern "C" int pidm_head_bwd(const void* x, const float* w, const float* y, cons
         return 0;
     }
 #define HEAD_B(OO)                                                                                     \
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_pdl(head_bwd_kernel<T, OO>, dim3(grid_for(M, 256, num_sms() * 2)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
+    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(head_bwd_kernel<T, OO>, dim3(grid_for(M, 256, num_sms() * 2)), dim3(256), (size_t)(smem), (cudaStream_t)stream, \
                                    (const T*)x, w, y, dy, (T*)dx, dw, db, C, HW, M, sigmoid_last)))
     switch (O) { case 1: HEAD_B(1); break; case 2: HEAD_B(2); break; case 3: HEAD_B(3); break; default: HEAD_B(4); }
 #undef HEAD_B

@@ -3,7 +3,6 @@
 //                  reference unet_model.py:147-159, 464-469
 //   * block_mlps : every ResnetBlock's Linear(4dim, 2*C_out) on SiLU(t) (unet_model.py:246-249,258-262),
 //                  ALL blocks in one launch through a device-side table (they share the same input).
-#define PIDM_PDL_GROUP 3
 #include "common.cuh"
 #include "pidm.h"
 
@@ -286,8 +285,8 @@ extern "C" int pidm_time_embed_fwd(const long long* t, const float* W1, const fl
                                    const float* b2, float* emb, float* h1, float* temb, float* silu_t, int B, int dim,
                                    int td, void* stream) {
     PIDM_REQUIRE(td <= 1024 && dim <= td && dim % 4 == 0 && td % 4 == 0 && dim >= 4, "time_embed: need 4<=dim<=td<=1024, dim and td multiples of 4");
-    PIDM_CUDA(launch_pdl(time_embed_fwd_kernel, dim3(B), dim3(td), (size_t)((dim + td) * sizeof(float)), (cudaStream_t)stream, t, W1, b1, W2, b2, emb, h1, temb,
-                                                                                      silu_t, dim, td));
+    PIDM_CUDA(launch_plain(time_embed_fwd_kernel, dim3(B), dim3(td), (size_t)((dim + td) * sizeof(float)), (cudaStream_t)stream, t, W1, b1, W2, b2, emb, h1, temb,
+                                                                                        silu_t, dim, td));
     PIDM_LAUNCH_CHECK("time_embed_fwd");
     return 0;
 }
@@ -304,11 +303,11 @@ extern "C" int pidm_time_embed_bwd(const float* d_silu_t, const float* emb, cons
     float* dt = workspace;
     float* dh = workspace + (size_t)B * td;
     if (parts & 2)
-        PIDM_CUDA(launch_pdl(time_embed_bwd_act_kernel, dim3(B), dim3(td), (size_t)(td * sizeof(float)), st, d_silu_t, h1, temb,
-                             W2, dt, dh, td));
+        PIDM_CUDA(launch_plain(time_embed_bwd_act_kernel, dim3(B), dim3(td), (size_t)(td * sizeof(float)), st, d_silu_t, h1, temb,
+                               W2, dt, dh, td));
     if (parts & 1)
-        PIDM_CUDA(launch_pdl(time_embed_bwd_wgrad_kernel, dim3(td), dim3(td), (size_t)0, st, (const float*)dt,
-                             (const float*)dh, emb, h1, dW1, db1, dW2, db2, B, dim, td));
+        PIDM_CUDA(launch_plain(time_embed_bwd_wgrad_kernel, dim3(td), dim3(td), (size_t)0, st, (const float*)dt,
+                               (const float*)dh, emb, h1, dW1, db1, dW2, db2, B, dim, td));
     PIDM_LAUNCH_CHECK("time_embed_bwd");
     return 0;
 }
@@ -331,7 +330,7 @@ extern "C" int pidm_block_mlps_fwd(const void* table_dev, int n_entries, int max
     size_t smem = (size_t)MLP_BCHUNK * (td + 1) * sizeof(float);
     if (int e = mlp_smem_attr(smem)) return e;
     dim3 grid(n_entries, ceil_div(max_rows, MLP_ROWS));
-    PIDM_CUDA(launch_pdl(block_mlps_fwd_kernel, dim3(grid), dim3(256), (size_t)(smem), (cudaStream_t)stream, (const MlpEntry*)table_dev, silu_t, B, td));
+    PIDM_CUDA(launch_plain(block_mlps_fwd_kernel, dim3(grid), dim3(256), (size_t)(smem), (cudaStream_t)stream, (const MlpEntry*)table_dev, silu_t, B, td));
     PIDM_LAUNCH_CHECK("block_mlps_fwd");
     return 0;
 }
@@ -347,12 +346,12 @@ extern "C" int pidm_block_mlps_bwd(const void* table_dev, int n_entries, int max
     if (int e = mlp_smem_attr(smem)) return e;
     if (parts & 1) {
         dim3 grid(n_entries, ceil_div(max_rows, MLP_ROWS));
-        PIDM_CUDA(launch_pdl(block_mlps_wgrad_kernel, dim3(grid), dim3(256), (size_t)(smem), st, (const MlpEntry*)table_dev, silu_t, B, td));
+        PIDM_CUDA(launch_plain(block_mlps_wgrad_kernel, dim3(grid), dim3(256), (size_t)(smem), st, (const MlpEntry*)table_dev, silu_t, B, td));
     }
     if (parts & 2) {
         PIDM_CUDA(cudaMemsetAsync(d_silu_t, 0, (size_t)B * td * sizeof(float), st));
         dim3 dgrid(n_entries, ceil_div(max_rows, MLP_DG_ROWS), ceil_div(B, MLP_BCHUNK));
-        PIDM_CUDA(launch_pdl(block_mlps_dgrad_kernel, dim3(dgrid), dim3(td), (size_t)(0), st, (const MlpEntry*)table_dev, d_silu_t, B, td));
+        PIDM_CUDA(launch_plain(block_mlps_dgrad_kernel, dim3(dgrid), dim3(td), (size_t)(0), st, (const MlpEntry*)table_dev, d_silu_t, B, td));
     }
     PIDM_LAUNCH_CHECK("block_mlps_bwd");
     return 0;

@@ -8,7 +8,6 @@
 #include "common.cuh"
 #include "pidm.h"
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 namespace pidm {
 
@@ -1098,11 +1097,6 @@ extern "C" int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const floa
             int cl = 1;
             while (cl < 8 && nv > (long long)cl * threads * 8) cl *= 2;
             while (cl < 8 && (long long)B * nslab * cl * 2 <= resident && nv > (long long)cl * threads) cl *= 2;
-            {   // tuning aid: PIDM_GN_CL pins the number of CTAs per piece
-                static int force_cl = -1;
-                if (force_cl < 0) { const char* ev = getenv("PIDM_GN_CL"); force_cl = ev ? atoi(ev) : 0; }
-                if (force_cl > 0) cl = force_cl;
-            }
             const int rpp = threads / so;
             int rows_per_cta = ceil_div(HW, cl);
             rows_per_cta = ceil_div(rows_per_cta, rpp) * rpp;
@@ -1118,12 +1112,9 @@ extern "C" int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const floa
                 cfg.dynamicSmemBytes = smem;
                 cfg.stream = st;
                 cudaLaunchAttribute attr[2];
-                int na = 0;
-                if (pdl_enabled(0)) {
-                    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-                    attr[na].val.programmaticStreamSerializationAllowed = 1;
-                    ++na;
-                }
+                attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+                attr[0].val.programmaticStreamSerializationAllowed = 1;
+                int na = 1;
                 if (cl > 1) {
                     attr[na].id = cudaLaunchAttributeClusterDimension;
                     attr[na].val.clusterDim.x = (unsigned)cl; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;

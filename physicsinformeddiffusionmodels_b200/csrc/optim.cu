@@ -3,22 +3,13 @@
 //   Adam(lr, betas=(0.9,0.999), eps=1e-8)                          (main.py:143,166)
 //   EMA shadow update mu=0.99                                       (denoising_utils.py:174-177, main.py:178-179)
 // and the error plumbing shared by all translation units.
-#define PIDM_PDL_GROUP 3
 #include "common.cuh"
-#include <stdlib.h>
 #include "pidm.h"
 #include <stdarg.h>
 
 namespace pidm {
 
 thread_local char g_last_error[512] = {0};
-
-bool pdl_enabled(int group) {
-    static int mask = -1;
-    // default 0x1: only group 0 (the prologue-heavy persistent kernels) gains, see common.cuh
-    if (mask < 0) { const char* e = getenv("PIDM_PDL"); mask = e ? atoi(e) : 0x1; }
-    return ((mask >> group) & 1) != 0;
-}
 
 int num_sms() {
     static int n = 0;
@@ -169,7 +160,7 @@ extern "C" int pidm_sumsq(const float* x, long long n, float* out, float* worksp
     int grid = (int)((n4 + 255) / 256);
     if (grid > 148 * 8) grid = 148 * 8;
     if (grid < 1) grid = 1;
-    PIDM_CUDA(launch_pdl(sumsq_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, (const float4*)x, n4, x + n4 * 4, (int)(n - n4 * 4), out, workspace));
+    PIDM_CUDA(launch_plain(sumsq_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, (const float4*)x, n4, x + n4 * 4, (int)(n - n4 * 4), out, workspace));
     PIDM_LAUNCH_CHECK("sumsq");
     return 0;
 }
@@ -181,13 +172,13 @@ extern "C" int pidm_adam_ema_step(float* param, float* grad, float* exp_avg, flo
     PIDM_REQUIRE(step >= 1 || step_counter_dev, "adam: step is 1-based");
     PIDM_REQUIRE((((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq |
                    (uintptr_t)(ema_first_step > 0 ? ema_shadow : param)) & 15) == 0, "adam: buffers must be 16-byte aligned");
-    if (step_counter_dev) PIDM_CUDA(launch_pdl(incr_kernel, dim3(1), dim3(1), (size_t)(0), (cudaStream_t)stream, step_counter_dev));   // counter holds steps done so far
+    if (step_counter_dev) PIDM_CUDA(launch_plain(incr_kernel, dim3(1), dim3(1), (size_t)(0), (cudaStream_t)stream, step_counter_dev));   // counter holds steps done so far
     int grid = (int)((n / 4 + 255) / 256);
     if (grid > num_sms() * 8) grid = num_sms() * 8;
     if (grid < 1) grid = 1;
-    PIDM_CUDA(launch_pdl(adam_ema_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, param, grad, exp_avg, exp_avg_sq, ema_shadow, n, lr, beta1,
-                                                           beta2, eps, step, step_counter_dev, grad_norm_sq_dev, grad_scale,
-                                                           max_norm, ema_mu, ema_first_step, zero_grad));
+    PIDM_CUDA(launch_plain(adam_ema_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, param, grad, exp_avg, exp_avg_sq, ema_shadow, n, lr, beta1,
+                                                             beta2, eps, step, step_counter_dev, grad_norm_sq_dev, grad_scale,
+                                                             max_norm, ema_mu, ema_first_step, zero_grad));
     PIDM_LAUNCH_CHECK("adam_ema_step");
     return 0;
 }

@@ -14,7 +14,6 @@
 // fp32 gradient with red.global.add (framework layout through strides), straight from the accumulator fragments.
 #include "hopper.cuh"
 #include "pidm.h"
-#include <stdlib.h>
 
 namespace pidm {
 
@@ -242,12 +241,6 @@ void wgrad3_geometry(int B, int GH, int GW, int CA, int CB, int* plan);
 int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB, int pad,
                long long s_col, cudaStream_t st);
 
-static bool wgrad3_enabled() {
-    static int use3 = -1;                       // PIDM_WGRAD3=0 falls back to the generic kernel (A/B testing)
-    if (use3 < 0) { const char* ev = getenv("PIDM_WGRAD3"); use3 = (ev && ev[0] == '0') ? 0 : 1; }
-    return use3 != 0;
-}
-
 // launch geometry of the generic kernel: M' tiles x n-tiles x pixel splits
 static bool wg_geometry(int B, int GH, int GW, int CA, int CB, int KH, int KW, int a_stride, WgPlan& pl, WgParams& p,
                         dim3& grid) {
@@ -282,7 +275,7 @@ extern "C" int pidm_conv2d_wgrad_tc_supported(int B, int GH, int GW, int CA, int
 extern "C" int pidm_conv2d_wgrad_tc_plan(int B, int HA, int WA, int CA, int CA_real, int GH, int GW, int CB, int KH,
                                          int KW, int a_stride, int pad, long long s_row, long long s_col, int* out) {
     (void)s_col;
-    if (wgrad3_enabled() && wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row)) {
+    if (wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row)) {
         out[0] = 1;
         wgrad3_geometry(B, GH, GW, CA, CB, out + 1);
         return 0;
@@ -301,7 +294,7 @@ extern "C" int pidm_conv2d_wgrad_tc_plan(int B, int HA, int WA, int CA, int CA_r
 extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int CA_real,
                                     int GH, int GW, int CB, int KH, int KW, int a_stride, int pad, long long s_row,
                                     long long s_col, void* stream) {
-    if (wgrad3_enabled() && wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row))
+    if (wgrad3_supported(B, HA, WA, CA, CA_real, GH, GW, CB, KH, KW, a_stride, pad, s_row))
         return wgrad3_run(a, b, dw, B, HA, WA, CA, GH, GW, CB, pad, s_col, (cudaStream_t)stream);
     WgPlan pl;
     WgParams p;

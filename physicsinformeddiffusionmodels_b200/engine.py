@@ -122,14 +122,13 @@ class TrainEngine:
         self.world, self.rank = world, rank
         self.ema_first_step = int(ema_start) + 2
         self.global_draws = bool(global_draws) and world > 1
-        # Overlap of the gradient exchange with backward (default for world > 1; PIDM_BUCKET_AR=0 or
-        # bucketed_allreduce=False selects the single all-reduce behind the last weight gradient): the flat gradient is
-        # laid out in three readiness groups and a group is all-reduced on its own stream as soon as backward has crossed
-        # the matching boundary of the U-Net.  scripts/check_ddp.py (2 GPUs): ranks stay bitwise identical, exchanged
-        # gradient equal to the single all-reduce to 2e-5 (fp32 atomics), eager and CUDA graph.
+        # Overlap of the gradient exchange with backward (default for world > 1; bucketed_allreduce=False selects the
+        # single all-reduce behind the last weight gradient): the flat gradient is laid out in three readiness groups
+        # and a group is all-reduced on its own stream as soon as backward has crossed the matching boundary of the U-Net.
+        # scripts/check_ddp.py (2 GPUs): ranks stay bitwise identical, exchanged gradient equal to the single all-reduce
+        # to 2e-5 (fp32 atomics), eager and CUDA graph.
         if bucketed_allreduce is None:
-            import os
-            bucketed_allreduce = world > 1 and os.environ.get('PIDM_BUCKET_AR', '1') != '0'
+            bucketed_allreduce = world > 1
         self.bucketed = bool(bucketed_allreduce) and hasattr(model, '_boundary_cb')
         self.fp = FlatParams(model, group_of=_unet_grad_group if self.bucketed else None, guidance=self.guidance)
         self._ar_stream = None
@@ -184,8 +183,7 @@ class TrainEngine:
         ar = self._ar_stream
         ar.wait_stream(torch.cuda.current_stream())
         if ops._SIDE['active']:
-            for st in ops._SIDE['streams']:
-                ar.wait_stream(st)
+            ar.wait_stream(ops._SIDE['stream'])
         lo, hi = self.fp.group_bounds[group]
         with torch.cuda.stream(ar):
             dist.all_reduce(self.fp.grad[lo:hi], op=dist.ReduceOp.SUM)

@@ -9,15 +9,12 @@ mode that buffer is a fresh zero tensor returned to autograd; when a parameter c
 `_pidm_grad` view (flat-buffer engine, engine.py) the kernel accumulates straight into it and autograd
 sees None, so one flat fp32 buffer is ready for the NCCL all-reduce / fused Adam with no per-tensor
 copies."""
-import os
-
 import torch
 
 from . import _lib
 from ._lib import call, stream
 
-_TC_HARD_OFF = os.environ.get('PIDM_DISABLE_TC') == '1'     # debugging aid: force the CUDA-core conv kernels
-_STATE = {'act_dtype': torch.bfloat16, 'use_tc': not _TC_HARD_OFF}
+_STATE = {'act_dtype': torch.bfloat16, 'use_tc': True}
 
 
 def set_precision(name):
@@ -26,7 +23,7 @@ def set_precision(name):
 
 
 def set_tensor_core_conv(flag):
-    _STATE['use_tc'] = bool(flag) and not _TC_HARD_OFF
+    _STATE['use_tc'] = bool(flag)
 
 
 def act_dtype():
@@ -320,25 +317,19 @@ class _Conv2d(torch.autograd.Function):
 # Weight-gradient kernels only feed the optimizer: inside TrainEngine they are launched on a side stream so that they
 # overlap the (latency-bound) dgrad / normalisation chain of the remaining layers.  Operand tensors are kept alive until
 # the join (they were allocated on the main stream).
-_SIDE = {'streams': [], 'next': 0, 'keep': [], 'active': False}
-_N_SIDE = max(1, int(os.environ.get('PIDM_SIDE_STREAMS', '1')))      # tuning aid: weight-gradient launches round-robin over
-                                                                      # this many side streams
+_SIDE = {'stream': None, 'keep': [], 'active': False}
 
 
 def side_stream_begin():
-    if os.environ.get('PIDM_NO_SIDE_STREAM') == '1':      # debugging aid: everything on one stream
-        return
-    while len(_SIDE['streams']) < _N_SIDE:
-        _SIDE['streams'].append(torch.cuda.Stream())
+    if _SIDE['stream'] is None:
+        _SIDE['stream'] = torch.cuda.Stream()
     _SIDE['active'] = True
-    _SIDE['next'] = 0
     _SIDE['keep'] = []
 
 
 def side_stream_join():
     if _SIDE['active']:
-        for st in _SIDE['streams']:
-            torch.cuda.current_stream().wait_stream(st)
+        torch.cuda.current_stream().wait_stream(_SIDE['stream'])
         _SIDE['keep'] = []
         _SIDE['active'] = False
 
@@ -358,8 +349,7 @@ def _wgrad_stream(*operands):
     """stream handle for a wgrad-type launch whose operands are ready on the current stream"""
     if not _SIDE['active']:
         return stream()
-    side = _SIDE['streams'][_SIDE['next']]
-    _SIDE['next'] = (_SIDE['next'] + 1) % len(_SIDE['streams'])
+    side = _SIDE['stream']
     side.wait_stream(torch.cuda.current_stream())
     _SIDE['keep'].extend(operands)
     return side.cuda_stream
