@@ -88,6 +88,14 @@ int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, const float
  * the 12288 x 4096 Jacobian per sample with vmap(jacfwd). */
 int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int B, int pixels, float domain_length, int reverse_d1,
                             int flags, void* stream);
+/* CoCoGen corrections (src/residuals_darcy.py:209-240, applied `steps` times), one launch for the batch.  x [B,2,P,P]
+ * fp32 (p, K) is updated in place: every active sample gets `steps` corrections
+ *   p <- p - (1e-6 / min(max_dr_dp, 1e12)) * d(sum r^2)/dp,
+ * and residual [B,P*P,3] receives the residual of the corrected fields.  Sample b is active when t == NULL or
+ * t[b] < n_active (t [B] int64 on the device, so a captured graph can predicate on the time index); an inactive
+ * sample is neither read nor written.  steps = 0 only evaluates the residual.  No allocation, no host synchronisation. */
+int pidm_darcy_cocogen(float* x, const float* f_s, float* residual, const long long* t, int n_active, int steps, int B,
+                       int pixels, float domain_length, int reverse_d1, int flags, void* stream);
 /* Residual-gradient guidance (src/residuals_darcy.py:116-120): cond = d (sum|r(x_t)|) / n_norm / d x_t, the residual
  * evaluated on x_t [B,2,P,P] itself, written in the b_xy_c layout [B,P*P,2] fp32 the network takes.  sign(0) = 0.  n_norm
  * is the count the mean divides by: B*P*P*3, or world*B*P*P*3 for a shard of a global batch. */

@@ -29,6 +29,7 @@ _SIGS = {
     'pidm_darcy_residual_fwd': [P, P, P, I, I, F, I, I, P],
     'pidm_darcy_residual_bwd': [P, P, P, P, I, I, F, I, I, P],
     'pidm_darcy_jacobian_max': [P, P, I, I, F, I, I, P],
+    'pidm_darcy_cocogen': [P, P, P, P, I, I, I, I, F, I, I, P],
     'pidm_darcy_abs_residual_grad': [P, P, P, I, L, I, F, I, I, P],
     'pidm_darcy_pidm_loss': [P, P, P, P, P, P, P, F, F, P, P, P, I, I, F, I, I, P],
     'pidm_nchw_to_nhwc': [P, P, I, I, I, I, I, P],

@@ -309,6 +309,32 @@ __device__ __forceinline__ void residual_quad_full(const float* sp, const float*
 // sign(x) * s for s > 0, with sign(0) = 0
 __device__ __forceinline__ float scaled_sign(float x, float s) { return x > 0.f ? s : (x < 0.f ? -s : 0.f); }
 
+// The p-side product planes of a quad from the cotangent (ge, g0, g1) of (eq_0, bc_x0, bc_x1):
+// A = -ge K, U0 = -ge K_0 + bc_x0 seed, U1 = -ge K_1 + bc_x1 seed.
+__device__ __forceinline__ void p_products(const float ge[4], const float g0[4], const float g1[4], const float kv[4],
+                                           const float k0[4], const float k1[4], int i, int j0, const DarcyGeom& g,
+                                           float a[4], float u0[4], float u1[4]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int j = j0 + k;
+        a[k] = -ge[k] * kv[k];
+        u0[k] = -ge[k] * k0[k] + ((i == 0) ? -g0[k] : ((i == P - 1) ? g0[k] : 0.f));
+        u1[k] = -ge[k] * k1[k] + ((j == 0) ? g.bc1_sign * g1[k] : ((j == P - 1) ? -g.bc1_sign * g1[k] : 0.f));
+    }
+}
+
+// d p at pixel (i, j): the transposed stencils gathered from the A, U0, U1 planes
+template <bool PER>
+__device__ __forceinline__ float p_adjoint(const float* sA, const float* sU0, const float* sU1, int i, int j,
+                                           const DarcyGeom& g) {
+    auto a_row = [&](int r) { return sA[r * P + j]; };
+    auto a_col = [&](int c) { return sA[i * P + c]; };
+    auto u0r = [&](int r) { return sU0[r * P + j]; };
+    auto u1c = [&](int c) { return sU1[i * P + c]; };
+    return adj_d2<PER>(a_row, i, g.inv_h0sq) + adj_d2<PER>(a_col, j, g.inv_h1sq) + adj_d1<PER>(u0r, i, g.inv_h0) +
+           adj_d1<PER>(u1c, j, g.inv_h1);
+}
+
 // MODE 1: generic backward (cotangent tensor given).  MODE 2: fused PIDM loss (data MSE + residual NLL sums, |r| sum)
 // and its gradient w.r.t. x0_hat / model_out in one pass.  MODE 3: gradient of sum|r| / n_norm (the cotangent sign(r) *
 // inv_norm is formed in registers), written in the b_xy_c layout [B,P*P,2] (residual-gradient guidance).  PER: periodic
@@ -399,12 +425,9 @@ __global__ void __launch_bounds__(DG_THREADS, MODE == 3 ? 1 : 0) darcy_grad_kern
                 }
             }
             float a[4], u0[4], u1[4], v0[4], v1[4];
+            p_products(ge, g0, g1, kv, k0, k1, i, j0, geom, a, u0, u1);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                const int j = j0 + k;
-                a[k] = -ge[k] * kv[k];
-                u0[k] = -ge[k] * k0[k] + ((i == 0) ? -g0[k] : ((i == P - 1) ? g0[k] : 0.f));
-                u1[k] = -ge[k] * k1[k] + ((j == 0) ? geom.bc1_sign * g1[k] : ((j == P - 1) ? -geom.bc1_sign * g1[k] : 0.f));
                 v0[k] = -ge[k] * p0[k];
                 v1[k] = -ge[k] * p1[k];
                 W[u][k] = -ge[k] * lap[k];
@@ -429,14 +452,9 @@ __global__ void __launch_bounds__(DG_THREADS, MODE == 3 ? 1 : 0) darcy_grad_kern
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
                     const int j = j0 + k;
-                    auto a_row = [&](int r) { return sA[r * P + j]; };
-                    auto a_col = [&](int c) { return sA[i * P + c]; };
-                    auto u0r = [&](int r) { return sU0[r * P + j]; };
-                    auto u1c = [&](int c) { return sU1[i * P + c]; };
                     auto v0r = [&](int r) { return sV0[r * P + j]; };
                     auto v1c = [&](int c) { return sV1[i * P + c]; };
-                    dp[k] = adj_d2<PER>(a_row, i, geom.inv_h0sq) + adj_d2<PER>(a_col, j, geom.inv_h1sq) +
-                            adj_d1<PER>(u0r, i, geom.inv_h0) + adj_d1<PER>(u1c, j, geom.inv_h1);
+                    dp[k] = p_adjoint<PER>(sA, sU0, sU1, i, j, geom);
                     dk[k] = W[u][k] + adj_d1<PER>(v0r, i, geom.inv_h0) + adj_d1<PER>(v1c, j, geom.inv_h1);
                 }
             }
@@ -533,6 +551,36 @@ __device__ __forceinline__ void dir_entries(int x, float kv, float kd, float inv
     n = stencil1<PER>(x, off, c);
     for (int k = 0; k < n; ++k) { e[off[k] + 3] += -kd * c[k] * inv_h; has[off[k] + 3] = true; }
 }
+// max(m, every Jacobian entry in the rows of pixel (i, j)), from the K plane sk
+template <bool PER>
+__device__ __forceinline__ float jacobian_max_pixel(const float* sk, int i, int j, const DarcyGeom& g, float m) {
+    const float kv = sk[i * P + j];
+    const float k0 = d_row<PER>(sk, i, j, g.inv_h0), k1 = d_col<PER>(sk, i, j, g.inv_h1);
+    float er[7], ec[7];
+    bool hr[7], hc[7];
+    dir_entries<PER>(i, kv, k0, g.inv_h0, g.inv_h0sq, er, hr);
+    dir_entries<PER>(j, kv, k1, g.inv_h1, g.inv_h1sq, ec, hc);
+    m = fmaxf(m, er[3] + ec[3]);                         // both directions touch the pixel itself
+#pragma unroll
+    for (int d = 0; d < 7; ++d) {
+        if (d == 3) continue;
+        if (hr[d]) m = fmaxf(m, er[d]);
+        if (hc[d]) m = fmaxf(m, ec[d]);
+    }
+    int off[4]; float c[4];
+    if (i == 0 || i == P - 1) {                          // bc_x0 = -p_0 (row 0), +p_0 (row P-1)
+        const int n = stencil1<PER>(i, off, c);
+        const float sg = (i == 0) ? -g.inv_h0 : g.inv_h0;
+        for (int k = 0; k < n; ++k) m = fmaxf(m, sg * c[k]);
+    }
+    if (j == 0 || j == P - 1) {                          // bc_x1 = +s p_1 (column 0), -s p_1 (column P-1)
+        const int n = stencil1<PER>(j, off, c);
+        const float sg = ((j == 0) ? g.bc1_sign : -g.bc1_sign) * g.inv_h1;
+        for (int k = 0; k < n; ++k) m = fmaxf(m, sg * c[k]);
+    }
+    return m;
+}
+
 template <bool PER>
 __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const float* __restrict__ x0hat,
                                                                           float* __restrict__ out, DarcyGeom g) {
@@ -547,30 +595,7 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const
     float m = 0.f;                                       // the Jacobian is sparse: zero entries take part in the max
     for (int q = threadIdx.x; q < PP; q += blockDim.x) {
         const int i = q / P, j = q - i * P;
-        const float kv = sk[q];
-        const float k0 = d_row<PER>(sk, i, j, g.inv_h0), k1 = d_col<PER>(sk, i, j, g.inv_h1);
-        float er[7], ec[7];
-        bool hr[7], hc[7];
-        dir_entries<PER>(i, kv, k0, g.inv_h0, g.inv_h0sq, er, hr);
-        dir_entries<PER>(j, kv, k1, g.inv_h1, g.inv_h1sq, ec, hc);
-        m = fmaxf(m, er[3] + ec[3]);                     // both directions touch the pixel itself
-#pragma unroll
-        for (int d = 0; d < 7; ++d) {
-            if (d == 3) continue;
-            if (hr[d]) m = fmaxf(m, er[d]);
-            if (hc[d]) m = fmaxf(m, ec[d]);
-        }
-        int off[4]; float c[4];
-        if (i == 0 || i == P - 1) {                      // bc_x0 = -p_0 (row 0), +p_0 (row P-1)
-            const int n = stencil1<PER>(i, off, c);
-            const float sg = (i == 0) ? -g.inv_h0 : g.inv_h0;
-            for (int k = 0; k < n; ++k) m = fmaxf(m, sg * c[k]);
-        }
-        if (j == 0 || j == P - 1) {                      // bc_x1 = +s p_1 (column 0), -s p_1 (column P-1)
-            const int n = stencil1<PER>(j, off, c);
-            const float sg = ((j == 0) ? g.bc1_sign : -g.bc1_sign) * g.inv_h1;
-            for (int k = 0; k < n; ++k) m = fmaxf(m, sg * c[k]);
-        }
+        m = jacobian_max_pixel<PER>(sk, i, j, g, m);
     }
     m = warp_max(m);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
@@ -579,6 +604,97 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_jacobian_max_kernel(const
         float r = red[0];
         for (int w = 1; w < DARCY_THREADS / 32; ++w) r = fmaxf(r, red[w]);
         out[b] = r;
+    }
+}
+
+// ---- CoCoGen corrections, all steps of a sample in one CTA ----------------------------------------------------------
+// The corrections move p only, so K -- and with it max dr/dp and the step size -- is fixed for the whole launch, and
+// the residual is affine in p: each step is a fixed-step gradient step on sum r^2 with the same operator.  One CTA owns
+// one sample; p, K and the A / U0 / U1 product planes of the p adjoint stay in shared memory (80 KB) for every step:
+//   forward stencil -> products of 2r -> barrier -> adjoint gather + update of p -> barrier.
+// Each step computes what one multi-launch correction does (residual, cotangent 2r, pidm_darcy_residual_bwd's p
+// component, p -= eps * dp with eps = 1e-6 / min(max dr/dp, 1e12)); the final residual is darcy_fwd_kernel's stencil.
+struct DarcyCocogenSmem {
+    float red[DG_THREADS / 32];
+    float p[PP];
+    float k[PP];
+    float prod[3][PP];         // A, U0, U1
+};
+
+template <bool PER>
+__global__ void __launch_bounds__(DG_THREADS, 1) darcy_cocogen_kernel(float* __restrict__ x /*[B,2,P,P]*/,
+                                                                     const float* __restrict__ fs,
+                                                                     float* __restrict__ residual /*[B,P*P,3]*/,
+                                                                     const long long* __restrict__ t, int n_active,
+                                                                     int steps, DarcyGeom g) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    DarcyCocogenSmem& S = *reinterpret_cast<DarcyCocogenSmem*>(smem_raw);
+    const int tid = threadIdx.x, b = blockIdx.x;
+    pdl_trigger();
+    pdl_wait();
+    if (t != nullptr && !(t[b] < n_active)) return;     // inactive sample: neither read nor written
+    float* xb = x + (size_t)b * 2 * PP;
+    for (int q = tid; q < PP / 4; q += DG_THREADS) {
+        reinterpret_cast<float4*>(S.p)[q] = reinterpret_cast<const float4*>(xb)[q];
+        reinterpret_cast<float4*>(S.k)[q] = reinterpret_cast<const float4*>(xb + PP)[q];
+    }
+    __syncthreads();
+    float m = 0.f;                                       // max dr/dp, as darcy_jacobian_max_kernel
+    for (int q = tid; q < PP; q += DG_THREADS) m = jacobian_max_pixel<PER>(S.k, q / P, q % P, g, m);
+    m = warp_max(m);
+    if ((tid & 31) == 0) S.red[tid >> 5] = m;
+    __syncthreads();
+    m = S.red[0];
+    for (int w = 1; w < DG_THREADS / 32; ++w) m = fmaxf(m, S.red[w]);
+    // torch: 1e-6 / clamp(m, max=1e12) is reciprocal(m) * 1e-6 (NaN propagates through the clamp)
+    const float eps = __fmul_rn(1.f / (m > 1e12f ? 1e12f : m), 1e-6f);
+    float* sA = S.prod[0];
+    float* sU0 = S.prod[1];
+    float* sU1 = S.prod[2];
+#pragma unroll 1
+    for (int s = 0; s < steps; ++s) {
+#pragma unroll
+        for (int u = 0; u < DG_QUADS; ++u) {
+            const int q = tid + u * DG_THREADS;
+            const int i = q / (P / 4), j0 = (q % (P / 4)) * 4;
+            float req[4], rb0[4], rb1[4], kv[4], k0[4], k1[4], p0[4], p1[4], lap[4];
+            residual_quad_full<PER>(S.p, S.k, fs, i, j0, g, req, rb0, rb1, kv, k0, k1, p0, p1, lap);
+            float ge[4], g0[4], g1[4], a[4], u0[4], u1[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { ge[k] = 2.f * req[k]; g0[k] = 2.f * rb0[k]; g1[k] = 2.f * rb1[k]; }
+            p_products(ge, g0, g1, kv, k0, k1, i, j0, g, a, u0, u1);
+            const int o = i * P + j0;
+            *reinterpret_cast<float4*>(sA + o) = make_float4(a[0], a[1], a[2], a[3]);
+            *reinterpret_cast<float4*>(sU0 + o) = make_float4(u0[0], u0[1], u0[2], u0[3]);
+            *reinterpret_cast<float4*>(sU1 + o) = make_float4(u1[0], u1[1], u1[2], u1[3]);
+        }
+        __syncthreads();
+        // the gather reads only the product planes, so p is updated in place
+#pragma unroll
+        for (int u = 0; u < DG_QUADS; ++u) {
+            const int q = tid + u * DG_THREADS;
+            const int i = q / (P / 4), j0 = (q % (P / 4)) * 4;
+            float4* pq = reinterpret_cast<float4*>(S.p + i * P + j0);
+            float4 pv = *pq;
+            pv.x -= __fmul_rn(eps, p_adjoint<PER>(sA, sU0, sU1, i, j0, g));   // eps * dp rounded, then subtracted
+            pv.y -= __fmul_rn(eps, p_adjoint<PER>(sA, sU0, sU1, i, j0 + 1, g));
+            pv.z -= __fmul_rn(eps, p_adjoint<PER>(sA, sU0, sU1, i, j0 + 2, g));
+            pv.w -= __fmul_rn(eps, p_adjoint<PER>(sA, sU0, sU1, i, j0 + 3, g));
+            *pq = pv;
+        }
+        __syncthreads();
+    }
+    float* out = residual + (size_t)b * PP * 3;
+#pragma unroll 1
+    for (int q = tid; q < PP / 4; q += DG_THREADS) {
+        const int i = q / (P / 4), j0 = (q % (P / 4)) * 4;
+        float req[4], rb0[4], rb1[4];
+        residual_quad<PER>(S.p, S.k, fs, i, j0, g, req, rb0, rb1);
+        float4* o = reinterpret_cast<float4*>(out + (size_t)(i * P + j0) * 3);
+        o[0] = make_float4(req[0], rb0[0], rb1[0], req[1]);
+        o[1] = make_float4(rb0[1], rb1[1], req[2], rb0[2]);
+        o[2] = make_float4(rb1[2], req[3], rb0[3], rb1[3]);
+        reinterpret_cast<float4*>(xb)[q] = reinterpret_cast<const float4*>(S.p)[q];   // K is left untouched
     }
 }
 
@@ -687,6 +803,21 @@ static int launch_darcy_grad(const float* x0hat, const float* fs, const float* c
     return 0;
 }
 
+template <bool PER>
+static int launch_darcy_cocogen(float* x, const float* fs, float* residual, const long long* t, int n_active, int steps,
+                                int B, float domain_length, int reverse_d1, int flags, cudaStream_t stream) {
+    const size_t smem = sizeof(DarcyCocogenSmem);
+    static bool attr_set = false;                             // one flag per PER instantiation
+    if (!attr_set) {
+        PIDM_CUDA(cudaFuncSetAttribute(darcy_cocogen_kernel<PER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr_set = true;
+    }
+    PIDM_CUDA(launch_plain(darcy_cocogen_kernel<PER>, dim3(B), dim3(DG_THREADS), smem, stream, x, fs, residual, t,
+                           n_active, steps, make_geom(domain_length, reverse_d1, flags)));
+    PIDM_LAUNCH_CHECK("darcy_cocogen_kernel");
+    return 0;
+}
+
 template <int MODE>
 static int launch_darcy_grad_any(const float* x0hat, const float* fs, const float* cot, float* grad_x0hat,
                                  const float* target, const float* model_out, float* grad_model_out, const long long* t,
@@ -769,4 +900,17 @@ extern "C" int pidm_darcy_jacobian_max(const float* x0hat, float* max_dr_dp, int
                            make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_jacobian_max");
     return 0;
+}
+
+/* `steps` CoCoGen corrections of every active sample in one launch (residuals_darcy.py:209-240 applied `steps` times) */
+extern "C" int pidm_darcy_cocogen(float* x, const float* f_s, float* residual, const long long* t, int n_active,
+                                  int steps, int B, int pixels, float domain_length, int reverse_d1, int flags,
+                                  void* stream) {
+    if (int e = check_flags(flags)) return e;
+    PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
+    PIDM_REQUIRE(B > 0, "empty batch");
+    PIDM_REQUIRE(steps >= 0, "darcy_cocogen: steps = %d must not be negative", steps);
+    PIDM_REQUIRE(x != nullptr && f_s != nullptr && residual != nullptr, "darcy_cocogen: x, f_s and residual must not be NULL");
+    auto launch = (flags & PIDM_DARCY_PERIODIC) ? launch_darcy_cocogen<true> : launch_darcy_cocogen<false>;
+    return launch(x, f_s, residual, t, n_active, steps, B, domain_length, reverse_d1, flags, (cudaStream_t)stream);
 }

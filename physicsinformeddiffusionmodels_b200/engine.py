@@ -277,10 +277,18 @@ class SampleEngine:
     (pidm_mech_sample_input) -> U-Net (or the DDIM walk) -> the posterior kernel (pidm_mech_posterior_step).  The
     residual, compliance and inequality are needed at t = 0 only and are evaluated once, on the last step's x0
     prediction; with residuals.topopt_eval and a solution the evaluation metrics use the fused solver.  A batch
-    smaller than `batch` is padded with copies of its last sample and the results are sliced."""
+    smaller than `batch` is padded with copies of its last sample and the results are sliced.
+
+    CoCoGen residual corrections (Darcy; N_correction, M_correction, correction_mode as in p_sample_loop, reference
+    denoising_utils.py:433-459,517-540): while t < N_correction a step corrects the x0 estimate before the posterior
+    step ('x0') or the new sample after it ('xt'), and the step's residual is the corrected one.  Every step launches
+    `pidm_darcy_cocogen` with the device-side time index and n_active = N_correction, so one captured graph serves the
+    whole loop.  After the loop, M_correction corrections of x run in one launch and the residual returned is the one
+    after the last of them.  With trajectory=True those M corrections add ONE entry, the final corrected state
+    (p_sample_loop records each of them).  N_correction = M_correction = 0 launches nothing extra."""
 
     def __init__(self, model, diffusion, residuals, batch, image_shape=(2, 64, 64), surpress_noise=True, use_graph=True,
-                 steps_per_graph=None, external_noise=False):
+                 steps_per_graph=None, external_noise=False, N_correction=0, M_correction=0, correction_mode='none'):
         from .denoising_utils import _axpby, image_to_b_xy_c, generalized_b_xy_c_to_image
         self._axpby, self._to_rows, self._to_img = _axpby, image_to_b_xy_c, generalized_b_xy_c_to_image
         self.model, self.diffusion, self.residuals = model, diffusion, residuals
@@ -294,6 +302,14 @@ class SampleEngine:
         self.k = steps_per_graph if use_graph else 1
         self.external_noise = external_noise
         self.mechanics = getattr(residuals, 'gov_eqs', 'darcy') == 'mechanics'
+        self.N_correction, self.M_correction = int(N_correction), int(M_correction)
+        if self.N_correction < 0 or self.M_correction < 0:
+            raise ValueError(f'N_correction = {N_correction} and M_correction = {M_correction} must not be negative')
+        if self.N_correction and correction_mode not in ('x0', 'xt'):
+            raise ValueError(f"correction_mode must be 'x0' or 'xt' with N_correction > 0 (got {correction_mode!r})")
+        if (self.N_correction or self.M_correction) and self.mechanics:
+            raise ValueError('CoCoGen correction is only implemented for the Darcy flow study (reference main.py:37-38).')
+        self.correction_mode = correction_mode
         if self.mechanics:
             assert tuple(image_shape) == (3, 65, 65), 'the topology-optimisation model samples [B, 3, 65, 65]'
             self.batch = batch
@@ -323,13 +339,19 @@ class SampleEngine:
             model_out = out['model_out']
             if model_out.dim() == 3:
                 model_out = self._to_img(model_out)
-            z = self.z[j] if self.external_noise else torch.randn_like(x)   # drawn at every step, t == 0 included
-            new_x = self._axpby(self.c1[t].contiguous(), model_out.float(), self.c2[t].contiguous(), x,
-                                self.sigma[t].contiguous(), z)
             if self.residual is None:
                 self.residual = torch.empty_like(out['residual'])
             self.residual.copy_(out['residual'])
+            correct = self.N_correction > 0
+            if correct and self.correction_mode == 'x0':   # the corrected x0 estimate feeds the posterior step
+                model_out = model_out.float().clone(memory_format=torch.contiguous_format)
+                self.residuals.cocogen(model_out, self.residual, 1, t, self.N_correction)
+            z = self.z[j] if self.external_noise else torch.randn_like(x)   # drawn at every step, t == 0 included
+            new_x = self._axpby(self.c1[t].contiguous(), model_out.float(), self.c2[t].contiguous(), x,
+                                self.sigma[t].contiguous(), z)
             self.x.copy_(new_x)
+            if correct and self.correction_mode == 'xt':
+                self.residuals.cocogen(self.x, self.residual, 1, t, self.N_correction)
             self.t.sub_(1)
 
     def _mech_step_body(self, j=0):
@@ -422,6 +444,10 @@ class SampleEngine:
                 self._graph.replay()
             else:
                 self._step_body()
+            if trajectory:
+                traj.append(self.x[:n].clone())
+        if self.M_correction:
+            self.residuals.cocogen(self.x, self.residual, self.M_correction)
             if trajectory:
                 traj.append(self.x[:n].clone())
         traj = torch.stack(traj) if trajectory else None

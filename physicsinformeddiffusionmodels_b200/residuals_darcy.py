@@ -120,25 +120,33 @@ class ResidualsDarcy:
             return output
         raise ValueError('Unknown reduction method.')
 
+    def cocogen(self, x, residual, steps, t=None, n_active=0):
+        """`steps` CoCoGen corrections of x [B,2,P,P] (contiguous fp32, updated in place) in one launch
+        (`pidm_darcy_cocogen`); residual [B,P*P,3] receives the residual of the corrected fields.  With t [B] int64 on
+        the device only the samples with t[b] < n_active are corrected, and the other rows of x and residual are left
+        as they are.  The step size 1e-6 / max dr/dp is computed once per launch: the corrections leave K unchanged."""
+        from ._lib import call, stream
+        ops._need_cuda(x, residual, t)
+        ops._need_f32(x=x, residual=residual)
+        B, C, P, _ = x.shape
+        assert C == 2 and residual.shape == (B, P * P, 3), (x.shape, residual.shape)
+        assert t is None or (t.dtype == torch.int64 and t.shape == (B,) and t.is_contiguous()), 't must be int64 [B]'
+        call('pidm_darcy_cocogen', x, self.f_s_flat, residual, t, int(n_active), int(steps), B, P, *self._abi_geometry(),
+             stream())
+        return x, residual
+
     def residual_correction(self, x0_pred_in):
         """CoCoGen correction step (reference :209-240): p <- p - (1e-6 / max|dr/dp|) * d(sum r^2)/dp, residual re-evaluated.
         x0_pred_in [B, P*P, 2] is updated IN PLACE like the reference and returned with the corrected residual.
         The reference materialises the per-sample Jacobian dr/dp (12288 x 4096, vmap(jacfwd)) to take its maximum; the
-        residual is linear in p, so the maximum is evaluated analytically from the stencil coefficients and K
-        (`pidm_darcy_jacobian_max`), and d(sum r^2)/dp is one adjoint-stencil launch (`pidm_darcy_residual_bwd`)."""
-        from ._lib import call, stream
+        residual is linear in p, so the maximum is evaluated analytically from the stencil coefficients and K, and the
+        whole step is one `pidm_darcy_cocogen` launch with steps = 1."""
         assert len(x0_pred_in.shape) == 3, 'Model output must be a tensor shaped as b_xy_c.'
         with torch.no_grad():
             img = generalized_b_xy_c_to_image(x0_pred_in).contiguous().float()          # [B,2,P,P]
             B, _, P, _ = img.shape
-            r = ops.darcy_residual(img, self.f_s_flat, *self.geometry)
-            gx = torch.empty_like(img)
-            call('pidm_darcy_residual_bwd', img, self.f_s_flat, (2.0 * r).contiguous(), gx, B, P, *self._abi_geometry(),
-                 stream())
-            mx = torch.empty(B, device=img.device, dtype=torch.float32)
-            call('pidm_darcy_jacobian_max', img, mx, B, P, *self._abi_geometry(), stream())
-            eps = 1.e-6 / torch.clamp(mx, max=1e12)
-            x0_pred_in[:, :, 0] -= eps.unsqueeze(1) * gx[:, 0].reshape(B, -1)
-            residual_corrected = ops.darcy_residual(generalized_b_xy_c_to_image(x0_pred_in).contiguous().float(),
-                                                    self.f_s_flat, *self.geometry)
+            residual_corrected = torch.empty(B, P * P, 3, device=img.device, dtype=torch.float32)
+            self.cocogen(img, residual_corrected, 1)
+            if img.data_ptr() != x0_pred_in.data_ptr():      # a copy was corrected: write p back into the caller's tensor
+                x0_pred_in[:, :, 0] = img[:, 0].reshape(B, -1)
         return x0_pred_in, residual_corrected
