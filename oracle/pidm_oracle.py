@@ -13,6 +13,11 @@ tables, solidspy Q4 stiffness, the authors' mesh files) parity is pinned analyti
 DESIGN.md "Oracle" for the list.
 
 Each function cites the reference file:line it follows (paths relative to the original project's root).
+
+The study options are arguments of the functions they change, so that they combine as in the product: `periodic`
+(bcs='periodic') of the Darcy functions, cfg['padding_mode'] (Unet3D(padding_mode='circular')) of the U-Net, CoCoGen
+corrections in `p_sample_loop`, and the conditional topology-optimisation sampler `mechanics_p_sample_loop`.  Their
+defaults run the reference's default path.
 """
 import math
 from collections import OrderedDict
@@ -90,15 +95,21 @@ def q_sample(x0, t, noise, tables):
 
 
 def unet_config(dim=32, channels=2, out_dim=None, dim_mults=(1, 2, 4, 8), heads=8, dim_head=32,
-                groups=8, sigmoid_last_channel=False):
+                groups=8, sigmoid_last_channel=False, padding_mode='zeros'):
     return dict(dim=dim, channels=channels, out_dim=channels if out_dim is None else out_dim,
                 dim_mults=tuple(dim_mults), heads=heads, dim_head=dim_head, groups=groups,
-                sigmoid_last_channel=sigmoid_last_channel)
+                sigmoid_last_channel=sigmoid_last_channel, padding_mode=padding_mode)
+
+
+def _up_key(cfg, i):
+    # with padding_mode='circular' the up-sampling layer is the periodic transposed-conv module (unet_model.py:164-194)
+    return f'ups.{i}.3.conv_transpose' if cfg['padding_mode'] == 'circular' else f'ups.{i}.3'
 
 
 def unet_param_shapes(cfg):
     """Every state_dict key of the reference Unet3D with its shape, in reference order
-    (unet_model.py:406-528).  Includes the parameter holders that forward never touches."""
+    (unet_model.py:406-528).  Includes the parameter holders that forward never touches.  The order, and so the weights
+    make_test_state_dict draws, is the same for both padding modes; only the six up-sampling keys differ."""
     dim, ch, od = cfg['dim'], cfg['channels'], cfg['out_dim']
     hid = cfg['heads'] * cfg['dim_head']
     td = dim * 4
@@ -162,8 +173,8 @@ def unet_param_shapes(cfg):
         resblock(f'ups.{i}.1', ci, ci)
         linattn(f'ups.{i}.2', ci)
         if i < nres - 1:
-            S[f'ups.{i}.3.weight'] = (ci, ci, 1, 4, 4)
-            S[f'ups.{i}.3.bias'] = (ci,)
+            S[_up_key(cfg, i) + '.weight'] = (ci, ci, 1, 4, 4)
+            S[_up_key(cfg, i) + '.bias'] = (ci,)
     mid = dims[-1]
     resblock('mid_block1', mid, mid)
     S['mid_spatial_attn.fn.fn.fn.to_qkv.weight'] = (hid * 3, mid)
@@ -218,15 +229,28 @@ def _gn_silu(x, w, b, groups, scale_shift=None):
     return F.silu(x)
 
 
-def _resblock(sd, p, x, temb, groups):
+def _conv(x, w, b, pad, padding_mode, stride=1):
+    # a padded Conv3d on F=1 frames; padding_mode='circular' wraps the pad (unet_model.py:196,226,452)
+    if padding_mode == 'circular':
+        return F.conv2d(F.pad(x, (pad,) * 4, mode='circular'), w, b, stride=stride)
+    return F.conv2d(x, w, b, stride=stride, padding=pad)
+
+
+def conv_transpose_circular(x, w, b):
+    """The periodic 4x4 / stride-2 up-sampling of padding_mode='circular' (unet_model.py:164-194): circular pad 1, then
+    conv_transpose2d with padding 3 -- equal to the reference's pad 2 / padding 5."""
+    return F.conv_transpose2d(F.pad(x, (1,) * 4, mode='circular'), w, b, stride=2, padding=3)
+
+
+def _resblock(sd, p, x, temb, groups, padding_mode='zeros'):
     # ResnetBlock.forward, unet_model.py:255-267
     ss = None
     if temb is not None and (p + '.mlp.1.weight') in sd:
         e = F.linear(F.silu(temb), sd[p + '.mlp.1.weight'], sd[p + '.mlp.1.bias'])
         ss = e[:, :, None, None].chunk(2, dim=1)
-    h = F.conv2d(x, sd[p + '.block1.proj.weight'][:, :, 0], sd[p + '.block1.proj.bias'], padding=1)
+    h = _conv(x, sd[p + '.block1.proj.weight'][:, :, 0], sd[p + '.block1.proj.bias'], 1, padding_mode)
     h = _gn_silu(h, sd[p + '.block1.norm.weight'], sd[p + '.block1.norm.bias'], groups, ss)
-    h = F.conv2d(h, sd[p + '.block2.proj.weight'][:, :, 0], sd[p + '.block2.proj.bias'], padding=1)
+    h = _conv(h, sd[p + '.block2.proj.weight'][:, :, 0], sd[p + '.block2.proj.bias'], 1, padding_mode)
     h = _gn_silu(h, sd[p + '.block2.norm.weight'], sd[p + '.block2.norm.bias'], groups)
     if (p + '.res_conv.weight') in sd:
         x = F.conv2d(x, sd[p + '.res_conv.weight'][:, :, 0], sd[p + '.res_conv.bias'])
@@ -284,18 +308,21 @@ def unet_forward(sd, cfg, x, time, return_taps=False, cond=None, null_mask=None)
     """Unet3D.forward with F=1, self_condition=False (unet_model.py:542-623).
     x: [B,C,P,P] (or [B,P*P,C], converted as at :554-556).  Returns [B,out_dim,P,P].
     cond [B,C,P,P] (optional, the residual gradient of the guidance branch, :585-603) with null_mask [B] bool = samples
-    whose conditioning is dropped (classifier-free guidance; the reference draws it with prob_mask_like)."""
+    whose conditioning is dropped (classifier-free guidance; the reference draws it with prob_mask_like).
+    cfg['padding_mode'] = 'circular' (unet_model.py:161-199, 452): the stem, every ResnetBlock 3x3 and the down-sampling
+    convolutions pad circularly and the up-sampling layers are conv_transpose_circular; emb_conv[2] stays zero-padded as
+    in the reference (:524)."""
     if x.ndim == 3:
         p = int(math.isqrt(x.shape[1]))
         x = x.reshape(x.shape[0], p, p, x.shape[2]).permute(0, 3, 1, 2)
-    heads, dh, groups = cfg['heads'], cfg['dim_head'], cfg['groups']
+    heads, dh, groups, pm = cfg['heads'], cfg['dim_head'], cfg['groups'], cfg['padding_mode']
     taps = OrderedDict()
-    x = F.conv2d(x, sd['init_conv.weight'][:, :, 0], sd['init_conv.bias'], padding=3)
+    x = _conv(x, sd['init_conv.weight'][:, :, 0], sd['init_conv.bias'], 3, pm)
     taps['init_conv'] = x
     if cond is not None:
         c = torch.where(null_mask[:, None, None, None], torch.zeros_like(cond), cond)
         e = F.conv2d(c, sd['emb_conv.0.weight'], sd['emb_conv.0.bias'])
-        e = F.conv2d(F.gelu(e), sd['emb_conv.2.weight'], sd['emb_conv.2.bias'], padding=1)
+        e = F.conv2d(F.gelu(e), sd['emb_conv.2.weight'], sd['emb_conv.2.bias'], padding=1)     # zeros in both modes
         x = F.conv2d(torch.cat((x, e), dim=1), sd['combine_conv.weight'], sd['combine_conv.bias'])
     r = x
     t = time_embedding(sd, time, cfg['dim'])
@@ -303,32 +330,36 @@ def unet_forward(sd, cfg, x, time, return_taps=False, cond=None, null_mask=None)
     n_res = len(cfg['dim_mults'])
     skips = []
     for i in range(n_res):
-        x = _resblock(sd, f'downs.{i}.0', x, t, groups)
+        x = _resblock(sd, f'downs.{i}.0', x, t, groups, pm)
         if i == 0:
             taps['downs.0.0'] = x
-        x = _resblock(sd, f'downs.{i}.1', x, t, groups)
+        x = _resblock(sd, f'downs.{i}.1', x, t, groups, pm)
         x = _linear_attention(sd, f'downs.{i}.2', x, heads, dh)
         if i == 0:
             taps['downs.0.2'] = x
         skips.append(x)
         if i < n_res - 1:
-            x = F.conv2d(x, sd[f'downs.{i}.3.weight'][:, :, 0], sd[f'downs.{i}.3.bias'], stride=2, padding=1)
+            x = _conv(x, sd[f'downs.{i}.3.weight'][:, :, 0], sd[f'downs.{i}.3.bias'], 1, pm, stride=2)
     taps['down_out'] = x
-    x = _resblock(sd, 'mid_block1', x, t, groups)
+    x = _resblock(sd, 'mid_block1', x, t, groups, pm)
     x = _mid_attention(sd, 'mid_spatial_attn', x, heads, dh)
     taps['mid_attn'] = x
-    x = _resblock(sd, 'mid_block2', x, t, groups)
+    x = _resblock(sd, 'mid_block2', x, t, groups, pm)
     for i in range(n_res):
         x = torch.cat((x, skips.pop()), dim=1)
-        x = _resblock(sd, f'ups.{i}.0', x, t, groups)
-        x = _resblock(sd, f'ups.{i}.1', x, t, groups)
+        x = _resblock(sd, f'ups.{i}.0', x, t, groups, pm)
+        x = _resblock(sd, f'ups.{i}.1', x, t, groups, pm)
         x = _linear_attention(sd, f'ups.{i}.2', x, heads, dh)
         if i < n_res - 1:
-            x = F.conv_transpose2d(x, sd[f'ups.{i}.3.weight'][:, :, 0], sd[f'ups.{i}.3.bias'], stride=2, padding=1)
+            w, b = sd[_up_key(cfg, i) + '.weight'][:, :, 0], sd[_up_key(cfg, i) + '.bias']
+            if pm == 'circular':
+                x = conv_transpose_circular(x, w, b)
+            else:
+                x = F.conv_transpose2d(x, w, b, stride=2, padding=1)
         if i == 0:
             taps['ups.0'] = x
     x = torch.cat((x, r), dim=1)
-    x = _resblock(sd, 'final_conv.0', x, None, groups)
+    x = _resblock(sd, 'final_conv.0', x, None, groups, pm)
     x = F.conv2d(x, sd['final_conv.1.weight'][:, :, 0], sd['final_conv.1.bias'])
     if cfg['sigmoid_last_channel']:
         x = torch.cat((x[:, :-1], torch.sigmoid(x[:, -1:])), dim=1)     # :619-621 (in place there)
@@ -342,10 +373,19 @@ def unet_forward(sd, cfg, x, time, return_taps=False, cond=None, null_mask=None)
 # --------------------------------------------------------------------------------------------
 
 
-def fd_first(u, axis, h):
+# bcs='periodic' (grad_utils.py:76-81): the reference pads by one pixel with mode='circular' and applies the interior
+# ('C', 'C') stencil, so every pixel, boundary pixels included, uses the central second-order stencil with wrapped
+# neighbours.  Everything else is kept as with bcs='none': h = domain_length / (P-1) when pixels_at_boundary, f_s, and
+# the two BC channels on rows 0 / P-1 and columns 0 / P-1 with the same signs (built from the wrapped p_0 / p_1).
+
+
+def fd_first(u, axis, h, periodic=False):
     """Second-order first derivative along `axis` (-2 = rows = x0, -1 = cols = x1): central in the
     interior, one-sided 3-point at the two ends.  Net effect of the 9 conv2d + 9 slice-assigns at
-    grad_utils.py:64-146 with the acc=2 stencils (corner assignments win)."""
+    grad_utils.py:64-146 with the acc=2 stencils (corner assignments win).  periodic: central everywhere, neighbours
+    wrapped."""
+    if periodic:
+        return (torch.roll(u, -1, axis) - torch.roll(u, 1, axis)) * (0.5 / h)
     u = u.movedim(axis, -1)
     d = torch.empty_like(u)
     d[..., 1:-1] = (u[..., 2:] - u[..., :-2]) * (0.5 / h)
@@ -354,8 +394,11 @@ def fd_first(u, axis, h):
     return d.movedim(-1, axis)
 
 
-def fd_second(u, axis, h):
-    """Second-order second derivative: central [1,-2,1]/h^2; 4-point one-sided [2,-5,4,-1]/h^2 at ends."""
+def fd_second(u, axis, h, periodic=False):
+    """Second-order second derivative: central [1,-2,1]/h^2; 4-point one-sided [2,-5,4,-1]/h^2 at ends.  periodic:
+    central everywhere, neighbours wrapped."""
+    if periodic:
+        return (torch.roll(u, -1, axis) - 2.0 * u + torch.roll(u, 1, axis)) / (h * h)
     u = u.movedim(axis, -1)
     d = torch.empty_like(u)
     h2 = h * h
@@ -363,6 +406,27 @@ def fd_second(u, axis, h):
     d[..., 0] = (2.0 * u[..., 0] - 5.0 * u[..., 1] + 4.0 * u[..., 2] - u[..., 3]) / h2
     d[..., -1] = (2.0 * u[..., -1] - 5.0 * u[..., -2] + 4.0 * u[..., -3] - u[..., -4]) / h2
     return d.movedim(-1, axis)
+
+
+def stencil_gradients(u, mode, d0, d1, periodic=False):
+    """StencilGradients(periodic=...).forward for one mode on [..., P, P]"""
+    if mode == 'd_d0':
+        return fd_first(u, -2, d0, periodic)
+    if mode == 'd_d1':
+        return fd_first(u, -1, d1, periodic)
+    if mode == 'd_d00':
+        return fd_second(u, -2, d0, periodic)
+    if mode == 'd_d11':
+        return fd_second(u, -1, d1, periodic)
+    if mode == 'd_d01':
+        return fd_first(fd_first(u, -1, d1, periodic), -2, d0, periodic)
+    raise ValueError(mode)
+
+
+def spacing(P, domain_length=1.0, reverse_d1=True, pixels_at_boundary=True):
+    """(d0, d1) of ResidualsDarcy (residuals_darcy.py:24-33)"""
+    d0 = domain_length / (P - 1) if pixels_at_boundary else domain_length / P
+    return d0, (-d0 if reverse_d1 else d0)
 
 
 def darcy_source(pixels=64, w=0.125, r=10.0, dtype=torch.float32):
@@ -376,17 +440,16 @@ def darcy_source(pixels=64, w=0.125, r=10.0, dtype=torch.float32):
     return f.to(dtype)
 
 
-def darcy_residual(x0_pred, domain_length=1.0, reverse_d1=True, pixels_at_boundary=True):
+def darcy_residual(x0_pred, domain_length=1.0, reverse_d1=True, pixels_at_boundary=True, periodic=False):
     """ResidualsDarcy.compute_residual on a given x0_pred [B,2,P,P] (residuals_darcy.py:134-183).
     Returns residual [B, P*P, 3] = (eq_0, bc_x0, bc_x1).
-    eq_0 = -(K p_00 + K_0 p_0) - (K p_11 + K_1 p_1) - f_s."""
+    eq_0 = -(K p_00 + K_0 p_0) - (K p_11 + K_1 p_1) - f_s.  periodic: bcs='periodic' (see fd_first)."""
     B, C, P, _ = x0_pred.shape
-    d0 = domain_length / (P - 1) if pixels_at_boundary else domain_length / P
-    d1 = -d0 if reverse_d1 else d0
+    d0, d1 = spacing(P, domain_length, reverse_d1, pixels_at_boundary)
     p, K = x0_pred[:, 0], x0_pred[:, 1]
-    p0, p1 = fd_first(p, -2, d0), fd_first(p, -1, d1)
-    p00, p11 = fd_second(p, -2, d0), fd_second(p, -1, d1)
-    K0, K1 = fd_first(K, -2, d0), fd_first(K, -1, d1)
+    p0, p1 = fd_first(p, -2, d0, periodic), fd_first(p, -1, d1, periodic)
+    p00, p11 = fd_second(p, -2, d0, periodic), fd_second(p, -1, d1, periodic)
+    K0, K1 = fd_first(K, -2, d0, periodic), fd_first(K, -1, d1, periodic)
     fs = darcy_source(P, dtype=x0_pred.dtype).to(x0_pred.device)     # (device-aware: bench's torch-CUDA leg runs this on the GPU)
     eq0 = (-K * p00 - K0 * p0) + (-K * p11 - K1 * p1) - fs
     bc0 = torch.zeros_like(p)
@@ -399,16 +462,86 @@ def darcy_residual(x0_pred, domain_length=1.0, reverse_d1=True, pixels_at_bounda
     return torch.stack([eq0, bc0, bc1], dim=-1).reshape(B, P * P, 3)
 
 
+def darcy_stencils(P, periodic=False):
+    """The stencils of darcy_residual at its default geometry as [P,P] fp64 matrices (D1_0, D2_0, D1_1, D2_1):
+    fd_first(u, -2, d0) = D1_0 u and fd_first(u, -1, d1) = u D1_1^T, likewise fd_second with D2.  Their absolute values
+    bound every rounding of an fp32 evaluation of the stencils."""
+    mats = []
+    for h in spacing(P):
+        D1 = torch.zeros(P, P, dtype=torch.float64)
+        D2 = torch.zeros(P, P, dtype=torch.float64)
+        for i in range(P):
+            if periodic or 0 < i < P - 1:
+                D1[i, (i - 1) % P] -= 0.5
+                D1[i, (i + 1) % P] += 0.5
+                D2[i, (i - 1) % P] += 1.
+                D2[i, i] -= 2.
+                D2[i, (i + 1) % P] += 1.
+            elif i == 0:
+                D1[0, :3] = torch.tensor([-1.5, 2., -0.5], dtype=torch.float64)
+                D2[0, :4] = torch.tensor([2., -5., 4., -1.], dtype=torch.float64)
+            else:
+                D1[-1, -3:] = torch.tensor([0.5, -2., 1.5], dtype=torch.float64)
+                D2[-1, -4:] = torch.tensor([-1., 4., -5., 2.], dtype=torch.float64)
+        mats += [D1 / h, D2 / (h * h)]
+    return mats
+
+
+def along_rows(M, u):
+    """M applied along axis -2 of u [B,P,P]"""
+    return torch.einsum('ij,bjk->bik', M, u)
+
+
+def along_cols(M, u):
+    """M applied along axis -1 of u [B,P,P]"""
+    return torch.einsum('kj,bij->bik', M, u)
+
+
+def darcy_residual_matrix(x, periodic=False, absolute=False, stencils=None):
+    """darcy_residual at its default geometry from the darcy_stencils matrices, x [B,2,P,P] fp64 -> [B,P*P,3]: the
+    fp64 reference the GPU tests compare fp32 kernels with.  absolute=True evaluates it with |stencils|, |fields| and
+    |f_s|, which bounds every intermediate of an fp32 evaluation.  `stencils` replaces darcy_stencils(P, periodic)."""
+    P = x.shape[-1]
+    mats = darcy_stencils(P, periodic) if stencils is None else stencils
+    if absolute:
+        mats, x = [m.abs() for m in mats], x.abs()
+    D1a, D2a, D1b, D2b = (m.to(x.device) for m in mats)
+    p, K = x[:, 0], x[:, 1]
+    p0, p1, K0, K1 = along_rows(D1a, p), along_cols(D1b, p), along_rows(D1a, K), along_cols(D1b, K)
+    lap = along_rows(D2a, p) + along_cols(D2b, p)
+    fs = darcy_source(P, dtype=torch.float64).to(x.device)
+    bc0, bc1 = torch.zeros_like(p), torch.zeros_like(p)
+    if absolute:
+        eq0 = K * lap + K0 * p0 + K1 * p1 + fs.abs()
+        bc0[:, 0], bc0[:, -1] = p0[:, 0], p0[:, -1]
+        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], p1[:, :, -1]
+    else:
+        eq0 = -K * lap - K0 * p0 - K1 * p1 - fs
+        bc0[:, 0], bc0[:, -1] = -p0[:, 0], p0[:, -1]
+        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], -p1[:, :, -1]
+    return torch.stack([eq0, bc0, bc1], dim=-1).reshape(x.shape[0], P * P, 3)
+
+
+def darcy_residual_vjp(x, cot, periodic=False, absolute=False):
+    """J^T cot of darcy_residual_matrix in fp64; absolute=True: |J|^T |cot| at |x| (the residual is bilinear in (p, K)
+    with non-negative coefficients in its absolute form, so this gradient bounds every product of the adjoint)"""
+    xa = (x.abs() if absolute else x).clone().requires_grad_(True)
+    r = darcy_residual_matrix(xa, periodic, absolute)
+    if absolute:
+        r = r - darcy_residual_matrix(torch.zeros_like(xa), periodic, True)      # drop the constant |f_s|
+    return torch.autograd.grad((r * (cot.abs() if absolute else cot)).sum(), xa)[0]
+
+
 # --------------------------------------------------------------------------------------------
 # A3/A10  training loss   (src/denoising_utils.py:554-558, 616-710)
 # --------------------------------------------------------------------------------------------
 
 
-def darcy_residual_gradient(x_t):
+def darcy_residual_gradient(x_t, periodic=False):
     """d mean|r(x_t)| / d x_t (residuals_darcy.py:117-120), [B,2,P,P]; a constant for the network (no graph kept)."""
     with torch.enable_grad():
         x = x_t.detach().clone().requires_grad_(True)
-        return torch.autograd.grad(darcy_residual(x).abs().mean(), x)[0]
+        return torch.autograd.grad(darcy_residual(x, periodic=periodic).abs().mean(), x)[0]
 
 
 def pidm_loss_from_x0pred(x0, x0_pred, residual, t, tables, c_data=1.0, c_residual=1e-3):
@@ -423,43 +556,60 @@ def pidm_loss_from_x0pred(x0, x0_pred, residual, t, tables, c_data=1.0, c_residu
 
 
 def darcy_training_loss(sd, cfg, x0, t, noise, tables, c_data=1.0, c_residual=1e-3, use_ddim_x0=False,
-                        guidance_null_mask=None):
+                        guidance_null_mask=None, periodic=False):
     """model_estimation_loss for gov_eqs='darcy' with t and eps supplied (so it is RNG-free).
-    guidance_null_mask [B] bool: residual-gradient guidance on (residuals_darcy.py:114-126) with that classifier-free mask."""
+    guidance_null_mask [B] bool: residual-gradient guidance on (residuals_darcy.py:114-126) with that classifier-free mask.
+    periodic: bcs='periodic' in the residual and in the guidance gradient."""
     xt = q_sample(x0, t, noise, tables)
     if guidance_null_mask is not None:
-        model_out = unet_forward(sd, cfg, xt, t, cond=darcy_residual_gradient(xt), null_mask=guidance_null_mask)
+        cond = darcy_residual_gradient(xt, periodic)
+        model_out = unet_forward(sd, cfg, xt, t, cond=cond, null_mask=guidance_null_mask)
         x0_hat = model_out
     elif use_ddim_x0:
         x0_hat, model_out = ddim_x0(sd, cfg, xt, t, tables)
     else:
         model_out = unet_forward(sd, cfg, xt, t)
         x0_hat = model_out
-    r = darcy_residual(x0_hat)
+    r = darcy_residual(x0_hat, periodic=periodic)
     loss, data, rabs = pidm_loss_from_x0pred(x0, model_out, r, t, tables, c_data, c_residual)
     return loss, dict(data=data, residual_abs=rabs, model_out=model_out, x0_hat=x0_hat, residual=r, x_t=xt)
 
 
-def cocogen_correction(x0_pred):
-    """ResidualsDarcy.residual_correction (residuals_darcy.py:209-240) on x0_pred [B,2,P,P]:
-    p <- p - (1e-6 / max(dr/dp)) * d(sum r^2)/dp, then the residual of the corrected field.  The reference obtains the
-    Jacobian dr/dp with vmap(jacfwd); the residual is affine in p, so here its columns are residual(e_j, K) - residual(0, K)
-    for the 4096 unit fields e_j (one batched call per sample)."""
+def jacobian_max(x0_pred, periodic=False):
+    """max_dr_dp [B]: the largest entry (signed, zeros included, as torch.max) of d residual / d p per sample, with the
+    reference's clamp(max=1e12).  The reference obtains the Jacobian with vmap(jacfwd); the residual is affine in p, so
+    here its columns are residual(e_j, K) - residual(0, K) for the P*P unit fields e_j (one batched call per sample)."""
     B, _, P, _ = x0_pred.shape
-    x = x0_pred.detach().clone().requires_grad_(True)
-    r = darcy_residual(x)
-    dr_dp = torch.autograd.grad((r ** 2).sum(), x)[0][:, 0]
-    out = x0_pred.detach().clone()
+    out = torch.empty(B, dtype=x0_pred.dtype)
     for b in range(B):
-        K = x0_pred[b, 1].detach()
         basis = torch.zeros(P * P + 1, 2, P, P, dtype=x0_pred.dtype)
-        basis[:, 1] = K
+        basis[:, 1] = x0_pred[b, 1].detach()
         basis[torch.arange(P * P), 0, torch.arange(P * P) // P, torch.arange(P * P) % P] = 1.0
-        rr = darcy_residual(basis)
-        J = rr[:-1] - rr[-1:]                                    # [column j][row (pixel, channel)]
-        mx = torch.clamp(J.max(), max=1e12)
-        out[b, 0] = out[b, 0] - (1e-6 / mx) * dr_dp[b]
-    return out, darcy_residual(out)
+        rr = darcy_residual(basis, periodic=periodic)
+        out[b] = torch.clamp((rr[:-1] - rr[-1:]).max(), max=1e12)
+    return out
+
+
+def cocogen_steps(x0_pred, steps, periodic=False):
+    """`steps` successive ResidualsDarcy.residual_correction calls (residuals_darcy.py:209-240) on x0_pred [B,2,P,P]:
+    p <- p - (1e-6 / jacobian_max) * d(sum r^2)/dp.  A correction changes p only, so K and the step size stay fixed over
+    successive corrections of a field.  Returns (x, residual of x, [p after each correction])."""
+    eps = (1e-6 / jacobian_max(x0_pred, periodic)).view(-1, 1, 1)
+    x = x0_pred.detach().clone()
+    p_iterates = []
+    for _ in range(steps):
+        with torch.enable_grad():
+            xg = x.clone().requires_grad_(True)
+            dr_dp = torch.autograd.grad((darcy_residual(xg, periodic=periodic) ** 2).sum(), xg)[0][:, 0]
+        x[:, 0] = x[:, 0] - eps * dr_dp
+        p_iterates.append(x[:, 0].clone())
+    return x, darcy_residual(x, periodic=periodic), p_iterates
+
+
+def cocogen_correction(x0_pred, periodic=False):
+    """One residual_correction: (corrected x0_pred, its residual)."""
+    x, r, _ = cocogen_steps(x0_pred, 1, periodic)
+    return x, r
 
 
 # --------------------------------------------------------------------------------------------
@@ -476,9 +626,11 @@ def posterior_step(x_t, x0_pred, z, i, tables, suppress_noise=True):
     return mean + mask * sig * z
 
 
-def ddim_x0(sd, cfg, xt, t, tables, ddim_steps=0):
+def ddim_x0(sd, cfg, xt, t, tables, ddim_steps=0, mechanics=False):
     """ddim_sample_x0 with eta=0 (denoising_utils.py:712-787), per-sample grids linspace(0,t,steps+2).
-    Reference quirk kept: every network call sees the ORIGINAL x_t (model_input never updated, :741-753)."""
+    Reference quirk kept: every network call sees the ORIGINAL x_t (model_input never updated, :741-753).
+    mechanics: gov_eqs='mechanics', xt is the network input and the walk runs on its three solution channels.  The walk
+    draws a noise tensor that eta = 0 never uses (the reference draws it for RNG parity), so there is none here."""
     B = xt.shape[0]
     dt = xt.dtype
     seqs, seqs_next = [], []
@@ -488,7 +640,7 @@ def ddim_x0(sd, cfg, xt, t, tables, ddim_steps=0):
         seqs_next.append(list(reversed([-1] + seq[:-1])))
     cur_t = torch.tensor(seqs).T
     nxt_t = torch.tensor(seqs_next).T
-    cur_x = xt
+    cur_x = xt[:, :3] if mechanics else xt
     model_out = None
     v4 = lambda name, idx: tables[name].to(dt)[idx].view(B, 1, 1, 1)
     for k in range(cur_t.shape[0]):
@@ -508,17 +660,32 @@ def ddim_x0(sd, cfg, xt, t, tables, ddim_steps=0):
     return cur_x, model_out
 
 
-def p_sample_loop(sd, cfg, x_T, noises, tables, n_steps):
+def p_sample_loop(sd, cfg, x_T, noises, tables, n_steps, periodic=False, N_correction=0, M_correction=0,
+                  correction_mode='none', trajectory=False):
     """Ancestral loop for Darcy, mean-mode x0 (denoising_utils.py:508-545).  noises[k] is the z drawn
-    at loop iteration k (drawn even at t=0).  Returns (x_0 sample, residual of the last x0_pred)."""
+    at loop iteration k (drawn even at t=0).  Returns (x_0 sample, residual of the last x0_pred).
+    CoCoGen corrections (the correction branches of denoising_utils.py:433-459,517-540): while t < N_correction the x0
+    estimate ('x0') or the new sample ('xt') is corrected once and the step's residual is the corrected one; then
+    M_correction corrections of the final sample, and the residual is that of the last correction.
+    trajectory=True returns [x_T, one entry per step, one per post-loop correction] in place of the sample."""
     x = x_T
+    seq = [x]
     r = None
     for k, i in enumerate(reversed(range(n_steps))):
         tt = torch.full((x.shape[0],), i, dtype=torch.long)
         x0p = unet_forward(sd, cfg, x, tt)
-        r = darcy_residual(x0p)
+        r = darcy_residual(x0p, periodic=periodic)
+        correct = i < N_correction
+        if correct and correction_mode == 'x0':
+            x0p, r = cocogen_correction(x0p, periodic)
         x = posterior_step(x, x0p, noises[k], i, tables)
-    return x, r
+        if correct and correction_mode == 'xt':
+            x, r = cocogen_correction(x, periodic)
+        seq.append(x)
+    for _ in range(M_correction):
+        x, r = cocogen_correction(x, periodic)
+        seq.append(x)
+    return (seq if trajectory else x), r
 
 
 # --------------------------------------------------------------------------------------------
@@ -605,6 +772,66 @@ def mechanics_training_loss(sd, cfg, inp, t, noise, tables, c_data=1.0, c_residu
     loss = loss + (lambda_opt * comp).mean()
     return loss, dict(data=data, residual_abs=r.abs().mean(), inequality=ineq.mean(), compliance=comp.mean(), model_out=out,
                       residual=r)
+
+
+def mechanics_p_sample_loop(sd, cfg, x_T, noises, conditioning, bcs, tables, n_steps, use_ddim_x0=False, ddim_steps=0):
+    """The reference's ancestral loop with a conditioning input (denoising_utils.py:388-545 with
+    residuals_mechanics_K.py:176-205).  x_T [B,3,65,65], noises[k] = the posterior z of loop iteration k (drawn at t = 0
+    too), conditioning [B,3,65,65], bcs [B,4,65,65].  Returns dict(x_first, x_final, x0_pred_last, residual, compliance,
+    inequality); the residual terms are those of the last step (t = 0)."""
+    x, out = x_T, {}
+    vf = conditioning[:, 0, 0, 0]
+    bcs_red = bilinear_resize(bcs, 64)
+    for k, i in enumerate(reversed(range(n_steps))):
+        tt = torch.full((x.shape[0],), i, dtype=torch.long)
+        net_in = torch.cat((bilinear_resize(torch.cat((x, conditioning), dim=1), 64), bcs_red), dim=1)
+        if use_ddim_x0:
+            x0p, mo = ddim_x0(sd, cfg, net_in, tt, tables, ddim_steps, mechanics=True)
+        else:
+            x0p = mo = unet_forward(sd, cfg, net_in, tt)
+        model_out = torch.cat((bilinear_resize(mo[:, :2], 65), F.pad(mo[:, 2], (0, 1, 0, 1)).unsqueeze(1)), dim=1)
+        x = posterior_step(x, model_out, noises[k], i, tables)
+        if k == 0:
+            out['x_first'] = x
+    r, comp, ineq = mechanics_residual(x0p, bcs, vf)
+    out.update(x_final=x, x0_pred_last=x0p, residual=r, compliance=comp, inequality=ineq)
+    return out
+
+
+def reduced_system(rho, bcs, KE=None):
+    """rho [nel,nel], bcs [4,nel+1,nel+1] -> (K scipy CSC fp64, f fp64) in the dof order 2*node + d: K(rho) with the
+    reference's modification (Dirichlet rows replaced by identity rows, columns kept, f zeroed on the Dirichlet dofs;
+    residuals_mechanics_K.py:296-325)."""
+    import numpy as np
+    import scipy.sparse as sp
+    rho = np.asarray(rho, dtype=np.float64)
+    bcs = np.asarray(bcs, dtype=np.float64)
+    nel = rho.shape[-1]
+    n = 2 * (nel + 1) ** 2
+    KE = (q4_plane_stress_stiffness() if KE is None else torch.as_tensor(KE)).double().numpy()
+    dofs = mechanics_mesh(nel).numpy()                                            # [nel^2, 8]
+    vals = rho.reshape(-1)[:, None, None] * KE[None]
+    rows = np.broadcast_to(dofs[:, :, None], vals.shape)
+    cols = np.broadcast_to(dofs[:, None, :], vals.shape)
+    K = sp.coo_matrix((vals.ravel(), (rows.ravel(), cols.ravel())), shape=(n, n)).tocsr()
+    fixed = np.stack((bcs[0].ravel(), bcs[1].ravel()), axis=1).ravel() != 0
+    f = np.stack((bcs[2].ravel(), bcs[3].ravel()), axis=1).ravel()
+    f[fixed] = 0.
+    K = sp.diags((~fixed).astype(np.float64)) @ K + sp.diags(fixed.astype(np.float64))
+    return K.tocsc(), f
+
+
+def fem_solve(rho, bcs, KE=None):
+    """u [B,2,nel+1,nel+1] fp64 with K(rho) u = f on the free dofs, u = 0 on the Dirichlet dofs: scipy's sparse direct
+    solve of reduced_system, the ground truth for the iterative solvers."""
+    import scipy.sparse.linalg as spla
+    rho, bcs = torch.as_tensor(rho), torch.as_tensor(bcs)
+    out = []
+    for b in range(rho.shape[0]):
+        K, f = reduced_system(rho[b].cpu().numpy(), bcs[b].cpu().numpy(), KE)
+        nn_ = bcs.shape[-1]
+        out.append(torch.from_numpy(spla.spsolve(K, f).reshape(nn_ * nn_, 2).T.reshape(2, nn_, nn_).copy()))
+    return torch.stack(out)
 
 
 # --------------------------------------------------------------------------------------------

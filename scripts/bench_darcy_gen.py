@@ -25,7 +25,6 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 N_PTS, BW = 4096, 195
 FACTOR_FLOP = N_PTS * BW * (BW + 3) + 2 * N_PTS * BW          # Cholesky + forward substitution, per sample
@@ -69,7 +68,7 @@ def main():
     __graft_entry__.build()
     from physicsinformeddiffusionmodels_b200._lib import call, stream
     from physicsinformeddiffusionmodels_b200.darcy_data_generation import DarcyDataGenerator
-    import darcy_gen_oracle as DO
+    from oracle import darcy_gen_oracle as DO
 
     out = {}
     out['card'], out['power_limit_and_max_sm_clock'] = card()

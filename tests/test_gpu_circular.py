@@ -2,24 +2,16 @@
 Darcy network (forward, dgrad, weight gradient) per element against fp64, the plans the halo'd operands get, and the
 network end to end against fixtures of the UNMODIFIED reference (scripts/make_golden_circular.py)."""
 import math
-import os
-import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import circular_oracle as CO  # noqa: E402
+from checks import rel
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 U = 2.0 ** -24
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 # ---- halo kernel --------------------------------------------------------------------------------------------------
@@ -206,17 +198,15 @@ def env():
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = CO.circular_state_dict(O.make_test_state_dict(cfg, 0))
 
     def build(n_steps=100, padding_mode='circular', **kw):
         model = Unet3D(dim=32, channels=2, padding_mode=padding_mode).to(DEV)
-        model.load_state_dict(sd if padding_mode == 'circular' else O.make_test_state_dict(cfg, 0))
+        model.load_state_dict(O.make_test_state_dict(O.unet_config(dim=32, channels=2, padding_mode=padding_mode), 0))
         diff = DenoisingDiffusion(n_steps, DEV, kw.get('residual_grad_guidance', False))
         res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
                              device=DEV, bcs='periodic', domain_length=1., **kw)
         return model, diff, res
-    yield dict(O=O, ops=ops, build=build, cfg=cfg, sd=sd)
+    yield dict(O=O, ops=ops, build=build)
     ops.set_precision('bf16')
 
 
@@ -331,8 +321,8 @@ def test_circular_mechanics_model_forward_matches_oracle(env, mode, tol):
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
     O = env['O']
     env['ops'].set_precision(mode)
-    cfg = O.unet_config(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True)
-    sd = CO.circular_state_dict(O.make_test_state_dict(cfg, 5))
+    cfg = O.unet_config(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True, padding_mode='circular')
+    sd = O.make_test_state_dict(cfg, 5)
     model = Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True, padding_mode='circular').to(DEV)
     model.load_state_dict(sd)
     model.eval()
@@ -341,7 +331,7 @@ def test_circular_mechanics_model_forward_matches_oracle(env, mode, tol):
     t = torch.tensor([5, 60], device=DEV)
     with torch.no_grad():
         y = model(x, t)
-        ref = CO.unet_forward({k: v.to(DEV).double() for k, v in sd.items()}, cfg, x.double(), t)
+        ref = O.unet_forward({k: v.to(DEV).double() for k, v in sd.items()}, cfg, x.double(), t)
     assert y.shape == (2, 3, 64, 64)
     assert rel(y, ref) < tol, rel(y, ref)
 

@@ -2,28 +2,19 @@
 unmodified reference's fixtures, against the multi-launch composition it replaces and against the fp64 oracle, its
 device-side predication, and the corrected `SampleEngine` (graph and eager) against the drop-in
 `DenoisingDiffusion.p_sample_loop` and the reference's corrected sampling loop."""
-import os
-import sys
-
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import cocogen_oracle as CO  # noqa: E402
+from checks import rel
+from oracle import pidm_oracle as O
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 P = 64
 
 
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
-
-
 @pytest.fixture(scope='module')
 def env():
-    from oracle import pidm_oracle as O
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
@@ -115,7 +106,7 @@ def test_steps_match_composition_and_reference(env, golden, bcs, fixture, steps)
     if bcs == 'none' and steps == 200:
         # fp64 oracle: p is rounded to fp32 after each of the 200 steps, and the residual, a small difference of
         # second-difference terms of order K p / h^2, magnifies those roundings (measured 1.0e-4 on an H100)
-        xo, ro, _ = CO.cocogen_steps(x0.double(), steps)
+        xo, ro, _ = O.cocogen_steps(x0.double(), steps)
         d_o = xo[:, 0] - x0.double()[:, 0]
         assert rel(d, d_o) < 1e-3, rel(d, d_o)
         assert rel(r, ro) < 3e-4, rel(r, ro)

@@ -2,15 +2,12 @@
 unmodified reference's output and the host oracle, the KLE product, consistency with the training residual kernel,
 determinism and batch independence, guard regions, TrainEngine fed by generated batches, and the CSV round trip."""
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import darcy_gen_oracle as DO  # noqa: E402
+from oracle import darcy_gen_oracle as DO
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'

@@ -6,13 +6,10 @@ tolerances) and 'bf16' (production mode: bf16 GEMM operands / activations, fp32 
 import pytest
 import torch
 
+from checks import rel
+
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 @pytest.fixture(scope='module')

@@ -3,113 +3,31 @@ rejected by the same bounds), and the engine end to end: graph replay against th
 one training iteration of the unmodified reference (scripts/make_golden_guidance.py), the optimizer update of the
 guidance layers, the in-graph mask draw, the sharded draw and the guided sampler."""
 import math
-import os
-import sys
 
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import circular_oracle as CO  # noqa: E402
+from checks import C_BOUND, P, U, fields, guarded, guards_intact, rel, within
+from oracle import pidm_oracle as O
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-P = 64
-U = 2.0 ** -24
-C_BOUND = 16            # |y - r| <= C_BOUND * 2^-24 * A, as for the other Darcy kernels
-GUARD = 1024            # NaN guard elements on each side of every output
 
 
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
-
-
-def guarded(n, dtype=torch.float32):
-    buf = torch.full((n + 2 * GUARD,), float('nan'), device=DEV, dtype=dtype)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def guards_intact(buf):
-    return bool(torch.isnan(buf[:GUARD]).all() and torch.isnan(buf[-GUARD:]).all())
-
-
-# ---- fp64 Darcy residual from explicit stencil matrices (|matrices| give the absolute operator) ---------------------
-def _mats(h, periodic):
-    D1 = torch.zeros(P, P, dtype=torch.float64)
-    D2 = torch.zeros(P, P, dtype=torch.float64)
-    for i in range(P):
-        if periodic or 0 < i < P - 1:
-            D1[i, (i - 1) % P] -= 0.5
-            D1[i, (i + 1) % P] += 0.5
-            D2[i, (i - 1) % P] += 1.
-            D2[i, i] -= 2.
-            D2[i, (i + 1) % P] += 1.
-        elif i == 0:
-            D1[0, :3] = torch.tensor([-1.5, 2., -0.5], dtype=torch.float64)
-            D2[0, :4] = torch.tensor([2., -5., 4., -1.], dtype=torch.float64)
-        else:
-            D1[-1, -3:] = torch.tensor([0.5, -2., 1.5], dtype=torch.float64)
-            D2[-1, -4:] = torch.tensor([-1., 4., -5., 2.], dtype=torch.float64)
-    return D1 / h, D2 / (h * h)
-
-
-def residual_op(x, periodic, absolute=False):
-    """[B,2,P,P] fp64 -> [B,P*P,3] (pixels_at_boundary, reverse_d1, domain 1); absolute=True: |stencils|, |fields|, |f_s|"""
-    from oracle import pidm_oracle as O
-    d0 = 1.0 / (P - 1)
-    D1a, D2a = _mats(d0, periodic)
-    D1b, D2b = _mats(-d0, periodic)
-    if absolute:
-        D1a, D2a, D1b, D2b, x = D1a.abs(), D2a.abs(), D1b.abs(), D2b.abs(), x.abs()
-    D1a, D2a, D1b, D2b = (m.to(x.device) for m in (D1a, D2a, D1b, D2b))
-    p, K = x[:, 0], x[:, 1]
-
-    def row(M, u):
-        return torch.einsum('ij,bjk->bik', M, u)
-
-    def col(M, u):
-        return torch.einsum('kj,bij->bik', M, u)
-    p0, p1, K0, K1 = row(D1a, p), col(D1b, p), row(D1a, K), col(D1b, K)
-    lap = row(D2a, p) + col(D2b, p)
-    fs = O.darcy_source(P, dtype=torch.float64).to(x.device)
-    bc0, bc1 = torch.zeros_like(p), torch.zeros_like(p)
-    if absolute:
-        eq0 = K * lap + K0 * p0 + K1 * p1 + fs.abs()
-        bc0[:, 0], bc0[:, -1] = p0[:, 0], p0[:, -1]
-        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], p1[:, :, -1]
-    else:
-        eq0 = -K * lap - K0 * p0 - K1 * p1 - fs
-        bc0[:, 0], bc0[:, -1] = -p0[:, 0], p0[:, -1]
-        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], -p1[:, :, -1]
-    return torch.stack([eq0, bc0, bc1], dim=-1).reshape(x.shape[0], P * P, 3)
-
-
+# ---- fp64 Darcy residual from explicit stencil matrices (oracle.pidm_oracle.darcy_residual_matrix) ------------------
 def cond_reference(x, periodic, n_norm, edit=None):
     """(cond, bound A) in fp64, [B,P*P,2]: cond = J^T sign(r) / n_norm, A = |J|^T |sign(r)| / n_norm at |x|"""
     B = x.shape[0]
-    xr = x.clone().requires_grad_(True)
-    r = residual_op(xr, periodic)
-    cot = torch.sign(r.detach()) / n_norm
+    cot = torch.sign(O.darcy_residual_matrix(x, periodic)) / n_norm
     if edit == 'bc_row_sign':                 # the bc_x0 seeds of row 0 with the wrong sign
         cot[:, :P, 1] = -cot[:, :P, 1]
-    g = torch.autograd.grad((r * cot).sum(), xr)[0]
-    xa = x.abs().clone().requires_grad_(True)
-    ra = residual_op(xa, periodic, True) - residual_op(torch.zeros_like(x), periodic, True)
-    A = torch.autograd.grad((ra * cot.abs()).sum(), xa)[0]
+    g = O.darcy_residual_vjp(x, cot, periodic)
+    A = O.darcy_residual_vjp(x, cot, periodic, absolute=True)
     to_rows = lambda t: t.permute(0, 2, 3, 1).reshape(B, P * P, 2)      # noqa: E731
     return to_rows(g), to_rows(A)
 
 
-def fields(B, seed):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(B, 2, P, P, generator=g, dtype=torch.float64)
-    x[:, 1] = torch.exp(0.5 * x[:, 1])
-    return x.float().double().to(DEV)         # fp32-representable inputs
-
-
 def launch_abs_residual_grad(x, periodic, n_norm):
-    from oracle import pidm_oracle as O
     from physicsinformeddiffusionmodels_b200._lib import call, stream
     B = x.shape[0]
     buf, out = guarded(B * P * P * 2)
@@ -119,23 +37,18 @@ def launch_abs_residual_grad(x, periodic, n_norm):
     return buf, out.reshape(B, P * P, 2)
 
 
-def within(y, r, A, c=C_BOUND):
-    return bool(((y.double() - r).abs() <= c * U * A).all())
-
-
 @pytest.mark.parametrize('bcs', ['none', 'periodic'])
 @pytest.mark.parametrize('B', [1, 3, 32, 400])
 def test_abs_residual_grad_per_element(B, bcs):
     periodic = bcs == 'periodic'
-    x = fields(B, 1008 if B == 400 else 600 + B + (7 if periodic else 0))     # seeds without sign-ambiguous entries
-    # the stencil matrices restate the oracles' residuals
-    from oracle import pidm_oracle as O
-    import periodic_oracle as PO
-    r = residual_op(x, periodic)
-    ref_r = (PO if periodic else O).darcy_residual(x[:2].cpu())
+    # seeds without sign-ambiguous entries
+    x = fields(B, 1008 if B == 400 else 600 + B + (7 if periodic else 0), DEV)
+    # the stencil matrices restate the oracle's residual
+    r = O.darcy_residual_matrix(x, periodic)
+    ref_r = O.darcy_residual(x[:2].cpu(), periodic=periodic)
     assert rel(r[:2], ref_r) < 1e-12
     # no sign-ambiguous entry: every entry that is not structurally zero lies outside the residual's rounding bound
-    Ar = residual_op(x, periodic, absolute=True)
+    Ar = O.darcy_residual_matrix(x, periodic, absolute=True)
     live = r != 0
     assert bool((r.abs()[live] > C_BOUND * U * Ar[live]).all())
     assert bool((r[:, :, 1:][~live[:, :, 1:]] == 0).all()) and bool(live[:, :, 0].all())
@@ -150,7 +63,7 @@ def test_abs_residual_grad_per_element(B, bcs):
 @pytest.mark.parametrize('edit', ['local_norm', 'bc_row_sign'])
 def test_abs_residual_grad_rejects_edited_references(bcs, edit):
     periodic = bcs == 'periodic'
-    x = fields(32, 77)
+    x = fields(32, 77, DEV)
     n = 32 * P * P * 3
     if edit == 'local_norm':              # a shard of a 2-rank global batch normalised by its local count
         _, y = launch_abs_residual_grad(x, periodic, 2 * n)
@@ -264,22 +177,19 @@ def test_cond_embed_wgrad_per_element(B, dtype):
 # ---- engine ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope='module')
 def env():
-    from oracle import pidm_oracle as O
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
 
     def build(n_steps=100, bcs='none', padding_mode='zeros'):
         model = Unet3D(dim=32, channels=2, padding_mode=padding_mode).to(DEV)
-        model.load_state_dict(CO.circular_state_dict(sd) if padding_mode == 'circular' else sd)
+        model.load_state_dict(O.make_test_state_dict(O.unet_config(dim=32, channels=2, padding_mode=padding_mode), 0))
         diff = DenoisingDiffusion(n_steps, DEV, residual_grad_guidance=True)
         res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
                              device=DEV, bcs=bcs, domain_length=1., residual_grad_guidance=True)
         return model, diff, res
-    yield dict(O=O, ops=ops, build=build)
+    yield dict(ops=ops, build=build)
     ops.set_precision('bf16')
 
 
@@ -339,7 +249,7 @@ def test_guidance_step_matches_reference(env, golden, mode, tol_loss, tol_grad, 
     loss.backward()
     named = dict(model.named_parameters())
     n = int(gd['grad_sample'])
-    worst = {k: rel(env['O'].golden_sample(named[k[5:]].grad, n), v) for k, v in gd.items()
+    worst = {k: rel(O.golden_sample(named[k[5:]].grad, n), v) for k, v in gd.items()
              if k.startswith('grad_') and k not in ('grad_norm', 'grad_sample')}
     assert max(worst.values()) < tol_grad, sorted(worst.items(), key=lambda kv: -kv[1])[:5]
     gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
@@ -392,7 +302,7 @@ def test_sharded_cond_and_mask_are_slices_of_the_global_batch(env):
     from physicsinformeddiffusionmodels_b200.unet_model import draw_null_mask
     _, _, res = env['build']()
     world, B = 4, 6
-    x = fields(world * B, 31).float().permute(0, 2, 3, 1).reshape(world * B, P * P, 2).contiguous()
+    x = fields(world * B, 31, DEV).float().permute(0, 2, 3, 1).reshape(world * B, P * P, 2).contiguous()
     full = res.residual_gradient(x)
     torch.manual_seed(9)
     mfull = draw_null_mask(world * B, 0.1, DEV)

@@ -1,24 +1,15 @@
 """Conditional sampling of the topology-optimisation model (configs[2]) on the graph-replayed SampleEngine and its
 evaluation solve, against the unmodified reference (tests/golden/mechanics_sample_loop.pt, mechanics_eval.pt) and the
-fp64 sparse direct solve of tests/mech_sample_oracle.py."""
-import os
-import sys
-
+fp64 sparse direct solve of oracle/pidm_oracle.py."""
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import mech_sample_inputs as MI  # noqa: E402
-import mech_sample_oracle as MO  # noqa: E402
+import mech_sample_inputs as MI
+from checks import rel
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 METRICS = ('rel_CE_error_full_batch', 'vf_error_full_batch', 'fm_error_full_batch')
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 @pytest.fixture(scope='module')
@@ -245,7 +236,7 @@ def test_fused_solver_against_sparse_direct_solve(env, golden):
     KE = res.KE.double().cpu()
     report = {}
     for name, rho, bc in cases:
-        u_ref = MO.fem_solve(rho, bc, KE)
+        u_ref = env['O'].fem_solve(rho, bc, KE)
         rho_d, bc_d = rho.contiguous().to(DEV), bc.contiguous().to(DEV)
         u_t = res.fem_solve(rho_d, bc_d)
         u_f, iters, relres = res.fem_solve_fused(rho_d, bc_d)

@@ -5,13 +5,10 @@ TrainEngine (flat buffers, fused Adam/EMA, CUDA graph) on that branch."""
 import pytest
 import torch
 
+from checks import rel
+
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 @pytest.fixture(scope='module')

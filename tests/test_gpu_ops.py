@@ -7,14 +7,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from checks import rel
+
 pytestmark = pytest.mark.gpu
 
 DEV = 'cuda'
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 def nhwc(x, dtype):      # test-side layout helper: NCHW fp32 -> NHWC activations

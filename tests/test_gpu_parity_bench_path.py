@@ -6,13 +6,10 @@ instantiations and the schedule the bench runs."""
 import pytest
 import torch
 
+from checks import rel
+
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 @pytest.fixture(scope='module')

@@ -1,67 +1,24 @@
 """bcs='periodic' on the GPU: every periodic Darcy kernel per element against the fp64 periodic oracle, edited references
 rejected by the same predicate, and the engine end to end against the fixtures of the unmodified reference
 (scripts/make_golden_periodic.py) at the tolerances of the matching 'none' tests."""
-import os
-import sys
-
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import periodic_oracle as PO  # noqa: E402
+from checks import C_BOUND, P, U, fields, guarded, guards_intact, rel, within
+from oracle import pidm_oracle as O
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-P = 64
-U = 2.0 ** -24
-C_BOUND = 16            # |y - r| <= C_BOUND * 2^-24 * A: a handful of fp32 roundings along each stencil / product chain
-GUARD = 1024            # NaN guard floats on each side of every output
 
 
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
-
-
-# ---- fp64 reference and its absolute-value operator -----------------------------------------------------------------
-def _d1(u, ax, h, absolute=False):
-    if absolute:
-        return (torch.roll(u, -1, ax) + torch.roll(u, 1, ax)) * (0.5 / abs(h))
-    return PO.fd_first(u, ax, h)
-
-
-def _d2(u, ax, h, absolute=False):
-    if absolute:
-        return (torch.roll(u, -1, ax) + 2.0 * u + torch.roll(u, 1, ax)) / (h * h)
-    return PO.fd_second(u, ax, h)
-
-
+# ---- fp64 reference (oracle.pidm_oracle.darcy_residual_matrix) and the edits the predicate has to reject -------------
 def residual_op(x, absolute=False, edit=None):
-    """the periodic residual in fp64 ([B,P*P,3]); absolute=True evaluates it with |coefficients| on the given
-    (non-negative) fields, which bounds every intermediate of the fp32 evaluation.  `edit` builds the wrong references
-    the predicate has to reject."""
-    d0, d1 = PO.spacing(P)
-    p, K = x[:, 0], x[:, 1]
-    p0, p1, K0, K1 = _d1(p, -2, d0, absolute), _d1(p, -1, d1, absolute), _d1(K, -2, d0, absolute), _d1(K, -1, d1, absolute)
-    p00, p11 = _d2(p, -2, d0, absolute), _d2(p, -1, d1, absolute)
+    """the periodic residual in fp64 ([B,P*P,3]); absolute=True: its absolute-value operator"""
+    stencils = None
     if edit == 'one_sided_row0':                 # the wrap dropped at row 0: the one-sided stencils of bcs='none' there
-        from oracle import pidm_oracle as O
-        p0[:, 0], p00[:, 0], K0[:, 0] = (O.fd_first(p, -2, d0)[:, 0], O.fd_second(p, -2, d0)[:, 0],
-                                         O.fd_first(K, -2, d0)[:, 0])
-    fs = PO.O.darcy_source(P, dtype=torch.float64).to(x.device)
-    if absolute:
-        eq0 = K * (p00 + p11) + K0 * p0 + K1 * p1 + fs.abs()
-        bc0 = torch.zeros_like(p)
-        bc1 = torch.zeros_like(p)
-        bc0[:, 0], bc0[:, -1] = p0[:, 0], p0[:, -1]
-        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], p1[:, :, -1]
-    else:
-        eq0 = (-K * p00 - K0 * p0) + (-K * p11 - K1 * p1) - fs
-        bc0 = torch.zeros_like(p)
-        bc1 = torch.zeros_like(p)
-        bc0[:, 0], bc0[:, -1] = -p0[:, 0], p0[:, -1]
-        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], -p1[:, :, -1]          # reverse_d1
-    r = torch.stack([eq0, bc0, bc1], dim=-1).reshape(x.shape[0], P * P, 3)
+        stencils, one_sided = O.darcy_stencils(P, periodic=True), O.darcy_stencils(P)
+        stencils[0][0], stencils[1][0] = one_sided[0][0], one_sided[1][0]
+    r = O.darcy_residual_matrix(x, True, absolute, stencils)
     if edit == 'corner_sign':
         r[:, 0, 1] = -r[:, 0, 1]
     if edit == 'last_row_zero':
@@ -69,41 +26,11 @@ def residual_op(x, absolute=False, edit=None):
     return r
 
 
-def vjp(x, cot, absolute=False):
-    """J^T cot in fp64; absolute=True: |J|^T |cot| at |x| (the residual is bilinear in (p, K) with non-negative
-    coefficients in its absolute form, so this gradient bounds every product of the adjoint)"""
-    xa = (x.abs() if absolute else x).clone().requires_grad_(True)
-    r = residual_op(xa, absolute)
-    if absolute:
-        r = r - residual_op(torch.zeros_like(xa), True)           # drop the constant |f_s|
-    return torch.autograd.grad((r * (cot.abs() if absolute else cot)).sum(), xa)[0]
-
-
-def within(y, r, A, c=C_BOUND):
-    return bool(((y.double() - r).abs() <= c * U * A).all())
-
-
-def guarded(n):
-    buf = torch.full((n + 2 * GUARD,), float('nan'), device=DEV)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def guards_intact(buf):
-    return bool(torch.isnan(buf[:GUARD]).all() and torch.isnan(buf[-GUARD:]).all())
-
-
-def fields(B, seed):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(B, 2, P, P, generator=g, dtype=torch.float64)
-    x[:, 1] = torch.exp(0.5 * x[:, 1])
-    return x.float().double()            # fp32-representable inputs
-
-
 FLAGS = 1 | 2             # PIDM_DARCY_PIXELS_AT_BOUNDARY | PIDM_DARCY_PERIODIC
 
 
 def fs_dev():
-    return PO.O.darcy_source(P).to(DEV).contiguous()
+    return O.darcy_source(P).to(DEV).contiguous()
 
 
 def launch_fwd(x):
@@ -148,8 +75,8 @@ def test_periodic_vjp_per_element(B):
     torch.cuda.synchronize()
     assert guards_intact(buf) and not torch.isnan(gx).any()
     gx = gx.reshape(B, 2, P, P).cpu()
-    assert within(gx, vjp(x, cot), vjp(x, cot, absolute=True)), \
-        ((gx.double() - vjp(x, cot)).abs() / (U * vjp(x, cot, absolute=True))).max().item()
+    ref, A = O.darcy_residual_vjp(x, cot, True), O.darcy_residual_vjp(x, cot, True, absolute=True)
+    assert within(gx, ref, A), ((gx.double() - ref).abs() / (U * A)).max().item()
 
 
 def _loss_reference(x, m, tgt, t, tab_p2, tab_var, c_data, c_res):
@@ -164,10 +91,10 @@ def _loss_reference(x, m, tgt, t, tab_p2, tab_var, c_data, c_res):
     sums_A = torch.stack([(wd[:, None, None, None] * (m.abs() + tgt.abs()) ** 2).sum(),
                           (wr[:, None, None] * Ar ** 2).sum(), Ar.mean()])
     cot = 2 * wr[:, None, None] * r
-    gx = vjp(x, cot)
+    gx = O.darcy_residual_vjp(x, cot, True)
     # the fp32 cotangent 2 wr r carries the residual's own error (<= C_BOUND 2^-24 Ar) and that of wr: the adjoint is
     # bounded with twice 2 wr Ar, which leaves C_BOUND 2^-24 for each of the two
-    A_gx = vjp(x, 4 * wr[:, None, None] * Ar, absolute=True)
+    A_gx = O.darcy_residual_vjp(x, 4 * wr[:, None, None] * Ar, True, absolute=True)
     gm = 2 * wd[:, None, None, None] * (m - tgt)
     A_gm = 2 * wd[:, None, None, None] * (m.abs() + tgt.abs())
     return sums, sums_A, gx, A_gx, gm, A_gm
@@ -213,9 +140,10 @@ def test_periodic_fused_loss_per_element(B, variant):
 
 def _jacobian_max_ref(x):
     """largest entry (signed, zeros included) of d r / d p per sample in fp64, with an absolute bound per sample"""
-    d0, d1 = PO.spacing(P)
+    d0, d1 = O.spacing(P)
+    D1a, _, D1b, _ = O.darcy_stencils(P, periodic=True)
     K = x[:, 1]
-    K0, K1 = PO.fd_first(K, -2, d0), PO.fd_first(K, -1, d1)
+    K0, K1 = O.along_rows(D1a, K), O.along_cols(D1b, K)
     e = torch.stack([-K / d0 ** 2 + K0 * 0.5 / d0, -K / d0 ** 2 - K0 * 0.5 / d0,      # rows i-1, i+1
                      -K / d1 ** 2 + K1 * 0.5 / d1, -K / d1 ** 2 - K1 * 0.5 / d1,      # columns j-1, j+1
                      2 * K / d0 ** 2 + 2 * K / d1 ** 2], dim=1)                     # the pixel itself
@@ -238,21 +166,22 @@ def test_periodic_jacobian_max_per_element(B):
     ref, A = _jacobian_max_ref(x)
     assert within(out.cpu(), ref, A)
     if B <= 3:                                    # the closed form above against the oracle's explicit Jacobian
-        assert torch.allclose(PO.jacobian_max(x), ref, rtol=1e-9, atol=0)
+        assert torch.allclose(O.jacobian_max(x, periodic=True), ref, rtol=1e-9, atol=0)
 
 
 @pytest.mark.parametrize('B', BATCHES)
 @pytest.mark.parametrize('mode', ['d_d0', 'd_d1', 'd_d00', 'd_d11', 'd_d01'])
 def test_periodic_fd_stencil_per_element(B, mode):
     from physicsinformeddiffusionmodels_b200.grad_utils import StencilGradients
-    d0, d1 = PO.spacing(P)
+    d0, d1 = O.spacing(P)
     u = fields(B, 50 + B)[:, 0]
     y = StencilGradients(d0=d0, d1=d1, periodic=True)(u.float().to(DEV), mode).cpu()
-    r = PO.stencil_gradients(u, mode, d0, d1)
+    r = O.stencil_gradients(u, mode, d0, d1, periodic=True)
     ua = u.abs()
-    A = {'d_d0': lambda: _d1(ua, -2, d0, True), 'd_d1': lambda: _d1(ua, -1, d1, True),
-         'd_d00': lambda: _d2(ua, -2, d0, True), 'd_d11': lambda: _d2(ua, -1, d1, True),
-         'd_d01': lambda: _d1(_d1(ua, -1, d1, True), -2, d0, True)}[mode]()
+    D1a, D2a, D1b, D2b = (m.abs() for m in O.darcy_stencils(P, periodic=True))
+    A = {'d_d0': lambda: O.along_rows(D1a, ua), 'd_d1': lambda: O.along_cols(D1b, ua),
+         'd_d00': lambda: O.along_rows(D2a, ua), 'd_d11': lambda: O.along_cols(D2b, ua),
+         'd_d01': lambda: O.along_rows(D1a, O.along_cols(D1b, ua))}[mode]()
     assert within(y, r, A)
     from physicsinformeddiffusionmodels_b200._lib import call, stream
     buf, out = guarded(B * P * P)
@@ -265,7 +194,6 @@ def test_periodic_fd_stencil_per_element(B, mode):
 # ---- end to end ---------------------------------------------------------------------------------------------------
 @pytest.fixture(scope='module')
 def env():
-    from oracle import pidm_oracle as O
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
@@ -281,7 +209,7 @@ def env():
                              device=DEV, bcs='periodic', domain_length=1., **kw)
         assert res.periodic
         return model, diff, res
-    yield dict(O=O, ops=ops, build=build, cfg=cfg, sd=sd)
+    yield dict(ops=ops, build=build, cfg=cfg, sd=sd)
     ops.set_precision('bf16')
 
 
@@ -297,7 +225,7 @@ def test_periodic_training_loss_and_gradients_match_reference(env, golden, mode,
     assert abs(rabs / gd['residual_abs'].item() - 1) < tol_loss
     loss.backward()
     named = dict(model.named_parameters())
-    worst = {k: rel(env['O'].golden_sample(named[k[5:]].grad), v) for k, v in gd.items()
+    worst = {k: rel(O.golden_sample(named[k[5:]].grad), v) for k, v in gd.items()
              if k.startswith('grad_') and k != 'grad_norm'}
     assert max(worst.values()) < tol_grad, worst
     gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
@@ -368,7 +296,6 @@ def test_periodic_residual_gradient_guidance_matches_oracle(env):
     """guidance branch (cond = d mean|r(x_t)| / d x_t with the periodic residual) through the engine vs the periodic
     oracle, fp32, with a classifier-free mask that drops one sample"""
     env['ops'].set_precision('fp32')
-    O = env['O']
     g = torch.Generator().manual_seed(77)
     B = 4
     x0 = torch.randn(B, 2, 64, 64, generator=g)
@@ -376,7 +303,8 @@ def test_periodic_residual_gradient_guidance_matches_oracle(env):
     e = torch.randn(B, 2, 64, 64, generator=g)
     mask = torch.tensor([False, True, False, False])
     sdr = {k: v.clone().requires_grad_('freqs' not in k) for k, v in env['sd'].items()}
-    loss_ref, _ = PO.darcy_training_loss(sdr, env['cfg'], x0, t, e, O.diffusion_tables(100), guidance_null_mask=mask)
+    loss_ref, _ = O.darcy_training_loss(sdr, env['cfg'], x0, t, e, O.diffusion_tables(100), guidance_null_mask=mask,
+                                        periodic=True)
     loss_ref.backward()
     model, diff, res = env['build'](residual_grad_guidance=True)
     model._null_mask_override = mask.to(DEV)

@@ -4,13 +4,10 @@ the UNMODIFIED reference module (tests/golden/toy.pt): loss, tracked scalars, gr
 import pytest
 import torch
 
+from checks import rel
+
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-
-
-def rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 def residual_func(x):

@@ -1,19 +1,14 @@
-"""Unet3D(padding_mode='circular') on the CPU: the parameter surface against the reference, and the circular oracle
-(tests/circular_oracle.py) against fixtures produced by the UNMODIFIED reference (scripts/make_golden_circular.py)."""
-import os
-import sys
-
+"""Unet3D(padding_mode='circular') on the CPU: the parameter surface against the reference, and the oracle's
+padding_mode='circular' (oracle/pidm_oracle.py) against fixtures produced by the UNMODIFIED reference
+(scripts/make_golden_circular.py)."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import circular_oracle as CO  # noqa: E402
-from oracle import pidm_oracle as O  # noqa: E402
+from checks import rel
+from oracle import pidm_oracle as O
 
-
-def rel(a, b):
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+CIRCULAR = O.unet_config(dim=32, channels=2, padding_mode='circular')
 
 
 def test_circular_unet_keys_and_seeded_init(golden):
@@ -23,12 +18,12 @@ def test_circular_unet_keys_and_seeded_init(golden):
     sd = Unet3D(dim=32, channels=2, padding_mode='circular').state_dict()
     assert list(sd.keys()) == golden('unet_circular_keys.pt')['keys']
     torch.manual_seed(0)
-    sd0 = CO.circular_state_dict(Unet3D(dim=32, channels=2).state_dict())
-    assert list(sd0.keys()) == list(sd.keys()) and len(sd) == 317
+    sd0 = Unet3D(dim=32, channels=2).state_dict()
+    assert [k.replace('.conv_transpose.', '.') for k in sd] == list(sd0.keys()) and len(sd) == 317
     renamed = [k for k in sd if 'conv_transpose' in k]
     assert len(renamed) == 6
     for k, v in sd.items():
-        assert torch.equal(v, sd0[k]), k
+        assert torch.equal(v, sd0[k.replace('.conv_transpose.', '.')]), k
     gd = golden('unet_init_seed0.pt')
     for k, v in sd.items():
         ref = gd[k.replace('.conv_transpose.', '.')]
@@ -37,12 +32,11 @@ def test_circular_unet_keys_and_seeded_init(golden):
 
 def test_circular_load_state_dict_is_strict():
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
     m = Unet3D(dim=32, channels=2, padding_mode='circular')
-    m.load_state_dict(CO.circular_state_dict(sd), strict=True)
+    m.load_state_dict(O.make_test_state_dict(CIRCULAR, 0), strict=True)
     with pytest.raises(RuntimeError):
-        m.load_state_dict(sd, strict=True)                  # a zeros checkpoint has the old up-sampling keys
+        # a zeros checkpoint has the old up-sampling keys
+        m.load_state_dict(O.make_test_state_dict(O.unet_config(dim=32, channels=2), 0), strict=True)
 
 
 def test_circular_conv_specs():
@@ -69,15 +63,14 @@ def test_periodic_transposed_conv_identity():
     x = torch.randn(2, 8, 8, 8, generator=g, dtype=torch.float64)
     w = torch.randn(8, 4, 4, 4, generator=g, dtype=torch.float64)
     ref = F.conv_transpose2d(F.pad(x, (2,) * 4, mode='circular'), w, stride=2, padding=5)
-    assert torch.equal(CO.up_circ(x, w, None), ref)
+    assert torch.equal(O.conv_transpose_circular(x, w, None), ref)
 
 
 def test_circular_oracle_forward_matches_reference(golden):
     gd = golden('unet_circular_fwd.pt')
     cfg = O.unet_config(dim=32, channels=2)
-    sd = CO.circular_state_dict(O.make_test_state_dict(cfg, 0))
     with torch.no_grad():
-        y, taps = CO.unet_forward(sd, cfg, gd['x'], gd['t'], return_taps=True)
+        y, taps = O.unet_forward(O.make_test_state_dict(CIRCULAR, 0), CIRCULAR, gd['x'], gd['t'], return_taps=True)
         y0 = O.unet_forward(O.make_test_state_dict(cfg, 0), cfg, gd['x'], gd['t'])
     for k in ('init_conv', 'downs.0.0', 'downs.0.2', 'mid_attn', 'ups.0'):
         assert rel(O.golden_sample(taps[k]), gd['tap_' + k]) < 2e-5, k
@@ -88,12 +81,11 @@ def test_circular_oracle_forward_matches_reference(golden):
 @pytest.mark.parametrize('shift', [(8, 16), (24, 40), (0, 8)])
 def test_circular_oracle_rolls_exactly(shift):
     """with periodic padding every layer commutes with a roll by a multiple of 8 pixels (the coarsest level is 8x8)"""
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = {k: v.double() for k, v in CO.circular_state_dict(O.make_test_state_dict(cfg, 0)).items()}
+    sd = {k: v.double() for k, v in O.make_test_state_dict(CIRCULAR, 0).items()}
     g = torch.Generator().manual_seed(11)
     x = torch.randn(1, 2, 64, 64, generator=g, dtype=torch.float64)
     t = torch.tensor([17])
     with torch.no_grad():
-        y = CO.unet_forward(sd, cfg, x, t)
-        ys = CO.unet_forward(sd, cfg, torch.roll(x, shift, (2, 3)), t)
+        y = O.unet_forward(sd, CIRCULAR, x, t)
+        ys = O.unet_forward(sd, CIRCULAR, torch.roll(x, shift, (2, 3)), t)
     assert (ys - torch.roll(y, shift, (2, 3))).abs().max().item() < 1e-10

@@ -1,25 +1,16 @@
-"""The CoCoGen oracle (tests/cocogen_oracle.py) against fixtures produced by the UNMODIFIED reference
+"""The oracle's CoCoGen corrections (oracle/pidm_oracle.py) against fixtures produced by the UNMODIFIED reference
 (scripts/make_golden_cocogen.py): successive residual_correction calls and the sampling loop with corrections."""
-import os
-import sys
-
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import cocogen_oracle as CO  # noqa: E402
-
-O = CO.O
-
-
-def rel(a, b):
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+from checks import rel
+from oracle import pidm_oracle as O
 
 
 def test_successive_corrections_match_reference(golden):
     gd = golden('cocogen_steps.pt')
     n = gd['p_iterates'].shape[0]
-    x, r, p_it = CO.cocogen_steps(gd['x0_pred'], n)
+    x, r, p_it = O.cocogen_steps(gd['x0_pred'], n)
     p0 = gd['x0_pred'][:, 0]
     for k in range(n):
         # each correction is tiny (step 1e-6 / max dr/dp): compare the accumulated CHANGE of p, not the field
@@ -35,7 +26,7 @@ def test_one_step_equals_pidm_oracle():
     g = torch.Generator().manual_seed(3)
     x = torch.randn(2, 2, 64, 64, generator=g, dtype=torch.float64)
     x[:, 1] = x[:, 1].exp()
-    xa, ra, _ = CO.cocogen_steps(x, 1)
+    xa, ra, _ = O.cocogen_steps(x, 1)
     xb, rb = O.cocogen_correction(x)
     assert torch.equal(xa, xb) and torch.equal(ra, rb)
 
@@ -46,8 +37,8 @@ def test_sampling_loop_with_corrections_matches_reference(golden, tag, N, M):
     cfg = O.unet_config(dim=32, channels=2)
     sd = O.make_test_state_dict(cfg, 0)
     with torch.no_grad():
-        seq, r = CO.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), O.diffusion_tables(6), 6, N_correction=N,
-                                  M_correction=M, correction_mode=tag)
+        seq, r = O.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), O.diffusion_tables(6), 6, N_correction=N,
+                                 M_correction=M, correction_mode=tag, trajectory=True)
     assert len(seq) == int(gd[f'{tag}_len']) == 7 + M
     tail = gd[f'{tag}_tail']
     for k in range(tail.shape[0]):

@@ -1,15 +1,11 @@
-"""Host checks of the Darcy data generator's spec (no GPU): the oracle of tests/darcy_gen_oracle.py against the unmodified
+"""Host checks of the Darcy data generator's spec (no GPU): oracle/darcy_gen_oracle.py against the unmodified
 reference's output (tests/golden/darcy_gen.pt, scripts/make_golden_darcy_gen.py), the pinned banded solve against the
 reference's lstsq, the set-up the generator computes on the host, and its constructor validation."""
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import darcy_gen_oracle as DO  # noqa: E402
+from oracle import darcy_gen_oracle as DO
 
 P = 64
 

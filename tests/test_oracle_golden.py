@@ -5,11 +5,8 @@ import math
 import pytest
 import torch
 
+from checks import rel
 from oracle import pidm_oracle as O
-
-
-def rel(a, b):
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 @pytest.mark.parametrize('n', [100, 250])

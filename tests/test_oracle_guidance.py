@@ -4,13 +4,10 @@ import os
 
 import torch
 
+from checks import rel
 from oracle import pidm_oracle as O
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
-
-
-def rel(a, b):
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
 def _names(fname):

@@ -1,23 +1,14 @@
-"""Host checks (no GPU) of the topology-optimisation sampling oracle (tests/mech_sample_oracle.py) against the unmodified
+"""Host checks (no GPU) of the topology-optimisation sampling oracle (oracle/pidm_oracle.py) against the unmodified
 reference: its ancestral loop with a conditioning input reproduces tests/golden/mechanics_sample_loop.pt
 (scripts/make_golden_mech_sample.py; inputs and draws rebuilt by tests/mech_sample_inputs.py) in both x0 modes, which
 pins the draw order, and its fp64 sparse solve reproduces the
 displacements of tests/golden/mechanics_eval.pt (the reference's dense fp64 solve)."""
-import os
-import sys
-
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import mech_sample_inputs as MI  # noqa: E402
-import mech_sample_oracle as MO  # noqa: E402
-from oracle import pidm_oracle as O  # noqa: E402
-
-
-def rel(a, b):
-    a, b = a.double(), b.double()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+import mech_sample_inputs as MI
+from checks import rel
+from oracle import pidm_oracle as O
 
 
 @pytest.mark.parametrize('mode', ['mean', 'sample'])
@@ -28,8 +19,8 @@ def test_oracle_sampler_reproduces_reference(golden, mode):
     n = int(gd['n_steps'])
     cond, bcs, _ = MI.inputs(gd)
     x_T, zs, _ = MI.replay_draws(gd, mode)
-    out = MO.p_sample_loop(sd, cfg, x_T.double(), zs.double(), cond.double(), bcs.double(), O.diffusion_tables(n), n,
-                           use_ddim_x0=mode == 'sample')
+    out = O.mechanics_p_sample_loop(sd, cfg, x_T.double(), zs.double(), cond.double(), bcs.double(), O.diffusion_tables(n),
+                                    n, use_ddim_x0=mode == 'sample')
     gs = lambda k: O.golden_sample(out[k], MI.SAMPLE)
     for k in ('x_first', 'x_final', 'x0_pred_last'):
         assert rel(gs(k), gd[f'{mode}_{k}']) < 1e-5, (k, rel(gs(k), gd[f'{mode}_{k}']))
@@ -44,10 +35,10 @@ def test_sparse_solve_reproduces_reference_solution(golden):
     ev = golden('mechanics_eval.pt')
     KE = golden('mechanics_residual.pt')['KE']                  # the reference's element matrix (fp32 values)
     rho = ev['solution'][:, 2, :-1, :-1]
-    u = MO.fem_solve(rho, ev['bcs'], KE)
+    u = O.fem_solve(rho, ev['bcs'], KE)
     assert rel(u, ev['solution'][:, :2]) < 1e-6, rel(u, ev['solution'][:, :2])
     _, bcs, sol = MI.inputs(golden('mechanics_sample_loop.pt'))
-    u = MO.fem_solve(sol[:, 2, :-1, :-1], bcs, KE)
+    u = O.fem_solve(sol[:, 2, :-1, :-1], bcs, KE)
     assert rel(u, sol[:, :2]) < 1e-6, rel(u, sol[:, :2])
 
 
@@ -59,7 +50,7 @@ def test_sparse_system_is_the_reference_modification():
     bcs[0, 0, :, 0] = 1.
     bcs[0, 1, 2, 0] = 1.
     bcs[0, 2:] = torch.randn(2, 5, 5, generator=g).double()
-    K, f = MO.reduced_system(rho[0], bcs[0])
+    K, f = O.reduced_system(rho[0], bcs[0])
     Kd = K.toarray()
     fixed = torch.stack((bcs[0, 0].reshape(-1), bcs[0, 1].reshape(-1)), dim=1).reshape(-1).numpy() != 0
     assert (Kd[fixed][:, fixed] == torch.eye(int(fixed.sum())).numpy()).all()

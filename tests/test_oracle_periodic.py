@@ -1,43 +1,36 @@
-"""bcs='periodic' on the CPU: the periodic oracle (tests/periodic_oracle.py) against fixtures produced by the UNMODIFIED
-reference with ResidualsDarcy(bcs='periodic') (scripts/make_golden_periodic.py), an fp64 known answer, and the host
-logic of the flag.  Tolerances are those of the matching 'none' tests in test_oracle_golden.py."""
+"""bcs='periodic' on the CPU: the oracle's periodic option (oracle/pidm_oracle.py) against fixtures produced by the
+UNMODIFIED reference with ResidualsDarcy(bcs='periodic') (scripts/make_golden_periodic.py), an fp64 known answer, and the
+host logic of the flag.  Tolerances are those of the matching 'none' tests in test_oracle_golden.py."""
 import math
-import os
-import sys
 
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import periodic_oracle as PO  # noqa: E402
-from oracle import pidm_oracle as O  # noqa: E402
-
-
-def rel(a, b):
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
+from checks import rel
+from oracle import pidm_oracle as O
 
 
 def test_periodic_residual_and_vjp_match_reference(golden):
     gd = golden('darcy_residual_periodic.pt')
     assert torch.equal(gd['x0_pred'], golden('darcy_residual.pt')['x0_pred'])
-    assert rel(PO.darcy_residual(gd['x0_pred']), gd['residual']) < 1e-5
+    assert rel(O.darcy_residual(gd['x0_pred'], periodic=True), gd['residual']) < 1e-5
     # periodic differs from 'none' (else this file would test nothing new)
     assert rel(O.darcy_residual(gd['x0_pred']), gd['residual']) > 1e-2
     x = gd['x0_pred'].clone().requires_grad_(True)
-    (PO.darcy_residual(x) * gd['cotangent']).sum().backward()
+    (O.darcy_residual(x, periodic=True) * gd['cotangent']).sum().backward()
     assert rel(x.grad, gd['grad_x0_pred']) < 1e-5
 
 
 @pytest.mark.parametrize('mode', ['d_d0', 'd_d1', 'd_d00', 'd_d11', 'd_d01'])
 def test_periodic_stencil_modes_match_reference(golden, mode):
     gd = golden('darcy_residual_periodic.pt')
-    d0, d1 = PO.spacing(64)
-    assert rel(PO.stencil_gradients(gd['x0_pred'][:, 0], mode, d0, d1), gd['stencil_' + mode]) < 1e-5
+    d0, d1 = O.spacing(64)
+    assert rel(O.stencil_gradients(gd['x0_pred'][:, 0], mode, d0, d1, periodic=True), gd['stencil_' + mode]) < 1e-5
 
 
 def test_periodic_cocogen_correction_matches_reference(golden):
     gd = golden('cocogen_periodic.pt')
-    xc, rc = PO.cocogen_correction(gd['x0_pred'])
+    xc, rc = O.cocogen_correction(gd['x0_pred'], periodic=True)
     d_ref = gd['corrected'] - gd['x0_pred']
     assert d_ref.abs().max() > 0
     assert rel(xc - gd['x0_pred'], d_ref) < 1e-3
@@ -51,7 +44,7 @@ def test_periodic_training_loss_and_grads_match_reference(golden):
     sd = {k: v.clone().requires_grad_(v.is_floating_point() and 'freqs' not in k)
           for k, v in O.make_test_state_dict(cfg, 0).items()}
     tables = O.diffusion_tables(100)
-    loss, aux = PO.darcy_training_loss(sd, cfg, gd['x0'], gd['t'], gd['noise'], tables)
+    loss, aux = O.darcy_training_loss(sd, cfg, gd['x0'], gd['t'], gd['noise'], tables, periodic=True)
     assert abs(loss.item() / gd['loss'].item() - 1) < 2e-5
     assert abs(aux['data'].item() / gd['data_loss'].item() - 1) < 2e-5
     assert abs(aux['residual_abs'].item() / gd['residual_abs'].item() - 1) < 2e-5
@@ -69,7 +62,7 @@ def test_periodic_sampling_loop_matches_reference(golden):
     sd = O.make_test_state_dict(cfg, 0)
     tables = O.diffusion_tables(6)
     with torch.no_grad():
-        x, r = PO.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), tables, 6)
+        x, r = O.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), tables, 6, periodic=True)
     assert rel(x, gd['x_final']) < 2e-4
     assert rel(r, gd['residual']) < 2e-3
 
@@ -86,7 +79,7 @@ def test_periodic_residual_known_answer_fourier_modes():
     I, J = torch.meshgrid(idx, idx, indexing='ij')
     p = torch.sin(a * I) * torch.cos(b * J)
     K = 2 + torch.cos(c * I) + torch.sin(e * J)
-    r = PO.darcy_residual(torch.stack([p, K])[None]).reshape(P, P, 3)
+    r = O.darcy_residual(torch.stack([p, K])[None], periodic=True).reshape(P, P, 3)
     p0 = math.sin(a) / h0 * torch.cos(a * I) * torch.cos(b * J)
     p1 = torch.sin(a * I) * (-math.sin(b) / h1 * torch.sin(b * J))
     p00 = -4 * math.sin(a / 2) ** 2 / h0 ** 2 * p
