@@ -1,6 +1,6 @@
 """Inputs of tests/golden/mechanics_sample_loop.pt, rebuilt rather than stored so that the fixture stays small.  TEST
-INFRASTRUCTURE ONLY; plain torch on the CPU, imported both by scripts/make_golden_mech_sample.py (which runs the
-reference) and by the tests.
+INFRASTRUCTURE ONLY; plain torch on the CPU, imported both by the mech_sample recipe of oracle/make_golden.py (which runs
+the reference) and by the tests.
 
 * `conditioning_batch()`: the B = 2 conditioning fields, boundary conditions and data densities of the fixture.
 * `replay_draws(gd, mode)`: the reference loop's draws regenerated from the fixture's seed on the CPU generator, checked

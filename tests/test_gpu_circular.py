@@ -1,6 +1,6 @@
 """Unet3D(padding_mode='circular') on the GPU: the wrap-pad (halo) kernel, every circular convolution geometry of the
 Darcy network (forward, dgrad, weight gradient) per element against fp64, the plans the halo'd operands get, and the
-network end to end against fixtures of the UNMODIFIED reference (scripts/make_golden_circular.py)."""
+network end to end against fixtures of the UNMODIFIED reference (oracle/make_golden.py circular)."""
 import math
 
 import pytest

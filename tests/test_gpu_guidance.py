@@ -1,6 +1,6 @@
 """Residual-gradient guidance on the GPU: the guidance kernels per element against fp64 references (edited references
 rejected by the same bounds), and the engine end to end: graph replay against the eager step, the eager step against
-one training iteration of the unmodified reference (scripts/make_golden_guidance.py), the optimizer update of the
+one training iteration of the unmodified reference (oracle/make_golden.py guidance), the optimizer update of the
 guidance layers, the in-graph mask draw, the sharded draw and the guided sampler."""
 import math
 

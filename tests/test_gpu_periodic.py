@@ -1,6 +1,6 @@
 """bcs='periodic' on the GPU: every periodic Darcy kernel per element against the fp64 periodic oracle, edited references
 rejected by the same predicate, and the engine end to end against the fixtures of the unmodified reference
-(scripts/make_golden_periodic.py) at the tolerances of the matching 'none' tests."""
+(oracle/make_golden.py periodic) at the tolerances of the matching 'none' tests."""
 import pytest
 import torch
 

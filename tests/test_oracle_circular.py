@@ -1,6 +1,6 @@
 """Unet3D(padding_mode='circular') on the CPU: the parameter surface against the reference, and the oracle's
 padding_mode='circular' (oracle/pidm_oracle.py) against fixtures produced by the UNMODIFIED reference
-(scripts/make_golden_circular.py)."""
+(oracle/make_golden.py circular)."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -1,5 +1,5 @@
 """The oracle's CoCoGen corrections (oracle/pidm_oracle.py) against fixtures produced by the UNMODIFIED reference
-(scripts/make_golden_cocogen.py): successive residual_correction calls and the sampling loop with corrections."""
+(oracle/make_golden.py cocogen): successive residual_correction calls and the sampling loop with corrections."""
 import pytest
 import torch
 

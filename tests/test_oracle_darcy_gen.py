@@ -1,5 +1,5 @@
 """Host checks of the Darcy data generator's spec (no GPU): oracle/darcy_gen_oracle.py against the unmodified
-reference's output (tests/golden/darcy_gen.pt, scripts/make_golden_darcy_gen.py), the pinned banded solve against the
+reference's output (tests/golden/darcy_gen.pt, oracle/make_golden.py darcy_gen), the pinned banded solve against the
 reference's lstsq, the set-up the generator computes on the host, and its constructor validation."""
 import numpy as np
 import pytest

@@ -1,12 +1,22 @@
 """The CPU oracle (oracle/pidm_oracle.py) against fixtures produced by the UNMODIFIED reference
 (oracle/make_golden.py), plus analytic known-answer tests (SURVEY.md section 4)."""
 import math
+import os
 
 import pytest
 import torch
 
 from checks import rel
+from oracle import make_golden
 from oracle import pidm_oracle as O
+
+
+def test_every_golden_file_has_a_recipe():
+    """The recipe table of oracle/make_golden.py (importable without a reference checkout) names every file under
+    tests/golden exactly once, so no fixture exists that the recipes cannot rewrite."""
+    files = [f for _, names in make_golden.RECIPES.values() for f in names]
+    assert len(files) == len(set(files))
+    assert sorted(files) == sorted(os.listdir(os.path.join(os.path.dirname(__file__), 'golden')))
 
 
 @pytest.mark.parametrize('n', [100, 250])
@@ -91,7 +101,6 @@ def test_training_loss_and_grads_match_reference(golden):
     gn = math.sqrt(sum((p.grad.double() ** 2).sum().item() for p in sd.values() if p.grad is not None))
     assert abs(gn / gd['grad_norm'].item() - 1) < 1e-4
     dead = sorted(k for k, p in sd.items() if p.requires_grad and p.grad is None)
-    import os
     with open(os.path.join(os.path.dirname(__file__), 'golden', 'params_without_grad.txt')) as f:
         ref_dead = [k for k in f.read().split() if not k.endswith('rotary_emb.freqs')]   # frozen, never trainable
     assert dead == ref_dead

@@ -1,5 +1,5 @@
 """Residual-gradient guidance on the CPU: the oracle against one training iteration of the unmodified reference
-(scripts/make_golden_guidance.py), the guidance no-grad list and the sharded classifier-free mask draw."""
+(oracle/make_golden.py guidance), the guidance no-grad list and the sharded classifier-free mask draw."""
 import os
 
 import torch

@@ -1,6 +1,6 @@
 """Host checks (no GPU) of the topology-optimisation sampling oracle (oracle/pidm_oracle.py) against the unmodified
 reference: its ancestral loop with a conditioning input reproduces tests/golden/mechanics_sample_loop.pt
-(scripts/make_golden_mech_sample.py; inputs and draws rebuilt by tests/mech_sample_inputs.py) in both x0 modes, which
+(oracle/make_golden.py mech_sample; inputs and draws rebuilt by tests/mech_sample_inputs.py) in both x0 modes, which
 pins the draw order, and its fp64 sparse solve reproduces the
 displacements of tests/golden/mechanics_eval.pt (the reference's dense fp64 solve)."""
 import pytest

@@ -1,5 +1,5 @@
 """bcs='periodic' on the CPU: the oracle's periodic option (oracle/pidm_oracle.py) against fixtures produced by the
-UNMODIFIED reference with ResidualsDarcy(bcs='periodic') (scripts/make_golden_periodic.py), an fp64 known answer, and the
+UNMODIFIED reference with ResidualsDarcy(bcs='periodic') (oracle/make_golden.py periodic), an fp64 known answer, and the
 host logic of the flag.  Tolerances are those of the matching 'none' tests in test_oracle_golden.py."""
 import math
 
