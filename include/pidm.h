@@ -211,7 +211,12 @@ int pidm_colsum(const void* x, float* out, long long M, int C, int dtype, void* 
 /* ---- normalisations ------------------------------------------------------------------------------------ */
 /* Block.forward tail: GroupNorm(G) -> *(scale+1)+shift -> SiLU (src/unet_model.py:233-241).  scale_shift [B,2C] or NULL.
  * residual (optional, same shape as y) is added after the SiLU: the `h + x` of a ResnetBlock whose res_conv is the
- * identity (:262).  sums [B,G,2] (sum, sum of squares) is written here and consumed by the backward. */
+ * identity (:262).  sums [B,G,2] (sum, sum of squares) is written here and consumed by the backward.
+ * With n = HW * C/G, s = sums[b][g][0], ss = sums[b][g][1]:  mean = s / n,  var = max(ss / n - mean^2, 0)  (biased, clamped),
+ * rstd = 1 / sqrt(var + eps),  y = silu(((x - mean) rstd gamma + beta)(scale + 1) + shift) (+ residual).  The sums are fp32, so
+ * the variance carries a relative error of about 2^-24 (1 + mean^2 / var): a group whose mean is tens of standard deviations
+ * away from zero loses that many digits (DESIGN.md section 2 has the measured figures).  A constant group has var = 0 up to
+ * that cancellation, hence rstd between 1 / sqrt(eps) and 1 / sqrt(eps + 2^-22 mean^2), and x - mean within 2^-23 |mean|. */
 int pidm_groupnorm_silu_fwd(const void* x, const float* gamma, const float* beta, const float* scale_shift,
                             const void* residual, void* y, float* sums, int stats_precomputed, int B, int HW, int C, int G,
                             float eps, int dtype, void* stream);
@@ -221,6 +226,11 @@ int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const float* sums, co
                             const float* scale_shift, void* dx, float* dgamma, float* dbeta, float* d_scale_shift,
                             float* dbias_of_producer, float* workspace, int B, int HW, int C, int G, float eps,
                             int dtype, void* stream);
+/* What the two GroupNorm entry points launch for a shape (test aid): out[10] = {statistics chunks, statistics block, apply
+ * chunks, apply grid rules that fired (bit 0 shrink the unroll, bit 1 halve, bit 2 one wave and loop), backward path
+ * (0 two-launch fallback, 1 / 2 piece kernel with 1 / 2 vectors per thread, 3 packed, 4 streaming), channel slab, threads,
+ * cluster size, pixel rows per CTA, vectors per thread}; the last five are 0 on the fallback path. */
+int pidm_groupnorm_plan(int B, int HW, int C, int G, int dtype, int* out);
 /* channel LayerNorm, gain only, biased variance (src/unet_model.py:201-210); dgamma ACCUMULATES */
 int pidm_layernorm_c_fwd(const void* x, const float* gamma, void* y, long long M, int C, float eps, int dtype, void* stream);
 int pidm_layernorm_c_bwd(const void* x, const void* dy, const float* gamma, void* dx, float* dgamma,

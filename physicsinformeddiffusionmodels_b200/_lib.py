@@ -55,6 +55,7 @@ _SIGS = {
     'pidm_colsum': [P, P, L, I, I, P],
     'pidm_groupnorm_silu_fwd': [P, P, P, P, P, P, P, I, I, I, I, I, F, I, P],
     'pidm_groupnorm_silu_bwd': [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, F, I, P],
+    'pidm_groupnorm_plan': [I, I, I, I, I, P],
     'pidm_layernorm_c_fwd': [P, P, P, L, I, F, I, P],
     'pidm_layernorm_c_bwd': [P, P, P, P, P, P, L, I, F, I, P],
     'pidm_linattn_workspace_floats': [I, I, I],
@@ -96,7 +97,7 @@ _RESTYPES = {'pidm_darcy_gen_workspace_bytes': ctypes.c_longlong}
 _VALUE_RETURN = {'pidm_pack_entry_size', 'pidm_pack_pair_entry_size', 'pidm_mlp_entry_size', 'pidm_linattn_workspace_floats', 'pidm_version',
                  'pidm_linattn_block_supported', 'pidm_linattn_block_workspace_floats',
                  'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported',
-                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_block_plan',
+                 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_block_plan', 'pidm_groupnorm_plan',
                  'pidm_darcy_gen_workspace_bytes'}
 
 if not os.path.exists(LIB_PATH):

@@ -1038,6 +1038,56 @@ static void gn_launch_dims(int HW, int C, int& block, int& chunks) {
     if (chunks < 1) chunks = 1;
 }
 
+// Grid of gn_apply_kernel: a thread owns one 16-byte channel vector position (ov of them per pixel row);
+// ~GN_APPLY_UNR vectors per thread, >= 2 waves of CTAs.  `rules` reports which adjustments fired (bit 0 shrink the unroll,
+// bit 1 halve, bit 2 one wave and loop).
+static int gn_apply_chunks(int B, int HW, int ov, int& rules) {
+    const int rpp = NORM_THREADS / ov;
+    int ach = ceil_div(HW, rpp * GN_APPLY_UNR);
+    rules = 0;
+    for (int u = GN_APPLY_UNR; u > 1 && (long long)B * ach < num_sms() * 2; u /= 2) { ach = ceil_div(HW, rpp * (u / 2)); rules |= 1; }
+    while (ach > 1 && (long long)B * ach > num_sms() * 8) { ach = (ach + 1) / 2; rules |= 2; }
+    // ~123 registers: two CTAs per SM are resident.  Between one and two waves the second wave runs mostly empty
+    // (e.g. 512 CTAs at 64x64x32, batch 32): size the grid to one wave and let the CTAs loop
+    if ((long long)B * ach > num_sms() * 2 && (long long)B * ach < num_sms() * 4 && B <= num_sms() * 2) { ach = (num_sms() * 2) / B; rules |= 4; }
+    return ach;
+}
+
+// Plan of pidm_groupnorm_silu_bwd: the single-launch piece kernel (see gn_bwd_piece_kernel) with its channel slab S,
+// thread count, cluster size cl, pixel rows per CTA and vectors per thread v, or the two-launch fallback (path 0).
+struct GnBwdPlan { int path /*0 fallback, 1 piece<1>, 2 piece<2>, 3 packed<4>, 4 stream*/, S, threads, cl, rows_per_cta, v; };
+static GnBwdPlan gn_bwd_plan(int B, int HW, int C, int G, int dtype) {
+    GnBwdPlan pl = {0, 0, 0, 0, 0, 0};
+    const int esz = dtype == PIDM_BF16 ? 2 : 4, ve = 16 / esz, cpg = C / G;
+    int S = cpg;
+    while (S * esz < 32 && S * 2 <= C && C % (S * 2) == 0) S *= 2;    // >= 32 bytes of channels per pixel row
+    const int so = S / ve;
+    const bool shape_ok = S % ve == 0 && so >= 1 && so <= 32 && (so & (so - 1)) == 0 && C % S == 0 && (C * esz) % 16 == 0;
+    if (!shape_ok) return pl;
+    const int nslab = C / S;
+    const long long nv = (long long)HW * so;            // 16-byte vectors per (sample, slab)
+    int threads = NORM_THREADS;
+    while (threads > 32 && threads / 2 >= nv && (threads / 2) % so == 0) threads /= 2;
+    // CTAs per piece.  A CTA of this kernel is a latency chain of a few microseconds whatever its size, a
+    // second wave of CTAs doubles the launch and a cluster costs ~1 us extra -- so: no cluster unless a piece
+    // has more than 8 vectors per thread, never more CTAs than are resident at once (2 per SM), and otherwise
+    // as many CTAs as that allows.
+    const int resident = num_sms() * 2;
+    int cl = 1;
+    while (cl < 8 && nv > (long long)cl * threads * 8) cl *= 2;
+    while (cl < 8 && (long long)B * nslab * cl * 2 <= resident && nv > (long long)cl * threads) cl *= 2;
+    const int rpp = threads / so;
+    int rows_per_cta = ceil_div(HW, cl);
+    rows_per_cta = ceil_div(rows_per_cta, rpp) * rpp;
+    const int v = rows_per_cta / rpp;                   // vectors per thread
+    if ((long long)rows_per_cta * (cl - 1) >= HW) return pl;        // a cluster rank would own no pixel
+    // three shapes of a piece: <= 2 vectors per thread stay in registers unpacked between the phases; 3-4 vectors are
+    // held packed (with 8 vectors that variant spills); larger pieces are streamed twice
+    pl.path = v <= 1 ? 1 : v <= 2 ? 2 : v <= 4 ? 3 : 4;
+    pl.S = S; pl.threads = threads; pl.cl = cl; pl.rows_per_cta = rows_per_cta; pl.v = v;
+    return pl;
+}
+
 // sums [B,G,2] holds (sum, sum of squares) per (sample, group): computed here unless stats_precomputed (then it was
 // filled by the producing convolution's epilogue); it must be kept for backward.
 extern "C" int pidm_groupnorm_silu_fwd(const void* x, const float* gamma, const float* beta, const float* scale_shift,
@@ -1051,16 +1101,10 @@ extern "C" int pidm_groupnorm_silu_fwd(const void* x, const float* gamma, const 
     PIDM_DISPATCH_DTYPE(dtype, {
         if (!stats_precomputed)
             gn_stats_kernel<T><<<dim3(chunks, B), block, 2 * G * sizeof(float), st>>>((const T*)x, sums, HW, C, G);
-        // apply: a thread owns one 16-byte channel vector position; ~GN_APPLY_UNR vectors per thread, >= 2 waves of CTAs
         const int ov = C / Vec<T>::N;
         PIDM_REQUIRE(ov <= NORM_THREADS && NORM_THREADS % ov == 0, "groupnorm: C=%d is not supported by the apply kernel", C);
-        const int rpp = NORM_THREADS / ov;
-        int ach = ceil_div(HW, rpp * GN_APPLY_UNR);
-        for (int u = GN_APPLY_UNR; u > 1 && (long long)B * ach < num_sms() * 2; u /= 2) ach = ceil_div(HW, rpp * (u / 2));
-        while (ach > 1 && (long long)B * ach > num_sms() * 8) ach = (ach + 1) / 2;
-        // ~123 registers: two CTAs per SM are resident.  Between one and two waves the second wave runs mostly empty
-        // (e.g. 512 CTAs at 64x64x32, batch 32): size the grid to one wave and let the CTAs loop
-        if ((long long)B * ach > num_sms() * 2 && (long long)B * ach < num_sms() * 4 && B <= num_sms() * 2) ach = (num_sms() * 2) / B;
+        int rules;
+        const int ach = gn_apply_chunks(B, HW, ov, rules);
         PIDM_CUDA(launch_pdl(gn_apply_kernel<T>, dim3(ach, B), dim3(NORM_THREADS), 0, st, (const T*)x, (const float*)sums,
                              gamma, beta, scale_shift, (const T*)residual, (T*)y, HW, C, G, eps));
     });
@@ -1078,78 +1122,36 @@ extern "C" int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const floa
     cudaStream_t st = (cudaStream_t)stream;
     int block, chunks;
     gn_launch_dims(HW, C, block, chunks);
-    {   // single-launch piece kernel (see gn_bwd_piece_kernel): plan (slab, cluster size, vectors per thread)
-        const int esz = dtype == PIDM_BF16 ? 2 : 4, ve = 16 / esz, cpg = C / G;
-        int S = cpg;
-        while (S * esz < 32 && S * 2 <= C && C % (S * 2) == 0) S *= 2;    // >= 32 bytes of channels per pixel row
-        const int so = S / ve;
-        const bool shape_ok = S % ve == 0 && so >= 1 && so <= 32 && (so & (so - 1)) == 0 && C % S == 0 && (C * esz) % 16 == 0;
-        if (shape_ok) {
-            const int nslab = C / S;
-            const long long nv = (long long)HW * so;            // 16-byte vectors per (sample, slab)
-            int threads = NORM_THREADS;
-            while (threads > 32 && threads / 2 >= nv && (threads / 2) % so == 0) threads /= 2;
-            // CTAs per piece.  A CTA of this kernel is a latency chain of a few microseconds whatever its size, a
-            // second wave of CTAs doubles the launch and a cluster costs ~1 us extra -- so: no cluster unless a piece
-            // has more than 8 vectors per thread, never more CTAs than are resident at once (2 per SM), and otherwise
-            // as many CTAs as that allows.
-            const int resident = num_sms() * 2;
-            int cl = 1;
-            while (cl < 8 && nv > (long long)cl * threads * 8) cl *= 2;
-            while (cl < 8 && (long long)B * nslab * cl * 2 <= resident && nv > (long long)cl * threads) cl *= 2;
-            const int rpp = threads / so;
-            int rows_per_cta = ceil_div(HW, cl);
-            rows_per_cta = ceil_div(rows_per_cta, rpp) * rpp;
-            const int v = rows_per_cta / rpp;                   // vectors per thread
-            if ((long long)rows_per_cta * (cl - 1) < HW) {
-                const int vt = v <= 1 ? 1 : 2;                  // vectors per chunk
-                const bool keep = v <= 2;                       // register-resident between the phases
-                const int nchunks = ceil_div(v, vt);
-                const size_t smem = (size_t)(7 * S + 2 * (S / cpg)) * sizeof(float);      // + 2 S: constants of the packed variant
-                cudaLaunchConfig_t cfg = {};
-                cfg.gridDim = dim3((unsigned)(B * nslab * cl));
-                cfg.blockDim = dim3((unsigned)threads);
-                cfg.dynamicSmemBytes = smem;
-                cfg.stream = st;
-                cudaLaunchAttribute attr[2];
-                attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-                attr[0].val.programmaticStreamSerializationAllowed = 1;
-                int na = 1;
-                if (cl > 1) {
-                    attr[na].id = cudaLaunchAttributeClusterDimension;
-                    attr[na].val.clusterDim.x = (unsigned)cl; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-                    ++na;
-                }
-                cfg.attrs = attr; cfg.numAttrs = na;
-#define GN_PIECE_CASE(VV, KK)                                                                                            \
-    if (vt == VV && keep == KK) {                                                                                                   \
-        PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_kernel<T, VV, KK>, (const T*)x, (const T*)dy, sums, gamma, beta, \
-                                     scale_shift, (T*)dx, d_scale_shift, dgamma, dbeta, dbias_of_producer, HW, C, G, eps, \
-                                     S, cl, rows_per_cta, nchunks));                                                     \
-    }
-#define GN_PACKED_CASE(NVV)                                                                                              \
-    PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_packed_kernel<T, NVV>, (const T*)x, (const T*)dy, sums, gamma, beta, \
-                                 scale_shift, (T*)dx, d_scale_shift, dgamma, dbeta, dbias_of_producer, HW, C, G, eps,    \
-                                 S, cl, rows_per_cta))
-                // three shapes of a piece: <= 2 vectors per thread stay in registers unpacked between the phases; 3-4 vectors are
-                // held packed (with 8 vectors that variant spills); larger pieces are streamed twice
-                if (keep) {
-                    PIDM_DISPATCH_DTYPE(dtype, { GN_PIECE_CASE(1, true) else GN_PIECE_CASE(2, true) });
-                } else if (v <= 4) {
-                    PIDM_DISPATCH_DTYPE(dtype, { GN_PACKED_CASE(4); });
-                } else {
-                    PIDM_DISPATCH_DTYPE(dtype, {
-                        PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_stream_kernel<T>, (const T*)x, (const T*)dy, sums, gamma,
-                                                     beta, scale_shift, (T*)dx, d_scale_shift, dgamma, dbeta, dbias_of_producer,
-                                                     HW, C, G, eps, S, cl, rows_per_cta));
-                    });
-                }
-#undef GN_PACKED_CASE
-#undef GN_PIECE_CASE
-                PIDM_LAUNCH_CHECK("groupnorm_silu_bwd(piece)");
-                return 0;
-            }
+    const GnBwdPlan pl = gn_bwd_plan(B, HW, C, G, dtype);
+    if (pl.path) {
+        const int S = pl.S, cl = pl.cl, rows_per_cta = pl.rows_per_cta;
+        const size_t smem = (size_t)(7 * S + 2 * (S / (C / G))) * sizeof(float);      // + 2 S: constants of the packed variant
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)(B * (C / S) * cl));
+        cfg.blockDim = dim3((unsigned)pl.threads);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        cudaLaunchAttribute attr[2];
+        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[0].val.programmaticStreamSerializationAllowed = 1;
+        int na = 1;
+        if (cl > 1) {
+            attr[na].id = cudaLaunchAttributeClusterDimension;
+            attr[na].val.clusterDim.x = (unsigned)cl; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
+            ++na;
         }
+        cfg.attrs = attr; cfg.numAttrs = na;
+#define GN_PIECE_ARGS (const T*)x, (const T*)dy, sums, gamma, beta, scale_shift, (T*)dx, d_scale_shift, dgamma, dbeta, \
+                      dbias_of_producer, HW, C, G, eps, S, cl, rows_per_cta
+        PIDM_DISPATCH_DTYPE(dtype, {
+            if (pl.path == 1) PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_kernel<T, 1, true>, GN_PIECE_ARGS, 1));
+            else if (pl.path == 2) PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_kernel<T, 2, true>, GN_PIECE_ARGS, 1));
+            else if (pl.path == 3) PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_packed_kernel<T, 4>, GN_PIECE_ARGS));
+            else PIDM_CUDA(cudaLaunchKernelEx(&cfg, gn_bwd_piece_stream_kernel<T>, GN_PIECE_ARGS));
+        });
+#undef GN_PIECE_ARGS
+        PIDM_LAUNCH_CHECK("groupnorm_silu_bwd(piece)");
+        return 0;
     }
     float* S = workspace;
     PIDM_CUDA(cudaMemsetAsync(S, 0, (size_t)B * C * 2 * sizeof(float), st));
@@ -1161,6 +1163,24 @@ extern "C" int pidm_groupnorm_silu_bwd(const void* x, const void* dy, const floa
             dbias_of_producer, HW, C, G, eps);
     });
     PIDM_LAUNCH_CHECK("groupnorm_silu_bwd");
+    return 0;
+}
+
+// What the two entry points above launch for a shape (test aid).  out[10] = {statistics chunks, statistics block, apply
+// chunks, apply grid rules (bit 0 shrink the unroll, bit 1 halve, bit 2 one wave and loop), backward path (0 two-launch
+// fallback, 1 piece<1>, 2 piece<2>, 3 packed<4>, 4 stream), channel slab S, threads, cluster size, pixel rows per CTA,
+// vectors per thread}; the last five are 0 on the fallback path.
+extern "C" int pidm_groupnorm_plan(int B, int HW, int C, int G, int dtype, int* out) {
+    if (int e = gn_check(C, G)) return e;
+    PIDM_REQUIRE(dtype == PIDM_BF16 || dtype == PIDM_F32, "unknown dtype code %d", dtype);
+    const int ov = C / (dtype == PIDM_BF16 ? 8 : 4);
+    PIDM_REQUIRE(ov <= NORM_THREADS && NORM_THREADS % ov == 0, "groupnorm: C=%d is not supported by the apply kernel", C);
+    int block, chunks, rules;
+    gn_launch_dims(HW, C, block, chunks);
+    const int ach = gn_apply_chunks(B, HW, ov, rules);
+    const GnBwdPlan pl = gn_bwd_plan(B, HW, C, G, dtype);
+    const int v[10] = {chunks, block, ach, rules, pl.path, pl.S, pl.threads, pl.cl, pl.rows_per_cta, pl.v};
+    for (int i = 0; i < 10; ++i) out[i] = v[i];
     return 0;
 }
 

@@ -468,7 +468,10 @@ _NAMES = {'pidm_conv2d_tc_general': 'conv', 'pidm_conv2d_wgrad_tc': 'wgrad', 'pi
 
 
 def _key_of(name, a):
-    kind = _NAMES[name]
+    """(family, key) of a tensor-core call, None for every other entry point"""
+    kind = _NAMES.get(name)
+    if kind is None:
+        return None
     if kind == 'conv':
         ints = tuple(int(v) for v in a[5:17])
         return 'conv', ints + (int(a[2] is not None), int(a[3] is not None), int(a[17] is not None), int(a[18]),
@@ -482,14 +485,15 @@ def _key_of(name, a):
     return 'laf', ('wgrad', int(a[14]), int(a[15]), int(a[9]), int(a[10]), int(a[12]), int(a[13]))
 
 
-def _record(fn):
+def _record(fn, key_of=_key_of):
     from physicsinformeddiffusionmodels_b200 import ops
     seen = set()
     orig = ops.call
 
     def rec(name, *a):
-        if name in _NAMES:
-            seen.add(_key_of(name, a))
+        k = key_of(name, a)
+        if k is not None:
+            seen.add(k)
         return orig(name, *a)
     ops.call = rec
     try:
@@ -506,8 +510,9 @@ def _darcy_model(dev):
     return Unet3D(dim=32, channels=2).to(dev)
 
 
-def run_census():
-    """{workload: set of (family, key)} for one eager step of every workload bench.py times (bf16)."""
+def run_census(key_of=_key_of):
+    """{workload: set of (family, key)} for one eager step of every workload bench.py times (bf16); key_of(name, args)
+    names the family and key of the calls to keep (test_gpu_norm_census.py asks for the normalisations)."""
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.engine import SampleEngine, TrainEngine
@@ -524,7 +529,7 @@ def run_census():
     eng = TrainEngine(model, DenoisingDiffusion(100, dev), res, lr=1e-4, max_norm=1.0, ema_mu=0.99, c_data=1.0,
                       c_residual=1e-3, use_graph=False)
     x0 = torch.randn(32, 2, 64, 64, generator=torch.Generator().manual_seed(1)).to(dev)
-    out['darcy_train_b32'] = _record(lambda: eng.step(x0))
+    out['darcy_train_b32'] = _record(lambda: eng.step(x0), key_of)
     del eng
     model.eval()
     diff = DenoisingDiffusion(250, dev)
@@ -537,7 +542,7 @@ def run_census():
             packer.refresh_if_stale(ops.act_dtype())
         se.x.normal_()
         se.t.fill_(diff.n_steps - 1)
-        out[f'darcy_sample_b{B}'] = _record(se._step_body)
+        out[f'darcy_sample_b{B}'] = _record(se._step_body, key_of)
         del se
     del model
     torch.manual_seed(0)
@@ -554,7 +559,7 @@ def run_census():
     bcs[:, 1, :, 0] = 1.
     bcs[:, 3, 32, 64] = -1.
     inp = torch.cat((cond, x0, bcs), dim=1).to(dev)
-    out['mech_train_b32'] = _record(lambda: eng.step(inp))
+    out['mech_train_b32'] = _record(lambda: eng.step(inp), key_of)
     del eng, mech
     torch.cuda.empty_cache()
     return out
