@@ -268,11 +268,23 @@ int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const void* w_ou
                              const float* dctx, const float* kmax, const float* kzinv, float* grad_w_qkv,
                              long long qkv_stride_n, long long qkv_stride_c, float* grad_w_out, long long out_stride_n,
                              long long out_stride_c, int B, int N, void* stream);
+/* Standalone linear attention (every layer that is not the 32-channel block), s = 32^-1/2, per sample and head h with
+ * q, k, v the head's [N][32] slices of qkv:
+ *   out[n, h*32+e] = s * sum_d softmax_d(q[n,:])[d] * ctx[h][d][e]
+ *   ctx[h][d][e]   = sum_n exp(k[n,d] - kmax[h][d]) * kzinv[h][d] * v[n,e] / N     (so ctx includes 1/(Z_d N))
+ *   kmax[b, h*32+d] = max_n k[n,d];   kzinv[b, h*32+d] = 1 / sum_n exp(k[n,d] - kmax)
+ * fwd WRITES out, ctx, kmax and kzinv; workspace holds pidm_linattn_workspace_floats(B, N, heads) floats of scratch.
+ * bwd WRITES dqkv from qkv, dout and the forward's ctx / kmax / kzinv (heads a multiple of 4); dctx_scratch
+ * [B,heads,32,32] is scratch. */
 int pidm_linattn_workspace_floats(int B, int N, int heads);
 int pidm_linattn_fwd(const void* qkv, void* out, float* ctx, float* kmax, float* kzinv, float* workspace, int B, int N,
                      int heads, int dtype, void* stream);
 int pidm_linattn_bwd(const void* qkv, const void* dout, const float* ctx, const float* kmax, const float* kzinv,
                      void* dqkv, float* dctx_scratch, int B, int N, int heads, int dtype, void* stream);
+/* What pidm_linattn_fwd / _bwd launch for a shape (test aid): out[8] = {forward path (0 one CTA per (sample, head),
+ * 1 mma.sync, 2 SIMT), backward path (0 mma.sync, 1 SIMT, -1 shape refused), statistics chunks, statistics rows per
+ * chunk, SIMT context rows per chunk, SIMT context chunks, mma.sync pixels per CTA, mma.sync chunks per sample}. */
+int pidm_linattn_plan(int B, int N, int heads, int dtype, int* out);
 /* mid-block softmax attention over <= 64 tokens (src/unet_model.py:341-367) */
 int pidm_attn_fwd(const void* qkv, void* out, int B, int n_tokens, int heads, int dtype, void* stream);
 int pidm_attn_bwd(const void* qkv, const void* dout, void* dqkv, int B, int n_tokens, int heads, int dtype, void* stream);

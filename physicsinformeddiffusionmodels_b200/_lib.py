@@ -67,6 +67,7 @@ _SIGS = {
     'pidm_linattn_block_wgrad': [P, P, P, P, P, P, P, P, P, L, L, P, L, L, I, I, P],
     'pidm_linattn_fwd': [P, P, P, P, P, P, I, I, I, I, P],
     'pidm_linattn_bwd': [P, P, P, P, P, P, P, I, I, I, I, P],
+    'pidm_linattn_plan': [I, I, I, I, P],
     'pidm_attn_fwd': [P, P, I, I, I, I, P],
     'pidm_attn_bwd': [P, P, P, I, I, I, I, P],
     'pidm_time_embed_fwd': [P, P, P, P, P, P, P, P, P, I, I, I, P],
@@ -98,6 +99,7 @@ _VALUE_RETURN = {'pidm_pack_entry_size', 'pidm_pack_pair_entry_size', 'pidm_mlp_
                  'pidm_linattn_block_supported', 'pidm_linattn_block_workspace_floats',
                  'pidm_conv2d_tc_supported', 'pidm_conv2d_wgrad_tc_supported', 'pidm_conv2d_tc_general_supported',
                  'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan', 'pidm_linattn_block_plan', 'pidm_groupnorm_plan',
+                 'pidm_linattn_plan',
                  'pidm_darcy_gen_workspace_bytes'}
 
 if not os.path.exists(LIB_PATH):

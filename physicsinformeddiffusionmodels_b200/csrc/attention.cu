@@ -443,6 +443,7 @@ int la_mma_ctx(int mode, const void* qkv, const void* dout, const float* part, i
 int la_mma_out(const void* qkv, const float* ctx, void* out, int B, int N, float scale, cudaStream_t st);
 int la_mma_bwd(const void* qkv, const void* dout, const float* ctx, const float* dctx, const float* kmax,
                const float* kzinv, void* dqkv, int B, int N, float scale, cudaStream_t st);
+int la_mma_chunk_px(int B, int N);
 
 // block = whole row groups of HID/8 threads, about 256 threads
 static int la_kstats_block(int HID) {
@@ -460,6 +461,23 @@ static int la_chunks(int N) {
     return c;
 }
 
+// forward path: one CTA per (sample, head) | mma.sync ctx / out | SIMT kstats -> context -> out
+enum { LA_FWD_SMALL = 0, LA_FWD_MMA = 1, LA_FWD_SIMT = 2 };
+static int la_fwd_path(int N, int heads, int dtype) {
+    if (la_small_supported(N, dtype)) return LA_FWD_SMALL;
+    return (dtype == PIDM_BF16 && heads == 8 && N % 64 == 0) ? LA_FWD_MMA : LA_FWD_SIMT;
+}
+static bool la_bwd_mma(int N, int heads, int dtype) { return dtype == PIDM_BF16 && heads == 8 && N % 64 == 0; }
+
+// statistics rows per chunk (the last chunk may be shorter)
+static int la_stat_rows(int N) { return (N + la_chunks(N) - 1) / la_chunks(N); }
+
+// SIMT context kernels: at most 16 pixel chunks, each a whole number of LA_TN-row tiles (the last may be ragged)
+static int la_ctx_rows(int N) {
+    const int cchunks = (N + 255) / 256 > 16 ? 16 : (N + 255) / 256;
+    return ((N + cchunks - 1) / cchunks + LA_TN - 1) / LA_TN * LA_TN;
+}
+
 }  // namespace pidm
 using namespace pidm;
 
@@ -470,20 +488,20 @@ extern "C" int pidm_linattn_fwd(const void* qkv, void* out, float* ctx, float* k
     cudaStream_t st = (cudaStream_t)stream;
     const int HID = heads * DH;
     const int chunks = la_chunks(N);
-    const int rpc = (N + chunks - 1) / chunks;
+    const int rpc = la_stat_rows(N);
     const float scale = 0.17677669529663687f;   // 32^-0.5
-    if (la_small_supported(N, dtype))     // 8x8 level: the whole (sample, head) problem in one CTA, one launch
+    const int path = la_fwd_path(N, heads, dtype);
+    if (path == LA_FWD_SMALL)     // 8x8 level: the whole (sample, head) problem in one CTA, one launch
         return la_small_fwd(qkv, out, ctx, kmax, kzinv, B, N, heads, scale, st);
     PIDM_CUDA(cudaMemsetAsync(ctx, 0, (size_t)B * heads * DH * DH * sizeof(float), st));
-    if (dtype == PIDM_BF16 && heads == 8 && N % 64 == 0) {
+    if (path == LA_FWD_MMA) {
         PIDM_CUDA(launch_plain(la_kstats_kernel<__nv_bfloat16>, dim3(dim3(chunks, B)), dim3(256), (size_t)(la_kstats_smem(HID)), st, (const __nv_bfloat16*)qkv, workspace, N, HID, rpc));
         if (int e = la_mma_ctx(0, qkv, nullptr, workspace, chunks, kmax, kzinv, ctx, B, N, scale, st)) return e;
         if (int e = la_mma_out(qkv, ctx, out, B, N, scale, st)) return e;
         PIDM_LAUNCH_CHECK("linattn_fwd");
         return 0;
     }
-    const int cchunks = (N + 255) / 256 > 16 ? 16 : (N + 255) / 256;
-    const int crpc = ((N + cchunks - 1) / cchunks + LA_TN - 1) / LA_TN * LA_TN;
+    const int crpc = la_ctx_rows(N);
     PIDM_DISPATCH_DTYPE(dtype, {
         PIDM_CUDA(launch_plain(la_kstats_kernel<T>, dim3(dim3(chunks, B)), dim3(la_kstats_block(HID)), (size_t)(la_kstats_smem(HID)), st, (const T*)qkv, workspace, N, HID, rpc));
         PIDM_CUDA(launch_plain(la_context_kernel<T, 0>, dim3(dim3((N + crpc - 1) / crpc, heads, B)), dim3(256), (size_t)(0), st, (const T*)qkv, nullptr, workspace, chunks, kmax, kzinv, ctx, N, heads, crpc, scale));
@@ -505,17 +523,30 @@ extern "C" int pidm_linattn_bwd(const void* qkv, const void* dout, const float* 
     cudaStream_t st = (cudaStream_t)stream;
     const float scale = 0.17677669529663687f;
     PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * heads * DH * DH * sizeof(float), st));
-    if (dtype == PIDM_BF16 && heads == 8 && N % 64 == 0) {
+    if (la_bwd_mma(N, heads, dtype)) {
         if (int e = la_mma_ctx(1, qkv, dout, nullptr, 0, nullptr, nullptr, dctx, B, N, scale, st)) return e;
         return la_mma_bwd(qkv, dout, ctx, dctx, kmax, kzinv, dqkv, B, N, scale, st);
     }
-    const int cchunks = (N + 255) / 256 > 16 ? 16 : (N + 255) / 256;
-    const int crpc = ((N + cchunks - 1) / cchunks + LA_TN - 1) / LA_TN * LA_TN;
+    const int crpc = la_ctx_rows(N);
     PIDM_DISPATCH_DTYPE(dtype, {
         PIDM_CUDA(launch_plain(la_context_kernel<T, 1>, dim3(dim3((N + crpc - 1) / crpc, heads, B)), dim3(256), (size_t)(0), st, (const T*)qkv, (const T*)dout, nullptr, 0, nullptr, nullptr, dctx, N, heads, crpc, scale));
         PIDM_CUDA(launch_plain(la_bwd_pixel_kernel<T>, dim3(dim3((unsigned)((long long)B * N / 32), heads / LA_HB)), dim3(32 * LA_HB), (size_t)(0), st, (const T*)qkv, (const T*)dout, ctx, dctx, kmax, kzinv, (T*)dqkv, N, heads, scale));
     });
     PIDM_LAUNCH_CHECK("linattn_bwd");
+    return 0;
+}
+
+// What pidm_linattn_fwd / _bwd launch for a shape (test aid), see pidm.h.
+extern "C" int pidm_linattn_plan(int B, int N, int heads, int dtype, int* out) {
+    PIDM_REQUIRE(B > 0 && N > 0 && N % 32 == 0 && heads >= 1 && heads * DH <= 1024,
+                 "linattn: N%%32==0 and heads*32<=1024 required");
+    PIDM_REQUIRE(dtype == PIDM_BF16 || dtype == PIDM_F32, "unknown dtype code %d", dtype);
+    const int fwd = la_fwd_path(N, heads, dtype);
+    const int bwd = heads % LA_HB != 0 ? -1 : la_bwd_mma(N, heads, dtype) ? 0 : 1;
+    const int crpc = la_ctx_rows(N);
+    const int cpx = la_mma_chunk_px(B, N);
+    const int v[8] = {fwd, bwd, la_chunks(N), la_stat_rows(N), crpc, (N + crpc - 1) / crpc, cpx, (N + cpx - 1) / cpx};
+    for (int i = 0; i < 8; ++i) out[i] = v[i];
     return 0;
 }
 

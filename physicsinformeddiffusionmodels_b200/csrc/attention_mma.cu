@@ -366,6 +366,7 @@ static int la_chunk_px(int B, int N, int ctas_per_sm) {
 }
 
 // entry points used by attention.cu for the bf16 / 8-head case
+int la_mma_chunk_px(int B, int N) { return la_chunk_px(B, N, 2); }
 int la_mma_ctx(int mode, const void* qkv, const void* dout, const float* part, int n_stat_chunks, float* kmax,
                float* kzinv, float* ctx, int B, int N, float scale, cudaStream_t st) {
     if (int e = la_mma_attrs()) return e;

@@ -307,8 +307,8 @@ def test_block_op_matches_unfused_composition(pk, B, H):
     residual and the bias are scaled to the rms of the attention term, so that all three terms of y count.  bf16
     activations: 3e-2 on y and 6e-2 on the gradients against fp32, like the other bf16 attention tests; the two libpidm
     compositions differ by the bf16 rounding of q, k, v, the attention output and its gradient, which only the unfused
-    one materialises: 1e-2 / 2e-2.  The per-element bounds of every launch the benchmark runs are checked against fp64
-    in test_gpu_launch_census.py."""
+    one materialises: 1e-2 / 2e-2.  The block's launches are checked per element against fp64 in
+    test_gpu_launch_census.py, the standalone linear attention's in test_gpu_attention_census.py."""
     ops, packing = pk
     ops.set_precision('bf16')
     ops.set_tensor_core_conv(True)
