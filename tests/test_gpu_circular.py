@@ -1,6 +1,8 @@
 """Unet3D(padding_mode='circular') on the GPU: the wrap-pad (halo) kernel, every circular convolution geometry of the
 Darcy network (forward, dgrad, weight gradient) per element against fp64, the plans the halo'd operands get, and the
-network end to end against fixtures of the UNMODIFIED reference (oracle/make_golden.py circular)."""
+network's forward, roll equivariance and guidance loss against fixtures of the UNMODIFIED reference
+(oracle/make_golden.py circular).  The circular training loss, graph-replayed step and sampling engine are the
+'circular' rows of test_gpu_e2e.py and test_gpu_parity_bench_path.py."""
 import math
 
 import pytest
@@ -8,6 +10,8 @@ import torch
 import torch.nn.functional as F
 
 from checks import rel
+from oracle import pidm_oracle as O
+from study import build_darcy
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -192,77 +196,46 @@ def test_circular_plans_match_the_zero_padded_layers(model):
 
 # ---- end to end -----------------------------------------------------------------------------------------------------
 @pytest.fixture(scope='module')
-def env():
-    from oracle import pidm_oracle as O
+def ops():
     from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-
-    def build(n_steps=100, padding_mode='circular', **kw):
-        model = Unet3D(dim=32, channels=2, padding_mode=padding_mode).to(DEV)
-        model.load_state_dict(O.make_test_state_dict(O.unet_config(dim=32, channels=2, padding_mode=padding_mode), 0))
-        diff = DenoisingDiffusion(n_steps, DEV, kw.get('residual_grad_guidance', False))
-        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                             device=DEV, bcs='periodic', domain_length=1., **kw)
-        return model, diff, res
-    yield dict(O=O, ops=ops, build=build)
+    yield ops
     ops.set_precision('bf16')
 
 
 @pytest.mark.parametrize('mode,tol', [('fp32', 1e-4), ('bf16', 3e-2)])
-def test_circular_unet_forward_matches_reference(env, golden, mode, tol):
-    env['ops'].set_precision(mode)
+def test_circular_unet_forward_matches_reference(ops, golden, mode, tol):
+    ops.set_precision(mode)
     gd = golden('unet_circular_fwd.pt')
-    model, _, _ = env['build']()
+    model, _, _ = build_darcy('circular')
     with torch.no_grad():
         y = model(gd['x'].to(DEV), gd['t'].to(DEV))
     assert rel(y, gd['y']) < tol, rel(y, gd['y'])
 
 
 @pytest.mark.parametrize('mode,tol', [('fp32', 1e-4), ('bf16', 3e-2)])
-def test_circular_unet_rolls_with_its_input(env, mode, tol):
+def test_circular_unet_rolls_with_its_input(ops, mode, tol):
     """rolling the input by (8, 16) pixels rolls the output; the zero-padded network fails the same check"""
-    env['ops'].set_precision(mode)
+    ops.set_precision(mode)
     g = torch.Generator().manual_seed(5)
     x = torch.randn(2, 2, 64, 64, generator=g).to(DEV)
     t = torch.tensor([3, 77], device=DEV)
     errs = {}
-    for pm in ('circular', 'zeros'):
-        model, _, _ = env['build'](padding_mode=pm)
+    for study in ('circular', 'periodic'):                  # 'periodic': periodic residual, zero-padded network
+        model, _, _ = build_darcy(study)
         with torch.no_grad():
             y = model(x, t)
             ys = model(torch.roll(x, (8, 16), (2, 3)), t)
-        errs[pm] = rel(ys, torch.roll(y, (8, 16), (2, 3)))
+        errs[study] = rel(ys, torch.roll(y, (8, 16), (2, 3)))
     assert errs['circular'] < tol, errs
-    assert errs['zeros'] > 0.1, errs
+    assert errs['periodic'] > 0.1, errs
 
 
 @pytest.mark.parametrize('mode,tol_loss,tol_grad', [('fp32', 5e-5, 1e-3), ('bf16', 3e-2, 8e-2)])
-def test_circular_training_loss_and_gradients_match_reference(env, golden, mode, tol_loss, tol_grad):
-    env['ops'].set_precision(mode)
-    gd = golden('darcy_loss_circular.pt')
-    model, diff, res = env['build']()
-    loss, data_l, rabs, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res,
-                                                          1.0, 1e-3)
-    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss
-    assert abs(data_l / gd['data_loss'].item() - 1) < tol_loss
-    assert abs(rabs / gd['residual_abs'].item() - 1) < tol_loss
-    loss.backward()
-    named = dict(model.named_parameters())
-    worst = {k: rel(env['O'].golden_sample(named[k[5:]].grad), v) for k, v in gd.items()
-             if k.startswith('grad_') and k != 'grad_norm'}
-    assert max(worst.values()) < tol_grad, worst
-    gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
-    assert abs(gn / gd['grad_norm'].item() - 1) < tol_grad
-
-
-@pytest.mark.parametrize('mode,tol_loss,tol_grad', [('fp32', 5e-5, 1e-3), ('bf16', 3e-2, 8e-2)])
-def test_circular_guidance_loss_matches_reference(env, golden, mode, tol_loss, tol_grad):
+def test_circular_guidance_loss_matches_reference(ops, golden, mode, tol_loss, tol_grad):
     """residual-gradient guidance: emb_conv[2] stays zero-padded inside the circular network"""
-    env['ops'].set_precision(mode)
+    ops.set_precision(mode)
     gd = golden('darcy_guidance_circular.pt')
-    model, diff, res = env['build'](residual_grad_guidance=True)
+    model, diff, res = build_darcy('circular', residual_grad_guidance=True)
     model._null_mask_override = gd['null_mask'].to(DEV)
     loss, _, _, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res, 1.0, 1e-3)
     model._null_mask_override = None
@@ -274,53 +247,12 @@ def test_circular_guidance_loss_matches_reference(env, golden, mode, tol_loss, t
         assert rel(named[k].grad, gd[gk]) < tol_grad, (k, rel(named[k].grad, gd[gk]))
 
 
-@pytest.mark.parametrize('mode,B,tol_loss,tol_grad', [('fp32', 32, 1e-5, 1e-4), ('bf16', 32, 2e-2, 6e-2)])
-def test_circular_graph_replayed_train_step_equals_eager(env, mode, B, tol_loss, tol_grad):
-    """the graph-replayed TrainEngine step (weight gradients on the side stream, the transposed layers' reading the
-    halo'd dy there) against the eager step: loss, flat gradient, step counter and the parameter / EMA update, with
-    the bounds of the zero-padded model's parity test"""
-    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    env['ops'].set_precision(mode)
-    g = torch.Generator().manual_seed(533 + B)
-    x0 = (0.7 * torch.randn(B, 2, 64, 64, generator=g)).to(DEV)
-    t = torch.randint(0, 100, (B,), generator=g).to(DEV)
-    e = torch.randn(B, 2, 64, 64, generator=g).to(DEV)
-    out = {}
-
-    def step(eng):
-        o1, o2 = torch.randint, torch.randn_like
-        torch.randint, torch.randn_like = (lambda *a, **k: t), (lambda *a, **k: e)
-        try:
-            return eng.step(x0)
-        finally:
-            torch.randint, torch.randn_like = o1, o2
-    for use_graph in (False, True):
-        model, diff, res = env['build']()
-        eng = TrainEngine(model, diff, res, use_graph=use_graph, snapshot_grad=True)
-        p0 = eng.fp.flat.clone()
-        loss, _, _ = step(eng)
-        torch.cuda.synchronize()
-        assert int(eng.fp.step_dev.item()) == 1
-        out[use_graph] = (loss.item(), eng.grad_snapshot.clone(), eng.fp.flat.clone() - p0, eng.fp.ema.clone() - p0)
-        if use_graph:
-            step(eng)
-            torch.cuda.synchronize()
-            assert int(eng.fp.step_dev.item()) == 2
-    (le, ge, pe, ee), (lg, gg, pg, eg) = out[False], out[True]
-    assert abs(lg / le - 1) < tol_loss, (lg, le)
-    assert rel(gg, ge) < tol_grad, rel(gg, ge)
-    assert (ge != 0).float().mean().item() > 0.8
-    assert rel(pg, pe) < (2e-2 if mode == 'fp32' else 0.5), rel(pg, pe)
-    assert rel(eg, ee) < (2e-2 if mode == 'fp32' else 0.5), rel(eg, ee)
-
-
 @pytest.mark.parametrize('mode,tol', [('fp32', 1e-4), ('bf16', 3e-2)])
-def test_circular_mechanics_model_forward_matches_oracle(env, mode, tol):
+def test_circular_mechanics_model_forward_matches_oracle(ops, mode, tol):
     """Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True, padding_mode='circular') at batch 2 against
     the circular oracle (fp64 on the device)"""
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    O = env['O']
-    env['ops'].set_precision(mode)
+    ops.set_precision(mode)
     cfg = O.unet_config(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True, padding_mode='circular')
     sd = O.make_test_state_dict(cfg, 5)
     model = Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True, padding_mode='circular').to(DEV)
@@ -334,24 +266,3 @@ def test_circular_mechanics_model_forward_matches_oracle(env, mode, tol):
         ref = O.unet_forward({k: v.to(DEV).double() for k, v in sd.items()}, cfg, x.double(), t)
     assert y.shape == (2, 3, 64, 64)
     assert rel(y, ref) < tol, rel(y, ref)
-
-
-def test_circular_sample_engine_matches_reference_and_graph_replay(env, golden, monkeypatch):
-    env['ops'].set_precision('fp32')
-    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
-    gd = golden('sample_loop_circular.pt')
-    model, diff, res = env['build'](n_steps=6)
-    model.eval()
-    it = iter(list(gd['noises']))
-    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: next(it).to(DEV))
-    x, r, traj = SampleEngine(model, diff, res, batch=1, use_graph=False).sample(x_init=gd['x_T'].to(DEV), trajectory=True)
-    monkeypatch.undo()
-    assert rel(traj[1], gd['x_after_first']) < 1e-4
-    assert rel(x, gd['x_final']) < 5e-4
-    assert rel(r, gd['residual']) < 5e-3
-    zfix = gd['noises'][0].to(DEV)
-    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: zfix)
-    xe = SampleEngine(model, diff, res, batch=1, use_graph=False).sample(x_init=gd['x_T'].to(DEV))[0].clone()
-    xg = SampleEngine(model, diff, res, batch=1, use_graph=True).sample(x_init=gd['x_T'].to(DEV))[0].clone()
-    monkeypatch.undo()
-    assert rel(xg, xe) < 1e-4, rel(xg, xe)

@@ -7,6 +7,7 @@ import torch
 
 from checks import rel
 from oracle import pidm_oracle as O
+from study import build_darcy
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -14,27 +15,16 @@ P = 64
 
 
 @pytest.fixture(scope='module')
-def env():
+def ops():
     from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
-
-    def residuals(bcs='none', model=None, **kw):
-        return ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=P, pixels_at_boundary=True, reverse_d1=True,
-                              device=DEV, bcs=bcs, domain_length=1., **kw)
-
-    def build(n_steps=6, bcs='none', use_ddim_x0=False, guidance=False):
-        model = Unet3D(dim=32, channels=2).to(DEV)
-        model.load_state_dict(sd)
-        model.eval()
-        diff = DenoisingDiffusion(n_steps, DEV, residual_grad_guidance=guidance)
-        res = residuals(bcs, model, use_ddim_x0=use_ddim_x0, ddim_steps=0, residual_grad_guidance=guidance)
-        return model, diff, res
-    yield dict(O=O, ops=ops, build=build, residuals=residuals)
+    yield ops
     ops.set_precision('bf16')
+
+
+def build(study='none', use_ddim_x0=False):
+    model, diff, res = build_darcy(study, n_steps=6, use_ddim_x0=use_ddim_x0)
+    model.eval()
+    return model, diff, res
 
 
 def compose(res, x, steps):
@@ -66,15 +56,20 @@ def kernel(res, x, steps, t=None, n_active=0, residual=None):
 
 
 # ---- kernel, one step: the reference's residual_correction ----------------------------------------------------------
-@pytest.mark.parametrize('bcs,fixture', [('none', 'cocogen.pt'), ('periodic', 'cocogen_periodic.pt')])
-def test_one_step_matches_reference(env, golden, bcs, fixture):
+@pytest.mark.parametrize('study,fixture', [('none', 'cocogen.pt'), ('periodic', 'cocogen_periodic.pt')])
+def test_one_step_matches_reference(golden, study, fixture):
+    """the kernel, and residual_correction, which applies it in place on the [B, P*P, 2] tensor like the reference"""
     gd = golden(fixture)
-    x, r = kernel(env['residuals'](bcs), gd['x0_pred'], 1)
-    x = x.cpu()
+    res = build(study)[2]
+    x, r = kernel(res, gd['x0_pred'], 1)
+    xin = gd['x0_pred'].permute(0, 2, 3, 1).reshape(2, P * P, 2).clone().to(DEV)
+    x_corr, r_corr = res.residual_correction(xin)
+    assert x_corr is xin
     d_ref = gd['corrected'] - gd['x0_pred']
-    assert rel(x - gd['x0_pred'], d_ref) < 1e-3, rel(x - gd['x0_pred'], d_ref)
-    assert torch.equal(x[:, 1], gd['x0_pred'][:, 1])
-    assert rel(r, gd['residual_corrected']) < 1e-5
+    for xc, rc in ((x.cpu(), r), (xin.reshape(2, P, P, 2).permute(0, 3, 1, 2).cpu(), r_corr)):
+        assert rel(xc - gd['x0_pred'], d_ref) < 1e-3, rel(xc - gd['x0_pred'], d_ref)
+        assert torch.equal(xc[:, 1], gd['x0_pred'][:, 1])
+        assert rel(rc, gd['residual_corrected']) < 1e-5
 
 
 # ---- kernel, several steps ------------------------------------------------------------------------------------------
@@ -85,9 +80,9 @@ def test_one_step_matches_reference(env, golden, bcs, fixture):
 # accumulated change of p is held to 1e-4 and the residual (a fixed linear map of that change plus f_s) to 1e-5.
 # Against the reference (fp32 vmap(jacfwd) path) and the fp64 oracle: the 1e-3 / 1e-5 of the one-step test.
 @pytest.mark.parametrize('steps', [2, 5, 200])
-@pytest.mark.parametrize('bcs,fixture', [('none', 'cocogen.pt'), ('periodic', 'cocogen_periodic.pt')])
-def test_steps_match_composition_and_reference(env, golden, bcs, fixture, steps):
-    res = env['residuals'](bcs)
+@pytest.mark.parametrize('study,fixture', [('none', 'cocogen.pt'), ('periodic', 'cocogen_periodic.pt')])
+def test_steps_match_composition_and_reference(golden, study, fixture, steps):
+    res = build(study)[2]
     x0 = golden(fixture)['x0_pred']
     x, r = kernel(res, x0, steps)
     xc, rc = compose(res, x0.to(DEV), steps)
@@ -97,13 +92,13 @@ def test_steps_match_composition_and_reference(env, golden, bcs, fixture, steps)
     assert torch.equal(x[:, 1], xc[:, 1])
     assert rel(d, dc) < 1e-4, rel(d, dc)
     assert rel(r, rc) < 1e-5, rel(r, rc)
-    if bcs == 'none' and steps <= 5:
+    if study == 'none' and steps <= 5:
         gd = golden('cocogen_steps.pt')
         d_ref = gd['p_iterates'][steps - 1] - gd['x0_pred'][:, 0]
         assert rel(d, d_ref) < 1e-3, rel(d, d_ref)
         if steps == gd['p_iterates'].shape[0]:
             assert rel(r, gd['residual_final']) < 1e-5
-    if bcs == 'none' and steps == 200:
+    if study == 'none' and steps == 200:
         # fp64 oracle: p is rounded to fp32 after each of the 200 steps, and the residual, a small difference of
         # second-difference terms of order K p / h^2, magnifies those roundings (measured 1.0e-4 on an H100)
         xo, ro, _ = O.cocogen_steps(x0.double(), steps)
@@ -112,18 +107,18 @@ def test_steps_match_composition_and_reference(env, golden, bcs, fixture, steps)
         assert rel(r, ro) < 3e-4, rel(r, ro)
 
 
-def test_zero_steps_is_the_residual(env, golden):
-    res = env['residuals']()
+def test_zero_steps_is_the_residual(ops, golden):
+    res = build()[2]
     x0 = golden('cocogen.pt')['x0_pred'].to(DEV)
     x, r = kernel(res, x0, 0)
     assert torch.equal(x, x0)
-    assert torch.equal(r, env['ops'].darcy_residual(x0, res.f_s_flat, *res.geometry))
+    assert torch.equal(r, ops.darcy_residual(x0, res.f_s_flat, *res.geometry))
 
 
 # ---- predication ----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize('bcs', ['none', 'periodic'])
-def test_inactive_samples_are_left_untouched(env, bcs):
-    res = env['residuals'](bcs)
+@pytest.mark.parametrize('study', ['none', 'periodic'])
+def test_inactive_samples_are_left_untouched(study):
+    res = build(study)[2]
     g = torch.Generator().manual_seed(5)
     B = 6
     x0 = torch.randn(B, 2, P, P, generator=g)
@@ -145,9 +140,9 @@ def test_inactive_samples_are_left_untouched(env, bcs):
     assert torch.equal(x, x0d) and torch.equal(r, r0)
 
 
-def test_abi_rejects_bad_arguments(env):
+def test_abi_rejects_bad_arguments():
     from physicsinformeddiffusionmodels_b200._lib import call, stream
-    res = env['residuals']()
+    res = build()[2]
     x = torch.zeros(1, 2, P, P, device=DEV)
     r = torch.zeros(1, P * P, 3, device=DEV)
     geo = res._abi_geometry()
@@ -189,18 +184,17 @@ CASES = {
     'xt_N2': dict(kw=dict(N_correction=2, correction_mode='xt')),
     'x0_N2': dict(kw=dict(N_correction=2, correction_mode='x0')),
     'M5': dict(kw=dict(M_correction=5)),
-    'periodic_xt_N3_M3': dict(bcs='periodic', kw=dict(N_correction=3, M_correction=3, correction_mode='xt')),
+    'periodic_xt_N3_M3': dict(study='periodic', kw=dict(N_correction=3, M_correction=3, correction_mode='xt')),
     'sample_mode_x0_N2_M2': dict(use_ddim_x0=True, kw=dict(N_correction=2, M_correction=2, correction_mode='x0')),
-    'guidance_xt_N2_M1': dict(guidance=True, kw=dict(N_correction=2, M_correction=1, correction_mode='xt')),
+    'guidance_xt_N2_M1': dict(study='guidance', kw=dict(N_correction=2, M_correction=1, correction_mode='xt')),
 }
 
 
 @pytest.mark.parametrize('case', list(CASES))
-def test_engine_matches_dropin(env, monkeypatch, case):
+def test_engine_matches_dropin(ops, monkeypatch, case):
     c = CASES[case]
-    env['ops'].set_precision('fp32')
-    model, diff, res = env['build'](bcs=c.get('bcs', 'none'), use_ddim_x0=c.get('use_ddim_x0', False),
-                                    guidance=c.get('guidance', False))
+    ops.set_precision('fp32')
+    model, diff, res = build(c.get('study', 'none'), c.get('use_ddim_x0', False))
     g = torch.Generator().manual_seed(21)
     x_T = torch.randn(2, 2, P, P, generator=g).to(DEV)
     zs = torch.randn(6, 2, 2, P, P, generator=g).to(DEV)
@@ -216,10 +210,10 @@ def test_engine_matches_dropin(env, monkeypatch, case):
 
 
 @pytest.mark.parametrize('tag,N,M', [('xt', 2, 3), ('x0', 2, 0)])
-def test_engine_and_dropin_match_reference(env, golden, monkeypatch, tag, N, M):
-    env['ops'].set_precision('fp32')
+def test_engine_and_dropin_match_reference(ops, golden, monkeypatch, tag, N, M):
+    ops.set_precision('fp32')
     gd = golden('sample_loop_cocogen.pt')
-    model, diff, res = env['build']()
+    model, diff, res = build()
     kw = dict(N_correction=N, M_correction=M, correction_mode=tag)
     x_T, zs = gd['x_T'].to(DEV), gd['noises'].to(DEV)
     xs, r_d = dropin(diff, res, x_T, zs, monkeypatch, **kw)
@@ -241,11 +235,11 @@ def test_engine_and_dropin_match_reference(env, golden, monkeypatch, tag, N, M):
 
 # ---- launches and validation ---------------------------------------------------------------------------------------
 @pytest.mark.parametrize('use_graph', [False, True])
-def test_engine_launch_count(env, monkeypatch, use_graph):
+def test_engine_launch_count(ops, monkeypatch, use_graph):
     from physicsinformeddiffusionmodels_b200 import _lib
     from physicsinformeddiffusionmodels_b200.engine import SampleEngine
-    env['ops'].set_precision('fp32')
-    model, diff, res = env['build']()
+    ops.set_precision('fp32')
+    model, diff, res = build()
     calls = []
     real = _lib.call
 
@@ -270,10 +264,10 @@ def test_engine_launch_count(env, monkeypatch, use_graph):
     assert n == (2 + k if use_graph else 2 * diff.n_steps) + 2, (n, k)
 
 
-def test_engine_rejects_bad_corrections(env):
+def test_engine_rejects_bad_corrections():
     from physicsinformeddiffusionmodels_b200.engine import SampleEngine
     from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
-    model, diff, res = env['build']()
+    model, diff, res = build()
     for mode in ('none', 'bad'):
         with pytest.raises(ValueError):
             SampleEngine(model, diff, res, batch=1, N_correction=1, correction_mode=mode)

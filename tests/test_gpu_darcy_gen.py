@@ -146,17 +146,11 @@ def test_guards(gen):
 
 
 def test_train_engine_on_generated_batches(gen):
-    from oracle import pidm_oracle as O
     from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
+    from study import build_darcy
     ops.set_precision('bf16')
-    model = Unet3D(dim=32, channels=2).to(DEV)
-    model.load_state_dict(O.make_test_state_dict(O.unet_config(dim=32, channels=2), 0))
-    diff = DenoisingDiffusion(100, DEV)
-    rd = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=P, pixels_at_boundary=True, reverse_d1=True, device=DEV)
+    model, diff, rd = build_darcy()
     eng = TrainEngine(model, diff, rd, use_graph=True)
     it = gen.batches(32, seed0=10)
     r_gen = []

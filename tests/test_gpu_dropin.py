@@ -1,6 +1,7 @@
 """The call sequence of the reference drivers (main.py:116-316, sample.py:112-150), written against the drop-in `src.*`
 module names with the reference's own glue (torch DataLoader, optim.Adam, clip_grad_norm_, EMA register/update/ema/
-restore, save_model/load_model, p_sample_loop).  Sizes are reduced (4 diffusion steps, 3 iterations)."""
+restore, save_model/load_model, p_sample_loop), with bcs = 'none' and with bcs = 'periodic' and CoCoGen corrections in
+the sampler.  Sizes are reduced (4 diffusion steps, 3 iterations)."""
 import os
 
 import numpy as np
@@ -10,7 +11,8 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-def test_reference_driver_sequence_runs_on_the_drop_in_modules(tmp_path):
+@pytest.mark.parametrize('bcs,M,N', [('none', 0, 0), ('periodic', 1, 1)])
+def test_reference_driver_sequence_runs_on_the_drop_in_modules(tmp_path, bcs, M, N):
     import torch.optim as optim
     from torch.utils.data import DataLoader
     from src.data_utils import Dataset, cycle  # noqa: F401
@@ -35,7 +37,7 @@ def test_reference_driver_sequence_runs_on_the_drop_in_modules(tmp_path):
     ema.register(model)
     assert sum(p.numel() for p in model.parameters() if p.requires_grad) == 10386482
     residuals = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                               device=device, bcs='none', domain_length=1., residual_grad_guidance=False,
+                               device=device, bcs=bcs, domain_length=1., residual_grad_guidance=False,
                                use_ddim_x0=False, ddim_steps=0)
     optimizer = optim.Adam(model.parameters(), lr=1.e-4)
     w_before = model.final_conv[1].weight.detach().clone()
@@ -62,13 +64,14 @@ def test_reference_driver_sequence_runs_on_the_drop_in_modules(tmp_path):
     # sampling exactly as main.py:220-225 / sample.py:145-150
     output = diffusion_utils.p_sample_loop(None, (2, 2, 64, 64), save_output=True, surpress_noise=True,
                                            use_dynamic_threshold=False, residual_func=residuals, eval_residuals=True,
-                                           return_optimizer=False, return_inequality=False, M_correction=0,
-                                           N_correction=0, correction_mode='xt')
+                                           return_optimizer=False, return_inequality=False, M_correction=M,
+                                           N_correction=N, correction_mode='xt')
     seqs, aux = output
+    assert torch.isfinite(aux['residual']).all()
     residual = aux['residual'].abs().mean(dim=tuple(range(1, aux['residual'].ndim)))
     assert residual.shape == (2,) and torch.isfinite(residual).all()
     seq = torch.stack(seqs[0], dim=0)
-    assert seq.shape == (5, 2, 2, 64, 64) and not seq.is_cuda and np.isfinite(seq[-1].numpy()).all()
+    assert seq.shape == (5 + M, 2, 2, 64, 64) and not seq.is_cuda and np.isfinite(seq[-1].numpy()).all()
     # checkpoint round trip in the reference's format
     ck = tmp_path / 'run' / 'model' / 'checkpoint_2.pt'
     assert ck.exists() and (tmp_path / 'run' / 'model' / 'model.yaml').exists()

@@ -1,44 +1,35 @@
 """End-to-end parity of the engine (U-Net, loss, gradients, sampler, training step) against the golden
-fixtures produced by the UNMODIFIED reference (tests/golden, oracle/make_golden.py) and against the CPU oracle.
+fixtures produced by the UNMODIFIED reference (tests/golden, oracle/make_golden.py) and against the CPU oracle.  The
+training loss and the sampling engine are checked for each study option (tests/study.py) that has a fixture.
 
 Two precision modes: 'fp32' activations (exact mode: only summation order differs from the reference -> tight
 tolerances) and 'bf16' (production mode: bf16 GEMM operands / activations, fp32 accumulate and statistics)."""
+import os
+
 import pytest
 import torch
 
 from checks import rel
+from oracle import pidm_oracle as O
+from study import build_darcy, config, fixed_draws, state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 
 
 @pytest.fixture(scope='module')
-def env():
-    from oracle import pidm_oracle as O
+def ops():
     from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
-
-    def build(n_steps=100, use_ddim_x0=False):
-        model = Unet3D(dim=32, channels=2).to(DEV)
-        model.load_state_dict(sd)
-        diff = DenoisingDiffusion(n_steps, DEV)
-        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                             device=DEV, bcs='none', domain_length=1., use_ddim_x0=use_ddim_x0, ddim_steps=0)
-        return model, diff, res
-    yield dict(O=O, ops=ops, build=build, cfg=cfg, sd=sd)
+    yield ops
     ops.set_precision('bf16')
 
 
 # fp32 mode: 1e-4 (accumulation order over K up to 4608 and ~60 layers); bf16 mode: 3e-2 (2^-9 per rounding)
 @pytest.mark.parametrize('mode,tol', [('fp32', 1e-4), ('bf16', 3e-2)])
-def test_unet_forward_matches_reference(env, golden, mode, tol):
-    env['ops'].set_precision(mode)
+def test_unet_forward_matches_reference(ops, golden, mode, tol):
+    ops.set_precision(mode)
     gd = golden('unet_darcy_fwd.pt')
-    model, _, _ = env['build']()
+    model, _, _ = build_darcy()
     with torch.no_grad():
         y = model(gd['x'].to(DEV), gd['t'].to(DEV))
         y2 = model(gd['x'].permute(0, 2, 3, 1).reshape(2, 4096, 2).to(DEV), gd['t'].to(DEV))
@@ -50,13 +41,12 @@ def test_unet_forward_matches_reference(env, golden, mode, tol):
     assert rel(y, gd['y']) < tol, rel(y, gd['y'])
 
 
-def test_unet_forward_tcgen05_vs_cuda_core_path(env, golden):
+def test_unet_forward_tcgen05_vs_cuda_core_path(ops, golden):
     """Same bf16 operands through the tensor-core (wgmma) kernels and through the CUDA-core implicit GEMM: both round the same
     activations to bf16, so they agree to accumulation order + 1-ulp bf16 flips that propagate through ~60 layers (2e-2)."""
-    ops = env['ops']
     ops.set_precision('bf16')
     gd = golden('unet_darcy_fwd.pt')
-    model, _, _ = env['build']()
+    model, _, _ = build_darcy()
     with torch.no_grad():
         ops.set_tensor_core_conv(True)
         y_tc = model(gd['x'].to(DEV), gd['t'].to(DEV))
@@ -66,36 +56,52 @@ def test_unet_forward_tcgen05_vs_cuda_core_path(env, golden):
     assert rel(y_tc, y_cc) < 2e-2, rel(y_tc, y_cc)
 
 
-@pytest.mark.parametrize('mode,tol_loss,tol_grad', [('fp32', 5e-5, 1e-3), ('bf16', 3e-2, 8e-2)])
-def test_training_loss_and_gradients_match_reference(env, golden, mode, tol_loss, tol_grad):
-    env['ops'].set_precision(mode)
-    gd = golden('darcy_loss_mean.pt')
-    model, diff, res = env['build']()
+# golden: (study, dead-parameter list or None, {mode: (loss, gradient, grad-norm tolerance)}).  A fixture with
+# 'null_mask' is a guidance step with that classifier-free mask; one with 'grad_sample' stores its gradients sampled
+# with that n.
+ZEROS_TOL = {'fp32': (5e-5, 1e-3, 1e-3), 'bf16': (3e-2, 8e-2, 8e-2)}
+LOSS_ROWS = {
+    'darcy_loss_mean': ('none', 'params_without_grad.txt', ZEROS_TOL),
+    'darcy_loss_periodic': ('periodic', None, ZEROS_TOL),
+    'darcy_loss_circular': ('circular', None, ZEROS_TOL),
+    'darcy_guidance_step': ('guidance', 'params_without_grad_guidance.txt',
+                            {'fp32': (5e-5, 2e-3, 1e-3), 'bf16': (3e-2, 1e-1, 8e-2)}),
+}
+
+
+@pytest.mark.parametrize('name,mode', [(n, m) for n in LOSS_ROWS for m in ('fp32', 'bf16')])
+def test_training_loss_and_gradients_match_reference(ops, golden, name, mode):
+    study, dead_list, tols = LOSS_ROWS[name]
+    tol_loss, tol_grad, tol_norm = tols[mode]
+    ops.set_precision(mode)
+    gd = golden(name + '.pt')
+    model, diff, res = build_darcy(study)
+    model._null_mask_override = gd['null_mask'].to(DEV) if 'null_mask' in gd else None
     loss, data_l, rabs, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res,
                                                           1.0, 1e-3)
-    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss
-    assert abs(data_l / gd['data_loss'].item() - 1) < tol_loss
-    assert abs(rabs / gd['residual_abs'].item() - 1) < tol_loss
+    model._null_mask_override = None
+    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss, (loss.item(), gd['loss'].item())
+    assert abs(float(data_l) / gd['data_loss'].item() - 1) < tol_loss
+    assert abs(float(rabs) / gd['residual_abs'].item() - 1) < tol_loss
     loss.backward()
     named = dict(model.named_parameters())
-    worst = {}
-    for k, v in gd.items():
-        if k.startswith('grad_') and k != 'grad_norm':
-            worst[k] = rel(env['O'].golden_sample(named[k[5:]].grad), v)
-    assert max(worst.values()) < tol_grad, worst
+    n = {'n': int(gd['grad_sample'])} if 'grad_sample' in gd else {}
+    worst = {k: rel(O.golden_sample(named[k[5:]].grad, **n), v) for k, v in gd.items()
+             if k.startswith('grad_') and k not in ('grad_norm', 'grad_sample')}
+    assert max(worst.values()) < tol_grad, sorted(worst.items(), key=lambda kv: -kv[1])[:5]
     gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
-    assert abs(gn / gd['grad_norm'].item() - 1) < tol_grad
-    import os
-    with open(os.path.join(os.path.dirname(__file__), 'golden', 'params_without_grad.txt')) as f:
-        ref_dead = sorted(k for k in f.read().split() if not k.endswith('rotary_emb.freqs'))
-    dead = sorted(k for k, p in named.items() if p.requires_grad and p.grad is None)
-    assert dead == ref_dead
+    assert abs(gn / gd['grad_norm'].item() - 1) < tol_norm
+    if dead_list is not None:
+        with open(os.path.join(os.path.dirname(__file__), 'golden', dead_list)) as f:
+            ref_dead = sorted(k for k in f.read().split() if not k.endswith('rotary_emb.freqs'))
+        dead = sorted(k for k, p in named.items() if p.requires_grad and p.grad is None)
+        assert dead == ref_dead
 
 
-def test_sample_mode_loss_matches_reference(env, golden):
-    env['ops'].set_precision('fp32')
+def test_sample_mode_loss_matches_reference(ops, golden):
+    ops.set_precision('fp32')
     gd = golden('darcy_loss_sample.pt')
-    model, diff, res = env['build'](use_ddim_x0=True)
+    model, diff, res = build_darcy(use_ddim_x0=True)
     loss, _, _, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res, 1.0, 1e-3)
     assert abs(loss.item() / gd['loss'].item() - 1) < 1e-4
     loss.backward()
@@ -103,11 +109,11 @@ def test_sample_mode_loss_matches_reference(env, golden):
     assert rel(model.init_conv.weight.grad, gd['grad_init_w']) < 2e-3
 
 
-def test_sampling_loop_matches_reference(env, golden, monkeypatch):
+def test_sampling_loop_matches_reference(ops, golden, monkeypatch):
     """p_sample_loop with the reference's own draws injected (x_T, then one z per step incl. t=0)."""
-    env['ops'].set_precision('fp32')
+    ops.set_precision('fp32')
     gd = golden('sample_loop_6.pt')
-    model, diff, res = env['build'](n_steps=6)
+    model, diff, res = build_darcy(n_steps=6)
     model.eval()
     draws = [gd['x_T']] + list(gd['noises'])
     it = iter(draws)
@@ -122,13 +128,15 @@ def test_sampling_loop_matches_reference(env, golden, monkeypatch):
     assert rel(aux['residual'], gd['residual']) < 5e-3      # residual amplifies x0 differences by 1/h^2
 
 
-def test_sample_engine_matches_reference_and_graph_replay(env, golden, monkeypatch):
+@pytest.mark.parametrize('name,study', [('sample_loop_6', 'none'), ('sample_loop_periodic', 'periodic'),
+                                        ('sample_loop_circular', 'circular')])
+def test_sample_engine_matches_reference_and_graph_replay(ops, golden, monkeypatch, name, study):
     """SampleEngine (device-side time index, one captured step replayed n_steps times) against the reference's
     trajectory with its own draws injected, and CUDA-graph replay against the eager loop on identical noise."""
-    env['ops'].set_precision('fp32')
+    ops.set_precision('fp32')
     from physicsinformeddiffusionmodels_b200.engine import SampleEngine
-    gd = golden('sample_loop_6.pt')
-    model, diff, res = env['build'](n_steps=6)
+    gd = golden(name + '.pt')
+    model, diff, res = build_darcy(study, n_steps=6)
     model.eval()
     it = iter(list(gd['noises']))
     monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: next(it).to(DEV))
@@ -146,34 +154,14 @@ def test_sample_engine_matches_reference_and_graph_replay(env, golden, monkeypat
     assert rel(xg, xe) < 1e-4, rel(xg, xe)
 
 
-def test_cocogen_correction_matches_reference(env, golden):
-    """SURVEY 8f.3 (residuals_darcy.py:209-240): the analytic Jacobian maximum + adjoint-stencil gradient against the
-    reference's vmap(jacfwd) path; the update is applied in place on the [B, P*P, 2] tensor like the reference."""
-    gd = golden('cocogen.pt')
-    _, _, res = env['build']()
-    xin = gd['x0_pred'].permute(0, 2, 3, 1).reshape(2, 4096, 2).clone().to(DEV)
-    x_corr, r_corr = res.residual_correction(xin)
-    assert x_corr is xin
-    img = xin.reshape(2, 64, 64, 2).permute(0, 3, 1, 2).cpu()
-    d_ref = gd['corrected'] - gd['x0_pred']
-    assert rel(img - gd['x0_pred'], d_ref) < 1e-3, rel(img - gd['x0_pred'], d_ref)
-    assert torch.equal(img[:, 1], gd['x0_pred'][:, 1])
-    assert rel(r_corr, gd['residual_corrected']) < 1e-5
-
-
 @pytest.mark.parametrize('mode,tol_loss,tol_grad', [('fp32', 5e-5, 2e-3), ('bf16', 3e-2, 1e-1)])
-def test_residual_gradient_guidance_matches_reference(env, golden, mode, tol_loss, tol_grad):
+def test_residual_gradient_guidance_matches_reference(ops, golden, mode, tol_loss, tol_grad):
     """SURVEY 8f.3 (residuals_darcy.py:114-126, unet_model.py:530-540,585-603): training loss and the gradients of the
     guidance-only layers with the reference's classifier-free mask, the forced-null-mask variant, and sampling with
     guidance scale 3, against the unmodified reference."""
-    env['ops'].set_precision(mode)
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
+    ops.set_precision(mode)
     gd = golden('darcy_guidance.pt')
-    model, _, _ = env['build']()
-    diff = DenoisingDiffusion(100, DEV, residual_grad_guidance=True)
-    res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True, device=DEV,
-                         bcs='none', domain_length=1., residual_grad_guidance=True)
+    model, diff, res = build_darcy('guidance')
     x0, t, e = gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV)
     model._null_mask_override = gd['null_mask'].to(DEV)
     loss, _, _, _, _ = diff.darcy_loss_from_draws(x0, t, e, res, 1.0, 1e-3)
@@ -194,12 +182,12 @@ def test_residual_gradient_guidance_matches_reference(env, golden, mode, tol_los
     assert rel(out['model_out'], gd['sample_x0']) < (2e-4 if mode == 'fp32' else 5e-2)
 
 
-def test_sampling_loop_with_cocogen_corrections(env, golden, monkeypatch):
+def test_sampling_loop_with_cocogen_corrections(ops, golden, monkeypatch):
     """p_sample_loop with N_correction / M_correction (reference :516-541): the corrected trajectory equals the plain
     one followed by explicit corrections where the reference applies them (correction_mode 'xt')."""
-    env['ops'].set_precision('fp32')
+    ops.set_precision('fp32')
     gd = golden('sample_loop_6.pt')
-    model, diff, res = env['build'](n_steps=6)
+    model, diff, res = build_darcy(n_steps=6)
     model.eval()
 
     def run(**kw):
@@ -224,11 +212,10 @@ def test_sampling_loop_with_cocogen_corrections(env, golden, monkeypatch):
 
 
 @pytest.mark.parametrize('B', [1, 3, 5, 16])
-def test_unet_tensor_core_path_at_odd_batch_sizes(env, B):
+def test_unet_tensor_core_path_at_odd_batch_sizes(ops, B):
     """Tile / chunk / cluster planning depends on the batch size (TN samples per pixel tile, per-sample pixel chunks of
     the attention kernels, one-wave pixel splits of the wgrads ...).  bf16 tensor-core path vs the fp32 CUDA-core path
     of the same engine (itself pinned to the oracle above) on the same weights and inputs: forward and gradients."""
-    ops = env['ops']
     g = torch.Generator().manual_seed(100 + B)
     x = torch.randn(B, 2, 64, 64, generator=g).to(DEV)
     t = torch.randint(0, 100, (B,), generator=g).to(DEV)
@@ -236,7 +223,7 @@ def test_unet_tensor_core_path_at_odd_batch_sizes(env, B):
     outs = {}
     for mode in ('fp32', 'bf16'):
         ops.set_precision(mode)
-        model, _, _ = env['build']()
+        model, _, _ = build_darcy()
         y = model(x, t)
         (y * cot).sum().backward()
         outs[mode] = (y.detach().clone(), model.init_conv.weight.grad.clone(),
@@ -246,12 +233,11 @@ def test_unet_tensor_core_path_at_odd_batch_sizes(env, B):
         assert rel(a, b) < 4e-2, rel(a, b)
 
 
-def test_mechanics_training_loss_matches_oracle(env, monkeypatch):
+def test_mechanics_training_loss_matches_oracle(ops, monkeypatch):
     """configs[2]: one loss evaluation + backward of the mechanics (topology-optimisation) branch -- q_sample on the
     65x65 fields, bilinear 65->64, Unet3D(channels=10, out_dim=3, sigmoid on the density channel), bilinear 64->65 of the
     displacements, matrix-free K(rho)u - f residual, compliance and volume-fraction terms (reference
     denoising_utils.py:629-710, residuals_mechanics_K.py:198-274) -- against the oracle composition in fp32."""
-    O, ops = env['O'], env['ops']
     ops.set_precision('fp32')
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
@@ -298,9 +284,8 @@ def test_mechanics_training_loss_matches_oracle(env, monkeypatch):
         assert rel(p.grad, params[name].grad) < 3e-3, (name, rel(p.grad, params[name].grad))
 
 
-def test_engine_training_steps_match_oracle(env):
+def test_engine_training_steps_match_oracle(ops):
     """3 optimizer steps of the flat-buffer engine (eager and CUDA-graph) vs the oracle's autograd + Adam + EMA."""
-    O, ops = env['O'], env['ops']
     ops.set_precision('fp32')
     from physicsinformeddiffusionmodels_b200.engine import TrainEngine
     B = 2
@@ -309,7 +294,8 @@ def test_engine_training_steps_match_oracle(env):
     ts = [torch.tensor([3, 70]), torch.tensor([50, 9]), torch.tensor([99, 0])]
     es = [torch.randn(B, 2, 64, 64, generator=g) for _ in ts]
     tables = O.diffusion_tables(100)
-    sdr = {k: v.clone().requires_grad_('freqs' not in k) for k, v in env['sd'].items()}
+    sd = state_dict()
+    sdr = {k: v.clone().requires_grad_('freqs' not in k) for k, v in sd.items()}
     train = [v for k, v in sdr.items() if v.requires_grad]
     m = [torch.zeros_like(p) for p in train]
     v = [torch.zeros_like(p) for p in train]
@@ -318,41 +304,35 @@ def test_engine_training_steps_match_oracle(env):
     for step, (t, e) in enumerate(zip(ts, es), 1):
         for p in train:
             p.grad = None
-        loss, _ = O.darcy_training_loss(sdr, env['cfg'], x0, t, e, tables)
+        loss, _ = O.darcy_training_loss(sdr, config(), x0, t, e, tables)
         loss.backward()
         ref_losses.append(loss.item())
         with torch.no_grad():
             grads = [p.grad if p.grad is not None else torch.zeros_like(p) for p in train]
             O.adam_ema_step(train, grads, m, v, ema, step)
-    model, diff, res = env['build']()
+    model, diff, res = build_darcy()
     eng = TrainEngine(model, diff, res, use_graph=False)
     losses = []
     for t, e in zip(ts, es):
-        draws = iter([e])
-        orig_randint, orig_randn_like = torch.randint, torch.randn_like
-        torch.randint = lambda *a, **k: t.to(DEV)
-        torch.randn_like = lambda *a, **k: next(draws).to(DEV)
-        try:
+        with fixed_draws(t.to(DEV), e.to(DEV)):
             loss, _, _ = eng.step(x0.to(DEV))
-        finally:
-            torch.randint, torch.randn_like = orig_randint, orig_randn_like
         losses.append(loss.item())
     for a, b in zip(losses, ref_losses):
         assert abs(a / b - 1) < 2e-3, (losses, ref_losses)
     named = dict(model.named_parameters())
     for k in ('final_conv.1.weight', 'downs.0.0.block1.proj.weight', 'mid_spatial_attn.fn.fn.fn.to_qkv.weight'):
         # Adam normalises every coordinate to |update| ~ lr, so parameters are compared by their UPDATE
-        upd = named[k].detach().cpu() - env['sd'][k]
-        upd_ref = sdr[k].detach() - env['sd'][k]
+        upd = named[k].detach().cpu() - sd[k]
+        upd_ref = sdr[k].detach() - sd[k]
         assert rel(upd, upd_ref) < 0.1, (k, rel(upd, upd_ref))
     sd_ema = eng.ema_state_dict()
-    assert set(sd_ema.keys()) == set(env['sd'].keys())
+    assert set(sd_ema.keys()) == set(sd.keys())
 
 
-def test_engine_cuda_graph_replay_runs_and_learns(env):
-    env['ops'].set_precision('bf16')
+def test_engine_cuda_graph_replay_runs_and_learns(ops):
+    ops.set_precision('bf16')
     from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    model, diff, res = env['build']()
+    model, diff, res = build_darcy()
     eng = TrainEngine(model, diff, res, use_graph=True, lr=1e-3)
     g = torch.Generator().manual_seed(22)
     x0 = (0.5 * torch.randn(4, 2, 64, 64, generator=g)).to(DEV)
@@ -368,11 +348,11 @@ def test_engine_cuda_graph_replay_runs_and_learns(env):
     assert int(eng.fp.step_dev.item()) == eng.steps_done
 
 
-def test_state_dict_roundtrip_and_cpu_rejection(env):
-    model, diff, res = env['build']()
+def test_state_dict_roundtrip_and_cpu_rejection():
+    model, diff, res = build_darcy()
     sd = model.state_dict()
     assert len(sd) == 317 and sum(v.numel() for v in sd.values()) == 10386514
-    assert list(sd.keys()) == list(env['sd'].keys())
+    assert list(sd.keys()) == list(state_dict().keys())
     with pytest.raises(RuntimeError):
         model(torch.zeros(1, 2, 64, 64), torch.zeros(1, dtype=torch.long))     # CPU tensor: no fallback
 

@@ -1,7 +1,8 @@
 """Residual-gradient guidance on the GPU: the guidance kernels per element against fp64 references (edited references
-rejected by the same bounds), and the engine end to end: graph replay against the eager step, the eager step against
-one training iteration of the unmodified reference (oracle/make_golden.py guidance), the optimizer update of the
-guidance layers, the in-graph mask draw, the sharded draw and the guided sampler."""
+rejected by the same bounds), and the engine end to end: the optimizer update of the guidance layers, the in-graph mask
+draw, the sharded draw and the guided sampler.  Graph replay against the eager step and the eager step against one
+training iteration of the unmodified reference (oracle/make_golden.py guidance) are the 'guidance' rows of
+test_gpu_parity_bench_path.py and test_gpu_e2e.py."""
 import math
 
 import pytest
@@ -9,6 +10,7 @@ import torch
 
 from checks import C_BOUND, P, U, fields, guarded, guards_intact, rel, within
 from oracle import pidm_oracle as O
+from study import build_darcy
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -176,20 +178,9 @@ def test_cond_embed_wgrad_per_element(B, dtype):
 
 # ---- engine ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope='module')
-def env():
+def ops():
     from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-
-    def build(n_steps=100, bcs='none', padding_mode='zeros'):
-        model = Unet3D(dim=32, channels=2, padding_mode=padding_mode).to(DEV)
-        model.load_state_dict(O.make_test_state_dict(O.unet_config(dim=32, channels=2, padding_mode=padding_mode), 0))
-        diff = DenoisingDiffusion(n_steps, DEV, residual_grad_guidance=True)
-        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                             device=DEV, bcs=bcs, domain_length=1., residual_grad_guidance=True)
-        return model, diff, res
-    yield dict(ops=ops, build=build)
+    yield ops
     ops.set_precision('bf16')
 
 
@@ -197,71 +188,10 @@ def _offset(eng, p):
     return eng.fp.offsets[next(i for i, q in enumerate(eng.fp.params) if q is p)]
 
 
-def _inject(t, e):
-    o1, o2 = torch.randint, torch.randn_like
-    torch.randint, torch.randn_like = (lambda *a, **k: t), (lambda *a, **k: e)
-    return lambda: setattr(torch, 'randint', o1) or setattr(torch, 'randn_like', o2)
-
-
-@pytest.mark.parametrize('B,bcs,padding_mode', [(32, 'none', 'zeros'), (5, 'none', 'zeros'),
-                                                (8, 'periodic', 'circular')])
-def test_graph_replayed_guidance_step_equals_eager(env, B, bcs, padding_mode):
+def test_guidance_layers_take_clip_and_adam_of_the_snapshot(ops):
     from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    env['ops'].set_precision('fp32')
-    g = torch.Generator().manual_seed(700 + B)
-    x0 = (0.7 * torch.randn(B, 2, 64, 64, generator=g)).to(DEV)
-    t = torch.randint(0, 100, (B,), generator=g).to(DEV)
-    e = torch.randn(B, 2, 64, 64, generator=g).to(DEV)
-    mask = (torch.arange(B) % 3 == 1).to(DEV)
-    out = {}
-    for use_graph in (False, True):
-        model, diff, res = env['build'](bcs=bcs, padding_mode=padding_mode)
-        model._null_mask_override = mask
-        eng = TrainEngine(model, diff, res, use_graph=use_graph, snapshot_grad=True)
-        restore = _inject(t, e)
-        try:
-            loss, _, _ = eng.step(x0)
-        finally:
-            restore()
-        torch.cuda.synchronize()
-        assert torch.equal(model._null_mask_last, mask)
-        out[use_graph] = (loss.item(), eng.grad_snapshot.clone())
-        named = dict(model.named_parameters())
-        for n in ('emb_conv.0.weight', 'emb_conv.2.weight', 'combine_conv.weight'):     # in the exchanged prefix
-            assert _offset(eng, named[n]) < eng.fp.live_total, n
-    (le, ge), (lg, gg) = out[False], out[True]
-    assert abs(lg / le - 1) < 1e-5, (lg, le)
-    assert rel(gg, ge) < 1e-4, rel(gg, ge)
-
-
-@pytest.mark.parametrize('mode,tol_loss,tol_grad,tol_norm', [('fp32', 5e-5, 2e-3, 1e-3), ('bf16', 3e-2, 1e-1, 8e-2)])
-def test_guidance_step_matches_reference(env, golden, mode, tol_loss, tol_grad, tol_norm):
-    env['ops'].set_precision(mode)
-    gd = golden('darcy_guidance_step.pt')
-    model, diff, res = env['build']()
-    model._null_mask_override = gd['null_mask'].to(DEV)
-    loss, data_l, rabs, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res,
-                                                          1.0, 1e-3)
-    model._null_mask_override = None
-    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss, (loss.item(), gd['loss'].item())
-    assert abs(float(data_l) / gd['data_loss'].item() - 1) < tol_loss
-    assert abs(float(rabs) / gd['residual_abs'].item() - 1) < tol_loss
-    loss.backward()
-    named = dict(model.named_parameters())
-    n = int(gd['grad_sample'])
-    worst = {k: rel(O.golden_sample(named[k[5:]].grad, n), v) for k, v in gd.items()
-             if k.startswith('grad_') and k not in ('grad_norm', 'grad_sample')}
-    assert max(worst.values()) < tol_grad, sorted(worst.items(), key=lambda kv: -kv[1])[:5]
-    gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
-    assert abs(gn / gd['grad_norm'].item() - 1) < tol_norm
-    dead = sorted(k for k, p in named.items() if p.requires_grad and p.grad is None)
-    assert dead == sorted(model.unused_parameter_names(guidance=True))
-
-
-def test_guidance_layers_take_clip_and_adam_of_the_snapshot(env):
-    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    env['ops'].set_precision('fp32')
-    model, diff, res = env['build']()
+    ops.set_precision('fp32')
+    model, diff, res = build_darcy('guidance')
     eng = TrainEngine(model, diff, res, use_graph=True, snapshot_grad=True)
     g = torch.Generator().manual_seed(11)
     x0 = (0.7 * torch.randn(8, 2, 64, 64, generator=g)).to(DEV)
@@ -282,10 +212,10 @@ def test_guidance_layers_take_clip_and_adam_of_the_snapshot(env):
         assert bool((err <= 4 * U * p0[sl].double().abs() + 1e-4 * eng.lr).all()), (name, err.max().item())
 
 
-def test_in_graph_mask_is_redrawn_every_replay(env):
+def test_in_graph_mask_is_redrawn_every_replay(ops):
     from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    env['ops'].set_precision('bf16')
-    model, diff, res = env['build']()
+    ops.set_precision('bf16')
+    model, diff, res = build_darcy('guidance')
     eng = TrainEngine(model, diff, res, use_graph=True)
     g = torch.Generator().manual_seed(12)
     x0 = (0.7 * torch.randn(32, 2, 64, 64, generator=g)).to(DEV)
@@ -298,9 +228,9 @@ def test_in_graph_mask_is_redrawn_every_replay(env):
     assert 0.07 <= m.mean().item() <= 0.13, m.mean().item()
 
 
-def test_sharded_cond_and_mask_are_slices_of_the_global_batch(env):
+def test_sharded_cond_and_mask_are_slices_of_the_global_batch():
     from physicsinformeddiffusionmodels_b200.unet_model import draw_null_mask
-    _, _, res = env['build']()
+    _, _, res = build_darcy('guidance')
     world, B = 4, 6
     x = fields(world * B, 31, DEV).float().permute(0, 2, 3, 1).reshape(world * B, P * P, 2).contiguous()
     full = res.residual_gradient(x)
@@ -313,10 +243,10 @@ def test_sharded_cond_and_mask_are_slices_of_the_global_batch(env):
         assert torch.equal(draw_null_mask(B, 0.1, DEV, (rank, world)), mfull[lo:hi])
 
 
-def test_guidance_sample_engine_graph_equals_eager(env, monkeypatch):
+def test_guidance_sample_engine_graph_equals_eager(ops, monkeypatch):
     from physicsinformeddiffusionmodels_b200.engine import SampleEngine
-    env['ops'].set_precision('fp32')
-    model, diff, res = env['build'](n_steps=6)
+    ops.set_precision('fp32')
+    model, diff, res = build_darcy('guidance', n_steps=6)
     model.eval()
     g = torch.Generator().manual_seed(13)
     x_T = torch.randn(2, 2, 64, 64, generator=g).to(DEV)

@@ -1,7 +1,8 @@
 """configs[2] (topology optimisation / linear elasticity): the mechanics branch of the training loss through the
 engine against the UNMODIFIED reference (tests/golden/mechanics_loss.pt, dense 8450 x 8450 assembly) and against the CPU
 oracle at the reference's model size (Unet3D dim=128, channels=10, out_dim=3; main.py:102-109,126), and the
-TrainEngine (flat buffers, fused Adam/EMA, CUDA graph) on that branch."""
+topology-optimisation evaluation metrics.  The TrainEngine (flat buffers, fused Adam/EMA, CUDA graph) on that branch is
+the 'mechanics' row of test_gpu_parity_bench_path.py, which builds it with `build` and `synthetic_batch`."""
 import pytest
 import torch
 
@@ -93,35 +94,6 @@ def test_mechanics_reference_model_size_matches_oracle(env, monkeypatch):
     named = dict(model.named_parameters())
     for k in ('final_conv.1.weight', 'init_conv.weight', 'downs.3.0.block1.proj.weight', 'ups.0.2.fn.fn.to_qkv.weight'):
         assert rel(named[k].grad, sdr[k].grad) < 1e-1, (k, rel(named[k].grad, sdr[k].grad))
-
-
-def test_mechanics_train_engine_graph_equals_eager(env):
-    """TrainEngine on the mechanics branch: the CUDA-graph step (no host synchronisation inside) against the eager step
-    on the same weights, batch and draws, fp32 mode; loss, flat gradient, and that the optimizer moved the weights."""
-    O, ops = env['O'], env['ops']
-    ops.set_precision('fp32')
-    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    inp, t, noise = synthetic_batch(2, 12)
-    inp, t, noise = inp.to(DEV), t.to(DEV), noise.to(DEV)
-    out = {}
-    for use_graph in (False, True):
-        _, _, model, diff, res = build(O, 32, 3)
-        eng = TrainEngine(model, diff, res, use_graph=use_graph, snapshot_grad=True, c_data=1.0, c_residual=1e-2,
-                          c_ineq=0.5, lambda_opt=1e-3)
-        p0 = eng.fp.flat.clone()
-        o1, o2 = torch.randint, torch.randn_like
-        torch.randint = lambda *a, **k: t
-        torch.randn_like = lambda *a, **k: noise
-        try:
-            loss, data_l, rabs = eng.step(inp)
-        finally:
-            torch.randint, torch.randn_like = o1, o2
-        torch.cuda.synchronize()
-        out[use_graph] = (loss.item(), eng.grad_snapshot.clone(), (eng.fp.flat - p0).abs().max().item())
-    (le, ge, de), (lg, gg, dg) = out[False], out[True]
-    assert abs(lg / le - 1) < 1e-5, (lg, le)
-    assert rel(gg, ge) < 1e-4, rel(gg, ge)
-    assert de > 0 and dg > 0
 
 
 def test_topopt_evaluation_metrics_match_reference(env, golden):

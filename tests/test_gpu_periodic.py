@@ -1,11 +1,13 @@
 """bcs='periodic' on the GPU: every periodic Darcy kernel per element against the fp64 periodic oracle, edited references
-rejected by the same predicate, and the engine end to end against the fixtures of the unmodified reference
-(oracle/make_golden.py periodic) at the tolerances of the matching 'none' tests."""
+rejected by the same predicate, and the guidance branch with the periodic residual against the oracle.  The engine
+against the periodic fixtures of the unmodified reference (oracle/make_golden.py periodic) runs as the 'periodic' rows
+of test_gpu_e2e.py, test_gpu_parity_bench_path.py, test_gpu_cocogen.py and test_gpu_dropin.py."""
 import pytest
 import torch
 
 from checks import C_BOUND, P, U, fields, guarded, guards_intact, rel, within
 from oracle import pidm_oracle as O
+from study import build_darcy, config, state_dict
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -193,120 +195,27 @@ def test_periodic_fd_stencil_per_element(B, mode):
 
 # ---- end to end ---------------------------------------------------------------------------------------------------
 @pytest.fixture(scope='module')
-def env():
+def ops():
     from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
-
-    def build(n_steps=100, **kw):
-        model = Unet3D(dim=32, channels=2).to(DEV)
-        model.load_state_dict(sd)
-        diff = DenoisingDiffusion(n_steps, DEV, kw.get('residual_grad_guidance', False))
-        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                             device=DEV, bcs='periodic', domain_length=1., **kw)
-        assert res.periodic
-        return model, diff, res
-    yield dict(ops=ops, build=build, cfg=cfg, sd=sd)
+    yield ops
     ops.set_precision('bf16')
 
 
-@pytest.mark.parametrize('mode,tol_loss,tol_grad', [('fp32', 5e-5, 1e-3), ('bf16', 3e-2, 8e-2)])
-def test_periodic_training_loss_and_gradients_match_reference(env, golden, mode, tol_loss, tol_grad):
-    env['ops'].set_precision(mode)
-    gd = golden('darcy_loss_periodic.pt')
-    model, diff, res = env['build']()
-    loss, data_l, rabs, _, _ = diff.darcy_loss_from_draws(gd['x0'].to(DEV), gd['t'].to(DEV), gd['noise'].to(DEV), res,
-                                                          1.0, 1e-3)
-    assert abs(loss.item() / gd['loss'].item() - 1) < tol_loss
-    assert abs(data_l / gd['data_loss'].item() - 1) < tol_loss
-    assert abs(rabs / gd['residual_abs'].item() - 1) < tol_loss
-    loss.backward()
-    named = dict(model.named_parameters())
-    worst = {k: rel(O.golden_sample(named[k[5:]].grad), v) for k, v in gd.items()
-             if k.startswith('grad_') and k != 'grad_norm'}
-    assert max(worst.values()) < tol_grad, worst
-    gn = torch.sqrt(sum((p.grad.double() ** 2).sum() for p in model.parameters() if p.grad is not None)).item()
-    assert abs(gn / gd['grad_norm'].item() - 1) < tol_grad
-
-
-def test_periodic_graph_replayed_train_step_equals_eager(env):
-    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
-    env['ops'].set_precision('fp32')
-    B = 32
-    g = torch.Generator().manual_seed(532)
-    x0 = (0.7 * torch.randn(B, 2, 64, 64, generator=g)).to(DEV)
-    t = torch.randint(0, 100, (B,), generator=g).to(DEV)
-    e = torch.randn(B, 2, 64, 64, generator=g).to(DEV)
-    out = {}
-    for use_graph in (False, True):
-        model, diff, res = env['build']()
-        eng = TrainEngine(model, diff, res, use_graph=use_graph, snapshot_grad=True)
-        o1, o2 = torch.randint, torch.randn_like
-        torch.randint, torch.randn_like = (lambda *a, **k: t), (lambda *a, **k: e)
-        try:
-            loss, _, _ = eng.step(x0)
-        finally:
-            torch.randint, torch.randn_like = o1, o2
-        torch.cuda.synchronize()
-        out[use_graph] = (loss.item(), eng.grad_snapshot.clone())
-    (le, ge), (lg, gg) = out[False], out[True]
-    assert abs(lg / le - 1) < 1e-5, (lg, le)
-    assert rel(gg, ge) < 1e-4, rel(gg, ge)
-    assert (ge != 0).float().mean().item() > 0.8
-
-
-def test_periodic_sample_engine_matches_reference_and_graph_replay(env, golden, monkeypatch):
-    env['ops'].set_precision('fp32')
-    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
-    gd = golden('sample_loop_periodic.pt')
-    model, diff, res = env['build'](n_steps=6)
-    model.eval()
-    it = iter(list(gd['noises']))
-    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: next(it).to(DEV))
-    x, r, traj = SampleEngine(model, diff, res, batch=1, use_graph=False).sample(x_init=gd['x_T'].to(DEV), trajectory=True)
-    monkeypatch.undo()
-    assert rel(traj[1], gd['x_after_first']) < 1e-4
-    assert rel(x, gd['x_final']) < 5e-4
-    assert rel(r, gd['residual']) < 5e-3
-    zfix = gd['noises'][0].to(DEV)
-    monkeypatch.setattr(torch, 'randn_like', lambda *a, **k: zfix)
-    xe = SampleEngine(model, diff, res, batch=1, use_graph=False).sample(x_init=gd['x_T'].to(DEV))[0].clone()
-    xg = SampleEngine(model, diff, res, batch=1, use_graph=True).sample(x_init=gd['x_T'].to(DEV))[0].clone()
-    monkeypatch.undo()
-    assert rel(xg, xe) < 1e-4, rel(xg, xe)
-
-
-def test_periodic_cocogen_correction_matches_reference(env, golden):
-    gd = golden('cocogen_periodic.pt')
-    _, _, res = env['build']()
-    xin = gd['x0_pred'].permute(0, 2, 3, 1).reshape(2, 4096, 2).clone().to(DEV)
-    x_corr, r_corr = res.residual_correction(xin)
-    assert x_corr is xin
-    img = xin.reshape(2, 64, 64, 2).permute(0, 3, 1, 2).cpu()
-    d_ref = gd['corrected'] - gd['x0_pred']
-    assert rel(img - gd['x0_pred'], d_ref) < 1e-3, rel(img - gd['x0_pred'], d_ref)
-    assert torch.equal(img[:, 1], gd['x0_pred'][:, 1])
-    assert rel(r_corr, gd['residual_corrected']) < 1e-5
-
-
-def test_periodic_residual_gradient_guidance_matches_oracle(env):
+def test_periodic_residual_gradient_guidance_matches_oracle(ops):
     """guidance branch (cond = d mean|r(x_t)| / d x_t with the periodic residual) through the engine vs the periodic
     oracle, fp32, with a classifier-free mask that drops one sample"""
-    env['ops'].set_precision('fp32')
+    ops.set_precision('fp32')
     g = torch.Generator().manual_seed(77)
     B = 4
     x0 = torch.randn(B, 2, 64, 64, generator=g)
     t = torch.randint(0, 100, (B,), generator=g)
     e = torch.randn(B, 2, 64, 64, generator=g)
     mask = torch.tensor([False, True, False, False])
-    sdr = {k: v.clone().requires_grad_('freqs' not in k) for k, v in env['sd'].items()}
-    loss_ref, _ = O.darcy_training_loss(sdr, env['cfg'], x0, t, e, O.diffusion_tables(100), guidance_null_mask=mask,
+    sdr = {k: v.clone().requires_grad_('freqs' not in k) for k, v in state_dict().items()}
+    loss_ref, _ = O.darcy_training_loss(sdr, config(), x0, t, e, O.diffusion_tables(100), guidance_null_mask=mask,
                                         periodic=True)
     loss_ref.backward()
-    model, diff, res = env['build'](residual_grad_guidance=True)
+    model, diff, res = build_darcy('periodic', residual_grad_guidance=True)
     model._null_mask_override = mask.to(DEV)
     loss, _, _, _, _ = diff.darcy_loss_from_draws(x0.to(DEV), t.to(DEV), e.to(DEV), res, 1.0, 1e-3)
     model._null_mask_override = None
@@ -315,48 +224,6 @@ def test_periodic_residual_gradient_guidance_matches_oracle(env):
     named = dict(model.named_parameters())
     for k in ('emb_conv.0.weight', 'combine_conv.weight', 'final_conv.1.weight'):
         assert rel(named[k].grad, sdr[k].grad) < 2e-3, (k, rel(named[k].grad, sdr[k].grad))
-
-
-def test_reference_driver_sequence_runs_with_periodic_bcs(tmp_path):
-    """main.py / sample.py with bcs = 'periodic' on the drop-in modules: training iterations with the reference glue,
-    then the ancestral sampler with the residual evaluated each step (4 diffusion steps, batch 3)."""
-    import numpy as np
-    import torch.optim as optim
-    from src.denoising_utils import DenoisingDiffusion, EMA, device
-    from src.residuals_darcy import ResidualsDarcy
-    from src.unet_model import Unet3D
-    from physicsinformeddiffusionmodels_b200 import ops
-    ops.set_precision('bf16')
-    diffusion_utils = DenoisingDiffusion(4, device, False)
-    model = Unet3D(dim=32, channels=2, sigmoid_last_channel=False).to(device)
-    ema = EMA(0.99)
-    ema.register(model)
-    residuals = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                               device=device, bcs='periodic', domain_length=1., residual_grad_guidance=False,
-                               use_ddim_x0=False, ddim_steps=0)
-    optimizer = optim.Adam(model.parameters(), lr=1.e-4)
-    w_before = model.final_conv[1].weight.detach().clone()
-    g = torch.Generator().manual_seed(5)
-    losses = []
-    for iteration in range(3):
-        model.train()
-        cur_batch = torch.randn(3, 2, 64, 64, generator=g).to(device)
-        loss, data_loss, residual_loss, _, _ = diffusion_utils.model_estimation_loss(
-            cur_batch, residual_func=residuals, c_data=1, c_residual=0.001, c_ineq=0, lambda_opt=0)
-        optimizer.zero_grad()
-        loss.backward()
-        torch.nn.utils.clip_grad_norm_(model.parameters(), 1.)
-        optimizer.step()
-        losses.append(loss.item())
-        if iteration > 0:
-            ema.update(model)
-    assert all(np.isfinite(losses)) and not torch.equal(model.final_conv[1].weight.detach(), w_before)
-    model.eval()
-    seqs, aux = diffusion_utils.p_sample_loop(None, (3, 2, 64, 64), save_output=True, surpress_noise=True,
-                                              use_dynamic_threshold=False, residual_func=residuals, eval_residuals=True,
-                                              return_optimizer=False, return_inequality=False, M_correction=1,
-                                              N_correction=1, correction_mode='xt')
-    assert torch.isfinite(aux['residual']).all() and torch.isfinite(seqs[0][-1]).all()
 
 
 def test_mechanics_periodic_equals_none():

@@ -1,14 +1,23 @@
 """The CPU oracle (oracle/pidm_oracle.py) against fixtures produced by the UNMODIFIED reference
-(oracle/make_golden.py), plus analytic known-answer tests (SURVEY.md section 4)."""
+(oracle/make_golden.py), plus analytic known-answer tests (SURVEY.md section 4).  The training loss, the sampling loop
+and the CoCoGen correction are checked for each study option (tests/study.py) that has a fixture."""
 import math
 import os
 
 import pytest
 import torch
 
+import study
 from checks import rel
 from oracle import make_golden
 from oracle import pidm_oracle as O
+
+
+def oracle_study(name):
+    """(config, seeded weights, periodic flag) of the oracle for a study of study.STUDIES"""
+    opts = study.STUDIES[name]
+    padding_mode = opts.get('padding_mode', 'zeros')
+    return study.config(padding_mode), study.state_dict(padding_mode), opts.get('bcs') == 'periodic'
 
 
 def test_every_golden_file_has_a_recipe():
@@ -84,27 +93,44 @@ def test_darcy_residual_manufactured_quadratic():
     assert r[1:-1, :, 1].abs().max() == 0 and r[:, 1:-1, 2].abs().max() == 0
 
 
-def test_training_loss_and_grads_match_reference(golden):
-    gd = golden('darcy_loss_mean.pt')
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = {k: v.clone().requires_grad_(v.is_floating_point() and 'freqs' not in k)
-          for k, v in O.make_test_state_dict(cfg, 0).items()}
-    tables = O.diffusion_tables(100)
-    loss, aux = O.darcy_training_loss(sd, cfg, gd['x0'], gd['t'], gd['noise'], tables)
+# golden: (study, gradient tolerance, extra assertions).  A fixture with 'null_mask' is a guidance step with that
+# classifier-free mask; one with 'grad_sample' stores its gradients sampled with that n.
+LOSS_ROWS = {
+    'darcy_loss_mean': ('none', 5e-4, dict(dead='params_without_grad.txt', dead_numel=1464432)),   # SURVEY.md 3.2
+    'darcy_loss_periodic': ('periodic', 5e-4, {}),
+    'darcy_loss_circular': ('circular', 5e-4, {}),
+    'darcy_guidance_step': ('guidance', 1e-3, dict(keys=('grad_emb_conv.0.weight', 'grad_combine_conv.bias'))),
+}
+
+
+@pytest.mark.parametrize('name', list(LOSS_ROWS))
+def test_training_loss_and_grads_match_reference(golden, name):
+    s, tol_grad, extra = LOSS_ROWS[name]
+    gd = golden(name + '.pt')
+    cfg, sd0, periodic = oracle_study(s)
+    sd = {k: v.clone().requires_grad_(v.is_floating_point() and 'freqs' not in k) for k, v in sd0.items()}
+    mask = gd.get('null_mask')
+    if mask is not None:
+        assert 0 < int(mask.sum()) < len(mask)                       # both branches of the mask are exercised
+    loss, aux = O.darcy_training_loss(sd, cfg, gd['x0'], gd['t'], gd['noise'], O.diffusion_tables(100),
+                                      guidance_null_mask=mask, periodic=periodic)
     assert abs(loss.item() / gd['loss'].item() - 1) < 2e-5
     assert abs(aux['data'].item() / gd['data_loss'].item() - 1) < 2e-5
     assert abs(aux['residual_abs'].item() / gd['residual_abs'].item() - 1) < 2e-5
     loss.backward()
-    for k, v in gd.items():
-        if k.startswith('grad_') and k != 'grad_norm':
-            assert rel(O.golden_sample(sd[k[5:]].grad), v) < 5e-4, k
+    n = {'n': int(gd['grad_sample'])} if 'grad_sample' in gd else {}
+    worst = {k: rel(O.golden_sample(sd[k[5:]].grad, **n), v) for k, v in gd.items()
+             if k.startswith('grad_') and k not in ('grad_norm', 'grad_sample')}
+    assert all(k in worst for k in extra.get('keys', ())), sorted(worst)
+    assert max(worst.values()) < tol_grad, sorted(worst.items(), key=lambda kv: -kv[1])[:5]
     gn = math.sqrt(sum((p.grad.double() ** 2).sum().item() for p in sd.values() if p.grad is not None))
     assert abs(gn / gd['grad_norm'].item() - 1) < 1e-4
-    dead = sorted(k for k, p in sd.items() if p.requires_grad and p.grad is None)
-    with open(os.path.join(os.path.dirname(__file__), 'golden', 'params_without_grad.txt')) as f:
-        ref_dead = [k for k in f.read().split() if not k.endswith('rotary_emb.freqs')]   # frozen, never trainable
-    assert dead == ref_dead
-    assert sum(sd[k].numel() for k in dead) == 1464432                                  # SURVEY.md section 3.2
+    if 'dead' in extra:
+        dead = sorted(k for k, p in sd.items() if p.requires_grad and p.grad is None)
+        with open(os.path.join(os.path.dirname(__file__), 'golden', extra['dead'])) as f:
+            ref_dead = [k for k in f.read().split() if not k.endswith('rotary_emb.freqs')]   # frozen, never trainable
+        assert dead == ref_dead
+        assert sum(sd[k].numel() for k in dead) == extra['dead_numel']
 
 
 def test_sample_mode_loss_matches_reference(golden):
@@ -119,13 +145,13 @@ def test_sample_mode_loss_matches_reference(golden):
     assert rel(sd['init_conv.weight'].grad, gd['grad_init_w']) < 5e-4
 
 
-def test_sampling_loop_matches_reference(golden):
-    gd = golden('sample_loop_6.pt')
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
-    tables = O.diffusion_tables(6)
+@pytest.mark.parametrize('name,s', [('sample_loop_6', 'none'), ('sample_loop_periodic', 'periodic'),
+                                    ('sample_loop_circular', 'circular')])
+def test_sampling_loop_matches_reference(golden, name, s):
+    gd = golden(name + '.pt')
+    cfg, sd, periodic = oracle_study(s)
     with torch.no_grad():
-        x, r = O.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), tables, 6)
+        x, r = O.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), O.diffusion_tables(6), 6, periodic=periodic)
     assert rel(x, gd['x_final']) < 2e-4
     assert rel(r, gd['residual']) < 2e-3          # residual amplifies x0 differences by 1/h^2
 
@@ -212,10 +238,11 @@ def test_toy_loss_matches_reference(golden, tag, mode, ddim):
     assert rel(sd['lin2.embed.weight'].grad, gd[tag + '_grad_embed2']) < 1e-4
 
 
-def test_cocogen_correction_matches_reference(golden):
+@pytest.mark.parametrize('name,s', [('cocogen', 'none'), ('cocogen_periodic', 'periodic')])
+def test_cocogen_correction_matches_reference(golden, name, s):
     """SURVEY 8f.3: ResidualsDarcy.residual_correction through the reference's vmap(jacfwd) Jacobian vs the oracle."""
-    gd = golden('cocogen.pt')
-    xc, rc = O.cocogen_correction(gd['x0_pred'])
+    gd = golden(name + '.pt')
+    xc, rc = O.cocogen_correction(gd['x0_pred'], periodic=oracle_study(s)[2])
     # the correction itself is tiny (step 1e-6 / max|J|): compare the CHANGE, not the field
     d_ref = gd['corrected'] - gd['x0_pred']
     assert d_ref.abs().max() > 0

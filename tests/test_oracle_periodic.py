@@ -1,6 +1,7 @@
-"""bcs='periodic' on the CPU: the oracle's periodic option (oracle/pidm_oracle.py) against fixtures produced by the
-UNMODIFIED reference with ResidualsDarcy(bcs='periodic') (oracle/make_golden.py periodic), an fp64 known answer, and the
-host logic of the flag.  Tolerances are those of the matching 'none' tests in test_oracle_golden.py."""
+"""bcs='periodic' on the CPU: the oracle's periodic residual, its VJP and stencils (oracle/pidm_oracle.py) against
+fixtures produced by the UNMODIFIED reference with ResidualsDarcy(bcs='periodic') (oracle/make_golden.py periodic), an
+fp64 known answer, and the host logic of the flag.  The periodic loss, sampling loop and CoCoGen correction are rows of
+test_oracle_golden.py."""
 import math
 
 import pytest
@@ -26,45 +27,6 @@ def test_periodic_stencil_modes_match_reference(golden, mode):
     gd = golden('darcy_residual_periodic.pt')
     d0, d1 = O.spacing(64)
     assert rel(O.stencil_gradients(gd['x0_pred'][:, 0], mode, d0, d1, periodic=True), gd['stencil_' + mode]) < 1e-5
-
-
-def test_periodic_cocogen_correction_matches_reference(golden):
-    gd = golden('cocogen_periodic.pt')
-    xc, rc = O.cocogen_correction(gd['x0_pred'], periodic=True)
-    d_ref = gd['corrected'] - gd['x0_pred']
-    assert d_ref.abs().max() > 0
-    assert rel(xc - gd['x0_pred'], d_ref) < 1e-3
-    assert torch.equal(xc[:, 1], gd['x0_pred'][:, 1])
-    assert rel(rc, gd['residual_corrected']) < 1e-5
-
-
-def test_periodic_training_loss_and_grads_match_reference(golden):
-    gd = golden('darcy_loss_periodic.pt')
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = {k: v.clone().requires_grad_(v.is_floating_point() and 'freqs' not in k)
-          for k, v in O.make_test_state_dict(cfg, 0).items()}
-    tables = O.diffusion_tables(100)
-    loss, aux = O.darcy_training_loss(sd, cfg, gd['x0'], gd['t'], gd['noise'], tables, periodic=True)
-    assert abs(loss.item() / gd['loss'].item() - 1) < 2e-5
-    assert abs(aux['data'].item() / gd['data_loss'].item() - 1) < 2e-5
-    assert abs(aux['residual_abs'].item() / gd['residual_abs'].item() - 1) < 2e-5
-    loss.backward()
-    for k, v in gd.items():
-        if k.startswith('grad_') and k != 'grad_norm':
-            assert rel(O.golden_sample(sd[k[5:]].grad), v) < 5e-4, k
-    gn = math.sqrt(sum((p.grad.double() ** 2).sum().item() for p in sd.values() if p.grad is not None))
-    assert abs(gn / gd['grad_norm'].item() - 1) < 1e-4
-
-
-def test_periodic_sampling_loop_matches_reference(golden):
-    gd = golden('sample_loop_periodic.pt')
-    cfg = O.unet_config(dim=32, channels=2)
-    sd = O.make_test_state_dict(cfg, 0)
-    tables = O.diffusion_tables(6)
-    with torch.no_grad():
-        x, r = O.p_sample_loop(sd, cfg, gd['x_T'], list(gd['noises']), tables, 6, periodic=True)
-    assert rel(x, gd['x_final']) < 2e-4
-    assert rel(r, gd['residual']) < 2e-3
 
 
 def test_periodic_residual_known_answer_fourier_modes():
