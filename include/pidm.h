@@ -78,7 +78,10 @@ int pidm_fd_stencil(const float* u, float* out, int planes, int pixels, int mode
 /* Fused PIDM loss (src/denoising_utils.py:669-692): sums3 = {c_data*mean_b(p2[t] mse_b), mean(c_res*0.5 r^2/var_t),
  * mean|r|}; optionally the gradient of (sums3[0]+sums3[1]) w.r.t. x0hat (residual operand) and model_out (data
  * operand; pass the same pointer twice in 'mean' mode, then only grad_x0hat is written).  The residual is never
- * materialised.  grad pointers may be NULL (loss only). */
+ * materialised.  The gradient pointers take one of three forms, any other is rejected before a launch:
+ *   grad_x0hat = grad_model_out = NULL                  loss only (either model_out);
+ *   grad_x0hat set, grad_model_out = NULL               model_out == x0hat: the data gradient is added into grad_x0hat;
+ *   grad_x0hat and grad_model_out both set              model_out != x0hat. */
 int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, const float* target, const float* f_s,
                          const long long* t, const float* p2_loss_weight, const float* posterior_var_clipped,
                          float c_data, float c_residual, float* sums3, float* grad_x0hat, float* grad_model_out, int B,

@@ -462,12 +462,12 @@ def darcy_residual(x0_pred, domain_length=1.0, reverse_d1=True, pixels_at_bounda
     return torch.stack([eq0, bc0, bc1], dim=-1).reshape(B, P * P, 3)
 
 
-def darcy_stencils(P, periodic=False):
-    """The stencils of darcy_residual at its default geometry as [P,P] fp64 matrices (D1_0, D2_0, D1_1, D2_1):
+def darcy_stencils(P, periodic=False, domain_length=1.0, reverse_d1=True, pixels_at_boundary=True):
+    """The stencils of darcy_residual at the geometry given (spacing) as [P,P] fp64 matrices (D1_0, D2_0, D1_1, D2_1):
     fd_first(u, -2, d0) = D1_0 u and fd_first(u, -1, d1) = u D1_1^T, likewise fd_second with D2.  Their absolute values
     bound every rounding of an fp32 evaluation of the stencils."""
     mats = []
-    for h in spacing(P):
+    for h in spacing(P, domain_length, reverse_d1, pixels_at_boundary):
         D1 = torch.zeros(P, P, dtype=torch.float64)
         D2 = torch.zeros(P, P, dtype=torch.float64)
         for i in range(P):
@@ -497,14 +497,17 @@ def along_cols(M, u):
     return torch.einsum('kj,bij->bik', M, u)
 
 
-def darcy_residual_matrix(x, periodic=False, absolute=False, stencils=None):
-    """darcy_residual at its default geometry from the darcy_stencils matrices, x [B,2,P,P] fp64 -> [B,P*P,3]: the
-    fp64 reference the GPU tests compare fp32 kernels with.  absolute=True evaluates it with |stencils|, |fields| and
-    |f_s|, which bounds every intermediate of an fp32 evaluation.  `stencils` replaces darcy_stencils(P, periodic)."""
+def darcy_residual_matrix(x, periodic=False, absolute=False, stencils=None, domain_length=1.0, reverse_d1=True,
+                          pixels_at_boundary=True):
+    """darcy_residual from the darcy_stencils matrices, x [B,2,P,P] fp64 -> [B,P*P,3]: the fp64 reference the GPU tests
+    compare fp32 kernels with.  absolute=True evaluates it with |stencils|, |fields| and |f_s|, which bounds every
+    intermediate of an fp32 evaluation.  `stencils` replaces darcy_stencils(P, periodic, <geometry>); reverse_d1 also
+    sets the sign of the bc_x1 channel, as in darcy_residual."""
     P = x.shape[-1]
-    mats = darcy_stencils(P, periodic) if stencils is None else stencils
-    if absolute:
-        mats, x = [m.abs() for m in mats], x.abs()
+    geom = dict(domain_length=domain_length, reverse_d1=reverse_d1, pixels_at_boundary=pixels_at_boundary)
+    mats = darcy_stencils(P, periodic, **geom) if stencils is None else stencils
+    if absolute:      # |x| as a select, not x.abs(): the derivative of abs vanishes at an exact zero, which would drop
+        mats, x = [m.abs() for m in mats], torch.where(x < 0, -x, x)     # that pixel from darcy_residual_vjp's bound
     D1a, D2a, D1b, D2b = (m.to(x.device) for m in mats)
     p, K = x[:, 0], x[:, 1]
     p0, p1, K0, K1 = along_rows(D1a, p), along_cols(D1b, p), along_rows(D1a, K), along_cols(D1b, K)
@@ -518,18 +521,21 @@ def darcy_residual_matrix(x, periodic=False, absolute=False, stencils=None):
     else:
         eq0 = -K * lap - K0 * p0 - K1 * p1 - fs
         bc0[:, 0], bc0[:, -1] = -p0[:, 0], p0[:, -1]
-        bc1[:, :, 0], bc1[:, :, -1] = p1[:, :, 0], -p1[:, :, -1]
+        sgn = 1.0 if reverse_d1 else -1.0
+        bc1[:, :, 0], bc1[:, :, -1] = sgn * p1[:, :, 0], -sgn * p1[:, :, -1]
     return torch.stack([eq0, bc0, bc1], dim=-1).reshape(x.shape[0], P * P, 3)
 
 
-def darcy_residual_vjp(x, cot, periodic=False, absolute=False):
+def darcy_residual_vjp(x, cot, periodic=False, absolute=False, **geom):
     """J^T cot of darcy_residual_matrix in fp64; absolute=True: |J|^T |cot| at |x| (the residual is bilinear in (p, K)
-    with non-negative coefficients in its absolute form, so this gradient bounds every product of the adjoint)"""
+    with non-negative coefficients in its absolute form, so this gradient bounds every product of the adjoint).
+    geom: the geometry keywords of darcy_residual_matrix."""
     xa = (x.abs() if absolute else x).clone().requires_grad_(True)
-    r = darcy_residual_matrix(xa, periodic, absolute)
-    if absolute:
-        r = r - darcy_residual_matrix(torch.zeros_like(xa), periodic, True)      # drop the constant |f_s|
-    return torch.autograd.grad((r * (cot.abs() if absolute else cot)).sum(), xa)[0]
+    with torch.enable_grad():
+        r = darcy_residual_matrix(xa, periodic, absolute, **geom)
+        if absolute:
+            r = r - darcy_residual_matrix(torch.zeros_like(xa), periodic, True, **geom)      # drop the constant |f_s|
+        return torch.autograd.grad((r * (cot.abs() if absolute else cot)).sum(), xa)[0]
 
 
 # --------------------------------------------------------------------------------------------
@@ -747,6 +753,30 @@ def mechanics_residual(x0_pred, bcs, vf, KE=None):
     compliance = (u * Ku).sum(dim=1)
     ineq = rho.mean(dim=1) - vf
     return residual, compliance, ineq
+
+
+def mechanics_matfree(u, rho, bcs, KE=None, absolute=False):
+    """pidm_mechanics_residual_fwd on its own operands, any nel: u [B,2,nn,nn] nodal displacements, rho [B,nel,nel],
+    bcs [B,4,nn,nn] = (bc_x, bc_y, load_x, load_y), nn = nel + 1.  Returns (residual [B, 2 nn^2] in the dof order
+    2*node + d, compliance [B]):
+       residual = K(rho) u - f with the Dirichlet rows (bcs[:, :2] != 0) replaced by identity rows and f zeroed there,
+       compliance = u^T (that modified K) u.
+    K(rho) u is formed from four shifted views of the node planes, one per local node of the Q4 element, so it shares no
+    indexing with mechanics_mesh.  Differentiable: its VJP comes from autograd.  absolute=True evaluates it with |KE|,
+    |u|, |rho| and |f|, which bounds every intermediate of an fp32 evaluation."""
+    KE = (q4_plane_stress_stiffness() if KE is None else torch.as_tensor(KE)).to(u)
+    fixed = bcs[:, :2] != 0
+    if absolute:      # selects, not abs(): as in darcy_residual_matrix, a VJP through them keeps exact zeros
+        KE, u, rho, bcs = (torch.where(v < 0, -v, v) for v in (KE, u, rho, bcs))
+    nel = rho.shape[-1]
+    corners = ((1, 0), (1, 1), (0, 1), (0, 0))              # local nodes n1..n4 of element (er, ec): (er + dr, ec + dc)
+    ue = torch.stack([u[:, d, dr:dr + nel, dc:dc + nel] for dr, dc in corners for d in (0, 1)], dim=1)
+    fe = torch.einsum('ij,bjrc->birc', KE, ue) * rho[:, None]
+    Ku = sum(F.pad(fe[:, 2 * k:2 * k + 2], (dc, 1 - dc, dr, 1 - dr)) for k, (dr, dc) in enumerate(corners))
+    f = torch.where(fixed, torch.zeros_like(u), bcs[:, 2:4])
+    w = torch.where(fixed, u, Ku)
+    r = w + f if absolute else w - f
+    return r.permute(0, 2, 3, 1).reshape(u.shape[0], -1), (u * w).sum(dim=(1, 2, 3))
 
 
 def mechanics_training_loss(sd, cfg, inp, t, noise, tables, c_data=1.0, c_residual=1e-2, c_ineq=0.0, lambda_opt=0.0):

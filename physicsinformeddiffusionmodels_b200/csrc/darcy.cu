@@ -870,6 +870,13 @@ extern "C" int pidm_darcy_pidm_loss(const float* x0hat, const float* model_out, 
                                     float* grad_model_out, int B, int pixels, float domain_length, int reverse_d1,
                                     int flags, void* stream) {
     if (int e = check_flags(flags)) return e;
+    // darcy_grad_kernel<2> writes grad_model_out only when model_out is a separate tensor, and then whenever grad_x0hat
+    // is written: any other combination would store through NULL or leave a requested gradient unwritten
+    PIDM_REQUIRE(x0hat != nullptr && model_out != nullptr, "darcy_pidm_loss: x0hat and model_out must not be NULL");
+    PIDM_REQUIRE(model_out == x0hat ? grad_model_out == nullptr : (grad_x0hat == nullptr) == (grad_model_out == nullptr),
+                 "darcy_pidm_loss: gradients must be both NULL, grad_x0hat alone (model_out == x0hat) or both "
+                 "(model_out != x0hat); got grad_x0hat %s, grad_model_out %s, model_out %s x0hat",
+                 grad_x0hat ? "set" : "NULL", grad_model_out ? "set" : "NULL", model_out == x0hat ? "==" : "!=");
     PIDM_CUDA(cudaMemsetAsync(sums3, 0, 3 * sizeof(float), (cudaStream_t)stream));
     return launch_darcy_grad_any<2>(x0hat, f_s, nullptr, grad_x0hat, target, model_out, grad_model_out, t, p2_loss_weight,
                                     posterior_var_clipped, c_data, c_residual, sums3, B, pixels, domain_length, reverse_d1,

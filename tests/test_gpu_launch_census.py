@@ -486,21 +486,29 @@ def _key_of(name, a):
 
 
 def _record(fn, key_of=_key_of):
-    from physicsinformeddiffusionmodels_b200 import ops
+    """the keys of the libpidm calls fn makes.  `call` is swapped in _lib and in every package module that imported it
+    (ops, engine, residuals_mechanics_K, ...), and put back in any module that imported the recorder meanwhile."""
+    from physicsinformeddiffusionmodels_b200 import _lib
     seen = set()
-    orig = ops.call
+    orig = _lib.call
 
     def rec(name, *a):
         k = key_of(name, a)
         if k is not None:
             seen.add(k)
         return orig(name, *a)
-    ops.call = rec
+
+    def package_modules(binding):
+        return [m for n, m in list(sys.modules.items())
+                if n.startswith('physicsinformeddiffusionmodels_b200') and getattr(m, 'call', None) is binding]
+    for m in package_modules(orig):
+        m.call = rec
     try:
         fn()
         torch.cuda.synchronize()
     finally:
-        ops.call = orig
+        for m in package_modules(rec):
+            m.call = orig
     return seen
 
 
