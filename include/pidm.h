@@ -327,6 +327,10 @@ int pidm_adam_ema_step(float* param, float* grad, float* exp_avg, float* exp_avg
                        float lr, double beta1, double beta2, float eps, int step, int* step_counter_dev,
                        const float* grad_norm_sq_dev, float grad_scale, float max_norm, float ema_mu,
                        int ema_first_step, int zero_grad, void* stream);
+/* a[i] <-> b[i] for i < n, in place, one pass (ema.ema / ema.restore of main.py:183,316 on the flat weight and EMA
+ * buffers: two calls restore every bit, and no pointer into either buffer changes).  n % 4 == 0 and both pointers
+ * 16-byte aligned, else an error is returned and nothing is launched. */
+int pidm_swap_f32(float* a, float* b, long long n, void* stream);
 
 /* ---- mechanics residual, matrix-free (src/residuals_mechanics_K.py:166-274) ------------------------------ */
 /* u [B,2,65,65] nodal displacements, rho [B,64,64], bcs [B,4,65,65] = (bc_x, bc_y, load_x, load_y), KE [8,8].
@@ -339,7 +343,10 @@ int pidm_mechanics_residual_bwd(const float* u, const float* rho, const float* b
 /* Fused PIDM loss of the mechanics branch + its gradients (src/denoising_utils.py:669-710), one launch:
  * u [B,2,n] displacements on the (nel+1)^2 node grid, rho [B,nel,nel], x0 [B,3,n] = (disp_x, disp_y, E) data target,
  * residual [B,2n], compliance [B], vf [B].  sums6 (zeroed here) = data, residual, inequality, optimisation loss terms,
- * mean|r|, mean_b(mean(rho_b) - vf_b).  grad_u / grad_rho / grad_residual / grad_compliance are overwritten. */
+ * mean|r|, mean_b(mean(rho_b) - vf_b).  grad_u / grad_rho / grad_residual / grad_compliance are overwritten, or all four
+ * are NULL: loss only (every CTA adds the same per-sample contributions to the sums, with atomics in any order, so
+ * the sums agree bitwise for B = 1 and to the order of the additions otherwise); any other combination is rejected
+ * before a launch. */
 int pidm_mech_pidm_loss(const float* u, const float* rho, const float* x0, const float* residual, const float* compliance,
                         const float* vf, const long long* t, const float* p2_loss_weight,
                         const float* posterior_var_clipped, float c_data, float c_residual, float c_ineq,

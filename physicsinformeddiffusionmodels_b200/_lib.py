@@ -79,6 +79,7 @@ _SIGS = {
     'pidm_head_bwd': [P, P, P, P, P, P, P, I, I, I, I, I, I, P],
     'pidm_sumsq': [P, L, P, P, P],
     'pidm_adam_ema_step': [P, P, P, P, P, L, F, D, D, F, I, P, P, F, F, F, I, I, P],
+    'pidm_swap_f32': [P, P, L, P],
     'pidm_mechanics_residual_fwd': [P, P, P, P, P, P, I, I, P],
     'pidm_mechanics_residual_bwd': [P, P, P, P, P, P, P, P, P, I, I, P],
     'pidm_mech_pidm_loss': [P, P, P, P, P, P, P, P, P, F, F, F, F, P, P, P, P, P, I, I, P],

@@ -221,6 +221,7 @@ __global__ void bilinear_bwd_kernel(const float* __restrict__ dy, float* __restr
 //          broadcast, :679,:694)                                             -> g_rho (+= dq_j / nel^2)
 //   opt  = lambda * mean_b(compliance_b)                                      -> g_c
 // sums[0..5] += data, res, ineq, opt, sum|r| / (B 2n), mean_b q_b   (caller zeroes; tracked scalars of the reference)
+// Loss only: g_u == NULL (the entry point admits all four gradients NULL or none); the sums are computed alike.
 __global__ void __launch_bounds__(256) mech_loss_kernel(
         const float* __restrict__ u, const float* __restrict__ rho, const float* __restrict__ x0,
         const float* __restrict__ r, const float* __restrict__ comp, const float* __restrict__ vf,
@@ -240,11 +241,13 @@ __global__ void __launch_bounds__(256) mech_loss_kernel(
     for (int i = tid; i < 2 * n; i += blockDim.x) {                 // displacement channels + residual (both 2n long)
         const float e = ub[i] - xb[i];
         a_data += wd * e * e;
-        g_u[(size_t)b * 2 * n + i] = 2.f * wd * e;
         const float rv = r[(size_t)b * 2 * n + i];
         a_res += wr * rv * rv;
         a_abs += fabsf(rv);
-        g_r[(size_t)b * 2 * n + i] = 2.f * wr * rv;
+        if (g_u) {
+            g_u[(size_t)b * 2 * n + i] = 2.f * wd * e;
+            g_r[(size_t)b * 2 * n + i] = 2.f * wr * rv;
+        }
     }
     for (int i = tid; i < n; i += blockDim.x) {                     // density channel on the node grid (zero outside nel x nel)
         const int row = i / nn, col = i - row * nn;
@@ -273,8 +276,9 @@ __global__ void __launch_bounds__(256) mech_loss_kernel(
         atomicAdd(&sums[3], lam * comp[b] / (float)B);
         atomicAdd(&sums[4], sa / ((float)B * 2.f * (float)n));
         atomicAdd(&sums[5], q / (float)B);
-        g_c[b] = lam / (float)B;
+        if (g_c) g_c[b] = lam / (float)B;
     }
+    if (!g_u) return;
     __syncthreads();
     const float dq = s_q / (float)ne;
     for (int i = tid; i < ne; i += blockDim.x) {
@@ -545,7 +549,7 @@ extern "C" int pidm_bilinear_resize_bwd(const float* dy, float* dx, int planes, 
     return 0;
 }
 
-/* fused mechanics PIDM loss + gradients, see mech_loss_kernel.  sums6 is zeroed here. */
+/* fused mechanics PIDM loss + gradients, see mech_loss_kernel.  sums6 is zeroed here; NULL gradients = loss only. */
 extern "C" int pidm_mech_pidm_loss(const float* u, const float* rho, const float* x0, const float* residual,
                                    const float* compliance, const float* vf, const long long* t,
                                    const float* p2_loss_weight, const float* posterior_var_clipped, float c_data,
@@ -553,6 +557,9 @@ extern "C" int pidm_mech_pidm_loss(const float* u, const float* rho, const float
                                    float* grad_rho, float* grad_residual, float* grad_compliance, int B, int nel,
                                    void* stream) {
     PIDM_REQUIRE(B > 0 && nel >= 2, "mech_pidm_loss: bad sizes B=%d nel=%d", B, nel);
+    const int n_grads = (grad_u != nullptr) + (grad_rho != nullptr) + (grad_residual != nullptr) + (grad_compliance != nullptr);
+    PIDM_REQUIRE(n_grads == 0 || n_grads == 4, "mech_pidm_loss: the four gradient pointers must be all set or all NULL "
+                 "(%d of 4 set)", n_grads);
     cudaStream_t st = (cudaStream_t)stream;
     PIDM_CUDA(cudaMemsetAsync(sums6, 0, 6 * sizeof(float), st));
     mech_loss_kernel<<<B, 256, 0, st>>>(u, rho, x0, residual, compliance, vf, t, p2_loss_weight, posterior_var_clipped, c_data,

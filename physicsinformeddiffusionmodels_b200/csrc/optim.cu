@@ -144,6 +144,17 @@ __global__ void incr_kernel(int* c) {
     pdl_trigger();
     pdl_wait(); *c += 1; }
 
+// a[i] <-> b[i] over n4 float4s: 16 bytes per element (each buffer read once and written once)
+__global__ void swap_kernel(float4* __restrict__ a, float4* __restrict__ b, long long n4) {
+    pdl_trigger();
+    pdl_wait();
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        const float4 x = a[i], y = b[i];
+        a[i] = y;
+        b[i] = x;
+    }
+}
+
 }  // namespace pidm
 using namespace pidm;
 
@@ -180,5 +191,16 @@ extern "C" int pidm_adam_ema_step(float* param, float* grad, float* exp_avg, flo
                                                              beta2, eps, step, step_counter_dev, grad_norm_sq_dev, grad_scale,
                                                              max_norm, ema_mu, ema_first_step, zero_grad));
     PIDM_LAUNCH_CHECK("adam_ema_step");
+    return 0;
+}
+
+extern "C" int pidm_swap_f32(float* a, float* b, long long n, void* stream) {
+    PIDM_REQUIRE(n >= 0 && n % 4 == 0, "swap_f32: n = %lld must be a non-negative multiple of 4", n);
+    PIDM_REQUIRE((((uintptr_t)a | (uintptr_t)b) & 15) == 0, "swap_f32: buffers must be 16-byte aligned");
+    if (n == 0) return 0;
+    const long long n4 = n / 4;
+    int grid = (int)std::min<long long>((n4 + 255) / 256, num_sms() * 8LL);
+    PIDM_CUDA(launch_plain(swap_kernel, dim3(grid), dim3(256), (size_t)(0), (cudaStream_t)stream, (float4*)a, (float4*)b, n4));
+    PIDM_LAUNCH_CHECK("swap_f32");
     return 0;
 }

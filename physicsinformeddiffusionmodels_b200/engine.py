@@ -11,6 +11,8 @@
 * Data parallel: one process per GPU; rank r owns rows [r*B, (r+1)*B) of the global batch; a single
   `all_reduce(SUM)` of the flat gradient per step, averaged inside the Adam kernel (grad_scale = 1/world).
 """
+import contextlib
+
 import torch
 import torch.distributed as dist
 
@@ -88,6 +90,16 @@ def allreduce_flat_grad(flat_grad, world, live=None):
     return flat_grad
 
 
+def allreduce_validation(vals, world):
+    """vals [5]: this rank's validation values (means over its equal shard) -> their mean over the ranks, in place: the
+    values of the global batch (one all-reduce; the mechanics inequality term, a product of two batch means, gets the
+    shard mean, as its gradient does in the training step)."""
+    if world > 1:
+        dist.all_reduce(vals, op=dist.ReduceOp.SUM)
+        vals.div_(world)
+    return vals
+
+
 def _unet_grad_group(name):
     """Gradient-readiness groups of Unet3D parameters (backward runs final -> ups -> mid -> downs -> stem; the time-MLP
     branches of every block finish last because they collect contributions from all blocks):
@@ -141,6 +153,9 @@ class TrainEngine:
         self._static_x0 = None
         self._static_out = None
         self.steps_done = 0
+        self._ema_active = False
+        self._val_graphs = {}           # (input shape, injected draws) -> (graph, static inputs, outputs)
+        self._val_masks = {}            # batch -> classifier-free mask tensor of the validation forward (guidance)
 
     # ---- one step, eager (also the body that gets captured) -------------------------------------------------
     def _step_body(self, x0):
@@ -191,6 +206,9 @@ class TrainEngine:
 
     def step(self, x0):
         """x0: [B, 2, 64, 64] fp32 on the device.  Returns (loss, data_loss, mean|r|) as device tensors."""
+        if self._ema_active:
+            raise RuntimeError('TrainEngine.step() inside ema_weights(): the model holds the EMA weights, and an optimizer '
+                               'step would train them; leave the context first')
         try:
             if not self.use_graph:
                 out = self._step_body(x0)
@@ -234,6 +252,105 @@ class TrainEngine:
         with torch.cuda.graph(self._graph):
             self._static_out = self._step_body(self._static_x0)
 
+    # ---- the EMA weights in the model, and the validation loss (reference main.py:181-198) ------------------------
+    def _swap_ema(self):
+        fp = self.fp
+        call('pidm_swap_f32', fp.flat, fp.ema, fp.total, stream())
+        packer = getattr(self.model, '_packer', None)
+        if packer is not None:
+            packer.invalidate()             # the swap rewrote the weights without bumping their version counters
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Inside the block the model's parameters hold the EMA shadow (reference main.py:183 `ema.ema(model)`, undone by
+        `ema.restore(model)` at :316): the flat weight buffer and the shadow are exchanged in place by one launch on the
+        current stream, and exchanged back on exit, also when the block raises, which restores every bit of both.  No
+        pointer moves, so the captured training graph, SampleEngine graphs built on the same model and every packing
+        table stay valid; before iteration ema_start + 1 the shadow still holds the initial weights, as in the
+        reference.  step() raises inside the block and the block does not nest."""
+        if self._ema_active:
+            raise RuntimeError('TrainEngine.ema_weights() is already active (the contexts do not nest)')
+        self._swap_ema()
+        self._ema_active = True
+        try:
+            yield self
+        finally:
+            self._swap_ema()
+            self._ema_active = False
+
+    def _validate_body(self, x0, t=None, noise=None):
+        shard = (self.rank, self.world) if self.global_draws else None
+        model = self.model
+        # the guided forward writes its classifier-free mask into model._null_mask_last, whose storage the captured
+        # training step holds: validation keeps a mask tensor of its own per batch size
+        train_mask = getattr(model, '_null_mask_last', None)
+        model._null_mask_last = self._val_masks.get(x0.shape[0])
+        try:
+            with torch.no_grad():
+                if t is None:
+                    out = self.diffusion.model_estimation_loss(
+                        x0, residual_func=self.residuals, c_data=self.c_data, c_residual=self.c_residual,
+                        c_ineq=self.c_ineq, lambda_opt=self.lambda_opt, sync_scalars=False, draw_shard=shard)
+                elif getattr(self.residuals, 'gov_eqs', 'darcy') == 'mechanics':
+                    out = self.residuals.training_loss(self.diffusion, x0, t, self.c_data, self.c_residual, self.c_ineq,
+                                                       self.lambda_opt, sync_scalars=False, draw_shard=shard, noise=noise)
+                else:
+                    out = self.diffusion.darcy_loss_from_draws(x0, t, noise, self.residuals, self.c_data, self.c_residual,
+                                                               sync_scalars=False, draw_shard=shard)
+                vals = torch.stack([v.detach().float().reshape(()) if isinstance(v, torch.Tensor)
+                                    else torch.full((), float(v), device=x0.device) for v in out])
+                allreduce_validation(vals, self.world)
+        finally:
+            self._val_masks[x0.shape[0]] = model._null_mask_last
+            model._null_mask_last = train_mask
+        return tuple(vals.unbind(0))
+
+    def _capture_validate(self, x0, t, noise):
+        static = [None if v is None else v.clone() for v in (x0, t, noise)]
+        dev = self.fp.flat.device
+        # warm-up as in _capture: it reads the weights and writes nothing the training step owns, and the RNG stream
+        # continues where the caller left it
+        rng = torch.cuda.get_rng_state(dev)
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            for _ in range(2):
+                self._validate_body(*static)
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        torch.cuda.set_rng_state(rng, dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = self._validate_body(*static)
+        return graph, static, out
+
+    def validate(self, x0, t=None, noise=None):
+        """The reference's validation loss (main.py:185-198: model_estimation_loss on a validation batch), forward only, on
+        whatever weights the model holds -- inside ema_weights() the EMA weights.  Returns (loss, data_loss, mean|r|,
+        inequality, optimisation) as 0-d device tensors (zero where a term does not apply) without synchronising with
+        the host; under world > 1 they are the mean over the ranks' equal shards, i.e. the values of the global batch
+        (except the mechanics inequality loss term, a product of two batch means: see allreduce_validation).
+        The draws come from the default CUDA generator in the reference's order (t, eps, then the classifier-free mask
+        under guidance) and leave it where the eager model_estimation_loss would; `t` and `noise` inject them instead.
+        use_graph: one CUDA graph per input shape, captured on first use (the last batch of an epoch may be smaller);
+        its outputs are static tensors, overwritten by the next validate() of that shape."""
+        if (t is None) != (noise is None):
+            raise ValueError('validate(): give both t and noise, or neither')
+        packer = getattr(self.model, '_packer', None)
+        if packer is not None:
+            packer.refresh_if_stale(ops.act_dtype())       # outside the graph, as in SampleEngine.sample
+        if not self.use_graph:
+            return self._validate_body(x0, t, noise)
+        key = (tuple(x0.shape), t is not None)
+        if key not in self._val_graphs:
+            self._val_graphs[key] = self._capture_validate(x0, t, noise)
+        graph, static, out = self._val_graphs[key]
+        for dst, src in zip(static, (x0, t, noise)):
+            if dst is not None:
+                dst.copy_(src, non_blocking=True)
+        graph.replay()
+        return out
+
     def close(self):
         """Release everything that pins NCCL / CUDA-graph resources: the captured graph (it holds NCCL kernels when
         world > 1, and ncclCommDestroy waits for it), the static tensors, and the model -> engine back reference of the
@@ -244,17 +361,20 @@ class TrainEngine:
         self._graph = None
         self._static_x0 = None
         self._static_out = None
+        self._val_graphs = {}
         if getattr(self.model, '_boundary_cb', None) is not None:
             self.model._boundary_cb = None
         gc.collect()
         torch.cuda.synchronize()
 
     def ema_state_dict(self):
-        """EMA weights keyed like model.state_dict() (what the reference checkpoints hold, main.py:314)."""
+        """EMA weights keyed like model.state_dict() (what the reference checkpoints hold, main.py:314), also inside
+        ema_weights(), where the reference saves its checkpoint and the shadow sits in the weight buffer."""
         sd = {k: v.clone() for k, v in self.model.state_dict().items()}
         name_of = {id(p): n for n, p in self.model.named_parameters()}
+        shadow = self.fp.flat if self._ema_active else self.fp.ema
         for p, o in zip(self.fp.params, self.fp.offsets):
-            sd[name_of[id(p)]] = self.fp.ema[o:o + p.numel()].view(p.shape).clone()
+            sd[name_of[id(p)]] = shadow[o:o + p.numel()].view(p.shape).clone()
         return sd
 
 

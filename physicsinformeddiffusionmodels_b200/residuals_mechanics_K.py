@@ -109,7 +109,10 @@ class _MechPidmLoss(torch.autograd.Function):
         B, _, nn_, _ = u.shape
         c_data, c_res, c_ineq, lam = coefs
         sums = torch.empty(6, device=u.device, dtype=torch.float32)
-        gu, grho, gr, gc = torch.empty_like(u), torch.empty_like(rho), torch.empty_like(residual), torch.empty_like(compliance)
+        gu = grho = gr = gc = None                          # loss only (validation under no_grad): no gradient written
+        if any(x.requires_grad for x in (u, rho, residual, compliance)):
+            gu, grho, gr, gc = (torch.empty_like(u), torch.empty_like(rho), torch.empty_like(residual),
+                                torch.empty_like(compliance))
         call('pidm_mech_pidm_loss', u, rho, x0, residual, compliance, vf, t, p2w, pvar, float(c_data), float(c_res),
              float(c_ineq), float(lam), sums, gu, grho, gr, gc, B, nn_ - 1, stream())
         ctx.save_for_backward(gu, grho, gr, gc)
@@ -277,21 +280,25 @@ class ResidualsMechanics:
 
     # ---- hooks used by DenoisingDiffusion (mechanics branch of the reference's loss / sampler) ------------------
     def training_loss(self, diffusion, input, t, c_data, c_residual, c_ineq, lambda_opt, sync_scalars=True,
-                      draw_shard=None):
+                      draw_shard=None, noise=None):
         """model_estimation_loss for gov_eqs='mechanics' (reference denoising_utils.py:629-710).
         input [B,10,65,65] = (vf, strain energy, von Mises | disp_x, disp_y, E | bc_x, bc_y, load_x, load_y).
         Mean-mode x0 (the reference default): q_sample, the two resamplings, the matrix-free residual and ONE fused loss
         kernel are libpidm launches; no host synchronisation unless sync_scalars (the reference reads four .item()s).
-        t=None: draw it here (the normal path); a given t is used as is (tests)."""
+        t=None: draw it here (the normal path); a given t is used as is (tests).  With t and noise [B,3,65,65] both given
+        nothing is drawn (injected draws)."""
         from . import ops
         from .denoising_utils import image_to_b_xy_c
         dd = diffusion.diff_dict
         conditioning, x_0, bcs = torch.tensor_split(input, (3, 6), dim=1)
         x_0 = x_0.contiguous().float()
         from .denoising_utils import draw_t_and_noise
-        t_drawn, e = draw_t_and_noise(diffusion.n_steps, x_0, draw_shard)      # reference order: t, then eps (:625,:636)
-        if t is None:
-            t = t_drawn
+        if t is None or noise is None:
+            t_drawn, e = draw_t_and_noise(diffusion.n_steps, x_0, draw_shard)  # reference order: t, then eps (:625,:636)
+            if t is None:
+                t = t_drawn
+        if noise is not None:
+            e = noise
         x = ops.q_sample(x_0, e, t, dd['alphas_bar_sqrt'], dd['one_minus_alphas_bar_sqrt'])
         x = torch.cat((x, conditioning), dim=1)
         vf = conditioning[:, 0, 0, 0].contiguous().float()

@@ -1,6 +1,6 @@
 """Multi-GPU consistency checks of the data-parallel training step (run with torchrun on >= 2 GPUs):
 
-  torchrun --nnodes=1 --nproc-per-node=2 --master-addr 127.0.0.1 scripts/check_ddp.py [--guidance]
+  torchrun --nnodes=1 --nproc-per-node=2 --master-addr 127.0.0.1 scripts/check_ddp.py [--guidance] [--validate]
 
 --guidance runs every check with residual-gradient guidance: the classifier-free mask is drawn for the global batch
 and sliced, and the guidance gradient is normalised by the global count, so part 1 holds with guidance too.
@@ -10,6 +10,9 @@ and sliced, and the guidance gradient is normalised by the global count, so part
  2. the bucketed / overlapped gradient exchange equals the single all-reduce: flat gradient after the exchange (5e-5)
     and bitwise-identical parameters on all ranks, eager and CUDA graph
  3. the process group is destroyed and the process exits normally (no os._exit) with captured NCCL graphs alive before.
+ 4. (--validate) TrainEngine.validate() inside ema_weights() on row shards, t / eps drawn for the global batch: every rank
+    reports the same five values, those of the ONE-process validation of the global batch        (fp32, 1e-5), eager and
+    CUDA graph (the all-reduce of the five values is captured in the graph).
 """
 import os
 import sys
@@ -31,6 +34,7 @@ dist.init_process_group('nccl', device_id=dev)
 ops.set_precision(os.environ.get('PIDM_CHECK_PRECISION', 'fp32'))
 PER = 8
 GUIDANCE = '--guidance' in sys.argv[1:]
+VALIDATE = '--validate' in sys.argv[1:]
 
 
 def rel(a, b):
@@ -96,6 +100,29 @@ for use_graph in (False, True):
               f'{worst:.3e}; max |rank diff| of the parameters {outs[True][1]:.1e} / {outs[False][1]:.1e}; groups reduced '
               f'early {outs[True][2]}', flush=True)
     ok = ok and worst < 5e-5 and outs[True][1] == 0.0 and outs[False][1] == 0.0      # fp32 atomics: order-dependent at 1e-5
+
+# ---- 4. validation loss of the global batch on every rank
+if VALIDATE:
+    for use_graph in (False, True):
+        model, eng = build(world, rank, use_graph, False)
+        model1, eng1 = build(1, 0, False, False)
+        vals = []
+        for e, x in ((eng, X[rank * PER:(rank + 1) * PER]), (eng1, X)):
+            torch.cuda.manual_seed(55)
+            with e.ema_weights():
+                vals.append(torch.stack(e.validate(x)).clone())
+        v_ddp, v_one = vals
+        ref = v_ddp.clone()
+        dist.broadcast(ref, 0)
+        same = torch.tensor([float(torch.equal(ref, v_ddp))], device=dev)
+        dist.all_reduce(same, op=dist.ReduceOp.MIN)
+        r4 = rel(v_ddp, v_one)
+        if rank == 0:
+            print(f'[4] graph={use_graph}: {world}-rank validation vs one process on the global batch: rel diff {r4:.3e}; '
+                  f'ranks identical {bool(same.item())}; values {v_ddp.tolist()}', flush=True)
+        ok = ok and r4 < 1e-5 and same.item() == 1.0
+        eng.close(); eng1.close()
+        del eng, eng1, model, model1
 
 # ---- 3. clean teardown (every engine was close()d: no captured NCCL kernel is alive any more)
 import threading

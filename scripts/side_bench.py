@@ -579,8 +579,49 @@ def darcy_gen(rounds):
     return out
 
 
+def ema_eval(rounds):
+    """Validation on the EMA weights (reference main.py:181-198), Darcy U-Net, bf16, batch 32:
+      - the EMA swap in and out of TrainEngine.ema_weights() (two pidm_swap_f32 over the flat buffers), in GB/s over
+        its algorithmic bytes (each of the two buffers read and written once per swap: 16 bytes per element);
+      - TrainEngine.validate() replayed from its CUDA graph, and eager;
+      - the whole evaluation as a training loop pays it: swap in, the repack of the bf16 operands the swap made stale,
+        validate() replayed from its graph, swap out;
+      - the drop-in evaluation as main.py runs it on a second model: ema.ema, model_estimation_loss (which reads the
+        tracked scalars on the host), ema.restore."""
+    from physicsinformeddiffusionmodels_b200.denoising_utils import EMA
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
+    sd = darcy_state_dict()
+    xv, _ = darcy_inputs()
+    te = TrainEngine(*darcy(sd), use_graph=True)
+    te_eager = TrainEngine(*darcy(sd), use_graph=False)
+    model_d, diff_d, res_d = darcy(sd)
+    ema = EMA(0.99)
+    ema.register(model_d)
+
+    def swap_in_out():
+        te._swap_ema()
+        te._swap_ema()
+
+    def dropin():
+        ema.ema(model_d)
+        diff_d.model_estimation_loss(xv, residual_func=res_d, c_data=1., c_residual=1e-3, c_ineq=0., lambda_opt=0.)
+        ema.restore(model_d)
+    def ema_validate():
+        with te.ema_weights():
+            te.validate(xv)
+    arms = {'swap_in_out_ms': (swap_in_out, 20, 2 * 16 * te.fp.total),
+            'validate_graph_ms': (lambda: te.validate(xv), 20),
+            'ema_validate_graph_ms': (ema_validate, 20),
+            'validate_eager_ms': (lambda: te_eager.validate(xv), 5),
+            'dropin_eval_ms': (dropin, 5)}
+    s = alternate(arms, rounds, {'family': 'ema_eval'})
+    s['flat_elements'] = te.fp.total
+    s['dropin/engine eval'] = s['dropin_eval_ms']['mean'] / s['ema_validate_graph_ms']['mean']
+    return s
+
+
 FAMILIES = {'periodic': periodic, 'circular': circular, 'guidance': guidance, 'cocogen': cocogen,
-            'mech_sample': mech_sample, 'darcy_gen': darcy_gen}
+            'mech_sample': mech_sample, 'darcy_gen': darcy_gen, 'ema_eval': ema_eval}
 
 
 def main(argv=None):
