@@ -27,10 +27,12 @@ __global__ void time_embed_fwd_kernel(const long long* __restrict__ t, const flo
     const int b = blockIdx.x, j = threadIdx.x;
     const int half = dim / 2;
     if (j < dim) {
-        int k = j < half ? j : j - half;
-        float f = expf((float)k * -(logf(10000.f) / (float)(half - 1)));
-        float arg = (float)t[b] * f;
-        float v = j < half ? sinf(arg) : cosf(arg);
+        // frequency, argument and sinusoid in double, which --use_fast_math leaves alone: with __expf / __sinf the
+        // error grew with t f and passed what fp32 PyTorch reaches (8 u (1 + |t f|)) at t = 999; B x dim evaluations
+        const int k = j < half ? j : j - half;
+        const double f = exp((double)k * -(log(10000.0) / (double)(half - 1)));
+        const double arg = (double)t[b] * f;
+        const float v = (float)(j < half ? sin(arg) : cos(arg));
         e[j] = v;
         emb[(size_t)b * dim + j] = v;
     }
@@ -124,6 +126,7 @@ constexpr int MLP_BCHUNK = 32;      // samples per pass = lanes of a warp
 constexpr int MLP_ROWS = 16;        // output rows per CTA (fwd / wgrad): two per warp.  The problem is latency-bound: ~240
                                     // CTAs (one wave at two CTAs per SM) each pay one table + one tile + four weight batches
 constexpr int MLP_DG_ROWS = 32;     // rows per CTA (dgrad)
+constexpr int MLP_TD_MAX = 704;     // largest td: the [32][td + 1] fp32 tile of fwd / wgrad fits in 96 KB of shared memory
 
 // out[b, j] = bias[j] + W[j,:] . s[b,:].  grid (entries, row chunks of MLP_ROWS), 256 threads.  A warp owns a row j,
 // its lanes are 32 samples: W[j,k] is one broadcast load per k, s[b,k] comes from a (td+1)-padded shared tile, and
@@ -232,7 +235,10 @@ __global__ void __launch_bounds__(256) block_mlps_wgrad_kernel(const MlpEntry* _
 // broadcast float4 reads, one atomicAdd per (sample, k) and CTA at the end.  ds zeroed by the caller.  (The first version
 // gave each of 37 CTAs a 128-row chunk found by scanning the table: 18 dependent table loads + 16 serial batches of
 // weight loads per CTA for a 30 MFLOP problem; now ~120 CTAs with 4 batches each, addressed directly.)
-__global__ void block_mlps_dgrad_kernel(const MlpEntry* __restrict__ table, float* __restrict__ ds, int B, int td) {
+// __launch_bounds__: blockDim = td goes up to MLP_TD_MAX; without the bound ptxas took 95 registers per thread and
+// a 704-thread block asked for more than the SM's 64 K registers (the launch failed for td > 672)
+__global__ void __launch_bounds__(MLP_TD_MAX) block_mlps_dgrad_kernel(const MlpEntry* __restrict__ table,
+                                                                      float* __restrict__ ds, int B, int td) {
     pdl_trigger();
     pdl_wait();
     __shared__ __align__(16) float sd[MLP_DG_ROWS][MLP_BCHUNK];
@@ -326,7 +332,7 @@ static int mlp_smem_attr(size_t bytes) {
 
 extern "C" int pidm_block_mlps_fwd(const void* table_dev, int n_entries, int max_rows, const float* silu_t, int B,
                                    int td, void* stream) {
-    PIDM_REQUIRE(td <= 704 && td % 32 == 0, "block_mlps: td must be a multiple of 32, <= 704");
+    PIDM_REQUIRE(td <= MLP_TD_MAX && td % 32 == 0, "block_mlps: td must be a multiple of 32, <= %d", MLP_TD_MAX);
     size_t smem = (size_t)MLP_BCHUNK * (td + 1) * sizeof(float);
     if (int e = mlp_smem_attr(smem)) return e;
     dim3 grid(n_entries, ceil_div(max_rows, MLP_ROWS));
@@ -340,7 +346,7 @@ extern "C" int pidm_block_mlps_fwd(const void* table_dev, int n_entries, int max
 // caller can put the weight-gradient half on the stream of its other weight-gradient kernels.
 extern "C" int pidm_block_mlps_bwd(const void* table_dev, int n_entries, int max_rows, const float* silu_t,
                                    float* d_silu_t, int B, int td, int parts, void* stream) {
-    PIDM_REQUIRE(td <= 704 && td % 32 == 0, "block_mlps: td must be a multiple of 32, <= 704");
+    PIDM_REQUIRE(td <= MLP_TD_MAX && td % 32 == 0, "block_mlps: td must be a multiple of 32, <= %d", MLP_TD_MAX);
     cudaStream_t st = (cudaStream_t)stream;
     size_t smem = (size_t)MLP_BCHUNK * (td + 1) * sizeof(float);
     if (int e = mlp_smem_attr(smem)) return e;

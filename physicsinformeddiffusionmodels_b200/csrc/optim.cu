@@ -98,7 +98,9 @@ __global__ void adam_ema_kernel(float* __restrict__ p, float* __restrict__ g, fl
         s_ema = (ema_first_step > 0 && st >= ema_first_step) ? 1 : 0;
     }
     __syncthreads();
-    const float b1 = (float)b1d, b2 = (float)b2d;
+    // 1 - beta in double: 1.f - (float)0.999 is 1.3e-5 too small (the same cancellation), which biased v by that much
+    // and made the step-1 update 6.4e-6 too large; torch rounds 1 - beta2 once
+    const float b1 = (float)b1d, b2 = (float)b2d, omb1 = (float)(1.0 - b1d), omb2 = (float)(1.0 - b2d);
     float coef = grad_scale;
     if (gnorm_sq && max_norm > 0.f) {
         float total = sqrtf(*gnorm_sq) * grad_scale;
@@ -120,8 +122,8 @@ __global__ void adam_ema_kernel(float* __restrict__ p, float* __restrict__ g, fl
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const float gi = gp[k] * coef;
-            mp[k] = b1 * mp[k] + (1.f - b1) * gi;
-            vp[k] = b2 * vp[k] + (1.f - b2) * gi * gi;
+            mp[k] = b1 * mp[k] + omb1 * gi;
+            vp[k] = b2 * vp[k] + omb2 * gi * gi;
             pp[k] = pp[k] - step * mp[k] / (sqrtf(vp[k]) * rs + eps);
             if (ema_on) ep[k] = ema_mu * ep[k] + (1.f - ema_mu) * pp[k];
         }
@@ -131,8 +133,8 @@ __global__ void adam_ema_kernel(float* __restrict__ p, float* __restrict__ g, fl
     }
     for (long long i = (n4 << 2) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         float gi = g[i] * coef;
-        float mi = b1 * m[i] + (1.f - b1) * gi;
-        float vi = b2 * v[i] + (1.f - b2) * gi * gi;
+        float mi = b1 * m[i] + omb1 * gi;
+        float vi = b2 * v[i] + omb2 * gi * gi;
         float pi = p[i] - step * mi / (sqrtf(vi) * rs + eps);
         m[i] = mi; v[i] = vi; p[i] = pi;
         if (ema_on) ema[i] = ema_mu * ema[i] + (1.f - ema_mu) * pi;

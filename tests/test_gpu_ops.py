@@ -374,40 +374,8 @@ def test_mid_attention(pk, dtype, tol):
 
 
 # ----------------------------------------------------------------------------------------------
-# time conditioning, head
+# output head (the time embedding and block MLPs are replayed per element in test_gpu_glue_census.py)
 # ----------------------------------------------------------------------------------------------
-def test_time_embed_and_block_mlps(pk):
-    ops, packing = pk
-    from oracle import pidm_oracle as O
-    g = torch.Generator().manual_seed(8)
-    B, dim, td = 5, 32, 128
-    sd = {'time_mlp.1.weight': torch.randn(td, dim, generator=g) / 6, 'time_mlp.1.bias': torch.randn(td, generator=g) * .1,
-          'time_mlp.3.weight': torch.randn(td, td, generator=g) / 11, 'time_mlp.3.bias': torch.randn(td, generator=g) * .1}
-    sdr = {k: v.clone().requires_grad_(True) for k, v in sd.items()}
-    t = torch.tensor([0, 3, 50, 99, 17])
-    temb_r = O.time_embedding(sdr, t, dim)
-    lins = [torch.nn.Linear(td, n) for n in (64, 128, 512)]
-    outs_r = [F.linear(F.silu(temb_r), l.weight, l.bias) for l in lins]
-    cots = [torch.randn(o.shape, generator=g) for o in outs_r]
-    sum((o * c).sum() for o, c in zip(outs_r, cots)).backward()
-    pd = {k: torch.nn.Parameter(v.to(DEV)) for k, v in sd.items()}
-    dl = [torch.nn.Linear(td, l.out_features).to(DEV) for l in lins]
-    for a, b_ in zip(dl, lins):
-        a.load_state_dict(b_.state_dict())
-    table = packing.MlpTable(dl)
-    silu_t, temb = ops.time_embed(t.to(DEV), pd['time_mlp.1.weight'], pd['time_mlp.1.bias'], pd['time_mlp.3.weight'],
-                                  pd['time_mlp.3.bias'])
-    assert rel(temb, temb_r) < 1e-5            # fp32 path: only op order / libm differences
-    outs = ops.block_mlps(silu_t, table)
-    for o, r in zip(outs, outs_r):
-        assert rel(o, r) < 1e-5
-    sum((o * c.to(DEV)).sum() for o, c in zip(outs, cots)).backward()
-    for a, b_ in zip(dl, lins):
-        assert rel(a.weight.grad, b_.weight.grad) < 1e-4 and rel(a.bias.grad, b_.bias.grad) < 1e-4
-    for k in sd:
-        assert rel(pd[k].grad, sdr[k].grad) < 1e-4, k
-
-
 @pytest.mark.parametrize('dtype,tol', DTYPES)
 @pytest.mark.parametrize('O_,sig', [(2, False), (3, True)])
 def test_head(pk, O_, sig, dtype, tol):
@@ -435,23 +403,19 @@ def test_head(pk, O_, sig, dtype, tol):
 
 
 # ----------------------------------------------------------------------------------------------
-# diffusion element-wise, Darcy residual + fused loss, optimizer glue
+# posterior step, Darcy residual + fused loss (q_sample and the optimizer: test_gpu_glue_census.py)
 # ----------------------------------------------------------------------------------------------
-def test_qsample_posterior(pk):
+def test_posterior_step(pk):
     ops, _ = pk
     from oracle import pidm_oracle as O
     tab = O.diffusion_tables(100)
     g = torch.Generator().manual_seed(10)
-    x0, e = torch.randn(5, 2, 64, 64, generator=g), torch.randn(5, 2, 64, 64, generator=g)
-    t = torch.tensor([0, 1, 50, 98, 99])
-    xt = ops.q_sample(x0.to(DEV), e.to(DEV), t.to(DEV), tab['alphas_bar_sqrt'].to(DEV),
-                      tab['one_minus_alphas_bar_sqrt'].to(DEV))
-    assert torch.allclose(xt.cpu(), O.q_sample(x0, t, e, tab), rtol=1e-6, atol=1e-6)
+    x0, xt = torch.randn(5, 2, 64, 64, generator=g), torch.randn(5, 2, 64, 64, generator=g)
     z = torch.randn(5, 2, 64, 64, generator=g)
     for i in (0, 7, 99):
-        ref = O.posterior_step(xt.cpu(), x0, z, i, tab)
+        ref = O.posterior_step(xt, x0, z, i, tab)
         sig = 0. if i == 0 else tab['betas'][i].sqrt().item()
-        got = ops.posterior_step(xt, x0.to(DEV), z.to(DEV), tab['posterior_mean_coef1'][i].item(),
+        got = ops.posterior_step(xt.to(DEV), x0.to(DEV), z.to(DEV), tab['posterior_mean_coef1'][i].item(),
                                  tab['posterior_mean_coef2'][i].item(), sig)
         assert torch.allclose(got.cpu(), ref, rtol=1e-5, atol=1e-5)
 
@@ -515,26 +479,6 @@ def test_fd_stencil(pk):
     assert rel(gh.stencil_gradients(ud, 'd_d00'), O.fd_second(u, -2, 1 / 63)) < 1e-5
     assert rel(gh.stencil_gradients(ud, 'd_d11'), O.fd_second(u, -1, -1 / 63)) < 1e-5
     assert rel(gh.stencil_gradients(ud, 'd_d01'), O.fd_first(O.fd_first(u, -1, -1 / 63), -2, 1 / 63)) < 1e-5
-
-
-def test_adam_ema_step(pk):
-    from physicsinformeddiffusionmodels_b200._lib import call, stream
-    from oracle import pidm_oracle as O
-    g = torch.Generator().manual_seed(14)
-    n = 100003
-    p, gr = torch.randn(n, generator=g), torch.randn(n, generator=g) * 0.01
-    m, v, ema = torch.zeros(n), torch.zeros(n), p.clone()
-    pr, mr, vr, er = p.clone(), m.clone(), v.clone(), ema.clone()
-    pd, gd, md, vd, ed = (a.to(DEV) for a in (p, gr, m, v, ema))
-    for step in (1, 2, 3):
-        O.adam_ema_step([pr], [gr], [mr], [vr], [er], step)
-        nsq = torch.zeros(1, device=DEV)
-        call('pidm_sumsq', gd, n, nsq, torch.zeros(1 + 148 * 8, device=DEV), stream())
-        call('pidm_adam_ema_step', pd, gd, md, vd, ed, n, 1e-4, 0.9, 0.999, 1e-8, step, None, nsq, 1.0, 1.0, 0.99, 1, 0,
-             stream())
-    assert abs(nsq.item() - (gr.double() ** 2).sum().item()) / nsq.item() < 1e-5
-    assert torch.allclose(pd.cpu(), pr, rtol=1e-5, atol=1e-7) and torch.allclose(ed.cpu(), er, rtol=1e-5, atol=1e-7)
-    assert torch.allclose(md.cpu(), mr, rtol=1e-4, atol=1e-9) and torch.allclose(vd.cpu(), vr, rtol=1e-4, atol=1e-12)
 
 
 def test_mechanics_residual_golden(pk, golden):

@@ -17,8 +17,8 @@ wave of CTAs cannot move.  Here, in the form of test_gpu_launch_census.py:
      the resize adds the error of its fp32 source coordinate (see resize_bounds);
   3. mutants: the same predicates reject the fp64 reference edited the way a subtle kernel bug would change it;
   4. plan coverage: the launch arithmetic, restated below, shows that the rows reach every grid case;
-  5. completeness: every entry point the benchmarked steps call is either checked by one of the four census files or
-     listed in NOT_PER_ELEMENT.
+  5. completeness: every entry point the benchmarked steps call is either checked by one of the five census files or
+     listed in LAUNCHES_NOTHING (host-side queries).
 """
 import math
 import os
@@ -32,6 +32,7 @@ if __name__ == '__main__':                       # --print-table: the repository
     sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from checks import P, U, guarded, guards_intact
 from oracle import pidm_oracle as O
+from test_gpu_glue_census import GLUE_NAMES
 from test_gpu_launch_census import _NAMES as LAUNCH_NAMES, _ratio, run_census
 
 pytestmark = pytest.mark.gpu
@@ -90,30 +91,16 @@ BENCH_ROWS = [
     ('mech_fwd', (8192, 64, 1), 'mechanics_bench'),
 ]
 
-# Entry points the benchmarked steps call that no census replays per element yet (glue, layout, optimizer).
-NOT_PER_ELEMENT = [
-    'pidm_adam_ema_step',
-    'pidm_axpby_per_sample',
-    'pidm_block_mlps_bwd',
-    'pidm_block_mlps_fwd',
-    'pidm_concat_channels',
+# Entry points the benchmarked steps call that launch nothing: host-side capability and size queries.
+LAUNCHES_NOTHING = [
     'pidm_conv2d_tc_general_supported',
     'pidm_conv2d_wgrad_tc_supported',
     'pidm_linattn_block_supported',
     'pidm_linattn_block_workspace_floats',
     'pidm_linattn_workspace_floats',
     'pidm_mlp_entry_size',
-    'pidm_nchw_to_nhwc',
     'pidm_pack_entry_size',
     'pidm_pack_pair_entry_size',
-    'pidm_pack_weights',
-    'pidm_pack_weights_pairs',
-    'pidm_qsample',
-    'pidm_scale',
-    'pidm_split_channels',
-    'pidm_sumsq',
-    'pidm_time_embed_bwd',
-    'pidm_time_embed_fwd',
 ]
 # the entry points each census file replays per element
 CENSUS_FAMILIES = {
@@ -125,6 +112,7 @@ CENSUS_FAMILIES = {
     'test_gpu_physics_census': {'pidm_darcy_residual_fwd', 'pidm_darcy_residual_bwd', 'pidm_darcy_pidm_loss',
                                 'pidm_mechanics_residual_fwd', 'pidm_mechanics_residual_bwd', 'pidm_mech_pidm_loss',
                                 'pidm_bilinear_resize_fwd', 'pidm_bilinear_resize_bwd'},
+    'test_gpu_glue_census': GLUE_NAMES,
 }
 
 
@@ -179,7 +167,7 @@ def print_table(keys, names):
             print(f'    {k!r},  # {" ".join(sorted(table[k]))}')
         print(']')
     covered = set().union(*CENSUS_FAMILIES.values())
-    print('NOT_PER_ELEMENT = [')
+    print('LAUNCHES_NOTHING = [')
     for n in sorted(names - covered):
         print(f'    {n!r},')
     print(']')
@@ -203,12 +191,12 @@ def test_every_table_row_is_produced_by_the_census():
 def test_every_benchmarked_entry_point_is_checked_or_listed():
     _, names = census()
     covered = set().union(*CENSUS_FAMILIES.values())
-    unchecked = sorted(names - covered - set(NOT_PER_ELEMENT))
+    unchecked = sorted(names - covered - set(LAUNCHES_NOTHING))
     assert not unchecked, ('entry points of the benchmarked steps that no census replays per element: add a census '
-                           'family or list them in NOT_PER_ELEMENT:\n' + '\n'.join(unchecked))
-    stale = sorted(set(NOT_PER_ELEMENT) - names)
-    assert not stale, f'NOT_PER_ELEMENT lists entry points the benchmarked steps no longer call: {stale}'
-    assert not set(NOT_PER_ELEMENT) & covered, 'an entry point is both checked and listed as unchecked'
+                           'family (a query that launches nothing goes in LAUNCHES_NOTHING):\n' + '\n'.join(unchecked))
+    stale = sorted(set(LAUNCHES_NOTHING) - names)
+    assert not stale, f'LAUNCHES_NOTHING lists entry points the benchmarked steps no longer call: {stale}'
+    assert not set(LAUNCHES_NOTHING) & covered, 'an entry point is both checked and listed as launching nothing'
 
 
 # ----------------------------------------------------------------------------------------------------------------------
