@@ -1,11 +1,21 @@
-"""Helpers shared by the tests: relative error, NaN-guarded output buffers and the per-element bound predicate of the
-fp32 Darcy kernels against their fp64 references."""
+"""Helpers shared by the tests: relative error, NaN-guarded output buffers, the per-element bound predicate of the fp32
+Darcy kernels against their fp64 references, and the seeding, launch, dtype and |err| / bound helpers of the census
+files."""
+import math
+import zlib
+
 import torch
 
 P = 64
 U = 2.0 ** -24
 C_BOUND = 16            # |y - r| <= C_BOUND * 2^-24 * A: a handful of fp32 roundings along each stencil / product chain
 GUARD = 1024            # NaN guard elements on each side of every output
+
+DTYPES = [torch.bfloat16, torch.float32]
+CODE = {torch.float32: 0, torch.bfloat16: 1}                      # the dtype code of the C ABI
+DTYPE = {c: t for t, c in CODE.items()}
+NAME = {torch.bfloat16: 'bf16', torch.float32: 'fp32'}
+RND = {torch.bfloat16: 2.0 ** -8, torch.float32: 2.0 ** -24}      # one rounding to the type, relative
 
 
 def rel(a, b):
@@ -33,3 +43,59 @@ def fields(B, seed, device='cpu'):
     x = torch.randn(B, 2, P, P, generator=g, dtype=torch.float64)
     x[:, 1] = torch.exp(0.5 * x[:, 1])
     return x.float().double().to(device)
+
+
+def sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def gen(key):
+    """a device generator: an int is the seed, anything else seeds by the crc32 of its repr"""
+    seed = key if isinstance(key, int) else zlib.crc32(repr(key).encode())
+    return torch.Generator(device='cuda').manual_seed(seed)
+
+
+def call_sync(name, *a):
+    """one C-ABI call on the package's stream, synchronized"""
+    from physicsinformeddiffusionmodels_b200._lib import call, stream
+    call(name, *a, stream())
+    torch.cuda.synchronize()
+
+
+def ratio(err, bound):
+    """worst |err| / bound; a non-finite error (an unwritten NaN sentinel) counts as infinitely bad"""
+    q = err / bound.clamp_min(1e-300)
+    q = torch.where(torch.isfinite(q), q, torch.full_like(q, math.inf))
+    return q.max().item() if q.numel() else 0.0
+
+
+def ratios(out, r, b, sl=slice(None)):
+    """worst |out - r| / bound of every output in the reference (an unwritten NaN counts as inf)"""
+    return {k: ratio((out[k][sl].double() - r[k]).abs(), b[k]) for k in r}
+
+
+def rounded(r, dtype, act):
+    """a reference as a correct kernel would return it: the outputs in `act` rounded to the activation type, the rest to
+    fp32"""
+    return {k: v.to(dtype if k in act else torch.float32) for k, v in r.items()}
+
+
+def note(tag, what, q):
+    """prints one worst |err| / bound, prefixed by the census tag"""
+    print(f'[{tag}] {what} |err|/bound {q:.4g}')
+
+
+def note_all(tag, what, rs):
+    for k, q in rs.items():
+        note(tag, f'{what} {k}', q)
+
+
+def assert_ok(rs, where):
+    assert max(rs.values()) <= 1.0, f'{where}: worst |err| / bound = {rs}'
+
+
+def check(tag, what, y, r, bound):
+    """notes and asserts the worst |y - r| / bound (y on the device, r and bound fp64)"""
+    q = ratio((y.double() - r).abs(), bound)
+    note(tag, what, q)
+    assert q <= 1.0, f'{what}: worst |err| / bound = {q:.4g}'

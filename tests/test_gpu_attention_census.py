@@ -7,11 +7,10 @@ bf16 with 8 heads and N % 64 == 0, SIMT statistics -> context -> output otherwis
 sizes its pixel chunks from the batch and the SM count; pidm_attn_* take the 64-token mma.sync kernels or the CUDA-core
 kernels with padded keys masked; pidm_head_bwd takes an octet kernel or a general one with a ragged last warp.  The
 operator tests in test_gpu_ops.py compare whole tensors at batch 2 or 3 by a norm ratio, which a wrong last chunk, a
-wrong head slice or a missing key mask at one shape cannot move.  Same four parts as test_gpu_launch_census.py, whose
-recorder and workload runner are used here:
+wrong head slice or a missing key mask at one shape cannot move.  Same four parts as the other census files:
 
   1. census: the distinct keys of the six entry points in one eager step of every workload bench.py times must equal
-     the tables below (`python tests/test_gpu_attention_census.py --print-table` regenerates them);
+     the tables below (`python tests/census.py --print-table` regenerates them);
   2. replay: every table row plus synthetic rows, through the C ABI, with bf16 and with fp32 activations, on seeded
      operands exact in the activation type, against the fp64 evaluation of the contract in include/pidm.h.  With
      u = 2^-24, rnd = 2^-8 (bf16 output) or 2^-24 (fp32 output) and A the absolute-value evaluation of the same chain
@@ -39,24 +38,19 @@ recorder and workload runner are used here:
      show that the rows reach every path, every hand-off, ragged last chunks and tiles, and capped grids.
 """
 import math
-import os
-import sys
 
 import pytest
 import torch
 
-from checks import guarded, guards_intact
-from test_gpu_launch_census import _gen, _ratio, run_census
+from census import assert_census_in_tables, assert_tables_in_census
+from checks import (CODE, DTYPES, NAME, RND, U, assert_ok, gen, guarded, guards_intact, note_all, ratios, rounded,
+                    sms)
 
 pytestmark = pytest.mark.gpu
 
 DEV = 'cuda'
-U = 2.0 ** -24
+TAG = 'attention census'
 BF = 2.0 ** -8
-RND = {torch.bfloat16: 2.0 ** -8, torch.float32: 2.0 ** -24}
-CODE = {torch.float32: 0, torch.bfloat16: 1}
-DTYPES = [torch.bfloat16, torch.float32]
-NAME = {torch.bfloat16: 'bf16', torch.float32: 'fp32'}
 SCALE = float(torch.tensor(32 ** -0.5, dtype=torch.float32))       # the kernels' fp32 32^-1/2
 # C_LA and C_ATT stayed at 1 after a run on an H100 80GB HBM3 (700 W).  C_HEAD is 2: at C = 8 over 570 k outputs the
 # largest fp32 accumulation error of y reached 1.2 sqrt(C) u A.  The worst |err| / bound per kernel path is recorded in
@@ -71,7 +65,7 @@ FWD_PATHS = {0: 'small', 1: 'mma', 2: 'simt'}
 BWD_PATHS = {0: 'mma', 1: 'simt'}
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the committed census tables (regenerate with --print-table)
+# the committed census tables (`python tests/census.py --print-table`)
 # ----------------------------------------------------------------------------------------------------------------------
 # pidm_linattn_fwd / _bwd: B, N, heads, dtype
 LA_FWD_TABLE = [
@@ -164,66 +158,12 @@ def _id(k):
 # ----------------------------------------------------------------------------------------------------------------------
 # census
 # ----------------------------------------------------------------------------------------------------------------------
-def _dt(code):
-    return 'bf16' if int(code) == 1 else 'fp32'
-
-
-def _key_of(name, a):
-    if name == 'pidm_linattn_fwd':
-        return 'la_fwd', (int(a[6]), int(a[7]), int(a[8]), _dt(a[9]))
-    if name == 'pidm_linattn_bwd':
-        return 'la_bwd', (int(a[7]), int(a[8]), int(a[9]), _dt(a[10]))
-    if name == 'pidm_attn_fwd':
-        return 'attn_fwd', (int(a[2]), int(a[3]), int(a[4]), _dt(a[5]))
-    if name == 'pidm_attn_bwd':
-        return 'attn_bwd', (int(a[3]), int(a[4]), int(a[5]), _dt(a[6]))
-    if name == 'pidm_head_fwd':
-        return 'head_fwd', (int(a[4]), int(a[5]), int(a[6]), int(a[7]), int(a[8]), _dt(a[9]))
-    if name == 'pidm_head_bwd':
-        return 'head_bwd', (int(a[7]), int(a[8]), int(a[9]), int(a[10]), int(a[11]), _dt(a[12]))
-    return None
-
-
-_CENSUS = {}
-
-
-def census():
-    if not _CENSUS:
-        _CENSUS.update(run_census(_key_of))
-    return _CENSUS
-
-
-def print_table(cen):
-    rows = {f: {} for f in TABLES}
-    for wl, keys in cen.items():
-        for fam, k in keys:
-            rows[fam].setdefault(k, []).append(wl)
-    for fam in TABLES:
-        print(f'{fam.upper()}_TABLE = [')
-        for k in sorted(rows[fam]):
-            print(f'    {k!r},  # {" ".join(sorted(rows[fam][k]))}')
-        print(']')
-    print('# distinct: ' + ', '.join(f'{f} {len(v)}' for f, v in rows.items()))
-
-
 def test_census_is_covered_by_the_table():
-    missing = []
-    for wl, keys in census().items():
-        for fam, k in sorted(keys):
-            if k not in set(TABLES[fam]):
-                missing.append(f'{fam} {k!r}  # {wl}')
-    assert not missing, ('attention and head launches of the benchmarked steps that the table does not replay (add '
-                         'them; `python tests/test_gpu_attention_census.py --print-table`):\n' + '\n'.join(missing))
+    assert_census_in_tables(TABLES)
 
 
 def test_every_table_row_is_produced_by_the_census():
-    produced = {f: set() for f in TABLES}
-    for keys in census().values():
-        for fam, k in keys:
-            produced[fam].add(k)
-    stale = [f'{fam} {k!r}' for fam, table in TABLES.items() for k in table if k not in produced[fam]]
-    assert not stale, ('table rows that no benchmarked step launches (drop them, or move a row kept for plan coverage '
-                       'to the synthetic rows):\n' + '\n'.join(stale))
+    assert_tables_in_census(TABLES)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -239,10 +179,6 @@ def plan_la(B, N, heads, dtype):
                 mma_chunks=v[7])
 
 
-def num_sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def attn_kernel(n, dtype):
     """pidm_attn_* restated: attention_mid.cu for bf16 at exactly 64 tokens, the CUDA-core kernels otherwise"""
     return 'mid' if dtype == torch.bfloat16 and n == 64 else 'core'
@@ -255,11 +191,11 @@ def plan_head(B, HW, C, O, bwd):
     M, lpp = B * HW, C // 8
     octet = lpp <= 32 and lpp & (lpp - 1) == 0
     if not bwd:
-        items, cap, kernel = M, num_sms() * 16, 'fwd'
+        items, cap, kernel = M, sms() * 16, 'fwd'
     elif octet:
-        items, cap, kernel = M * lpp, num_sms() * 4, 'octet'
+        items, cap, kernel = M * lpp, sms() * 4, 'octet'
     else:
-        items, cap, kernel = M, num_sms() * 2, 'general'
+        items, cap, kernel = M, sms() * 2, 'general'
     grid = max(1, min(-(-items // 256), cap))
     return dict(kernel=kernel, lpp=lpp, grid=grid, passes=-(-items // (grid * 256)), ragged_warp=M % 32 != 0)
 
@@ -288,7 +224,7 @@ class LaCase:
 
     def __init__(self, B, N, heads, dtype, edge=None):
         self.B, self.N, self.heads, self.dtype, self.HID = B, N, heads, dtype, heads * 32
-        g = _gen(('la', B, N, heads, edge))
+        g = gen(('la', B, N, heads, edge))
         qkv = _randn(g, B, N, 3, heads, 32, scale=1.5)
         if edge == 'spike in the last statistics chunk':
             qkv[:, N - 1, 1] = 40.0
@@ -422,21 +358,10 @@ class LaCase:
         return {'dq': d[:, :, 0], 'dk': d[:, :, 1], 'dv': d[:, :, 2]}, guards_intact(dbuf) and guards_intact(cbuf)
 
 
-def ratios(out, r, b, sl=slice(None)):
-    """worst |out - r| / bound of every output in the reference (an unwritten NaN counts as inf)"""
-    return {k: _ratio((out[k][sl].double() - r[k]).abs(), b[k]) for k in r}
-
-
 def _merge(acc, rs):
     for k, v in rs.items():
         acc[k] = max(acc.get(k, 0.0), v)
     return acc
-
-
-def rounded(r, dtype, act):
-    """a reference as a correct kernel would return it: activation outputs rounded to the activation type, the rest to
-    fp32"""
-    return {k: v.to(dtype if k in act else torch.float32) for k, v in r.items()}
 
 
 LA_ACT = ('out', 'dq', 'dk', 'dv')
@@ -445,7 +370,7 @@ LA_ACT = ('out', 'dq', 'dk', 'dv')
 class AttnCase:
     def __init__(self, B, n, heads, dtype, edge=None):
         self.B, self.n, self.heads, self.dtype, self.HID = B, n, heads, dtype, heads * 32
-        g = _gen(('attn', B, n, heads, edge))
+        g = gen(('attn', B, n, heads, edge))
         qkv = _randn(g, B, n, 3, heads, 32)
         if edge == 'dominant key':
             qkv[:, :, 0, :, 0] = 8.0
@@ -504,7 +429,7 @@ class AttnCase:
 class HeadCase:
     def __init__(self, B, HW, C, O, sig, dtype, edge=None):
         self.shape, self.sig, self.dtype = (B, HW, C, O), sig, dtype
-        g = _gen(('head', B, HW, C, O, sig, edge))
+        g = gen(('head', B, HW, C, O, sig, edge))
         self.x = _randn(g, B * HW, C).to(dtype)
         self.w = _randn(g, O, C, scale=1 / math.sqrt(C))
         self.bias = _randn(g, O, scale=0.1)
@@ -577,28 +502,14 @@ class HeadCase:
 # ----------------------------------------------------------------------------------------------------------------------
 # replay
 # ----------------------------------------------------------------------------------------------------------------------
-WORST = {}
-
-
-def _note(what, rs):
-    for k, v in rs.items():
-        name = f'{what} {k}'
-        WORST[name] = max(WORST.get(name, 0.0), v)
-        print(f'[attention census] {name} |err|/bound {v:.4g}')
-
-
-def _assert_ok(rs, where):
-    assert max(rs.values()) <= 1.0, f'{where}: worst |err| / bound = {rs}'
-
-
 def replay_la_fwd(c, where):
     out, ok = c.run_fwd()
     assert ok, f'{where}: a store landed outside out, ctx, kmax or kzinv'
     rs = {}
     for sl in c.slices():
         _merge(rs, ratios(out, *c.ref_fwd(sl), sl))
-    _note(f'linattn_fwd {FWD_PATHS[c.plan["fwd"]]} {NAME[c.dtype]}', rs)
-    _assert_ok(rs, f'{where} (plan {c.plan})')
+    note_all(TAG, f'linattn_fwd {FWD_PATHS[c.plan["fwd"]]} {NAME[c.dtype]}', rs)
+    assert_ok(rs, f'{where} (plan {c.plan})')
     return out
 
 
@@ -611,8 +522,8 @@ def replay_la_bwd(c, where, fwd_out=None):
     rs = {}
     for sl in c.slices():
         _merge(rs, ratios(out, *c.ref_bwd(sl, given['ctx'][sl], given['kmax'][sl], given['kzinv'][sl]), sl))
-    _note(path + ' given statistics', rs)
-    _assert_ok(rs, f'{where} given the statistics (plan {c.plan})')
+    note_all(TAG, path + ' given statistics', rs)
+    assert_ok(rs, f'{where} given the statistics (plan {c.plan})')
     fo = fwd_out if fwd_out is not None else replay_la_fwd(c, where)
     out, ok = c.run_bwd(fo['ctx'], fo['kmax'], fo['kzinv'])
     assert ok, f'{where}: a store landed outside dqkv or dctx'
@@ -621,8 +532,8 @@ def replay_la_bwd(c, where, fwd_out=None):
         r, b = c.ref_bwd(sl, st['ctx'][sl], st['kmax'][sl], st['kzinv'][sl], e_ctx=e_ctx[sl], eps_kz=c.eps32 + U)
         _merge(rs, ratios(out, r, b, sl))
     hand = f'{FWD_PATHS[c.plan["fwd"]]}->{BWD_PATHS[c.plan["bwd"]]}'
-    _note(f'{path} end to end ({hand})', rs)
-    _assert_ok(rs, f'{where} end to end, {hand} (plan {c.plan})')
+    note_all(TAG, f'{path} end to end ({hand})', rs)
+    assert_ok(rs, f'{where} end to end, {hand} (plan {c.plan})')
     return out
 
 
@@ -642,8 +553,8 @@ def replay_attn(c, backward, where):
     out, ok = c.run(backward)
     assert ok, f'{where}: a store landed outside the output (padded query rows must not be written)'
     rs = ratios(out, *c.ref(backward))
-    _note(f'attn_{"bwd" if backward else "fwd"} {c.kernel} {NAME[c.dtype]}', rs)
-    _assert_ok(rs, where)
+    note_all(TAG, f'attn_{"bwd" if backward else "fwd"} {c.kernel} {NAME[c.dtype]}', rs)
+    assert_ok(rs, where)
     return out
 
 
@@ -663,15 +574,15 @@ def replay_head(c, backward, where):
     out, ok = c.run_fwd()
     assert ok, f'{where}: a store landed outside y'
     rs = ratios(out, *c.ref_fwd())
-    _note(f'head_fwd {NAME[c.dtype]}', rs)
-    _assert_ok(rs, where)
+    note_all(TAG, f'head_fwd {NAME[c.dtype]}', rs)
+    assert_ok(rs, where)
     if not backward:
         return out, None
     dout, ok = c.run_bwd(out['y'])
     assert ok, f'{where}: a store landed outside dx, dW or db'
     rs = ratios(dout, *c.ref_bwd(out['y']))
-    _note(f'head_bwd {plan_head(*c.shape, True)["kernel"]} {NAME[c.dtype]}', rs)
-    _assert_ok(rs, f'{where} (plan {plan_head(*c.shape, True)})')
+    note_all(TAG, f'head_bwd {plan_head(*c.shape, True)["kernel"]} {NAME[c.dtype]}', rs)
+    assert_ok(rs, f'{where} (plan {plan_head(*c.shape, True)})')
     return out, dout
 
 
@@ -833,7 +744,7 @@ def la_coverage():
         'bwd paths': {(p['bwd'], NAME[dt]) for _, dt, p in bwd},
         'hand-offs (bf16)': {(p['fwd'], p['bwd']) for _, dt, p in bwd if dt == torch.bfloat16},
         'mma one chunk per sample': any(p['mma_chunks'] == 1 and k[0] == 256 for k, p in mma_fwd),
-        'mma clamped to 64 pixels': any(p['mma_px'] == 64 and -(-k[1] // (num_sms() * 2 // k[0])) < 64
+        'mma clamped to 64 pixels': any(p['mma_px'] == 64 and -(-k[1] // (sms() * 2 // k[0])) < 64
                                         for k, p in mma_fwd),
         'mma ragged last chunk': any(k[1] % p['mma_px'] for k, p in mma_fwd
                                      if any(kb == k and pb['bwd'] == 0 for kb, _, pb in bwd)),
@@ -858,7 +769,7 @@ def head_coverage():
 
 
 def test_plan_coverage():
-    assert num_sms() == 132, 'the synthetic rows are chosen for the 132-SM H100'
+    assert sms() == 132, 'the synthetic rows are chosen for the 132-SM H100'
     cv = la_coverage()
     print(f'[attention census] linear attention coverage {cv}')
     assert cv['fwd paths'] == {(0, 'bf16'), (1, 'bf16'), (2, 'bf16'), (2, 'fp32')}, cv
@@ -911,8 +822,3 @@ def test_rejected_shapes_are_refused_before_any_launch():
         assert torch.isnan(buf.float()).all()
     assert not x.any() and not w.any()
 
-
-if __name__ == '__main__':
-    if '--print-table' in sys.argv:
-        sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-        print_table(run_census(_key_of))

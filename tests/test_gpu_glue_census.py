@@ -4,12 +4,12 @@ element by element against an fp64 reference.
 These entry points run on every training or sampling step, but the per-op tests compared them by a norm ratio at a few
 small shapes: a time embedding at B = 5, t <= 99; block MLPs whose backward only ever saw one 32-sample chunk; an Adam
 step with a host step count, no gradient scale and no zeroing; a weight packer whose output only the end-to-end
-tolerances looked at.  Here, in the form of test_gpu_launch_census.py:
+tolerances looked at.  Here, in the four parts of the other census files:
 
   1. census: one eager step of every workload bench.py times is recorded at the C ABI, and the distinct keys of the
-     glue entry points must equal the tables below (`python tests/test_gpu_glue_census.py --print-table` regenerates
-     them).  Keys are the integer and flag arguments and the geometry decoded from the device tables (packing._PACK_DT,
-     _PAIR_DT, _MLP_DT), never pointers;
+     glue entry points must equal the tables below (`python tests/census.py --print-table` regenerates them).  Keys
+     are the integer and flag arguments and the geometry decoded from the device tables (packing._PACK_DT, _PAIR_DT,
+     _MLP_DT), never pointers;
   2. replay: every table row and synthetic row runs through the C ABI on seeded operands, outputs between NaN guards,
      accumulating outputs prefilled, against fp64 references of the semantics in oracle/pidm_oracle.py:
         packing, concat, split, nchw_to_nhwc, scale    bitwise (packing: the torch permutation of fp32 weights that are
@@ -26,22 +26,19 @@ Two tests run without a GPU: the fp64 references against the oracle (test_refere
 reciprocal division of pack_pair_kernel, exhaustively (test_pack_pair_reciprocal_division).
 """
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-if __name__ == '__main__':                       # --print-table: the repository root, as conftest.py sets it
-    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from checks import U, guarded, guards_intact
+from census import assert_census_in_tables, assert_tables_in_census, census
+from checks import DTYPE, U, call_sync, check, gen, guarded, guards_intact, note, sms
 from oracle import pidm_oracle as O
-from test_gpu_launch_census import _ratio, run_census
 
 gpu = pytest.mark.gpu                            # per test: the two CPU tests run without a GPU
 DEV = 'cuda'
+TAG = 'glue census'
 
 # Bound constants, each the smallest power of two that passes on an H100; the worst |err| / bound per output is
 # recorded in DESIGN.md section 2.
@@ -54,7 +51,7 @@ C_SUM = 4          # sumsq: roundings beside the accumulation depth
 GELU_LIP, SILU_LIP = 1.13, 1.10        # max |gelu'|, max |silu'|
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the committed census tables (regenerate with --print-table)
+# the committed census tables (`python tests/census.py --print-table`)
 # ----------------------------------------------------------------------------------------------------------------------
 # time_fwd: B, dim, td;  time_bwd: B, dim, td, parts
 # mlp_fwd: B, td, max_rows, rows of every entry;  mlp_bwd: B, td, max_rows, rows of every entry, parts
@@ -225,95 +222,14 @@ GLUE_NAMES = {'pidm_time_embed_fwd', 'pidm_time_embed_bwd', 'pidm_block_mlps_fwd
 # ----------------------------------------------------------------------------------------------------------------------
 # census
 # ----------------------------------------------------------------------------------------------------------------------
-def _decode(table_dev, dt, n):
-    return np.frombuffer(table_dev.cpu().numpy().tobytes(), dtype=dt)[:n]
-
-
-def _glue_keys(name, a):
-    """[(family, key)] of one call (a: the arguments, stream last)"""
-    from physicsinformeddiffusionmodels_b200 import packing
-    if name == 'pidm_time_embed_fwd':
-        return [('time_fwd', (int(a[9]), int(a[10]), int(a[11])))]
-    if name == 'pidm_time_embed_bwd':
-        return [('time_bwd', (int(a[10]), int(a[11]), int(a[12]), int(a[13])))]
-    if name in ('pidm_block_mlps_fwd', 'pidm_block_mlps_bwd'):
-        ns = tuple(int(r['n']) for r in _decode(a[0], packing._MLP_DT, int(a[1])))
-        if name.endswith('fwd'):
-            return [('mlp_fwd', (int(a[4]), int(a[5]), int(a[2]), ns))]
-        return [('mlp_bwd', (int(a[5]), int(a[6]), int(a[2]), ns, int(a[7])))]
-    if name == 'pidm_sumsq':
-        return [('sumsq', (int(a[1]),))]
-    if name == 'pidm_adam_ema_step':
-        return [('adam', (int(a[5]), int(a[11] is not None), float(a[13]), float(a[14]), int(a[16]), int(a[17])))]
-    if name == 'pidm_pack_weights':
-        return [('pack', (int(a[2]), int(r['N']), int(r['C']), int(r['Cpad']), int(r['taps']), int(r['flip']),
-                          int(r['s_n']), int(r['s_c']))) for r in _decode(a[0], packing._PACK_DT, int(a[1]))]
-    if name == 'pidm_pack_weights_pairs':
-        tile_base, n_tiles = int(a[2]), int(a[3])
-        tmap = a[1].cpu().numpy().view(np.int32)
-        used = sorted(set(tmap[tile_base:tile_base + n_tiles].tolist()))
-        rows = _decode(a[0], packing._PAIR_DT, max(used) + 1)
-        keys = [('pair_launch', (int(a[5]), tile_base, n_tiles, int(a[4])))]
-        for i in used:
-            r = rows[i]
-            keys.append(('pair', (int(a[5]), int(r['Cout']), int(r['Cin']), int(r['taps']), int(r['flip']),
-                                  int(int(r['s_ci']) == int(r['taps'])), int(int(r['dst_d']) != 0))))
-        return keys
-    if name in ('pidm_qsample', 'pidm_axpby_per_sample'):
-        i = 6 if name == 'pidm_qsample' else 7
-        return [(name[5:].split('_')[0], (int(a[i]), int(a[i + 1])))]
-    if name == 'pidm_scale':
-        return [('scale', (int(a[3]),))]
-    if name in ('pidm_concat_channels', 'pidm_split_channels'):
-        return [(name[5:].split('_')[0], (int(a[3]), int(a[4]), int(a[5]), int(a[6])))]
-    if name == 'pidm_nchw_to_nhwc':
-        return [('nchw', tuple(int(v) for v in a[2:7]))]
-    return []
-
-
-def _key_of(name, a):
-    return 'call', (name, tuple(_glue_keys(name, a)))
-
-
-_CENSUS = {}
-
-
-def census():
-    """{workload: set of (family, key)} of the glue calls, and the set of every entry point called"""
-    if not _CENSUS:
-        raw = run_census(_key_of)
-        _CENSUS['keys'] = {wl: {fk for _, (_, ks) in calls for fk in ks} for wl, calls in raw.items()}
-        _CENSUS['names'] = {n for calls in raw.values() for _, (n, _) in calls}
-    return _CENSUS['keys'], _CENSUS['names']
-
-
-def print_table(keys):
-    rows = {f: {} for f in TABLES}
-    for wl, ks in keys.items():
-        for fam, k in ks:
-            rows[fam].setdefault(k, []).append(wl)
-    for fam, table in rows.items():
-        print(f'{fam.upper()}_TABLE = [')
-        for k in sorted(table):
-            print(f'    {k!r},  # {" ".join(sorted(table[k]))}')
-        print(']')
-
-
 @gpu
 def test_census_is_covered_by_the_table():
-    keys, _ = census()
-    missing = [f'{fam} {k!r}  # {wl}' for wl, ks in keys.items() for fam, k in sorted(ks) if k not in TABLES[fam]]
-    assert not missing, ('glue launches of the benchmarked steps that the tables do not replay (add them; '
-                         '`python tests/test_gpu_glue_census.py --print-table`):\n' + '\n'.join(missing))
+    assert_census_in_tables(TABLES)
 
 
 @gpu
 def test_every_table_row_is_produced_by_the_census():
-    keys, _ = census()
-    produced = {(fam, k) for ks in keys.values() for fam, k in ks}
-    stale = [f'{fam} {k!r}' for fam, table in TABLES.items() for k in table if (fam, k) not in produced]
-    assert not stale, ('table rows that no benchmarked step launches (drop them; '
-                       '`python tests/test_gpu_glue_census.py --print-table`):\n' + '\n'.join(stale))
+    assert_tables_in_census(TABLES)
 
 
 @gpu
@@ -327,10 +243,6 @@ def test_every_glue_entry_point_is_recorded():
 # ----------------------------------------------------------------------------------------------------------------------
 MLP_BCHUNK, MLP_ROWS, MLP_DG_ROWS = 32, 16, 32          # linear.cu
 SUMSQ_CAP = 148 * 8                                     # optim.cu pidm_sumsq (and its workspace: 1 + SUMSQ_CAP floats)
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def sumsq_grid(n):                   # pidm_sumsq: 256 threads, ceil(n/4 / 256) CTAs, capped at 148 * 8
@@ -361,21 +273,6 @@ def mlp_smem(td):                    # pidm_block_mlps_fwd / _bwd: [32][td + 1] 
 # ----------------------------------------------------------------------------------------------------------------------
 # shared helpers
 # ----------------------------------------------------------------------------------------------------------------------
-WORST = {}
-
-
-def _note(what, ratio):
-    WORST[what] = max(WORST.get(what, 0.0), ratio)
-    print(f'[glue census] {what} |err|/bound {ratio:.4g}')
-
-
-def _check(what, y, r, bound):
-    """records and asserts the worst |y - r| / bound (y on the device, r and bound fp64 on the device)"""
-    q = _ratio((y.double() - r).abs(), bound)
-    _note(what, q)
-    assert q <= 1.0, f'{what}: worst |err| / bound = {q:.4g}'
-
-
 def _within(y, r, bound):
     d = (y.double() - r).abs()
     return bool((d <= bound).all())
@@ -387,31 +284,13 @@ def _bits(t):
 
 def _exact(what, y, r):
     bad = int((_bits(y.contiguous()) != _bits(r.contiguous())).sum())
-    _note(what + ' (elements differing)', float(bad))
+    note(TAG, what + ' (elements differing)', float(bad))
     assert bad == 0, f'{what}: {bad} elements differ bitwise'
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def _call(name, *a):
-    from physicsinformeddiffusionmodels_b200._lib import call, stream
-    call(name, *a, stream())
-    torch.cuda.synchronize()
 
 
 def _upload(rows, dt):
     arr = np.array(rows, dtype=dt)
     return torch.from_numpy(arr.view(np.uint8).copy()).to(DEV)
-
-
-def _code(dtype):
-    return {torch.float32: 0, torch.bfloat16: 1}[dtype]
-
-
-def _dt(code):
-    return {0: torch.float32, 1: torch.bfloat16}[code]
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -452,7 +331,7 @@ def time_fwd_ref(t, W1, b1, W2, b2, edit=None):
 
 
 def time_operands(B, dim, td, t_spec, seed):
-    g = _gen(seed)
+    g = gen(seed)
     W1 = torch.randn(td, dim, generator=g, device=DEV) / math.sqrt(dim)
     b1 = torch.randn(td, generator=g, device=DEV) * 0.1
     W2 = torch.randn(td, td, generator=g, device=DEV) / math.sqrt(td)
@@ -468,7 +347,7 @@ def time_operands(B, dim, td, t_spec, seed):
 def time_fwd_launch(t, W1, b1, W2, b2):
     B, (td, dim) = t.shape[0], W1.shape
     bufs = [guarded(B * dim)] + [guarded(B * td) for _ in range(3)]
-    _call('pidm_time_embed_fwd', t, W1, b1, W2, b2, *(o for _, o in bufs), B, dim, td)
+    call_sync('pidm_time_embed_fwd', t, W1, b1, W2, b2, *(o for _, o in bufs), B, dim, td)
     assert all(guards_intact(b) for b, _ in bufs)
     emb, h1, temb, s = (o.view(B, -1) for _, o in bufs)
     return {'emb': emb, 'h1': h1, 'temb': temb, 'silu_t': s}
@@ -496,7 +375,7 @@ def test_time_embed_fwd_replay(row):
     tag = ' (t = 999, outside sin.approx range)' if ts == 999 else ''
     print(f'[glue census] time_fwd emb max |err| {(y["emb"].double() - ref["emb"][0]).abs().max().item():.3g}{tag}')
     for k in ('emb', 'h1', 'temb', 'silu_t'):
-        _check(f'time_fwd {k}{tag}', y[k], *ref[k])
+        check(TAG, f'time_fwd {k}{tag}', y[k], *ref[k])
 
 
 def time_bwd_ref(d_silu, emb, h1, temb, W2, ws_dt, ws_dh, prefill, edit=None):
@@ -534,7 +413,7 @@ def time_bwd_ref(d_silu, emb, h1, temb, W2, ws_dt, ws_dh, prefill, edit=None):
 def time_bwd_launch(B, dim, td, ts, parts, seed):
     t, W1, b1, W2, b2 = time_operands(B, dim, td, ts, seed)
     fw = time_fwd_launch(t, W1, b1, W2, b2)
-    g = _gen(seed + 1)
+    g = gen(seed + 1)
     d_silu = torch.randn(B, td, generator=g, device=DEV)
     prefill = [torch.randn(*s, generator=g, device=DEV) * 0.01 for s in ((td, dim), (td,), (td, td), (td,))]
     outs = [guarded(p.numel()) for p in prefill]
@@ -543,8 +422,8 @@ def time_bwd_launch(B, dim, td, ts, parts, seed):
     bw, ws = guarded(2 * B * td)
     for p in (2, 1):                           # stage 1 then stage 2, as ops._TimeEmbed.backward issues them; a
         if p == 2 or parts & 1:                # parts = 1 row reads the workspace a stage-1 call left
-            _call('pidm_time_embed_bwd', d_silu, fw['emb'], fw['h1'], fw['temb'], W2, *(o for _, o in outs), ws, B, dim,
-                  td, p)
+            call_sync('pidm_time_embed_bwd', d_silu, fw['emb'], fw['h1'], fw['temb'], W2, *(o for _, o in outs), ws, B,
+                      dim, td, p)
     assert guards_intact(bw) and all(guards_intact(b) for b, _ in outs)
     grads = [o.view(p.shape) for (_, o), p in zip(outs, prefill)]
     return (d_silu, fw, W2, prefill), ws.view(2, B, td), grads
@@ -557,11 +436,11 @@ def test_time_embed_bwd_replay(row):
     B, dim, td, parts = row
     (d_silu, fw, W2, prefill), ws, grads = time_bwd_launch(B, dim, td, 'mix', parts, 200 + dim)
     ref = time_bwd_ref(d_silu, fw['emb'], fw['h1'], fw['temb'], W2, ws[0], ws[1], prefill)
-    _check('time_bwd dt', ws[0], *ref['dt'])           # stage 1 runs in every row
-    _check('time_bwd dh', ws[1], *ref['dh'])
+    check(TAG, 'time_bwd dt', ws[0], *ref['dt'])           # stage 1 runs in every row
+    check(TAG, 'time_bwd dh', ws[1], *ref['dh'])
     for name, y, p in zip(('dW1', 'db1', 'dW2', 'db2'), grads, prefill):
         if parts & 1:
-            _check(f'time_bwd {name}', y, *ref[name])
+            check(TAG, f'time_bwd {name}', y, *ref[name])
         else:
             _exact(f'time_bwd {name} untouched by stage 1', y, p)
 
@@ -573,7 +452,7 @@ class MlpCase:
     """operands, device table and guarded outputs of one block-MLP launch"""
 
     def __init__(self, B, td, ns, seed, with_grad=False):
-        g = _gen(seed)
+        g = gen(seed)
         self.B, self.td, self.ns = B, td, list(ns)
         self.s = torch.randn(B, td, generator=g, device=DEV)
         self.W = [torch.randn(n, td, generator=g, device=DEV) / math.sqrt(td) for n in ns]
@@ -597,12 +476,13 @@ class MlpCase:
         return all(guards_intact(b) for b, _ in self.out + self.dW + self.db + [self.ds])
 
     def fwd(self):
-        _call('pidm_block_mlps_fwd', self.table, len(self.ns), max(self.ns), self.s, self.B, self.td)
+        call_sync('pidm_block_mlps_fwd', self.table, len(self.ns), max(self.ns), self.s, self.B, self.td)
         assert self.guards()
         return [o.view(self.B, n) for (_, o), n in zip(self.out, self.ns)]
 
     def bwd(self, parts):
-        _call('pidm_block_mlps_bwd', self.table, len(self.ns), max(self.ns), self.s, self.ds[1], self.B, self.td, parts)
+        call_sync('pidm_block_mlps_bwd', self.table, len(self.ns), max(self.ns), self.s, self.ds[1], self.B, self.td,
+                  parts)
         assert self.guards()
         return ([o.view(n, self.td) for (_, o), n in zip(self.dW, self.ns)], [o for _, o in self.db],
                 self.ds[1].view(self.B, self.td))
@@ -662,7 +542,7 @@ def _mlp_id(r):
 def test_block_mlps_fwd_replay(row):
     c = MlpCase(*row, seed=300 + row[0])
     for y, (r, bound) in zip(c.fwd(), mlp_fwd_ref(c)):
-        _check('mlp_fwd out', y, r, bound)
+        check(TAG, 'mlp_fwd out', y, r, bound)
 
 
 @gpu
@@ -674,14 +554,14 @@ def test_block_mlps_bwd_replay(row):
     dWs, dbs, ds = c.bwd(parts)
     if parts & 1:
         for y, yb, ((r, bd), (rb, bdb)) in zip(dWs, dbs, mlp_wgrad_ref(c)):
-            _check('mlp_bwd dW', y, r, bd)
-            _check('mlp_bwd db', yb, rb, bdb)
+            check(TAG, 'mlp_bwd dW', y, r, bd)
+            check(TAG, 'mlp_bwd db', yb, rb, bdb)
     else:
         for y, yb, pW, pb in zip(dWs, dbs, c.pW, c.pb):
             _exact('mlp_bwd dW untouched', y, pW)
             _exact('mlp_bwd db untouched', yb, pb)
     if parts & 2:
-        _check('mlp_bwd d_silu', ds, *mlp_dgrad_ref(c))
+        check(TAG, 'mlp_bwd d_silu', ds, *mlp_dgrad_ref(c))
     else:
         assert torch.isnan(ds).all(), 'd_silu was written without parts & 2'
 
@@ -704,7 +584,7 @@ def sumsq_launch(x, prefill, ws=None):
     if ws is None:
         bw, ws = guarded(1 + SUMSQ_CAP)
         ws.zero_()
-    _call('pidm_sumsq', x, n, out, ws)
+    call_sync('pidm_sumsq', x, n, out, ws)
     assert guards_intact(bo)
     assert int(ws[:1].view(torch.int32).item()) == 0, 'the ticket counter was not reset'
     return out
@@ -719,7 +599,7 @@ def sumsq_ref(x, prefill, edit=None):
 
 
 def _sumsq_x(n, seed):
-    x = torch.randn(n, generator=_gen(seed), device=DEV)
+    x = torch.randn(n, generator=gen(seed), device=DEV)
     x[-(n % 4 or 1):] *= 8                     # a tail that weighs: dropping it must be visible
     return x
 
@@ -738,7 +618,7 @@ def test_sumsq_replay(n):
     b = sumsq_launch(x, 0.375, ws)                 # the same workspace: the ticket reset that graph replay relies on
     assert guards_intact(bw)
     _exact('sumsq twice on one workspace', b, a)
-    _check('sumsq', a, *sumsq_ref(x, 0.375))
+    check(TAG, 'sumsq', a, *sumsq_ref(x, 0.375))
 
 
 F32 = lambda v: float(np.float32(v))           # the fp32 ABI arguments, as the kernel receives them
@@ -747,7 +627,7 @@ LR, EPS, MU, B1, B2 = F32(1e-4), F32(1e-8), F32(0.99), 0.9, 0.999
 
 def adam_state(n, seed, fresh):
     """p with a block of exact zeros (and ema = 0 there), g ~ 1e-2, m, v zero at a fresh start, else drawn"""
-    g_ = _gen(seed)
+    g_ = gen(seed)
     p = torch.randn(n, generator=g_, device=DEV)
     gr = torch.randn(n, generator=g_, device=DEV) * 0.01
     if fresh:
@@ -808,9 +688,9 @@ def adam_launch(state, st, device_step, gnorm_sq, grad_scale, max_norm, ema_firs
         bc = torch.full((3,), -7, dtype=torch.int32, device=DEV)
         bc[1] = st - 1                                   # the counter holds the steps done so far
     p, g, m, v, e = (o for _, o in bufs)
-    _call('pidm_adam_ema_step', p, g, m, v, e, n, LR, B1, B2, EPS, 0 if device_step else st,
-          bc[1:2] if device_step else None, gn if gnorm_sq is not None else None, grad_scale, max_norm, MU, ema_first,
-          zero_grad)
+    call_sync('pidm_adam_ema_step', p, g, m, v, e, n, LR, B1, B2, EPS, 0 if device_step else st,
+              bc[1:2] if device_step else None, gn if gnorm_sq is not None else None, grad_scale, max_norm, MU, ema_first,
+              zero_grad)
     assert all(guards_intact(b) for b, _ in bufs) and guards_intact(bg)
     if device_step:
         assert bc.tolist() == [-7, st, -7], 'the device step counter must advance by exactly one'
@@ -822,7 +702,7 @@ def check_adam(y, state, st, gnorm_sq, grad_scale, max_norm, ema_first, zero_gra
     ok = True
     for k in ('m', 'v', 'p', 'ema'):
         if edit is None:
-            _check(f'adam {k}', y[k], *ref[k])
+            check(TAG, f'adam {k}', y[k], *ref[k])
         ok &= _within(y[k], *ref[k])
     if edit is None:
         if zero_grad:
@@ -883,14 +763,14 @@ def test_adam_three_chained_steps(device_step):
     counter = torch.zeros(1, dtype=torch.int32, device=DEV)
     pr, mr, vr, er = (x.double().cpu() for x in (p, m, v, ema))
     for st in (1, 2, 3):
-        gr = torch.randn(n, generator=_gen(710 + st), device=DEV) * 0.01
+        gr = torch.randn(n, generator=gen(710 + st), device=DEV) * 0.01
         state = [x.clone() for x in (p, gr, m, v, ema)]
         nsq = torch.zeros(1, device=DEV)
         call('pidm_sumsq', gr, n, nsq, ws, stream())
         call('pidm_adam_ema_step', p, gr, m, v, ema, n, LR, B1, B2, EPS, 0 if device_step else st,
              counter if device_step else None, nsq, 1.0, 1.0, MU, 1, 0, stream())
         torch.cuda.synchronize()
-        _check('sumsq (chained)', nsq[0], *sumsq_ref(state[1], 0.0))
+        check(TAG, 'sumsq (chained)', nsq[0], *sumsq_ref(state[1], 0.0))
         assert check_adam({'p': p, 'g': gr, 'm': m, 'v': v, 'ema': ema}, state, st, nsq.item(), 1.0, 1.0, 1, 0)
         O.adam_ema_step([pr], [state[1].double().cpu()], [mr], [vr], [er], st, lr=LR, eps=EPS, ema_mu=MU)
     if device_step:
@@ -947,18 +827,18 @@ def pack_ref(src, N, C, Cpad, taps, flip, s_n, s_c, dtype, edit=None):
 def pack_src(N, C, taps, s_n, s_c, seed):
     """fp32 weights that are not bf16-exact (a truncating conversion differs from rounding on about half of them)"""
     size = (N - 1) * s_n + (C - 1) * s_c + taps
-    return torch.randn(size, generator=_gen(seed), device=DEV) * (1 + 2.0 ** -12)
+    return torch.randn(size, generator=gen(seed), device=DEV) * (1 + 2.0 ** -12)
 
 
 def replay_pack(rows, seed, edit=None):
     """one pidm_pack_weights launch over rows (dtype, N, C, Cpad, taps, flip, s_n, s_c) of one dtype"""
-    dtype = _dt(rows[0][0])
+    dtype = DTYPE[rows[0][0]]
     srcs = [pack_src(k[1], k[2], k[4], k[6], k[7], seed + i) for i, k in enumerate(rows)]
     arena = Arena([k[1] * k[4] * k[3] for k in rows], dtype)
     from physicsinformeddiffusionmodels_b200 import packing
     table = _upload([(s.data_ptr(), arena.view(i).data_ptr(), k[6], k[7], k[1], k[2], k[3], k[4], k[5], 0)
                      for i, (s, k) in enumerate(zip(srcs, rows))], packing._PACK_DT)
-    _call('pidm_pack_weights', table, len(rows), rows[0][0])
+    call_sync('pidm_pack_weights', table, len(rows), rows[0][0])
     assert arena.gaps_intact(), 'pidm_pack_weights wrote outside its matrices'
     return [(arena.view(i), pack_ref(s, *k[1:], dtype=dtype, edit=edit)) for i, (s, k) in enumerate(zip(srcs, rows))]
 
@@ -1000,8 +880,8 @@ def replay_pairs(entries, dtype_code, seed, splits=(0,), max_taps=None, edit=Non
     """pidm_pack_weights_pairs over entries (Cout, Cin, taps, flip, ci_inner, has_dgrad), the tile list cut into launches
     at `splits` (tile_base > 0 for all but the first); -> [(y_f, r_f, y_d or None, r_d)] and the arena"""
     from physicsinformeddiffusionmodels_b200 import packing
-    dtype = _dt(dtype_code)
-    srcs = [torch.randn(co * ci * t, generator=_gen(seed + i), device=DEV) * (1 + 2.0 ** -12)
+    dtype = DTYPE[dtype_code]
+    srcs = [torch.randn(co * ci * t, generator=gen(seed + i), device=DEV) * (1 + 2.0 ** -12)
             for i, (co, ci, t, *_) in enumerate(entries)]
     sizes = []
     for co, ci, t, _, _, hd in entries:
@@ -1021,7 +901,7 @@ def replay_pairs(entries, dtype_code, seed, splits=(0,), max_taps=None, edit=Non
     mt = max_taps or max(e[2] for e in entries)
     cuts = list(splits) + [len(tmap)]
     for lo, hi in zip(cuts[:-1], cuts[1:]):
-        _call('pidm_pack_weights_pairs', table, tm, lo, hi - lo, mt, dtype_code)
+        call_sync('pidm_pack_weights_pairs', table, tm, lo, hi - lo, mt, dtype_code)
     out = []
     for (co, ci, t, fl, inner, hd), s, (vf, vd) in zip(entries, srcs, views):
         rf, rd = pair_ref(s, co, ci, t, fl, inner, dtype, edit)
@@ -1037,7 +917,7 @@ def _check_pairs(what, out, arena):
         if vd is not None:
             bad['dgrad'] += int((_bits(vd) != _bits(rd)).sum())
     for k, v in bad.items():
-        _note(f'{what} {k} operand (elements differing)', float(v))
+        note(TAG, f'{what} {k} operand (elements differing)', float(v))
     assert not any(bad.values()), f'{what}: packed operands differ bitwise from the permutation: {bad}'
 
 
@@ -1165,14 +1045,14 @@ def qsample_ref(x0, eps, t, sa, sb, edit=None):
 
 
 def qsample_launch(B, per, seed):
-    g = _gen(seed)
+    g = gen(seed)
     tab = O.diffusion_tables(250)
     sa, sb = tab['alphas_bar_sqrt'].float().to(DEV), tab['one_minus_alphas_bar_sqrt'].float().to(DEV)
     x0, eps = torch.randn(B, per, generator=g, device=DEV), torch.randn(B, per, generator=g, device=DEV)
     t = torch.randint(0, 250, (B,), generator=g, device=DEV)
     t[0] = 249
     bo, xt = guarded(B * per)
-    _call('pidm_qsample', x0, eps, t, sa, sb, xt, B, per)
+    call_sync('pidm_qsample', x0, eps, t, sa, sb, xt, B, per)
     assert guards_intact(bo)
     return (x0, eps, t, sa, sb), xt.view(B, per)
 
@@ -1185,7 +1065,7 @@ EW_SYNTH = [(1, 8192), (3, 4225), (5, 3 * 4225), ('multi', 8192), ('multi', 4225
 @pytest.mark.parametrize('row', [k for k in QSAMPLE_TABLE] + EW_SYNTH, ids=lambda k: f'B{k[0]}_per{k[1]}')
 def test_qsample_replay(row):
     ops, y = qsample_launch(_ew_B(row[0], row[1]), row[1], 1000 + row[1] % 89)
-    _check('qsample', y, *qsample_ref(*ops))
+    check(TAG, 'qsample', y, *qsample_ref(*ops))
     if row == (5, 3 * 4225):                   # the oracle's own q_sample (fp32) on the same operands
         x0, eps, t, sa, sb = ops
         tab = {'alphas_bar_sqrt': sa.cpu(), 'one_minus_alphas_bar_sqrt': sb.cpu()}
@@ -1201,22 +1081,22 @@ def axpby_ref(a, x, b, y, c, z):
 @pytest.mark.parametrize('row', [k for k in AXPBY_TABLE] + EW_SYNTH, ids=lambda k: f'B{k[0]}_per{k[1]}')
 def test_axpby_replay(row):
     B, per = _ew_B(row[0], row[1]), row[1]
-    g = _gen(1100 + per % 89)
+    g = gen(1100 + per % 89)
     a, b, c = (torch.randn(B, generator=g, device=DEV) for _ in range(3))
     x, y, z = (torch.randn(B, per, generator=g, device=DEV) for _ in range(3))
     bo, out = guarded(B * per)
-    _call('pidm_axpby_per_sample', a, x, b, y, c, z, out, B, per)
+    call_sync('pidm_axpby_per_sample', a, x, b, y, c, z, out, B, per)
     assert guards_intact(bo)
-    _check('axpby', out.view(B, per), *axpby_ref(a, x, b, y, c, z))
+    check(TAG, 'axpby', out.view(B, per), *axpby_ref(a, x, b, y, c, z))
 
 
 @gpu
 @pytest.mark.parametrize('n', [k[0] for k in SCALE_TABLE] + [1, 7, 4225, 3 * 16 * 256 * 132 * 3 + 5])
 def test_scale_replay(n):
-    g = _gen(1200 + n % 89)
+    g = gen(1200 + n % 89)
     x, alpha = torch.randn(n, generator=g, device=DEV), torch.randn(1, generator=g, device=DEV)
     bo, out = guarded(n)
-    _call('pidm_scale', x, alpha, out, n)
+    call_sync('pidm_scale', x, alpha, out, n)
     assert guards_intact(bo)
     _exact('scale', out, x * alpha)
 
@@ -1232,12 +1112,12 @@ CONCAT_SYNTH = [(1, 8, 8, 1), (1, 8, 8, 0), (37, 32, 64, 1), (37, 64, 8, 0), ('m
 @pytest.mark.parametrize('row', [k for k in CONCAT_TABLE] + CONCAT_SYNTH, ids=lambda k: 'rows{}_Ca{}_Cb{}_dt{}'.format(*k))
 def test_concat_replay(row):
     rows, Ca, Cb, code = _rows_spec(row[0], row[1] + row[2]), *row[1:]
-    dtype = _dt(code)
-    g = _gen(1300 + Ca)
+    dtype = DTYPE[code]
+    g = gen(1300 + Ca)
     a = torch.randn(rows, Ca, generator=g, device=DEV).to(dtype)
     b = torch.randn(rows, Cb, generator=g, device=DEV).to(dtype)
     bo, out = guarded(rows * (Ca + Cb), dtype)
-    _call('pidm_concat_channels', a, b, out, rows, Ca, Cb, code)
+    call_sync('pidm_concat_channels', a, b, out, rows, Ca, Cb, code)
     assert guards_intact(bo)
     _exact('concat', out.view(rows, Ca + Cb), concat_ref(a, b))
 
@@ -1250,11 +1130,11 @@ def concat_ref(a, b, edit=None):
 @pytest.mark.parametrize('row', [k for k in SPLIT_TABLE] + CONCAT_SYNTH, ids=lambda k: 'rows{}_Ca{}_Cb{}_dt{}'.format(*k))
 def test_split_replay(row):
     rows, Ca, Cb, code = _rows_spec(row[0], row[1] + row[2]), *row[1:]
-    dtype = _dt(code)
-    gsrc = torch.randn(rows, Ca + Cb, generator=_gen(1400 + Ca), device=DEV).to(dtype)
+    dtype = DTYPE[code]
+    gsrc = torch.randn(rows, Ca + Cb, generator=gen(1400 + Ca), device=DEV).to(dtype)
     ba, ga = guarded(rows * Ca, dtype)
     bb, gb = guarded(rows * Cb, dtype)
-    _call('pidm_split_channels', gsrc, ga, gb, rows, Ca, Cb, code)
+    call_sync('pidm_split_channels', gsrc, ga, gb, rows, Ca, Cb, code)
     assert guards_intact(ba) and guards_intact(bb)
     _exact('split a', ga.view(rows, Ca), gsrc[:, :Ca])
     _exact('split b', gb.view(rows, Cb), gsrc[:, Ca:])
@@ -1276,10 +1156,10 @@ def test_nchw_to_nhwc_replay(row):
     B, C, HW, Cpad, code = row
     if B == 'multi':                           # grid_for(B * HW, 128) capped, three or more passes
         B = -(-3 * 16 * sms() * 128 // HW) + 1
-    dtype = _dt(code)
-    x = torch.randn(B, C, HW, generator=_gen(1500 + C), device=DEV)
+    dtype = DTYPE[code]
+    x = torch.randn(B, C, HW, generator=gen(1500 + C), device=DEV)
     bo, out = guarded(B * HW * Cpad, dtype)    # NaN: a padding lane left unwritten would stay NaN
-    _call('pidm_nchw_to_nhwc', x, out, B, C, HW, Cpad, code)
+    call_sync('pidm_nchw_to_nhwc', x, out, B, C, HW, Cpad, code)
     assert guards_intact(bo)
     _exact('nchw_to_nhwc (padding included)', out.view(B, HW, Cpad), nchw_ref(x, Cpad, dtype))
 
@@ -1388,10 +1268,10 @@ def test_mutant_qsample_indexed_by_element():
 
 @gpu
 def test_mutant_concat_halves_swapped():
-    a = torch.randn(9, 32, generator=_gen(94), device=DEV).bfloat16()
-    b = torch.randn(9, 32, generator=_gen(95), device=DEV).bfloat16()
+    a = torch.randn(9, 32, generator=gen(94), device=DEV).bfloat16()
+    b = torch.randn(9, 32, generator=gen(95), device=DEV).bfloat16()
     out = torch.empty(9, 64, dtype=torch.bfloat16, device=DEV)
-    _call('pidm_concat_channels', a, b, out, 9, 32, 32, 1)
+    call_sync('pidm_concat_channels', a, b, out, 9, 32, 32, 1)
     assert torch.equal(_bits(out), _bits(concat_ref(a, b)))
     assert not torch.equal(_bits(out), _bits(concat_ref(a, b, 'halves_swapped')))
 
@@ -1476,7 +1356,3 @@ def test_plan_coverage():
     missing = [c for c, ok in cases.items() if not ok]
     assert not missing, f'element-wise rows miss {missing}'
 
-
-if __name__ == '__main__':
-    if '--print-table' in sys.argv:
-        print_table(census()[0])

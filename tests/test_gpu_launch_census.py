@@ -5,10 +5,9 @@ The convolution (conv_tc.cu), the two weight-gradient kernels (wgrad_tc.cu, wgra
 size and the SM count.  The per-op tests in test_gpu_ops.py run small batches, so they see few of the plans the
 benchmark runs, and they compare whole tensors by a norm ratio, which a bug confined to one tile row cannot move.  Here:
 
-  1. census: one eager step of every workload bench.py times (Darcy training at batch 32, mechanics training at batch 32
-     with Unet3D(dim=128), one Darcy sampling step at batch 16 / 64 / 256) is run with `ops.call` swapped for a recorder,
-     and the distinct integer arguments of every tensor-core call are kept.  They must equal the tables below
-     (`python tests/test_gpu_launch_census.py --print-table` regenerates them);
+  1. census: the distinct integer arguments of every tensor-core call in one eager step of every workload bench.py times
+     (recorded by tests/census.py) must equal the tables below (`python tests/census.py --print-table` regenerates
+     them);
   2. replay: every table row (plus a few synthetic rows that reach the planner choices the workloads do not) is run
      directly through the C ABI on fresh seeded bf16-exact operands and compared with an fp64 reference of the contract
      in include/pidm.h, per element:
@@ -23,13 +22,13 @@ benchmark runs, and they compare whole tensors by a norm ratio, which a bug conf
      every planner branch (ragged persistent waves, short last splits, ragged last chunks, odd batch with TN = 2).
 """
 import math
-import os
-import sys
-import zlib
 
 import pytest
 import torch
 import torch.nn.functional as F
+
+from census import assert_census_in_tables, assert_tables_in_census
+from checks import gen, note, ratio
 
 pytestmark = pytest.mark.gpu
 
@@ -49,7 +48,7 @@ GUARD_BF16 = 0x7FBF            # a NaN bit pattern: an unwritten output element 
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the committed census table (regenerate with --print-table); distinct keys per workload:
+# the committed census tables (`python tests/census.py --print-table`); distinct keys per workload:
 #   darcy_train_b32: conv 81, wgrad 34, laf 6
 #   darcy_sample_b16: conv 38, wgrad 0, laf 2
 #   darcy_sample_b64: conv 38, wgrad 0, laf 2
@@ -431,6 +430,7 @@ LAF_TABLE = [
     ('wgrad', 32, 1024, 32, 1, 256, 1),  # darcy_train_b32
     ('wgrad', 32, 4096, 32, 1, 256, 1),  # darcy_train_b32
 ]
+TABLES = {'conv': CONV_TABLE, 'wgrad': WGRAD_TABLE, 'laf': LAF_TABLE}
 
 # rows no benchmarked step produces, for planner branches the workloads do not reach (see test_plan_coverage)
 CONV_SYNTHETIC = [
@@ -463,180 +463,19 @@ def laf_id(k):
 # ----------------------------------------------------------------------------------------------------------------------
 # census
 # ----------------------------------------------------------------------------------------------------------------------
-_NAMES = {'pidm_conv2d_tc_general': 'conv', 'pidm_conv2d_wgrad_tc': 'wgrad', 'pidm_linattn_block_fwd': 'fwd',
-          'pidm_linattn_block_bwd': 'bwd', 'pidm_linattn_block_wgrad': 'wgrad_laf'}
-
-
-def _key_of(name, a):
-    """(family, key) of a tensor-core call, None for every other entry point"""
-    kind = _NAMES.get(name)
-    if kind is None:
-        return None
-    if kind == 'conv':
-        ints = tuple(int(v) for v in a[5:17])
-        return 'conv', ints + (int(a[2] is not None), int(a[3] is not None), int(a[17] is not None), int(a[18]),
-                               int(a[19]))
-    if kind == 'wgrad':
-        return 'wgrad', tuple(int(v) for v in a[3:17])
-    if kind == 'fwd':
-        return 'laf', ('fwd', int(a[10]), int(a[11]), 0, 0, 0, 0)
-    if kind == 'bwd':
-        return 'laf', ('bwd', int(a[9]), int(a[10]), 0, 0, 0, 0)
-    return 'laf', ('wgrad', int(a[14]), int(a[15]), int(a[9]), int(a[10]), int(a[12]), int(a[13]))
-
-
-def _record(fn, key_of=_key_of):
-    """the keys of the libpidm calls fn makes.  `call` is swapped in _lib and in every package module that imported it
-    (ops, engine, residuals_mechanics_K, ...), and put back in any module that imported the recorder meanwhile."""
-    from physicsinformeddiffusionmodels_b200 import _lib
-    seen = set()
-    orig = _lib.call
-
-    def rec(name, *a):
-        k = key_of(name, a)
-        if k is not None:
-            seen.add(k)
-        return orig(name, *a)
-
-    def package_modules(binding):
-        return [m for n, m in list(sys.modules.items())
-                if n.startswith('physicsinformeddiffusionmodels_b200') and getattr(m, 'call', None) is binding]
-    for m in package_modules(orig):
-        m.call = rec
-    try:
-        fn()
-        torch.cuda.synchronize()
-    finally:
-        for m in package_modules(rec):
-            m.call = orig
-    return seen
-
-
-def _darcy_model(dev):
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    torch.manual_seed(0)
-    return Unet3D(dim=32, channels=2).to(dev)
-
-
-def run_census(key_of=_key_of):
-    """{workload: set of (family, key)} for one eager step of every workload bench.py times (bf16); key_of(name, args)
-    names the family and key of the calls to keep (test_gpu_norm_census.py asks for the normalisations)."""
-    from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.engine import SampleEngine, TrainEngine
-    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
-    from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
-    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
-    dev = torch.device(DEV)
-    ops.set_precision('bf16')
-    ops.set_tensor_core_conv(True)
-    out = {}
-    model = _darcy_model(dev)
-    res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True, device=dev,
-                         bcs='none', domain_length=1.)
-    eng = TrainEngine(model, DenoisingDiffusion(100, dev), res, lr=1e-4, max_norm=1.0, ema_mu=0.99, c_data=1.0,
-                      c_residual=1e-3, use_graph=False)
-    x0 = torch.randn(32, 2, 64, 64, generator=torch.Generator().manual_seed(1)).to(dev)
-    out['darcy_train_b32'] = _record(lambda: eng.step(x0), key_of)
-    del eng
-    model.eval()
-    diff = DenoisingDiffusion(250, dev)
-    for B in (16, 64, 256):
-        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                             device=dev, bcs='none', domain_length=1., use_ddim_x0=False, ddim_steps=0)
-        se = SampleEngine(model, diff, res, batch=B, use_graph=False)
-        packer = getattr(model, '_packer', None)
-        if packer is not None:
-            packer.refresh_if_stale(ops.act_dtype())
-        se.x.normal_()
-        se.t.fill_(diff.n_steps - 1)
-        out[f'darcy_sample_b{B}'] = _record(se._step_body, key_of)
-        del se
-    del model
-    torch.manual_seed(0)
-    mech = Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True).to(dev)
-    res = ResidualsMechanics(model=mech, pixels_per_dim=64, pixels_at_boundary=True, no_BC_folder='', device=dev)
-    eng = TrainEngine(mech, DenoisingDiffusion(100, dev), res, lr=1e-4, max_norm=1.0, ema_mu=0.99, c_data=1.0,
-                      c_residual=1e-2, c_ineq=0., lambda_opt=1e-3, use_graph=False)
-    g = torch.Generator().manual_seed(5)
-    B = 32
-    cond = torch.rand(B, 3, 65, 65, generator=g)
-    x0 = torch.cat((0.2 * torch.randn(B, 2, 65, 65, generator=g), torch.rand(B, 1, 65, 65, generator=g).clamp(1e-3, 1.)), 1)
-    bcs = torch.zeros(B, 4, 65, 65)
-    bcs[:, 0, :, 0] = 1.
-    bcs[:, 1, :, 0] = 1.
-    bcs[:, 3, 32, 64] = -1.
-    inp = torch.cat((cond, x0, bcs), dim=1).to(dev)
-    out['mech_train_b32'] = _record(lambda: eng.step(inp), key_of)
-    del eng, mech
-    torch.cuda.empty_cache()
-    return out
-
-
-_CENSUS = {}
-
-
-def census():
-    if not _CENSUS:
-        _CENSUS.update(run_census())
-    return _CENSUS
-
-
-def print_table(cen):
-    rows = {'conv': {}, 'wgrad': {}, 'laf': {}}
-    for wl, keys in cen.items():
-        for fam, k in keys:
-            rows[fam].setdefault(k, []).append(wl)
-    for fam, name in (('conv', 'CONV_TABLE'), ('wgrad', 'WGRAD_TABLE'), ('laf', 'LAF_TABLE')):
-        print(f'{name} = [')
-        for k in sorted(rows[fam]):
-            print(f'    {k!r},  # {" ".join(sorted(rows[fam][k]))}')
-        print(']')
-    for wl, keys in cen.items():
-        n = {f: sum(1 for ff, _ in keys if ff == f) for f in ('conv', 'wgrad', 'laf')}
-        print(f'# {wl}: ' + ', '.join(f'{f} {v}' for f, v in n.items()))
-    print('# distinct: ' + ', '.join(f'{f} {len(v)}' for f, v in rows.items()))
-
-
 def test_census_is_covered_by_the_table():
-    tables = {'conv': set(CONV_TABLE), 'wgrad': set(WGRAD_TABLE), 'laf': set(LAF_TABLE)}
-    missing = []
-    for wl, keys in census().items():
-        for fam, k in sorted(keys):
-            if k not in tables[fam]:
-                missing.append(f'{fam} {k!r}  # {wl}')
-    assert not missing, ('launches of the benchmarked steps that the table does not replay (add them; '
-                         '`python tests/test_gpu_launch_census.py --print-table`):\n' + '\n'.join(missing))
+    assert_census_in_tables(TABLES)
 
 
 def test_every_table_row_is_produced_by_the_census():
-    produced = {'conv': set(), 'wgrad': set(), 'laf': set()}
-    for keys in census().values():
-        for fam, k in keys:
-            produced[fam].add(k)
-    stale = [f'{fam} {k!r}' for fam, table in (('conv', CONV_TABLE), ('wgrad', WGRAD_TABLE), ('laf', LAF_TABLE))
-             for k in table if k not in produced[fam]]
-    assert not stale, ('table rows that no benchmarked step launches (drop them, or move a row kept for planner coverage '
-                       'to the synthetic rows; `python tests/test_gpu_launch_census.py --print-table`):\n'
-                       + '\n'.join(stale))
+    assert_tables_in_census(TABLES)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # operands, references, predicates
 # ----------------------------------------------------------------------------------------------------------------------
-def _gen(key):
-    return torch.Generator(device=DEV).manual_seed(zlib.crc32(repr(key).encode()))
-
-
 def _randn(g, *shape, scale=1.0, dtype=torch.bfloat16):
     return (torch.randn(*shape, generator=g, device=DEV) * scale).to(dtype)
-
-
-def _ratio(err, bound):
-    """worst |err| / bound; a non-finite error (an unwritten NaN sentinel) counts as infinitely bad"""
-    q = err / bound.clamp_min(1e-300)
-    q = torch.where(torch.isfinite(q), q, torch.full_like(q, math.inf))
-    return q.max().item() if q.numel() else 0.0
 
 
 def _guarded(n, fill_bits):
@@ -703,7 +542,7 @@ class ConvCase:
     def __init__(self, k):
         B, H, W, Cin, Ho, Wo, Cout, KH, KW, s, p, tr, hb, hr, hg, G, z = k
         self.k, self.K = k, KH * KW * Cin
-        g = _gen(('conv',) + tuple(k))
+        g = gen(('conv',) + tuple(k))
         self.x = _randn(g, B, H, W, Cin)
         self.wp = _randn(g, Cout, self.K, scale=1.0 / math.sqrt(self.K))
         self.bias = torch.randn(Cout, generator=g, device=DEV) if hb else None
@@ -720,11 +559,11 @@ class ConvCase:
         """worst |y - r| / (2^-8 |r| + C_ACC sqrt(K) 2^-24 A) over all elements.  The first term is the exact worst case
         of one round-to-nearest bf16 rounding, reached by values just above a power of two, so on large tensors this
         ratio approaches 1 by construction; the margin lies in the accumulation term (acc_ratio)."""
-        return _ratio((y.double() - self.r).abs(), 2.0 ** -8 * self.r.abs() + self.acc_bound())
+        return ratio((y.double() - self.r).abs(), 2.0 ** -8 * self.r.abs() + self.acc_bound())
 
     def acc_ratio(self, y):
         """worst (|y - r| - 2^-8 |r|) / (C_ACC sqrt(K) 2^-24 A): the share of the accumulation term that is used"""
-        return _ratio(((y.double() - self.r).abs() - 2.0 ** -8 * self.r.abs()).clamp_min(0), self.acc_bound())
+        return ratio(((y.double() - self.r).abs() - 2.0 ** -8 * self.r.abs()).clamp_min(0), self.acc_bound())
 
     def run(self):
         from physicsinformeddiffusionmodels_b200._lib import call, stream
@@ -750,7 +589,7 @@ class ConvCase:
         b1 = e.sum(dim=(1, 3)) + c * r.abs().sum(dim=(1, 3))
         b2 = (2 * r.abs() * e + e * e).sum(dim=(1, 3)) + c * s2
         sd = sums.double()
-        return max(_ratio((sd[..., 0] - s1).abs(), b1), _ratio((sd[..., 1] - s2).abs(), b2))
+        return max(ratio((sd[..., 0] - s1).abs(), b1), ratio((sd[..., 1] - s2).abs(), b2))
 
 
 # ---- weight gradient --------------------------------------------------------------------------------------------------
@@ -781,7 +620,7 @@ class WgradCase:
     def __init__(self, k):
         B, HA, WA, CA, CAr, GH, GW, CB, KH, KW, s, p, sr, sc = k
         self.k, self.K = k, B * GH * GW
-        g = _gen(('wgrad',) + tuple(k))
+        g = gen(('wgrad',) + tuple(k))
         self.a = _randn(g, B, HA, WA, CA)                    # padding channels (>= CA_real) are random: must be dropped
         self.b = _randn(g, B, GH, GW, CB)
         self.idx = _wgrad_index(k)
@@ -796,12 +635,12 @@ class WgradCase:
     def ratio(self, dw):
         """dw: the accumulated fp32 buffer (prefill + D) at the contract's positions"""
         got = dw.double()[self.idx] - self.prefill.double()[self.idx]
-        return _ratio((got - self.D).abs(), self.bound())
+        return ratio((got - self.D).abs(), self.bound())
 
     def run(self):
         from physicsinformeddiffusionmodels_b200._lib import call, stream
         guard = 4096
-        buf = torch.randn(self.n + 2 * guard, generator=_gen(('wgrad-guard',) + tuple(self.k)), device=DEV)
+        buf = torch.randn(self.n + 2 * guard, generator=gen(('wgrad-guard',) + tuple(self.k)), device=DEV)
         buf[guard:guard + self.n] = self.prefill
         keep = buf.clone()
         dw = buf[guard:]
@@ -879,7 +718,7 @@ class BlockCase:
     def __init__(self, k):
         kind, B, N = k[:3]
         self.k = k
-        g = _gen(('linattn-block', B, N))                   # same operands for the fwd / bwd / wgrad rows of a shape
+        g = gen(('linattn-block', B, N))                   # same operands for the fwd / bwd / wgrad rows of a shape
         self.xn = _randn(g, B, N, 32)
         self.wq = _randn(g, 768, 32, scale=1.5 / math.sqrt(32))
         self.wo = _randn(g, 32, 256, scale=1.0 / math.sqrt(256))
@@ -913,11 +752,11 @@ class BlockCase:
         call('pidm_linattn_block_bwd', self.xn, self.wq, self.wo, self.dy, ctx, kmax, kzinv, dx, dctx, B, N, stream())
         if kind == 'bwd':
             torch.cuda.synchronize()
-            r = _ratio((dx.view(B, N, 32).double() - self.dx_r).abs(), dx_bound(self.dx_r))
+            r = ratio((dx.view(B, N, 32).double() - self.dx_r).abs(), dx_bound(self.dx_r))
             return {'dxn': r}, _guards_intact(buf, guard, n, GUARD_BF16)
         # both weight gradients accumulate into strided views of one prefilled flat buffer (as the engine's flat
         # gradient buffer), and pidm_colsum the bias gradient into the same buffer
-        g = _gen(('linattn-block-gw', B, N))
+        g = gen(('linattn-block-gw', B, N))
         guard = 1024
         nq, no = 767 * sn + 31 * sc + 1, 31 * osn + 255 * osc + 1
         oq, oo, ob = guard, 2 * guard + nq, 3 * guard + nq + no
@@ -937,28 +776,20 @@ class BlockCase:
             v.fill_(True)
         ok = bool((gbuf[~touched] == keep[~touched]).all())
         pq, po, pb = (v.double() for v in views(keep))
-        return {'dWqkv': _ratio((gq.double() - pq - self.gq_r).abs(), gq_bound(self.gq_r, pq)),
+        return {'dWqkv': ratio((gq.double() - pq - self.gq_r).abs(), gq_bound(self.gq_r, pq)),
                 'dWout': self.go_ratio(go.double() - po, po),
-                'db': _ratio((gb.double() - pb - self.db_r).abs(), db_bound(self.db_r, pb))}, ok
+                'db': ratio((gb.double() - pb - self.db_r).abs(), db_bound(self.db_r, pb))}, ok
 
     def y_ratio(self, y):
-        return _ratio((y.double() - self.y_r).abs(), y_bound(self.y_r))
+        return ratio((y.double() - self.y_r).abs(), y_bound(self.y_r))
 
     def go_ratio(self, go, prefill):
-        return _ratio((go.double() - self.go_r).abs(), go_bound(self.go_r, prefill))
+        return ratio((go.double() - self.go_r).abs(), go_bound(self.go_r, prefill))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # replay
 # ----------------------------------------------------------------------------------------------------------------------
-WORST = {}
-
-
-def _note(family, r):
-    WORST[family] = max(WORST.get(family, 0.0), r)
-    print(f'[census] {family} worst |err|/bound {r:.4g}')
-
-
 @pytest.fixture(scope='module', autouse=True)
 def _bf16_mode():
     from physicsinformeddiffusionmodels_b200 import ops
@@ -978,12 +809,12 @@ def test_conv_replay(k):
     buf, y, guard, n, sums = c.run()
     assert _guards_intact(buf, guard, n, GUARD_BF16), f'{conv_id(k)}: a store landed outside y'
     r = c.ratio(y)
-    _note('conv', r)
-    _note('conv_accumulation', c.acc_ratio(y))
+    note('census', 'conv worst', r)
+    note('census', 'conv_accumulation worst', c.acc_ratio(y))
     assert r <= 1.0, f'{conv_id(k)}: worst |err| / bound = {r:.3g} (plan {plan_conv(k)})'
     if k[14]:
         rg = c.gn_ratio(sums)
-        _note('gn_sums', rg)
+        note('census', 'gn_sums worst', rg)
         assert rg <= 1.0, f'{conv_id(k)}: fused GroupNorm statistics off, worst |err| / bound = {rg:.3g}'
 
 
@@ -993,7 +824,7 @@ def test_wgrad_replay(k):
     dw, untouched_ok = c.run()
     assert untouched_ok, f'{wgrad_id(k)}: an element outside the contract (guard, padding row cA >= CA_real) changed'
     r = c.ratio(dw)
-    _note('wgrad3' if plan_wgrad(k)['w3'] else 'wgrad', r)
+    note('census', ('wgrad3' if plan_wgrad(k)['w3'] else 'wgrad') + ' worst', r)
     assert r <= 1.0, f'{wgrad_id(k)}: worst |err| / bound = {r:.3g} (plan {plan_wgrad(k)})'
 
 
@@ -1002,7 +833,7 @@ def test_attention_block_replay(k):
     ratios, ok = BlockCase(k).run()
     assert ok, f'{laf_id(k)}: a store landed outside the outputs'
     for name, r in ratios.items():
-        _note('laf_' + name, r)
+        note('census', f'laf_{name} worst', r)
     assert max(ratios.values()) <= 1.0, f'{laf_id(k)}: worst |err| / bound = {ratios} (plan {plan_laf(k[1], k[2])})'
 
 
@@ -1183,8 +1014,3 @@ def test_attention_block_plan_coverage():
     la = laf_coverage()
     assert all(la.values()), la
 
-
-if __name__ == '__main__':
-    if '--print-table' in sys.argv:
-        sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-        print_table(run_census())

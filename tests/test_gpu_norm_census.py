@@ -4,11 +4,11 @@ element by element against an fp64 reference.
 pidm_groupnorm_silu_bwd picks a channel slab, a thread count, a cluster size 1..8 and one of five code paths from the
 shape, the batch and the SM count; the forward sizes its apply grid by three rules; the LayerNorm kernels cap their grid
 and loop.  The operator tests in test_gpu_ops.py compare whole tensors by a norm ratio against an fp32 reference, which a
-bug confined to one cluster rank, one channel slab or the last pixel rows cannot move.  Same four parts as
-test_gpu_launch_census.py, whose recorder and workload runner are used here:
+bug confined to one cluster rank, one channel slab or the last pixel rows cannot move.  Same four parts as the other
+census files:
 
   1. census: the distinct keys of the five entry points in one eager step of every workload bench.py times must equal the
-     tables below (`python tests/test_gpu_norm_census.py --print-table` regenerates them);
+     tables below (`python tests/census.py --print-table` regenerates them);
   2. replay: every table row plus synthetic rows, through the C ABI, with bf16 and with fp32 activations, on seeded
      inputs, against the fp64 evaluation of the contract in include/pidm.h.  With u = 2^-24, rnd = 2^-8 (bf16 output) or
      2^-24 (fp32 output) and A(.) the absolute-value evaluation of the same expression:
@@ -31,23 +31,19 @@ test_gpu_launch_census.py, whose recorder and workload runner are used here:
      backward path, every cluster size, a ragged last cluster rank on every path, every thread count and grid rule.
 """
 import math
-import os
-import sys
-import zlib
 
 import pytest
 import torch
 
-from checks import guarded, guards_intact
-from test_gpu_launch_census import _ratio, run_census
+from census import assert_census_in_tables, assert_tables_in_census
+from checks import (CODE, DTYPES, NAME, RND, U, assert_ok, gen, guarded, guards_intact, note_all, ratio, ratios,
+                    rounded, sms)
 
 pytestmark = pytest.mark.gpu
 
 DEV = 'cuda'
-U = 2.0 ** -24
-RND = {torch.bfloat16: 2.0 ** -8, torch.float32: 2.0 ** -24}
-CODE = {torch.float32: 0, torch.bfloat16: 1}
-DTYPES = [torch.bfloat16, torch.float32]
+TAG = 'norm census'
+ACT = ('y', 'dx')            # the outputs in the activation type
 EPS = float(torch.tensor(1e-5, dtype=torch.float32))      # the entry points take eps as a float
 # Both stayed at 1 after a run on an H100 80GB HBM3 (700 W); the worst |err| / bound per kernel path is recorded in
 # DESIGN.md section 2.
@@ -56,7 +52,7 @@ C_EL = 1.0
 PATHS = {0: 'fallback', 1: 'piece1', 2: 'piece2', 3: 'packed4', 4: 'stream'}
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the committed census tables (regenerate with --print-table)
+# the committed census tables (`python tests/census.py --print-table`)
 # ----------------------------------------------------------------------------------------------------------------------
 # pidm_groupnorm_silu_fwd: B, HW, C, G, scale_shift, residual, stats_precomputed
 GN_FWD_TABLE = [
@@ -310,68 +306,15 @@ def _id(k):
     return '_'.join(str(v) for v in k)
 
 
-def _tname(dtype):
-    return 'bf16' if dtype == torch.bfloat16 else 'fp32'
-
-
 # ----------------------------------------------------------------------------------------------------------------------
 # census
 # ----------------------------------------------------------------------------------------------------------------------
-def _key_of(name, a):
-    has = lambda t: int(t is not None)
-    if name == 'pidm_groupnorm_silu_fwd':
-        return 'gn_fwd', (int(a[8]), int(a[9]), int(a[10]), int(a[11]), has(a[3]), has(a[4]), int(a[7]))
-    if name == 'pidm_groupnorm_silu_bwd':
-        return 'gn_bwd', (int(a[12]), int(a[13]), int(a[14]), int(a[15]), has(a[5]), has(a[9]), has(a[10]))
-    if name == 'pidm_layernorm_c_fwd':
-        return 'ln_fwd', (int(a[3]), int(a[4]))
-    if name == 'pidm_layernorm_c_bwd':
-        return 'ln_bwd', (int(a[6]), int(a[7]), has(a[5]))
-    if name == 'pidm_colsum':
-        return 'colsum', (int(a[2]), int(a[3]))
-    return None
-
-
-_CENSUS = {}
-
-
-def census():
-    if not _CENSUS:
-        _CENSUS.update(run_census(_key_of))
-    return _CENSUS
-
-
-def print_table(cen):
-    rows = {f: {} for f in TABLES}
-    for wl, keys in cen.items():
-        for fam, k in keys:
-            rows[fam].setdefault(k, []).append(wl)
-    for fam in TABLES:
-        print(f'{fam.upper()}_TABLE = [' if fam != 'colsum' else 'COLSUM_TABLE = [')
-        for k in sorted(rows[fam]):
-            print(f'    {k!r},  # {" ".join(sorted(rows[fam][k]))}')
-        print(']')
-    print('# distinct: ' + ', '.join(f'{f} {len(v)}' for f, v in rows.items()))
-
-
 def test_census_is_covered_by_the_table():
-    missing = []
-    for wl, keys in census().items():
-        for fam, k in sorted(keys):
-            if k not in set(TABLES[fam]):
-                missing.append(f'{fam} {k!r}  # {wl}')
-    assert not missing, ('normalisation launches of the benchmarked steps that the table does not replay (add them; '
-                         '`python tests/test_gpu_norm_census.py --print-table`):\n' + '\n'.join(missing))
+    assert_census_in_tables(TABLES)
 
 
 def test_every_table_row_is_produced_by_the_census():
-    produced = {f: set() for f in TABLES}
-    for keys in census().values():
-        for fam, k in keys:
-            produced[fam].add(k)
-    stale = [f'{fam} {k!r}' for fam, table in TABLES.items() for k in table if k not in produced[fam]]
-    assert not stale, ('table rows that no benchmarked step launches (drop them, or move a row kept for planner coverage '
-                       'to the synthetic rows):\n' + '\n'.join(stale))
+    assert_tables_in_census(TABLES)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -381,14 +324,10 @@ def plan_gn(B, HW, C, G, dtype):
     from physicsinformeddiffusionmodels_b200._lib import call
     out = torch.zeros(10, dtype=torch.int32)
     rc = call('pidm_groupnorm_plan', B, HW, C, G, CODE[dtype], out.data_ptr())
-    assert rc == 0, f'groupnorm rejects B={B} HW={HW} C={C} G={G} {_tname(dtype)}'
+    assert rc == 0, f'groupnorm rejects B={B} HW={HW} C={C} G={G} {NAME[dtype]}'
     v = out.tolist()
     return dict(stats_chunks=v[0], stats_block=v[1], apply_chunks=v[2], rules=v[3], path=v[4], S=v[5], threads=v[6],
                 cl=v[7], rows_per_cta=v[8], v=v[9])
-
-
-def num_sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count if DEV == 'cuda' else 132
 
 
 def plan_ln(M, C, bwd):
@@ -399,7 +338,7 @@ def plan_ln(M, C, bwd):
         L *= 2
     reg = L == oct_
     rows = (32 // L) * 8 * (4 if reg else 1)            # rows per CTA and iteration
-    want, cap = max(1, -(-M // rows)), num_sms() * (4 if bwd else 8)
+    want, cap = max(1, -(-M // rows)), sms() * (4 if bwd else 8)
     grid = min(want, cap)
     return dict(kernel='ln1' if reg else 'ln', capped=want > cap, ragged=M % (grid * rows) != 0, grid=grid, rows=rows)
 
@@ -407,10 +346,6 @@ def plan_ln(M, C, bwd):
 # ----------------------------------------------------------------------------------------------------------------------
 # operands, references, bounds
 # ----------------------------------------------------------------------------------------------------------------------
-def _gen(key):
-    return torch.Generator(device=DEV).manual_seed(zlib.crc32(repr(key).encode()))
-
-
 def _randn(g, *shape, dtype=torch.float32):
     return torch.randn(*shape, generator=g, device=DEV).to(dtype)
 
@@ -443,7 +378,7 @@ class GnCase:
 
     def __init__(self, B, HW, C, G, dtype, ss=1, res=0, m_over_sigma=None, constant_group=False):
         self.shape, self.dtype = (B, HW, C, G), dtype
-        g = _gen(('gn', B, HW, C, G, m_over_sigma))
+        g = gen(('gn', B, HW, C, G, m_over_sigma))
         if m_over_sigma is None:
             x = torch.randn(B, HW, C, generator=g, device=DEV) * 1.5 + 0.3
         else:
@@ -587,20 +522,10 @@ class GnCase:
         return out, all(guards_intact(t[0]) for t in bufs.values())
 
 
-def ratios(out, r, b):
-    """worst |out - r| / bound of every output in the reference (an unwritten NaN or a missing output counts as inf)"""
-    return {k: _ratio((out[k].double() - r[k]).abs(), b[k]) for k in r}
-
-
-def rounded(r, dtype):
-    """a reference as a correct kernel would return it: activations rounded to the activation type, the rest to fp32"""
-    return {k: v.to(dtype if k in ('y', 'dx') else torch.float32) for k, v in r.items()}
-
-
 class LnCase:
     def __init__(self, M, C, dtype, res=0):
         self.M, self.C, self.dtype = M, C, dtype
-        g = _gen(('ln', M, C))
+        g = gen(('ln', M, C))
         self.x = (torch.randn(M, C, generator=g, device=DEV) * 2 + 0.5).to(dtype)
         self.dy = _randn(g, M, C, dtype=dtype)
         self.gamma = 1 + 0.2 * _randn(g, C)
@@ -661,25 +586,11 @@ class LnCase:
 # ----------------------------------------------------------------------------------------------------------------------
 # replay
 # ----------------------------------------------------------------------------------------------------------------------
-WORST = {}
-
-
-def _note(what, rs):
-    for k, v in rs.items():
-        name = f'{what} {k}'
-        WORST[name] = max(WORST.get(name, 0.0), v)
-        print(f'[norm census] {name} |err|/bound {v:.4g}')
-
-
-def _assert_ok(rs, where):
-    assert max(rs.values()) <= 1.0, f'{where}: worst |err| / bound = {rs}'
-
-
 def _check_stats(c, sums, where):
-    rs = {'sum': _ratio((sums[..., 0].double() - c.sums[..., 0]).abs(), c.e_sums[..., 0]),
-          'sum of squares': _ratio((sums[..., 1].double() - c.sums[..., 1]).abs(), c.e_sums[..., 1])}
-    _note(f'gn_stats {_tname(c.dtype)}', rs)
-    _assert_ok(rs, where + ' statistics')
+    rs = {'sum': ratio((sums[..., 0].double() - c.sums[..., 0]).abs(), c.e_sums[..., 0]),
+          'sum of squares': ratio((sums[..., 1].double() - c.sums[..., 1]).abs(), c.e_sums[..., 1])}
+    note_all(TAG, f'gn_stats {NAME[c.dtype]}', rs)
+    assert_ok(rs, where + ' statistics')
 
 
 def replay_gn_fwd(c, where):
@@ -687,14 +598,14 @@ def replay_gn_fwd(c, where):
     out, _, ok = c.run_fwd(given)
     assert ok, f'{where}: a store landed outside y or the sums'
     rs = ratios(out, *c.eval(given, end_to_end=False, backward=False))
-    _note(f'gn_apply {_tname(c.dtype)} given statistics', rs)
-    _assert_ok(rs, where + ' given the statistics')
+    note_all(TAG, f'gn_apply {NAME[c.dtype]} given statistics', rs)
+    assert_ok(rs, where + ' given the statistics')
     out, sums, ok = c.run_fwd(None)
     assert ok, f'{where}: a store landed outside y or the sums'
     _check_stats(c, sums, where)
     rs = ratios(out, *c.eval(c.sums, end_to_end=True, backward=False))
-    _note(f'gn_apply {_tname(c.dtype)} end to end', rs)
-    _assert_ok(rs, where + ' end to end')
+    note_all(TAG, f'gn_apply {NAME[c.dtype]} end to end', rs)
+    assert_ok(rs, where + ' end to end')
     return out, sums
 
 
@@ -706,45 +617,45 @@ def replay_gn_bwd(c, dss, dbias, where):
     r, b = c.eval(given, end_to_end=False, dss=dss, dbias=dbias)
     del r['y']
     rs = ratios(out, r, b)
-    _note(f'gn_bwd {path} {_tname(c.dtype)} given statistics', rs)
-    _assert_ok(rs, f'{where} given the statistics (plan {c.plan()})')
+    note_all(TAG, f'gn_bwd {path} {NAME[c.dtype]} given statistics', rs)
+    assert_ok(rs, f'{where} given the statistics (plan {c.plan()})')
     _, sums, _ = c.run_fwd(None)
     out, ok = c.run_bwd(sums, dss, dbias)
     assert ok, f'{where}: a store landed outside the outputs'
     r, b = c.eval(c.sums, end_to_end=True, dss=dss, dbias=dbias)
     del r['y']
     rs = ratios(out, r, b)
-    _note(f'gn_bwd {path} {_tname(c.dtype)} end to end', rs)
-    _assert_ok(rs, f'{where} end to end (plan {c.plan()})')
+    note_all(TAG, f'gn_bwd {path} {NAME[c.dtype]} end to end', rs)
+    assert_ok(rs, f'{where} end to end (plan {c.plan()})')
     return out
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 @pytest.mark.parametrize('k', GN_FWD_ROWS, ids=_id)
 def test_groupnorm_fwd_replay(k, dtype):
     B, HW, C, G, ss, res, _ = k
-    replay_gn_fwd(GnCase(B, HW, C, G, dtype, ss, res), f'gn_fwd {k} {_tname(dtype)}')
+    replay_gn_fwd(GnCase(B, HW, C, G, dtype, ss, res), f'gn_fwd {k} {NAME[dtype]}')
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 @pytest.mark.parametrize('k', GN_BWD_ROWS, ids=_id)
 def test_groupnorm_bwd_replay(k, dtype):
     B, HW, C, G, ss, dss, dbias = k
-    replay_gn_bwd(GnCase(B, HW, C, G, dtype, ss), dss, dbias, f'gn_bwd {k} {_tname(dtype)}')
+    replay_gn_bwd(GnCase(B, HW, C, G, dtype, ss), dss, dbias, f'gn_bwd {k} {NAME[dtype]}')
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 @pytest.mark.parametrize('k', LN_FWD_ROWS, ids=_id)
 def test_layernorm_fwd_replay(k, dtype):
     c = LnCase(*k, dtype)
     out, ok = c.run(False)
     assert ok, f'ln_fwd {k}: a store landed outside y'
     rs = ratios(out, *c.eval(False))
-    _note(f'{plan_ln(*k, False)["kernel"]}_fwd {_tname(dtype)}', rs)
-    _assert_ok(rs, f'ln_fwd {k} {_tname(dtype)} (plan {plan_ln(*k, False)})')
+    note_all(TAG, f'{plan_ln(*k, False)["kernel"]}_fwd {NAME[dtype]}', rs)
+    assert_ok(rs, f'ln_fwd {k} {NAME[dtype]} (plan {plan_ln(*k, False)})')
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 @pytest.mark.parametrize('k', LN_BWD_ROWS, ids=_id)
 def test_layernorm_bwd_replay(k, dtype):
     M, C, res = k
@@ -752,8 +663,8 @@ def test_layernorm_bwd_replay(k, dtype):
     out, ok = c.run(True)
     assert ok, f'ln_bwd {k}: a store landed outside dx or dgamma'
     rs = ratios(out, *c.eval(True))
-    _note(f'{plan_ln(M, C, True)["kernel"]}_bwd {_tname(dtype)}', rs)
-    _assert_ok(rs, f'ln_bwd {k} {_tname(dtype)} (plan {plan_ln(M, C, True)})')
+    note_all(TAG, f'{plan_ln(M, C, True)["kernel"]}_bwd {NAME[dtype]}', rs)
+    assert_ok(rs, f'ln_bwd {k} {NAME[dtype]} (plan {plan_ln(M, C, True)})')
 
 
 def colsum_eval(x, pre, M):
@@ -762,12 +673,12 @@ def colsum_eval(x, pre, M):
             {'colsum': C_ACC * math.sqrt(M) * U * (pre.double().abs() + xd.abs().sum(dim=0))})
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 @pytest.mark.parametrize('k', COLSUM_ROWS, ids=_id)
 def test_colsum_replay(k, dtype):
     from physicsinformeddiffusionmodels_b200._lib import call, stream
     M, C = k
-    g = _gen(('colsum', M, C))
+    g = gen(('colsum', M, C))
     x, pre = _randn(g, M, C, dtype=dtype), _randn(g, C)
     buf, out = guarded(C)
     out.copy_(pre)
@@ -775,8 +686,8 @@ def test_colsum_replay(k, dtype):
     torch.cuda.synchronize()
     assert guards_intact(buf), f'colsum {k}: a store landed outside the output'
     rs = ratios({'colsum': out}, *colsum_eval(x, pre, M))
-    _note(f'colsum {_tname(dtype)}', rs)
-    _assert_ok(rs, f'colsum {k} {_tname(dtype)}')
+    note_all(TAG, f'colsum {NAME[dtype]}', rs)
+    assert_ok(rs, f'colsum {k} {NAME[dtype]}')
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -785,14 +696,14 @@ def test_colsum_replay(k, dtype):
 COND_SHAPE = (4, 1024, 64, 8)
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 @pytest.mark.parametrize('m_over_sigma', [0, 8, 64])
 def test_groupnorm_conditioning(m_over_sigma, dtype):
     """x = m + z: the variance loses a factor kappa = 1 + (m / sigma)^2 of accuracy (sum of squares minus squared mean
     in fp32) and the bound follows it, so the assertion is that the kernels lose no more than the formula in pidm.h
     must.  The worst absolute error of y is printed; DESIGN.md section 2 records it."""
     c = GnCase(*COND_SHAPE, dtype, ss=1, m_over_sigma=m_over_sigma)
-    where = f'm/sigma = {m_over_sigma} {_tname(dtype)}'
+    where = f'm/sigma = {m_over_sigma} {NAME[dtype]}'
     out, _ = replay_gn_fwd(c, where)
     r, _ = c.eval(c.sums, end_to_end=True, backward=False)
     err = (out['y'].double() - r['y']).abs()
@@ -802,14 +713,14 @@ def test_groupnorm_conditioning(m_over_sigma, dtype):
     replay_gn_bwd(c, 1, 1, where)
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 def test_groupnorm_constant_group(dtype):
     """a group that is one constant has var = 0: rstd = 1/sqrt(eps), xhat = 0, y = silu(beta (1 + scale) + shift), and dx
     is rstd times the mean-free part of gamma (1 + scale) dz; all finite and inside the same bounds"""
     c = GnCase(*COND_SHAPE, dtype, ss=1, constant_group=True)
-    out, sums = replay_gn_fwd(c, f'constant group {_tname(dtype)}')
+    out, sums = replay_gn_fwd(c, f'constant group {NAME[dtype]}')
     assert sums[0, 0, 0].item() == 2.0 * c.n and sums[0, 0, 1].item() == 4.0 * c.n
-    dout = replay_gn_bwd(c, 1, 1, f'constant group {_tname(dtype)}')
+    dout = replay_gn_bwd(c, 1, 1, f'constant group {NAME[dtype]}')
     assert torch.isfinite(out['y']).all() and torch.isfinite(dout['dx']).all()
     r, _ = c.eval(c.sums, end_to_end=False)
     cpg = c.shape[2] // c.shape[3]
@@ -823,9 +734,9 @@ def _gn_mutant(shape, dtype, mutation, output, ss=1, res=0):
     c = GnCase(*shape, dtype, ss, res)
     sums = c.sums.float()
     r, b = c.eval(sums, end_to_end=False)
-    assert max(ratios(rounded(r, dtype), r, b).values()) <= 1.0
+    assert max(ratios(rounded(r, dtype, ACT), r, b).values()) <= 1.0
     m, _ = c.eval(sums, end_to_end=False, mut=(mutation,))
-    return ratios(rounded(m, dtype), r, b)[output]
+    return ratios(rounded(m, dtype, ACT), r, b)[output]
 
 
 def test_mutant_variance_over_n_minus_1():
@@ -838,7 +749,7 @@ def test_mutant_variance_over_n_minus_1():
     assert _gn_mutant(shape, torch.bfloat16, 'variance over n - 1', 'dgamma') > 1.0
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 def test_mutant_last_cluster_rank_missing_from_the_group_sums(dtype):
     hit = set()
     for shape in GN_SHAPES_SYNTHETIC:
@@ -849,7 +760,7 @@ def test_mutant_last_cluster_rank_missing_from_the_group_sums(dtype):
     assert len(hit) >= 3, hit
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 def test_mutant_groupnorm_terms(dtype):
     shape = (5, 400, 256, 8)
     assert _gn_mutant(shape, dtype, 'one channel slab missing from dgamma', 'dgamma') > 1.0
@@ -859,18 +770,18 @@ def test_mutant_groupnorm_terms(dtype):
     assert _gn_mutant(shape, dtype, 'dbeta overwritten', 'dbeta') > 1.0
 
 
-@pytest.mark.parametrize('dtype', DTYPES, ids=_tname)
+@pytest.mark.parametrize('dtype', DTYPES, ids=NAME.get)
 def test_mutant_layernorm(dtype):
     c = LnCase(257, 32, dtype)
     r, b = c.eval(False)
-    assert max(ratios(rounded(r, dtype), r, b).values()) <= 1.0
+    assert max(ratios(rounded(r, dtype, ACT), r, b).values()) <= 1.0
     m, _ = c.eval(False, mut=('last row taken from the previous row',))
-    assert ratios(rounded(m, dtype), r, b)['y'] > 1.0
+    assert ratios(rounded(m, dtype, ACT), r, b)['y'] > 1.0
     c = LnCase(257, 32, dtype, res=1)
     r, b = c.eval(True)
-    assert max(ratios(rounded(r, dtype), r, b).values()) <= 1.0
+    assert max(ratios(rounded(r, dtype, ACT), r, b).values()) <= 1.0
     m, _ = c.eval(True, mut=('dx_residual missing',))
-    assert ratios(rounded(m, dtype), r, b)['dx'] > 1.0
+    assert ratios(rounded(m, dtype, ACT), r, b)['dx'] > 1.0
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -936,8 +847,3 @@ def test_rejected_shapes_are_refused_before_any_launch():
     for B, HW, C, G, code in ((1, 16, 24, 2, 1), (1, 16, 36, 4, 1), (1, 16, 32, 3, 1), (1, 16, 4096, 8, 0)):
         assert call('pidm_groupnorm_plan', B, HW, C, G, code, out.data_ptr()) != 0, (B, HW, C, G, code)
 
-
-if __name__ == '__main__':
-    if '--print-table' in sys.argv:
-        sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-        print_table(run_census(_key_of))

@@ -4,11 +4,11 @@ The Darcy residual (darcy.cu), the mechanics residual, its fused loss and the bi
 grids from the batch, the SM count and the mesh size: persistent Darcy CTAs that walk the batch with a double-buffered
 bulk copy, 8-row mechanics bands with a ragged last band, grid-stride resize loops.  The per-op tests in test_gpu_ops.py
 compare whole tensors by a norm ratio at a few small batches, which a bug confined to one band, one BC column or the last
-wave of CTAs cannot move.  Here, in the form of test_gpu_launch_census.py:
+wave of CTAs cannot move.  Here, in the four parts of the other census files and one more:
 
   1. census: one eager step of every workload bench.py times is recorded at the C ABI, and the distinct keys of the
      physics entry points (entry point, integer and flag arguments, which optional pointers are set) must equal the
-     tables below (`python tests/test_gpu_physics_census.py --print-table` regenerates them).  The standalone sweeps of
+     tables below (`python tests/census.py --print-table` regenerates them).  The standalone sweeps of
      bench.py are fixed rows that name the function they come from;
   2. replay: every table row and synthetic row runs through the C ABI on seeded fp32-exact operands, between NaN guards,
      against the fp64 references of oracle/pidm_oracle.py, per element:
@@ -17,26 +17,22 @@ wave of CTAs cannot move.  Here, in the form of test_gpu_launch_census.py:
      the resize adds the error of its fp32 source coordinate (see resize_bounds);
   3. mutants: the same predicates reject the fp64 reference edited the way a subtle kernel bug would change it;
   4. plan coverage: the launch arithmetic, restated below, shows that the rows reach every grid case;
-  5. completeness: every entry point the benchmarked steps call is either checked by one of the five census files or
-     listed in LAUNCHES_NOTHING (host-side queries).
+  5. completeness: every entry point the benchmarked steps call is either checked by one of the five census files (has
+     a key in census.KEYS) or listed in census.LAUNCHES_NOTHING (host-side queries).
 """
 import math
-import os
-import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-if __name__ == '__main__':                       # --print-table: the repository root, as conftest.py sets it
-    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from checks import P, U, guarded, guards_intact
+from census import KEYS, LAUNCHES_NOTHING, assert_census_in_tables, assert_tables_in_census, census
+from checks import P, U, call_sync, check, gen, guarded, guards_intact, sms
 from oracle import pidm_oracle as O
-from test_gpu_glue_census import GLUE_NAMES
-from test_gpu_launch_census import _NAMES as LAUNCH_NAMES, _ratio, run_census
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
+TAG = 'physics census'
 
 # Bound constants: C fp32 roundings of the absolute-value chain, each the smallest power of two that passes on an H100
 # (the worst |err| / (2^-24 A) seen was 6.6 for Darcy, 4.4 for mechanics, 6.2 for the fused losses); the worst
@@ -48,7 +44,7 @@ C_RESIZE = 4
 CHUNK = 2048                     # samples per fp64 reference chunk on the device
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the committed census tables (regenerate with --print-table)
+# the committed census tables (`python tests/census.py --print-table`)
 # ----------------------------------------------------------------------------------------------------------------------
 # darcy_fwd / darcy_bwd: B, P, domain_length, reverse_d1, flags
 # darcy_loss: B, P, domain_length, reverse_d1, flags, model_out == x0hat, grad_x0hat set, grad_model_out set
@@ -91,106 +87,21 @@ BENCH_ROWS = [
     ('mech_fwd', (8192, 64, 1), 'mechanics_bench'),
 ]
 
-# Entry points the benchmarked steps call that launch nothing: host-side capability and size queries.
-LAUNCHES_NOTHING = [
-    'pidm_conv2d_tc_general_supported',
-    'pidm_conv2d_wgrad_tc_supported',
-    'pidm_linattn_block_supported',
-    'pidm_linattn_block_workspace_floats',
-    'pidm_linattn_workspace_floats',
-    'pidm_mlp_entry_size',
-    'pidm_pack_entry_size',
-    'pidm_pack_pair_entry_size',
-]
-# the entry points each census file replays per element
-CENSUS_FAMILIES = {
-    'test_gpu_launch_census': set(LAUNCH_NAMES),
-    'test_gpu_norm_census': {'pidm_groupnorm_silu_fwd', 'pidm_groupnorm_silu_bwd', 'pidm_layernorm_c_fwd',
-                             'pidm_layernorm_c_bwd', 'pidm_colsum'},
-    'test_gpu_attention_census': {'pidm_linattn_fwd', 'pidm_linattn_bwd', 'pidm_attn_fwd', 'pidm_attn_bwd',
-                                  'pidm_head_fwd', 'pidm_head_bwd'},
-    'test_gpu_physics_census': {'pidm_darcy_residual_fwd', 'pidm_darcy_residual_bwd', 'pidm_darcy_pidm_loss',
-                                'pidm_mechanics_residual_fwd', 'pidm_mechanics_residual_bwd', 'pidm_mech_pidm_loss',
-                                'pidm_bilinear_resize_fwd', 'pidm_bilinear_resize_bwd'},
-    'test_gpu_glue_census': GLUE_NAMES,
-}
-
 
 # ----------------------------------------------------------------------------------------------------------------------
 # census
 # ----------------------------------------------------------------------------------------------------------------------
-def _physics_key(name, a):
-    has = lambda t: int(t is not None)
-    if name in ('pidm_darcy_residual_fwd', 'pidm_darcy_residual_bwd'):
-        i = 3 if name.endswith('fwd') else 4
-        return ('darcy_fwd' if name.endswith('fwd') else 'darcy_bwd',
-                (int(a[i]), int(a[i + 1]), float(a[i + 2]), int(a[i + 3]), int(a[i + 4])))
-    if name == 'pidm_darcy_pidm_loss':
-        return 'darcy_loss', (int(a[12]), int(a[13]), float(a[14]), int(a[15]), int(a[16]),
-                              int(a[1] is a[0] or a[1].data_ptr() == a[0].data_ptr()), has(a[10]), has(a[11]))
-    if name == 'pidm_mechanics_residual_fwd':
-        return 'mech_fwd', (int(a[6]), int(a[7]), has(a[5]))
-    if name == 'pidm_mechanics_residual_bwd':
-        return 'mech_bwd', (int(a[9]), int(a[10]), has(a[4]), has(a[5]))
-    if name == 'pidm_mech_pidm_loss':
-        return 'mech_loss', (int(a[18]), int(a[19]))
-    if name in ('pidm_bilinear_resize_fwd', 'pidm_bilinear_resize_bwd'):
-        return 'resize_' + name[-3:], (int(a[2]), int(a[3]), int(a[4]))
-    return None
-
-
-def _key_of(name, a):
-    """every call: (entry point, its physics key or None)"""
-    return 'call', (name, _physics_key(name, a))
-
-
-_CENSUS = {}
-
-
-def census():
-    """{workload: set of (family, key)} of the physics calls, and the set of every entry point called"""
-    if not _CENSUS:
-        raw = run_census(_key_of)
-        _CENSUS['keys'] = {wl: {k for _, (_, k) in calls if k is not None} for wl, calls in raw.items()}
-        _CENSUS['names'] = {n for calls in raw.values() for _, (n, _) in calls}
-    return _CENSUS['keys'], _CENSUS['names']
-
-
-def print_table(keys, names):
-    rows = {f: {} for f in TABLES}
-    for wl, ks in keys.items():
-        for fam, k in ks:
-            rows[fam].setdefault(k, []).append(wl)
-    for fam, table in rows.items():
-        print(f'{fam.upper()}_TABLE = [')
-        for k in sorted(table):
-            print(f'    {k!r},  # {" ".join(sorted(table[k]))}')
-        print(']')
-    covered = set().union(*CENSUS_FAMILIES.values())
-    print('LAUNCHES_NOTHING = [')
-    for n in sorted(names - covered):
-        print(f'    {n!r},')
-    print(']')
-
-
 def test_census_is_covered_by_the_table():
-    keys, _ = census()
-    missing = [f'{fam} {k!r}  # {wl}' for wl, ks in keys.items() for fam, k in sorted(ks) if k not in TABLES[fam]]
-    assert not missing, ('physics launches of the benchmarked steps that the tables do not replay (add them; '
-                         '`python tests/test_gpu_physics_census.py --print-table`):\n' + '\n'.join(missing))
+    assert_census_in_tables(TABLES)
 
 
 def test_every_table_row_is_produced_by_the_census():
-    keys, _ = census()
-    produced = {(fam, k) for ks in keys.values() for fam, k in ks}
-    stale = [f'{fam} {k!r}' for fam, table in TABLES.items() for k in table if (fam, k) not in produced]
-    assert not stale, ('table rows that no benchmarked step launches (drop them; '
-                       '`python tests/test_gpu_physics_census.py --print-table`):\n' + '\n'.join(stale))
+    assert_tables_in_census(TABLES)
 
 
 def test_every_benchmarked_entry_point_is_checked_or_listed():
     _, names = census()
-    covered = set().union(*CENSUS_FAMILIES.values())
+    covered = set(KEYS)
     unchecked = sorted(names - covered - set(LAUNCHES_NOTHING))
     assert not unchecked, ('entry points of the benchmarked steps that no census replays per element: add a census '
                            'family (a query that launches nothing goes in LAUNCHES_NOTHING):\n' + '\n'.join(unchecked))
@@ -202,10 +113,6 @@ def test_every_benchmarked_entry_point_is_checked_or_listed():
 # ----------------------------------------------------------------------------------------------------------------------
 # launch arithmetic (restated from the launches; no ABI query needed)
 # ----------------------------------------------------------------------------------------------------------------------
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def darcy_fwd_grid(B):          # launch_darcy_fwd: 220 KB / sizeof(DarcySmem) (64 KB) = 3 CTAs per SM, capped at B
     return min(B, 3 * sms())
 
@@ -222,34 +129,6 @@ def resize_passes(planes, out):  # pidm_bilinear_resize_fwd / _bwd: 256 threads,
     total = planes * out * out
     grid = min(-(-total // 256), 8 * sms())
     return -(-total // (grid * 256))
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# shared helpers
-# ----------------------------------------------------------------------------------------------------------------------
-WORST = {}
-
-
-def _note(what, ratio):
-    WORST[what] = max(WORST.get(what, 0.0), ratio)
-    print(f'[physics census] {what} |err|/bound {ratio:.4g}')
-
-
-def _check(what, y, r, bound):
-    """records and asserts the worst |y - r| / bound (y on the device, r and bound fp64 on the device)"""
-    q = _ratio((y.double() - r).abs(), bound)
-    _note(what, q)
-    assert q <= 1.0, f'{what}: worst |err| / bound = {q:.4g}'
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def _call(name, *a):
-    from physicsinformeddiffusionmodels_b200._lib import call, stream
-    call(name, *a, stream())
-    torch.cuda.synchronize()
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -289,7 +168,7 @@ def _geom(L, rev, flags):
 
 def _fields(B, seed):
     """Darcy fields [B,2,P,P] on the device, fp32 (p normal, K log-normal): exactly what the fp64 reference reads"""
-    x = torch.randn(B, 2, P, P, generator=_gen(seed), device=DEV)
+    x = torch.randn(B, 2, P, P, generator=gen(seed), device=DEV)
     x[:, 1] = torch.exp(0.5 * x[:, 1])
     return x
 
@@ -329,7 +208,7 @@ CH_NAMES = ('eq_0', 'bc_x0', 'bc_x1')
 def _fwd_launch(x, L, rev, flags):
     B = x.shape[0]
     buf, out = guarded(B * P * P * 3)
-    _call('pidm_darcy_residual_fwd', x, fs_dev(), out, B, P, float(L), int(rev), int(flags))
+    call_sync('pidm_darcy_residual_fwd', x, fs_dev(), out, B, P, float(L), int(rev), int(flags))
     assert guards_intact(buf), 'a store landed outside the residual'
     return out.view(B, P * P, 3)
 
@@ -344,7 +223,7 @@ def replay_darcy_fwd(row, seed):
         xs = x[lo:lo + CHUNK]
         r, A = darcy_residual(xs, per, geom), darcy_residual(xs.abs(), per, geom, absolute=True)
         for c, name in enumerate(CH_NAMES):
-            _check(f'darcy_fwd {tag} {name}', y[lo:lo + CHUNK, :, c], r[..., c], C_DARCY * U * A[..., c])
+            check(TAG, f'darcy_fwd {tag} {name}', y[lo:lo + CHUNK, :, c], r[..., c], C_DARCY * U * A[..., c])
 
 
 @pytest.mark.parametrize('row', _darcy_rows(DARCY_FWD_TABLE + [k for f, k, _ in BENCH_ROWS if f == 'darcy_fwd']),
@@ -358,9 +237,9 @@ def test_darcy_vjp_replay(row):
     B = _bspec(row[0])
     geom, per = _geom(*row[1:])
     x = _fields(B, 21)
-    cot = torch.randn(B, P * P, 3, generator=_gen(22), device=DEV)
+    cot = torch.randn(B, P * P, 3, generator=gen(22), device=DEV)
     buf, gx = guarded(B * 2 * P * P)
-    _call('pidm_darcy_residual_bwd', x, fs_dev(), cot, gx, B, P, float(row[1]), int(row[2]), int(row[3]))
+    call_sync('pidm_darcy_residual_bwd', x, fs_dev(), cot, gx, B, P, float(row[1]), int(row[2]), int(row[3]))
     assert guards_intact(buf), 'a store landed outside grad_x0hat'
     gx = gx.view(B, 2, P, P)
     for lo in range(0, B, CHUNK):
@@ -368,8 +247,8 @@ def test_darcy_vjp_replay(row):
         ref = O.darcy_residual_vjp(xs, cs, per, **geom)
         A = O.darcy_residual_vjp(xs, cs, per, absolute=True, **geom)
         for c, name in enumerate(('dp', 'dK')):
-            _check(f'darcy_bwd {"periodic" if per else "none"} {name}', gx[lo:lo + CHUNK, c], ref[:, c],
-                   C_DARCY * U * A[:, c])
+            check(TAG, f'darcy_bwd {"periodic" if per else "none"} {name}', gx[lo:lo + CHUNK, c], ref[:, c],
+                  C_DARCY * U * A[:, c])
 
 
 def _tables():
@@ -390,16 +269,16 @@ def replay_darcy_loss(B, L, rev, flags, variant, seed):
     geom, per = _geom(L, rev, flags)
     p2, var = _tables()
     x = _fields(B, seed)
-    tgt = torch.randn(B, 2, P, P, generator=_gen(seed + 1), device=DEV)
-    t = torch.randint(0, 100, (B,), generator=_gen(seed + 2), device=DEV)
-    m = torch.randn(B, 2, P, P, generator=_gen(seed + 3), device=DEV) if variant == 'sample' else x
+    tgt = torch.randn(B, 2, P, P, generator=gen(seed + 1), device=DEV)
+    t = torch.randint(0, 100, (B,), generator=gen(seed + 2), device=DEV)
+    m = torch.randn(B, 2, P, P, generator=gen(seed + 3), device=DEV) if variant == 'sample' else x
     bs, sums = guarded(3)
     bx, gx = guarded(B * 2 * P * P)
     bm, gm = guarded(B * 2 * P * P)
     c_data, c_res = 1.0, 1e-3
-    _call('pidm_darcy_pidm_loss', x, m, tgt, fs_dev(), t, p2, var, c_data, c_res, sums,
-          None if variant == 'loss_only' else gx, gm if variant == 'sample' else None, B, P, float(L), int(rev),
-          int(flags))
+    call_sync('pidm_darcy_pidm_loss', x, m, tgt, fs_dev(), t, p2, var, c_data, c_res, sums,
+              None if variant == 'loss_only' else gx, gm if variant == 'sample' else None, B, P, float(L), int(rev),
+              int(flags))
     assert guards_intact(bs) and guards_intact(bx) and guards_intact(bm)
     if variant != 'sample':
         assert torch.isnan(gm).all(), 'grad_model_out was written although it was not passed'
@@ -425,12 +304,12 @@ def replay_darcy_loss(B, L, rev, flags, variant, seed):
         A_gx = O.darcy_residual_vjp(xs, 4 * wr * Ar, per, absolute=True, **geom)
         rgm, A_gm = 2 * wd * (ms - ts), 2 * wd * (ms.abs() + ts.abs())
         if variant == 'mean':                   # the data gradient folded into grad_x0hat
-            _check(f'{tag} grad_x0hat (mean)', gx[sl], rgx + rgm, C_LOSS * U * (A_gx + A_gm))
+            check(TAG, f'{tag} grad_x0hat (mean)', gx[sl], rgx + rgm, C_LOSS * U * (A_gx + A_gm))
         else:
-            _check(f'{tag} grad_x0hat', gx[sl], rgx, C_LOSS * U * A_gx)
-            _check(f'{tag} grad_model_out', gm[sl], rgm, C_LOSS * U * A_gm)
+            check(TAG, f'{tag} grad_x0hat', gx[sl], rgx, C_LOSS * U * A_gx)
+            check(TAG, f'{tag} grad_model_out', gm[sl], rgm, C_LOSS * U * A_gm)
     for i, name in enumerate(('data', 'residual', 'mean|r|')):
-        _check(f'{tag} sum {name}', sums[i], rs[i], (darcy_loss_depth(B) + 2 * C_LOSS) * U * rA[i])
+        check(TAG, f'{tag} sum {name}', sums[i], rs[i], (darcy_loss_depth(B) + 2 * C_LOSS) * U * rA[i])
 
 
 LOSS_VARIANTS = ('mean', 'sample', 'loss_only')
@@ -468,7 +347,8 @@ def test_darcy_loss_rejects_unsupported_gradient_pointers(case):
     gx_arg = None if case == 'grad_model_out_without_grad_x0hat' else gx
     gm_arg = None if case == 'grad_x0hat_without_grad_model_out' else gm
     with pytest.raises(RuntimeError, match='darcy_pidm_loss: gradients'):
-        _call('pidm_darcy_pidm_loss', x, m, tgt, fs_dev(), t, p2, var, 1.0, 1e-3, sums, gx_arg, gm_arg, B, P, 1.0, 1, 1)
+        call_sync('pidm_darcy_pidm_loss', x, m, tgt, fs_dev(), t, p2, var, 1.0, 1e-3, sums, gx_arg, gm_arg, B, P, 1.0,
+                  1, 1)
     assert torch.isnan(bs).all() and torch.isnan(bx).all() and torch.isnan(bm).all(), 'a rejected call wrote'
 
 
@@ -507,10 +387,10 @@ def test_darcy_jacobian_max_replay(row):
     if B == 3:
         x[1, 1] = -x[1, 1]                        # negative K: the maximum comes from the BC rows / zero entries
     buf, out = guarded(B)
-    _call('pidm_darcy_jacobian_max', x, out, B, P, float(row[1]), int(row[2]), int(row[3]))
+    call_sync('pidm_darcy_jacobian_max', x, out, B, P, float(row[1]), int(row[2]), int(row[3]))
     assert guards_intact(buf)
     ref, A = torch.cat([torch.stack(jacobian_max_ref(x[lo:lo + 64], per, geom)) for lo in range(0, B, 64)], dim=1)
-    _check(f'darcy_jacobian_max {"periodic" if per else "none"}', out, ref, C_DARCY * U * A)
+    check(TAG, f'darcy_jacobian_max {"periodic" if per else "none"}', out, ref, C_DARCY * U * A)
     if B <= 3 and row[1:3] == (1.0, 1) and row[3] & 1:      # the matrix form against the oracle's explicit Jacobian
         assert torch.allclose(O.jacobian_max(x.double().cpu(), periodic=per), ref.cpu(), rtol=1e-9, atol=0)
 
@@ -533,9 +413,9 @@ def test_darcy_fd_stencil_replay(mode, B, periodic):
     A = {'d_d0': lambda: O.along_rows(D1a, ua), 'd_d1': lambda: O.along_cols(D1b, ua),
          'd_d00': lambda: O.along_rows(D2a, ua), 'd_d11': lambda: O.along_cols(D2b, ua),
          'd_d01': lambda: O.along_rows(D1a, O.along_cols(D1b, ua))}[mode]()
-    _check(f'fd_stencil {"periodic" if periodic else "none"} {mode}', y, r, C_DARCY * U * A)
+    check(TAG, f'fd_stencil {"periodic" if periodic else "none"} {mode}', y, r, C_DARCY * U * A)
     buf, out = guarded(B * P * P)
-    _call('pidm_fd_stencil', u, out, B, P, FD_MODES.index(mode) | (8 if periodic else 0), float(d0), float(d1))
+    call_sync('pidm_fd_stencil', u, out, B, P, FD_MODES.index(mode) | (8 if periodic else 0), float(d0), float(d1))
     assert guards_intact(buf) and torch.equal(out.view(B, P, P), y)
 
 
@@ -548,7 +428,7 @@ NELS = [2, 7, 63, 64, 100, 256]       # one band, one exact band, eight full ban
 def mech_operands(B, nel, seed):
     """fp32-exact u [B,2,nn,nn], rho [B,nel,nel] with exact zeros, bcs [B,4,nn,nn] with Dirichlet values 1, 0.5 and -1,
     loads on fixed dofs (which must be dropped) and at the four corner nodes"""
-    g = _gen(seed)
+    g = gen(seed)
     nn = nel + 1
     u = torch.randn(B, 2, nn, nn, generator=g, device=DEV) * 0.1
     rho = torch.rand(B, nel, nel, generator=g, device=DEV)
@@ -579,7 +459,7 @@ def mech_fwd_launch(u, rho, bcs, with_compliance=True):
     nn = nel + 1
     br, r = guarded(B * 2 * nn * nn)
     bc, c = guarded(B)
-    _call('pidm_mechanics_residual_fwd', u, rho, bcs, ke_dev(), r, c if with_compliance else None, B, nel)
+    call_sync('pidm_mechanics_residual_fwd', u, rho, bcs, ke_dev(), r, c if with_compliance else None, B, nel)
     assert guards_intact(br) and guards_intact(bc)
     if not with_compliance:
         assert torch.isnan(bc).all()
@@ -605,9 +485,9 @@ def test_mechanics_residual_replay(row):
         sl = slice(lo, lo + ch)
         rr, rc = mech_ref(u[sl], rho[sl], bcs[sl])
         Ar, Ac = mech_ref(u[sl], rho[sl], bcs[sl], absolute=True)
-        _check('mech_fwd residual', r[sl], rr, C_MECH * U * Ar)
+        check(TAG, 'mech_fwd residual', r[sl], rr, C_MECH * U * Ar)
         if with_c:
-            _check('mech_fwd compliance', c[sl], rc, (C_MECH + mech_depth(nel)) * U * Ac)
+            check(TAG, 'mech_fwd compliance', c[sl], rc, (C_MECH + mech_depth(nel)) * U * Ac)
 
 
 def mech_bwd_ref(u, rho, bcs, gr, gc, absolute=False, bcs_for_grad=None):
@@ -636,7 +516,7 @@ def mech_bwd_launch(u, rho, bcs, gr, gc):
     bu, du = guarded(B * 2 * nn * nn)
     bw, ws = guarded(B * 2 * nn * nn)
     bp, dp = guarded(B * nel * nel)
-    _call('pidm_mechanics_residual_bwd', u, rho, bcs, ke_dev(), gr, gc, du, dp, ws, B, nel)
+    call_sync('pidm_mechanics_residual_bwd', u, rho, bcs, ke_dev(), gr, gc, du, dp, ws, B, nel)
     assert guards_intact(bu) and guards_intact(bw) and guards_intact(bp)
     return du.view(B, 2, nn, nn), dp.view(B, nel, nel)
 
@@ -654,13 +534,13 @@ def test_mechanics_vjp_replay(row):
     B, nel, cm = row
     nn = nel + 1
     u, rho, bcs = mech_operands(B, nel, 70 + nel)
-    gr = torch.randn(B, 2 * nn * nn, generator=_gen(71), device=DEV) if cm != 'compliance' else None
-    gc = torch.randn(B, generator=_gen(72), device=DEV) if cm != 'residual' else None
+    gr = torch.randn(B, 2 * nn * nn, generator=gen(71), device=DEV) if cm != 'compliance' else None
+    gc = torch.randn(B, generator=gen(72), device=DEV) if cm != 'residual' else None
     du, drho = mech_bwd_launch(u, rho, bcs, gr, gc)
     rdu, rdrho = mech_bwd_ref(u, rho, bcs, gr, gc)
     Adu, Adrho = mech_bwd_ref(u, rho, bcs, gr, gc, absolute=True)
-    _check(f'mech_bwd grad_u ({cm})', du, rdu, C_MECH * U * Adu)
-    _check(f'mech_bwd grad_rho ({cm})', drho, rdrho, C_MECH * U * Adrho)
+    check(TAG, f'mech_bwd grad_u ({cm})', du, rdu, C_MECH * U * Adu)
+    check(TAG, f'mech_bwd grad_rho ({cm})', drho, rdrho, C_MECH * U * Adrho)
 
 
 def mech_loss_ref(u, rho, x0, r, comp, vf, t, p2, var, c_data, c_res, c_ineq, lam, edit=None):
@@ -698,7 +578,7 @@ def mech_loss_ref(u, rho, x0, r, comp, vf, t, p2, var, c_data, c_res, c_ineq, la
 def mech_loss_launch(B, nel, c_ineq, lam, t_kind, seed):
     nn = nel + 1
     n, ne = nn * nn, nel * nel
-    g = _gen(seed)
+    g = gen(seed)
     u = torch.randn(B, 2 * n, generator=g, device=DEV) * 0.1
     rho = torch.rand(B, nel, nel, generator=g, device=DEV)
     x0 = torch.rand(B, 3 * n, generator=g, device=DEV)
@@ -713,8 +593,8 @@ def mech_loss_launch(B, nel, c_ineq, lam, t_kind, seed):
     bp, grho = guarded(B * ne)
     br, gr = guarded(B * 2 * n)
     bc, gc = guarded(B)
-    _call('pidm_mech_pidm_loss', u, rho, x0, r, comp, vf, t, p2, var, 1.0, 1e-2, float(c_ineq), float(lam), sums, gu,
-          grho, gr, gc, B, nel)
+    call_sync('pidm_mech_pidm_loss', u, rho, x0, r, comp, vf, t, p2, var, 1.0, 1e-2, float(c_ineq), float(lam), sums,
+              gu, grho, gr, gc, B, nel)
     assert all(guards_intact(b) for b in (bs, bu, bp, br, bc))
     operands = (u, rho, x0, r, comp, vf, t, p2, var, 1.0, 1e-2, c_ineq, lam)
     return operands, sums, (gu.view(B, 2 * n), grho.view(B, nel, nel), gr.view(B, 2 * n), gc)
@@ -735,13 +615,13 @@ def check_mech_loss(operands, sums, grads, edit=None):
     for i, name in enumerate(('data', 'residual', 'inequality', 'optimisation', 'mean|r|', 'mean q')):
         bound = ((2 if i == 2 else 1) * depth + C_LOSS) * U * rA[i]
         if edit is None:
-            _check(f'mech_loss sum {name}', sums[i], rs[i], bound)
+            check(TAG, f'mech_loss sum {name}', sums[i], rs[i], bound)
         ok &= bool((sums[i].double() - rs[i]).abs() <= bound)
     A_gu, A_grho, A_dq, A_gr, A_gc = Ag
     bounds = (C_LOSS * U * A_gu, C_LOSS * U * A_grho + (depth + C_LOSS) * U * A_dq, C_LOSS * U * A_gr, C_LOSS * U * A_gc)
     for name, y, r, b in zip(('grad_u', 'grad_rho', 'grad_residual', 'grad_compliance'), grads, rg, bounds):
         if edit is None:
-            _check(f'mech_loss {name}', y, r, b)
+            check(TAG, f'mech_loss {name}', y, r, b)
         ok &= bool(((y.double() - r).abs() <= b).all())
     return ok
 
@@ -803,14 +683,14 @@ def resize_bounds(x, n_out):
                          ids=lambda k: f'planes{k[0]}_{k[1]}to{k[2]}')
 def test_resize_fwd_replay(row):
     planes, n_in, n_out = _planes(row[0], row[2]), row[1], row[2]
-    x = torch.randn(planes, n_in, n_in, generator=_gen(90 + n_in), device=DEV)
+    x = torch.randn(planes, n_in, n_in, generator=gen(90 + n_in), device=DEV)
     buf, y = guarded(planes * n_out * n_out)
-    _call('pidm_bilinear_resize_fwd', x, y, planes, n_in, n_out)
+    call_sync('pidm_bilinear_resize_fwd', x, y, planes, n_in, n_out)
     assert guards_intact(buf)
     xd = x.double().cpu()
     r = F.interpolate(xd[:, None], size=(n_out, n_out), mode='bilinear', align_corners=False)[:, 0]
     A, coord = resize_bounds(xd, n_out)
-    _check('resize_fwd', y.view(planes, n_out, n_out).cpu(), r, C_RESIZE * U * A + coord)
+    check(TAG, 'resize_fwd', y.view(planes, n_out, n_out).cpu(), r, C_RESIZE * U * A + coord)
 
 
 def resize_bwd_bounds(dy, n_in):
@@ -840,14 +720,14 @@ def resize_adjoint(dy, n_in):
                          ids=lambda k: f'planes{k[0]}_{k[1]}to{k[2]}')
 def test_resize_bwd_replay(row):
     planes, n_in, n_out = _planes(row[0], row[2]), row[1], row[2]
-    dy = torch.randn(planes, n_out, n_out, generator=_gen(95 + n_in), device=DEV)
+    dy = torch.randn(planes, n_out, n_out, generator=gen(95 + n_in), device=DEV)
     buf, dx = guarded(planes * n_in * n_in)          # NaN-filled: the entry point must zero dx itself
-    _call('pidm_bilinear_resize_bwd', dy, dx, planes, n_in, n_out)
+    call_sync('pidm_bilinear_resize_bwd', dy, dx, planes, n_in, n_out)
     assert guards_intact(buf)
     dyd = dy.double().cpu()
     r = resize_adjoint(dyd, n_in)
     A, T, depth = resize_bwd_bounds(dyd, n_in)
-    _check('resize_bwd', dx.view(planes, n_in, n_in).cpu(), r, (C_RESIZE + depth) * U * A + T)
+    check(TAG, 'resize_bwd', dx.view(planes, n_in, n_in).cpu(), r, (C_RESIZE + depth) * U * A + T)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -888,8 +768,8 @@ def test_mutant_mechanics(edit):
     B, nel = 3, 64
     u, rho, bcs = mech_operands(B, nel, 99)
     if edit == 'drho_from_unmasked_cotangent':
-        gr = torch.randn(B, 2 * (nel + 1) ** 2, generator=_gen(98), device=DEV)
-        gc = torch.randn(B, generator=_gen(97), device=DEV)
+        gr = torch.randn(B, 2 * (nel + 1) ** 2, generator=gen(98), device=DEV)
+        gc = torch.randn(B, generator=gen(97), device=DEV)
         _, drho = mech_bwd_launch(u, rho, bcs, gr, gc)
         bound = C_MECH * U * mech_bwd_ref(u, rho, bcs, gr, gc, absolute=True)[1]
         assert _within(drho, mech_bwd_ref(u, rho, bcs, gr, gc)[1], bound)
@@ -930,9 +810,9 @@ def test_mutant_mech_loss(edit):
 @pytest.mark.parametrize('shape', [(65, 64), (64, 128), (2, 5)], ids=lambda s: f'{s[0]}to{s[1]}')
 def test_mutant_resize(edit, shape):
     n_in, n_out = shape
-    x = torch.randn(3, n_in, n_in, generator=_gen(91), device=DEV)
+    x = torch.randn(3, n_in, n_in, generator=gen(91), device=DEV)
     _, y = guarded(3 * n_out * n_out)
-    _call('pidm_bilinear_resize_fwd', x, y, 3, n_in, n_out)
+    call_sync('pidm_bilinear_resize_fwd', x, y, 3, n_in, n_out)
     y = y.view(3, n_out, n_out).cpu()
     xd = x.double().cpu()
     A, coord = resize_bounds(xd, n_out)
@@ -977,7 +857,3 @@ def test_plan_coverage():
         assert max(resize_passes(_planes(k[0], k[2]), k[2]) for k in rows) >= 3, 'no multi-pass resize grid'
         assert any(resize_passes(_planes(k[0], k[2]), k[2]) == 1 for k in rows)
 
-
-if __name__ == '__main__':
-    if '--print-table' in sys.argv:
-        print_table(*census())
