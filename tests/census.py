@@ -1,12 +1,15 @@
-"""The census of the benchmarked steps, shared by the five per-element census files (tests/test_gpu_*_census.py).
+"""The census of the benchmarked steps, shared by the six per-element census files (tests/test_gpu_*_census.py).
 
 One eager step of every workload bench.py times (Darcy training at batch 32, one Darcy sampling step at batch 16 / 64 /
 256, mechanics training at batch 32 with Unet3D(dim=128)) is run with the C ABI's `call` swapped for a recorder, which
 keeps every entry point called and, for the entry points in KEYS, the distinct (family, key) pairs of their arguments.
 Keys are integer and flag arguments, which optional pointers are set and geometry decoded from device tables, never
-pointers.  Each census file commits one table per family and checks it against census() both ways;
-`python tests/census.py --print-table` regenerates every table.  The product package is imported inside the functions,
-so importing this module builds nothing."""
+pointers.  There are two recordings: census() runs the workloads as bench.py does (bf16), census_exact() runs them and
+the guidance and circular training steps in the fp32 exact mode that every oracle-parity test uses, where every
+convolution runs on the CUDA-core kernels of conv_simt.cu.  Each census file commits one table per family and checks it
+against its recording (census_exact() for the files in EXACT_FILES) both ways; `python tests/census.py --print-table`
+regenerates every table.  The product package is imported inside the functions, so importing this module builds
+nothing."""
 import functools
 import os
 import sys
@@ -114,6 +117,9 @@ KEYS = {
     'pidm_concat_channels': lambda a: [('concat', (int(a[3]), int(a[4]), int(a[5]), int(a[6])))],
     'pidm_split_channels': lambda a: [('split', (int(a[3]), int(a[4]), int(a[5]), int(a[6])))],
     'pidm_nchw_to_nhwc': lambda a: [('nchw', tuple(int(v) for v in a[2:7]))],
+    # test_gpu_simt_census.py (the dtype is left out: every row is replayed in both)
+    'pidm_conv2d_simt': lambda a: [('simt', tuple(int(v) for v in a[5:17]) + (_has(a[2]), _has(a[3])))],
+    'pidm_conv2d_wgrad_simt': lambda a: [('simt_wgrad', tuple(int(v) for v in a[4:19]) + (_has(a[3]),))],
 }
 
 # the families of KEYS by the census file that holds their tables, in the order of its tables
@@ -125,7 +131,10 @@ FAMILIES = {
                                    'resize_fwd', 'resize_bwd'),
     'test_gpu_glue_census.py': ('time_fwd', 'time_bwd', 'mlp_fwd', 'mlp_bwd', 'sumsq', 'adam', 'pack', 'pair',
                                 'pair_launch', 'qsample', 'axpby', 'scale', 'concat', 'split', 'nchw'),
+    'test_gpu_simt_census.py': ('simt', 'simt_wgrad'),
 }
+# the files whose tables are checked against census_exact(); every other file against census()
+EXACT_FILES = ('test_gpu_simt_census.py',)
 
 # Entry points the benchmarked steps call that launch nothing: host-side capability and size queries.
 LAUNCHES_NOTHING = [
@@ -177,8 +186,8 @@ def _darcy_model(dev):
     return Unet3D(dim=32, channels=2).to(dev)
 
 
-def run_census():
-    """{workload: _record(one eager step of it)} for every workload bench.py times (bf16)"""
+def run_census(precision='bf16'):
+    """{workload: _record(one eager step of it)} for every workload bench.py times, in ops precision `precision`"""
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
     from physicsinformeddiffusionmodels_b200.engine import SampleEngine, TrainEngine
@@ -186,7 +195,7 @@ def run_census():
     from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
     dev = torch.device(DEV)
-    ops.set_precision('bf16')
+    ops.set_precision(precision)
     ops.set_tensor_core_conv(True)
     out = {}
     model = _darcy_model(dev)
@@ -231,18 +240,71 @@ def run_census():
     return out
 
 
+def _train_step(model, diff, res, B, seed):
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
+    eng = TrainEngine(model, diff, res, lr=1e-4, max_norm=1.0, ema_mu=0.99, c_data=1.0, c_residual=1e-3,
+                      use_graph=False)
+    x0 = torch.randn(B, 2, 64, 64, generator=torch.Generator().manual_seed(seed)).to(DEV)
+    return _record(lambda: eng.step(x0))
+
+
+def run_census_exact():
+    """{workload: _record(one eager step of it)} in the fp32 exact mode: the workloads of run_census(), the Darcy
+    training step of the guidance study and of the circular study with residual-gradient guidance (the halo'd
+    geometries, and emb_conv[2], which stays zero-padded inside a circular model), and forward + backward of a scalar
+    loss through the circular mechanics U-Net.  Leaves the package in bf16."""
+    from physicsinformeddiffusionmodels_b200 import ops
+    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
+    from study import build_darcy
+    try:
+        out = run_census('fp32')
+        out['guidance_train_b32'] = _train_step(*build_darcy('guidance'), 32, 2)
+        out['circular_train_b32'] = _train_step(*build_darcy('circular', residual_grad_guidance=True), 32, 3)
+        torch.manual_seed(0)
+        mech = Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True, padding_mode='circular').to(DEV)
+        g = torch.Generator().manual_seed(4)
+        x = torch.randn(32, 10, 64, 64, generator=g).to(DEV)
+        t = torch.randint(0, 100, (32,), generator=g).to(DEV)
+        out['circular_mech_b32'] = _record(lambda: mech(x, t).square().mean().backward())
+        del mech
+        torch.cuda.empty_cache()
+    finally:
+        ops.set_precision('bf16')
+    return out
+
+
+def _summary(raw):
+    return {wl: keys for wl, (keys, _) in raw.items()}, set().union(*(names for _, names in raw.values()))
+
+
 @functools.cache
 def census():
     """({workload: set of (family, key)}, set of every entry point called), recorded once per process"""
-    raw = run_census()
-    return {wl: keys for wl, (keys, _) in raw.items()}, set().union(*(names for _, names in raw.values()))
+    return _summary(run_census())
+
+
+@functools.cache
+def census_exact():
+    """census() of the fp32 exact mode (run_census_exact), recorded once per process"""
+    return _summary(run_census_exact())
+
+
+def _recording(file):
+    return census_exact if file in EXACT_FILES else census
+
+
+def _file_of(tables):
+    """the census file whose families are the keys of `tables`"""
+    files = [f for f, fams in FAMILIES.items() if set(tables) <= set(fams)]
+    assert len(files) == 1, f'tables of no single census file: {sorted(tables)}'
+    return files[0]
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # the two-way check of a census file's tables ({family: rows})
 # ----------------------------------------------------------------------------------------------------------------------
 def assert_census_in_tables(tables):
-    keys, _ = census()
+    keys, _ = _recording(_file_of(tables))()
     missing = [f'{fam} {k!r}  # {wl}' for wl, ks in keys.items()
                for fam, k in sorted(fk for fk in ks if fk[0] in tables) if k not in tables[fam]]
     assert not missing, ('launches of the benchmarked steps that the tables do not replay (add them; '
@@ -250,7 +312,7 @@ def assert_census_in_tables(tables):
 
 
 def assert_tables_in_census(tables):
-    keys, _ = census()
+    keys, _ = _recording(_file_of(tables))()
     produced = {fk for ks in keys.values() for fk in ks}
     stale = [f'{fam} {k!r}' for fam, table in tables.items() for k in table if (fam, k) not in produced]
     assert not stale, ('table rows that no benchmarked step launches (drop them, or move a row kept for plan coverage '
@@ -258,8 +320,8 @@ def assert_tables_in_census(tables):
 
 
 def print_tables():
-    keys, names = census()
     for file, families in FAMILIES.items():
+        keys, _ = _recording(file)()
         rows = {f: {} for f in families}
         for wl, ks in keys.items():
             for fam, k in ks:
@@ -274,6 +336,7 @@ def print_tables():
         for wl, ks in keys.items():
             print(f'# {wl}: ' + ', '.join(f'{f} {sum(1 for ff, _ in ks if ff == f)}' for f in families))
         print('# distinct: ' + ', '.join(f'{f} {len(v)}' for f, v in rows.items()))
+    _, names = census()
     print('# tests/census.py')
     print('LAUNCHES_NOTHING = [')
     for n in sorted(names - set(KEYS)):

@@ -1,10 +1,11 @@
 """Helpers shared by the tests: relative error, NaN-guarded output buffers, the per-element bound predicate of the fp32
-Darcy kernels against their fp64 references, and the seeding, launch, dtype and |err| / bound helpers of the census
-files."""
+Darcy kernels against their fp64 references, the seeding, launch, dtype and |err| / bound helpers of the census files,
+and the fp64 reference of the implicit-GEMM convolution contract that both convolution census files replay."""
 import math
 import zlib
 
 import torch
+import torch.nn.functional as F
 
 P = 64
 U = 2.0 ** -24
@@ -99,3 +100,23 @@ def check(tag, what, y, r, bound):
     q = ratio((y.double() - r).abs(), bound)
     note(tag, what, q)
     assert q <= 1.0, f'{what}: worst |err| / bound = {q:.4g}'
+
+
+def conv_ref(x, wp, bias, res, k):
+    """fp64 y of the implicit-GEMM convolution contract of include/pidm.h (pidm_conv2d_simt, pidm_conv2d_tc_general):
+    y = sum A(m,k) Wp[n,k] (+ bias) (+ residual), NHWC, for k = (B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad,
+    transposed, ...)"""
+    B, H, W, Cin, Ho, Wo, Cout, KH, KW, s, p, tr = k[:12]
+    w4 = wp.view(Cout, KH, KW, Cin)
+    xn = x.permute(0, 3, 1, 2)
+    if not tr:
+        y = F.conv2d(xn, w4.permute(0, 3, 1, 2), stride=s, padding=p)
+    else:                           # gather at ((oh + p - r) / s, ...) == ConvTranspose with w[c][n][r][q] = Wp[n][r][q][c]
+        op = Ho - ((H - 1) * s - 2 * p + KH)
+        y = F.conv_transpose2d(xn, w4.permute(3, 0, 1, 2), stride=s, padding=p, output_padding=op)
+    y = y.permute(0, 2, 3, 1)
+    if bias is not None:
+        y = y + bias
+    if res is not None:
+        y = y + res
+    return y

@@ -28,7 +28,7 @@ import torch
 import torch.nn.functional as F
 
 from census import assert_census_in_tables, assert_tables_in_census
-from checks import gen, note, ratio
+from checks import conv_ref, gen, note, ratio
 
 pytestmark = pytest.mark.gpu
 
@@ -518,24 +518,6 @@ def plan_laf(B, N):
 
 
 # ---- convolution ------------------------------------------------------------------------------------------------------
-def _conv_ref(x, wp, bias, res, k):
-    """fp64 y of the pidm_conv2d_tc_general contract: y = sum A(m,k) Wp[n,k] (+ bias) (+ residual), NHWC"""
-    B, H, W, Cin, Ho, Wo, Cout, KH, KW, s, p, tr = k[:12]
-    w4 = wp.view(Cout, KH, KW, Cin)
-    xn = x.permute(0, 3, 1, 2)
-    if not tr:
-        y = F.conv2d(xn, w4.permute(0, 3, 1, 2), stride=s, padding=p)
-    else:                           # gather at ((oh + p - r) / s, ...) == ConvTranspose with w[c][n][r][q] = Wp[n][r][q][c]
-        op = Ho - ((H - 1) * s - 2 * p + KH)
-        y = F.conv_transpose2d(xn, w4.permute(3, 0, 1, 2), stride=s, padding=p, output_padding=op)
-    y = y.permute(0, 2, 3, 1)
-    if bias is not None:
-        y = y + bias
-    if res is not None:
-        y = y + res
-    return y
-
-
 class ConvCase:
     """operands + fp64 reference (r) + absolute-value reference (A) of one table row"""
 
@@ -548,9 +530,9 @@ class ConvCase:
         self.bias = torch.randn(Cout, generator=g, device=DEV) if hb else None
         self.res = _randn(g, B, Ho, Wo, Cout) if hr else None
         d = lambda t: None if t is None else t.double()
-        self.r = _conv_ref(d(self.x), d(self.wp), d(self.bias), d(self.res), k)
-        self.A = _conv_ref(d(self.x).abs(), d(self.wp).abs(), None if self.bias is None else d(self.bias).abs(),
-                           None if self.res is None else d(self.res).abs(), k)
+        self.r = conv_ref(d(self.x), d(self.wp), d(self.bias), d(self.res), k)
+        self.A = conv_ref(d(self.x).abs(), d(self.wp).abs(), None if self.bias is None else d(self.bias).abs(),
+                          None if self.res is None else d(self.res).abs(), k)
 
     def acc_bound(self):
         return C_ACC * math.sqrt(self.K) * 2.0 ** -24 * self.A
@@ -864,7 +846,7 @@ def test_mutant_conv_dropped_k_slice():
     tap, c0 = (KH * KW) // 2, Cin // 2 // 32 * 32
     wm = torch.zeros(Cout, KH * KW, Cin, dtype=torch.float64, device=DEV)
     wm[:, tap, c0:c0 + 32] = c.wp.double().view(Cout, KH * KW, Cin)[:, tap, c0:c0 + 32]
-    part = _conv_ref(c.x.double(), wm.view(Cout, -1), None, None, k)
+    part = conv_ref(c.x.double(), wm.view(Cout, -1), None, None, k)
     assert c.ratio(_bf16(c.r - part)) > 1.0, conv_id(k)
 
 
