@@ -554,14 +554,8 @@ extern "C" int pidm_attn_fwd(const void* qkv, void* out, int B, int n_tokens, in
     PIDM_REQUIRE(n_tokens >= 1 && n_tokens <= AT_N, "attn: at most %d tokens supported (got %d)", AT_N, n_tokens);
     const float scale = 0.17677669529663687f;
     if (attn_mid_supported(n_tokens, dtype)) return attn_mid_fwd(qkv, out, B, heads, scale, (cudaStream_t)stream);
-    static bool set0 = false, set1 = false;
     PIDM_DISPATCH_DTYPE(dtype, {
-        bool& flag = (sizeof(T) == 4) ? set0 : set1;
-        if (!flag) {
-            PIDM_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)sizeof(AttnSmemF)));
-            flag = true;
-        }
+        PIDM_CUDA(allow_smem(attn_fwd_kernel<T>, sizeof(AttnSmemF)));
         PIDM_CUDA(launch_plain(attn_fwd_kernel<T>, dim3(dim3(heads, B)), dim3(256), (size_t)(sizeof(AttnSmemF)), (cudaStream_t)stream, (const T*)qkv, (T*)out,
                                                                                               n_tokens, heads, scale));
     });
@@ -574,14 +568,8 @@ extern "C" int pidm_attn_bwd(const void* qkv, const void* dout, void* dqkv, int 
     PIDM_REQUIRE(n_tokens >= 1 && n_tokens <= AT_N, "attn: at most %d tokens supported (got %d)", AT_N, n_tokens);
     const float scale = 0.17677669529663687f;
     if (attn_mid_supported(n_tokens, dtype)) return attn_mid_bwd(qkv, dout, dqkv, B, heads, scale, (cudaStream_t)stream);
-    static bool set0 = false, set1 = false;
     PIDM_DISPATCH_DTYPE(dtype, {
-        bool& flag = (sizeof(T) == 4) ? set0 : set1;
-        if (!flag) {
-            PIDM_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)sizeof(AttnSmemB)));
-            flag = true;
-        }
+        PIDM_CUDA(allow_smem(attn_bwd_kernel<T>, sizeof(AttnSmemB)));
         PIDM_CUDA(launch_plain(attn_bwd_kernel<T>, dim3(dim3(heads, B)), dim3(256), (size_t)(sizeof(AttnSmemB)), (cudaStream_t)stream, (const T*)qkv, (const T*)dout, (T*)dqkv, n_tokens, heads, scale));
     });
     PIDM_LAUNCH_CHECK("attn_bwd");

@@ -875,30 +875,6 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
 
 constexpr size_t LAF_STATS_SMEM = (size_t)LM_HEADS * LFS_STAGES * LW_TILE * 2;
 
-static int laf_attrs() {
-    static bool done = false;
-    if (!done) {
-        PIDM_CUDA(cudaFuncSetAttribute(laf_kmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_STATS_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_ctx_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfcCfg<0>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_ctx_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfcCfg<1>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAF_OUT_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfbCfg::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<0>::SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(laf_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LfwCfg<1>::SMEM));
-        done = true;
-    }
-    return 0;
-}
-
-static int laf_chunk_px(int B, int N, int ctas_per_sm) {
-    // chunks are per sample: k chunks per sample with B * k <= resident CTA slots (one wave), 32-pixel granularity
-    int k = (num_sms() * ctas_per_sm) / B;
-    if (k < 1) k = 1;
-    int px = ((N + k - 1) / k + 31) / 32 * 32;
-    if (px < 64) px = 64;
-    if (px > N) px = N;
-    return px;
-}
 static int laf_stat_chunks(int N) {
     int c = N / 128;
     if (c < 1) c = 1;
@@ -918,8 +894,7 @@ extern "C" int pidm_linattn_block_workspace_floats(int B, int N) { return B * la
 // pixel chunking of the block's kernels: out[5] = {statistics chunks (kmax), ctx px, fwd (y) px, bwd px, wgrad px}
 extern "C" int pidm_linattn_block_plan(int B, int N, int* out) {
     PIDM_REQUIRE(N % 128 == 0 && B > 0, "linattn_block_plan: N must be a multiple of 128 (got %d)", N);
-    const int v[5] = {laf_stat_chunks(N), laf_chunk_px(B, N, 2), laf_chunk_px(B, N, 2), laf_chunk_px(B, N, 1),
-                      laf_chunk_px(B, N, 1)};
+    const int v[5] = {laf_stat_chunks(N), chunk_px(B, N, 2), chunk_px(B, N, 2), chunk_px(B, N, 1), chunk_px(B, N, 1)};
     for (int i = 0; i < 5; ++i) out[i] = v[i];
     return 0;
 }
@@ -931,7 +906,6 @@ extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const v
     PIDM_REQUIRE(w_out && b_out && residual, "linattn_block_fwd: w_out, b_out and residual are required");
     PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
-    if (int e = laf_attrs()) return e;
     const float scale = 0.17677669529663687f;   // 32^-0.5
     const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
     const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
@@ -940,12 +914,15 @@ extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const v
     const int chunks = laf_stat_chunks(N);
     const int rpc = N / chunks;
     PIDM_REQUIRE(rpc % 32 == 0 && rpc * chunks == N, "linattn_block: bad statistics chunking for N=%d", N);
+    PIDM_CUDA(allow_smem(laf_kmax_kernel, LAF_STATS_SMEM));
     PIDM_CUDA(launch_plain(laf_kmax_kernel, dim3(dim3(chunks, B)), dim3(256), (size_t)(LAF_STATS_SMEM), st, x, w, workspace, N, rpc));
-    const int px = laf_chunk_px(B, N, 2);         // the context and output kernels: two CTAs per SM
+    const int px = chunk_px(B, N, 2);             // the context and output kernels: two CTAs per SM
     const dim3 grid((N + px - 1) / px, B);
+    PIDM_CUDA(allow_smem(laf_ctx_kernel<0>, LfcCfg<0>::SMEM));
     PIDM_CUDA(launch_plain(laf_ctx_kernel<0>, grid, dim3(256), LfcCfg<0>::SMEM, st, x, w, nullptr, workspace, chunks, kmax, kzinv,
                            ctx, N, px, scale, nullptr));
     PIDM_CUDA(launch_plain(laf_finalize_kernel, dim3((B * LM_HID + 7) / 8), dim3(256), (size_t)(0), st, ctx, kzinv, B * LM_HID));
+    PIDM_CUDA(allow_smem(laf_out_kernel, LAF_OUT_SMEM));
     PIDM_CUDA(launch_plain(laf_out_kernel, grid, dim3(256), LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)y, N, px, scale,
                            (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
     PIDM_LAUNCH_CHECK("linattn_block_fwd");
@@ -957,17 +934,18 @@ extern "C" int pidm_linattn_block_bwd(const void* xn, const void* w_qkv, const v
                                       void* stream) {
     PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
-    if (int e = laf_attrs()) return e;
     const float scale = 0.17677669529663687f;
     const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
     const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
     const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
     const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
     PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * LM_HEADS * LM_D * LM_D * sizeof(float), st));
-    const int cpx = laf_chunk_px(B, N, 2);
+    const int cpx = chunk_px(B, N, 2);
+    PIDM_CUDA(allow_smem(laf_ctx_kernel<1>, LfcCfg<1>::SMEM));
     PIDM_CUDA(launch_plain(laf_ctx_kernel<1>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), LfcCfg<1>::SMEM, st, x, w, g,
                            nullptr, 0, nullptr, nullptr, dctx, N, cpx, scale, wo));
-    const int bpx = laf_chunk_px(B, N, 1);
+    const int bpx = chunk_px(B, N, 1);
+    PIDM_CUDA(allow_smem(laf_bwd_kernel, LfbCfg::SMEM));
     PIDM_CUDA(launch_plain(laf_bwd_kernel, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), LfbCfg::SMEM, st, x, w, g, ctx, dctx,
                            kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, scale, wo));
     PIDM_LAUNCH_CHECK("linattn_block_bwd");
@@ -981,16 +959,17 @@ extern "C" int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const
                                         void* stream) {
     PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
-    if (int e = laf_attrs()) return e;
     const float scale = 0.17677669529663687f;
     const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
     const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
     const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
     const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
-    const int px = laf_chunk_px(B, N, 1);
+    const int px = chunk_px(B, N, 1);
     const dim3 grid((N + px - 1) / px, B);
+    PIDM_CUDA(allow_smem(laf_wgrad_kernel<0>, LfwCfg<0>::SMEM));
     PIDM_CUDA(launch_plain(laf_wgrad_kernel<0>, grid, dim3(256), LfwCfg<0>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
                            N, px, qkv_stride_n, qkv_stride_c, scale, wo, grad_w_out, out_stride_n, out_stride_c));
+    PIDM_CUDA(allow_smem(laf_wgrad_kernel<1>, LfwCfg<1>::SMEM));
     PIDM_CUDA(launch_plain(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
                            N, px, qkv_stride_n, qkv_stride_c, scale, nullptr, nullptr, 0LL, 0LL));
     PIDM_LAUNCH_CHECK("linattn_block_wgrad");

@@ -342,58 +342,37 @@ constexpr size_t LA_CTX_SMEM = (size_t)LM_HEADS * LC_STAGES * 2 * LW_TILE * 2 + 
 constexpr size_t LA_OUT_SMEM = (size_t)LM_HEADS * LO_STAGES * LW_TILE * 2;
 constexpr size_t LA_BWD_SMEM = (size_t)LM_HEADS * LB_STAGES * LB_TILE * 2 + (size_t)LM_HEADS * 3 * LM_D * 4;
 
-static int la_mma_attrs() {
-    static bool done = false;
-    if (!done) {
-        PIDM_CUDA(cudaFuncSetAttribute(la_ctx_mma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LA_CTX_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(la_ctx_mma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LA_CTX_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(la_out_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LA_OUT_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(la_bwd_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LA_BWD_SMEM));
-        done = true;
-    }
-    return 0;
-}
-
-// pixels per CTA: about two CTAs per SM over the whole batch, a multiple of 32, never more than the image
-static int la_chunk_px(int B, int N, int ctas_per_sm) {
-    // chunks are per sample: k chunks per sample with B * k <= resident CTA slots (one wave), 32-pixel granularity
-    int k = (num_sms() * ctas_per_sm) / B;
-    if (k < 1) k = 1;
-    int px = ((N + k - 1) / k + 31) / 32 * 32;
-    if (px < 64) px = 64;
-    if (px > N) px = N;
-    return px;
-}
-
-// entry points used by attention.cu for the bf16 / 8-head case
-int la_mma_chunk_px(int B, int N) { return la_chunk_px(B, N, 2); }
+// entry points used by attention.cu for the bf16 / 8-head case: about two CTAs per SM
+int la_mma_chunk_px(int B, int N) { return chunk_px(B, N, 2); }
 int la_mma_ctx(int mode, const void* qkv, const void* dout, const float* part, int n_stat_chunks, float* kmax,
                float* kzinv, float* ctx, int B, int N, float scale, cudaStream_t st) {
-    if (int e = la_mma_attrs()) return e;
-    const int cpx = la_chunk_px(B, N, 2);
+    const int cpx = chunk_px(B, N, 2);
     dim3 grid((N + cpx - 1) / cpx, B);
-    if (mode == 0)
+    if (mode == 0) {
+        PIDM_CUDA(allow_smem(la_ctx_mma_kernel<0>, LA_CTX_SMEM));
         PIDM_CUDA(launch_plain(la_ctx_mma_kernel<0>, dim3(grid), dim3(256), (size_t)(LA_CTX_SMEM), st, (const __nv_bfloat16*)qkv, nullptr, part, n_stat_chunks, kmax,
                                                               kzinv, ctx, N, cpx, scale));
-    else
+    } else {
+        PIDM_CUDA(allow_smem(la_ctx_mma_kernel<1>, LA_CTX_SMEM));
         PIDM_CUDA(launch_plain(la_ctx_mma_kernel<1>, dim3(grid), dim3(256), (size_t)(LA_CTX_SMEM), st, (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)dout, nullptr,
                                                               0, nullptr, nullptr, ctx, N, cpx, scale));
+    }
     PIDM_LAUNCH_CHECK("la_ctx_mma");
     return 0;
 }
 int la_mma_out(const void* qkv, const float* ctx, void* out, int B, int N, float scale, cudaStream_t st) {
-    if (int e = la_mma_attrs()) return e;
-    const int cpx = la_chunk_px(B, N, 2);
+    const int cpx = chunk_px(B, N, 2);
     dim3 grid((N + cpx - 1) / cpx, B);
+    PIDM_CUDA(allow_smem(la_out_mma_kernel, LA_OUT_SMEM));
     PIDM_CUDA(launch_plain(la_out_mma_kernel, dim3(grid), dim3(256), (size_t)(LA_OUT_SMEM), st, (const __nv_bfloat16*)qkv, ctx, (__nv_bfloat16*)out, N, cpx, scale));
     PIDM_LAUNCH_CHECK("la_out_mma");
     return 0;
 }
 int la_mma_bwd(const void* qkv, const void* dout, const float* ctx, const float* dctx, const float* kmax,
                const float* kzinv, void* dqkv, int B, int N, float scale, cudaStream_t st) {
-    if (int e = la_mma_attrs()) return e;
-    const int cpx = la_chunk_px(B, N, 2);
+    const int cpx = chunk_px(B, N, 2);
     dim3 grid((N + cpx - 1) / cpx, B);
+    PIDM_CUDA(allow_smem(la_bwd_mma_kernel, LA_BWD_SMEM));
     PIDM_CUDA(launch_plain(la_bwd_mma_kernel, dim3(grid), dim3(256), (size_t)(LA_BWD_SMEM), st, (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)dout, ctx, dctx, kmax,
                                                        kzinv, (__nv_bfloat16*)dqkv, N, cpx, scale));
     PIDM_LAUNCH_CHECK("la_bwd_mma");

@@ -182,11 +182,7 @@ bool la_small_supported(int N, int dtype) { return dtype == PIDM_BF16 && N >= 32
 
 int la_small_fwd(const void* qkv, void* out, float* ctx, float* kmax, float* kzinv, int B, int N, int heads, float scale,
                  cudaStream_t st) {
-    static bool attr = false;
-    if (!attr) {
-        PIDM_CUDA(cudaFuncSetAttribute(la_small_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ls_smem(LS_MAXN, false)));
-        attr = true;
-    }
+    PIDM_CUDA(allow_smem(la_small_fwd_kernel, ls_smem(LS_MAXN, false)));
     PIDM_CUDA(launch_plain(la_small_fwd_kernel, dim3(heads, B), dim3(LS_THREADS), ls_smem(N, false), st, (const __nv_bfloat16*)qkv,
                            (__nv_bfloat16*)out, ctx, kmax, kzinv, N, heads, scale));
     PIDM_LAUNCH_CHECK("la_small_fwd");

@@ -109,16 +109,32 @@ __device__ __forceinline__ bool reduce_same_octet(float (&v)[NV], int oct) {
     return (threadIdx.x & 31) < oct;
 }
 
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
 __device__ __forceinline__ float silu_f(float z) { return z / (1.f + __expf(-z)); }
 __device__ __forceinline__ float silu_grad_f(float z) {
     float s = 1.f / (1.f + __expf(-z));
     return s * (1.f + z * (1.f - s));
+}
+// GELU, exact erf form (nn.GELU()); each translation unit compiles it under its own arithmetic flags
+__device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+__device__ __forceinline__ float gelu_erf_grad_f(float x) {
+    return 0.5f * (1.f + erff(x * 0.70710678118654752f)) + x * 0.3989422804014327f * expf(-0.5f * x * x);
 }
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // streaming multiprocessors of the current device (queried once; sizes persistent grids and one-wave splits)
 int num_sms();
+
+// Opt a kernel into `bytes` of dynamic shared memory (needed above 48 KB).  The attribute is set only when `bytes`
+// exceeds what was last set for that kernel, so a call before every launch costs a lookup; safe from several host
+// threads (the autograd worker and the main thread) at once.
+cudaError_t allow_smem(const void* kernel, size_t bytes);
+template <typename... KArgs>
+static inline cudaError_t allow_smem(void (*kernel)(KArgs...), size_t bytes) {
+    return allow_smem((const void*)kernel, bytes);
+}
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------------------
 // The step is a chain of ~420 dependent kernels, many of them a few microseconds long: the kernel-to-kernel launch

@@ -381,11 +381,7 @@ extern "C" int pidm_pack_weights_pairs(const void* table_dev, const int* tile_ma
     PIDM_REQUIRE(max_taps >= 1 && max_taps <= 16, "pack_weights_pairs: taps must be 1..16 (got %d)", max_taps);
     const size_t esz = dtype == PIDM_BF16 ? 2 : 4;
     const size_t smem = (size_t)32 * (32 * (max_taps | 1) + 2) * esz;
-    static bool attr = false;
-    if (!attr) {
-        PIDM_CUDA(cudaFuncSetAttribute(pack_pair_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * (32 * 17 + 2) * 4));
-        attr = true;
-    }
+    PIDM_CUDA(allow_smem(pack_pair_kernel<float>, 32 * (32 * 17 + 2) * 4));
     PIDM_DISPATCH_DTYPE(dtype, (pack_pair_kernel<T><<<n_tiles, 256, smem, (cudaStream_t)stream>>>((const PackPairEntry*)table_dev,
                                                                                                     tile_map_dev, tile_base)));
     PIDM_LAUNCH_CHECK("pack_weights_pairs");

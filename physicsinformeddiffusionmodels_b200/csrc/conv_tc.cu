@@ -415,16 +415,37 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 }
 
 // ---- host side ------------------------------------------------------------------------------------------
-EncodeTiledFn tensor_map_encoder() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
+int tensor_map_encoder(const char* who, EncodeTiledFn* enc) {
+    static thread_local bool ctx_bound = false;
+    if (!ctx_bound) {
+        PIDM_CUDA(cudaFree(0));
+        ctx_bound = true;
+    }
+    static const EncodeTiledFn fn = [] {
         void* p = nullptr;
         cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
+        const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+                        qres == cudaDriverEntryPointSuccess;
+        return ok ? (EncodeTiledFn)p : nullptr;
+    }();
+    PIDM_REQUIRE(fn != nullptr, "%s: cuTensorMapEncodeTiled is not available from the driver", who);
+    *enc = fn;
+    return 0;
+}
+
+int encode_nhwc_map(CUtensorMap* map, const char* who, const void* ptr, int B, int H, int W, int C, int atom, int box_w,
+                    int box_h, int box_n, int elem_stride) {
+    EncodeTiledFn enc;
+    if (int e = tensor_map_encoder(who, &enc)) return e;
+    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+    cuuint32_t box[4] = {(cuuint32_t)atom, (cuuint32_t)box_w, (cuuint32_t)box_h, (cuuint32_t)box_n};
+    cuuint32_t es[4] = {1, (cuuint32_t)elem_stride, (cuuint32_t)elem_stride, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, atom == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    PIDM_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed with %d", who, (int)r);
+    return 0;
 }
 
 // resident weights + operand ring of an n-tile width (TcCfg<BN, *>::OPERAND_BYTES)
@@ -444,17 +465,9 @@ static bool tc_plan(int B, int GH, int GW, int Cin, int Cout, int KH, int KW, in
     pl.rg = (mode == 0 && in_stride == 1 && KH > 1 && KH <= 7 && GW % 8 == 0 && GH % 16 == 0) ? 1 : 0;
     if (pl.rg) {
         pl.TW = 8; pl.TH = 16; pl.TN = 1;
-    } else {
-        if (GW > 128 || GW < 1 || (128 % GW) != 0) return false;
-        pl.TW = GW;
-        int th = 128 / GW;
-        if (th > GH) th = GH;
-        if (GH % th != 0) return false;
-        pl.TH = th;
-        pl.TN = 128 / (pl.TW * pl.TH);
+    } else if (!box_tiling(GH, GW, 128, in_stride, pl.TW, pl.TH, pl.TN)) {
+        return false;
     }
-    if (pl.TW * pl.TH * pl.TN != 128) return false;
-    if (pl.TW * in_stride > 256 || pl.TH * in_stride > 256) return false;      // TMA box limit
     pl.nb = pl.rg ? KH : 1;
     pl.a_bytes = (pl.TH + (pl.rg ? KH - 1 : 0)) * pl.TW * pl.TN * pl.BK * 2;
     const long long K = (long long)KH * KW * Cin;
@@ -484,12 +497,7 @@ static bool tc_plan(int B, int GH, int GW, int Cin, int Cout, int KH, int KW, in
 
 template <int BN, int BK>
 static int launch_tc(const CUtensorMap& mx, const CUtensorMap& mw, const TcParams& p, dim3 grid, cudaStream_t st) {
-    static bool attr = false;
-    if (!attr) {
-        PIDM_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BN, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       TcCfg<BN, BK>::SMEM_BYTES));
-        attr = true;
-    }
+    PIDM_CUDA(allow_smem(conv_tc_kernel<BN, BK>, TcCfg<BN, BK>::SMEM_BYTES));
     const size_t smem = (size_t)p.operand_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + 4 * 4096 /*epilogue staging*/ +
                         TcCfg<BN, BK>::ACC_BYTES;
     PIDM_CUDA(launch_pdl(conv_tc_kernel<BN, BK>, grid, dim3(TC_THREADS), smem, st, mx, mw, p));
@@ -556,40 +564,22 @@ static int tc_run(const void* x, const void* w_packed, const float* bias, const 
     int classes = 1;
     PIDM_REQUIRE(tc_geometry(B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad, transposed, p, pl, classes),
                  "conv2d_tc: unsupported geometry");
-    // cuTensorMapEncodeTiled is a driver-API call: the calling thread (e.g. the autograd worker) may not have the
-    // primary context bound yet if no runtime call has run in it
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        PIDM_CUDA(cudaFree(0));
-        ctx_bound = true;
-    }
-    EncodeTiledFn enc = tensor_map_encoder();
-    PIDM_REQUIRE(enc != nullptr, "conv2d_tc: cuTensorMapEncodeTiled is not available from the driver");
     PIDM_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w_packed & 15) == 0, "conv2d_tc: operands must be 16-byte aligned");
     CUtensorMap mx, mw;
-    const CUtensorMapSwizzle sw = pl.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    const int s = p.in_stride;
+    const int box_h = pl.rg ? pl.TH + KH - 1 : pl.TH * s;
+    if (int e = encode_nhwc_map(&mx, "conv2d_tc", x, B, H, W, Cin, pl.BK, pl.TW * s, box_h, pl.TN, s)) return e;
     {
-        const int s = p.in_stride;
-        cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
-        // with elementStrides = s the box spans boxDim global elements and loads boxDim / s of them
-        const int box_h = pl.rg ? pl.TH + KH - 1 : pl.TH * s;
-        cuuint32_t box[4] = {(cuuint32_t)pl.BK, (cuuint32_t)(pl.TW * s), (cuuint32_t)box_h, (cuuint32_t)pl.TN};
-        cuuint32_t es[4] = {1, (cuuint32_t)s, (cuuint32_t)s, 1};
-        CUresult r = enc(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, es,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        PIDM_REQUIRE(r == CUDA_SUCCESS, "conv2d_tc: cuTensorMapEncodeTiled(x) failed with %d", (int)r);
-    }
-    {
+        EncodeTiledFn enc;
+        if (int e = tensor_map_encoder("conv2d_tc", &enc)) return e;
         const int K = KH * KW * Cin;
         cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)Cout};
         cuuint64_t strides[1] = {(cuuint64_t)K * 2};
         cuuint32_t box[2] = {(cuuint32_t)pl.BK, (cuuint32_t)pl.BN};
         cuuint32_t es[2] = {1, 1};
         CUresult r = enc(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_packed), dims, strides, box, es,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, pl.BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         PIDM_REQUIRE(r == CUDA_SUCCESS, "conv2d_tc: cuTensorMapEncodeTiled(w) failed with %d", (int)r);
     }
     p.bias = bias; p.residual = (const __nv_bfloat16*)residual; p.y = (__nv_bfloat16*)y;

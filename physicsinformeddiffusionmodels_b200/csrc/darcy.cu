@@ -28,8 +28,8 @@ constexpr int P = 64;             // pixels per dim (reference: pixels_per_dim =
 constexpr int PP = P * P;
 constexpr int DARCY_THREADS = 256;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
+// the mbarrier helpers of hopper.cuh: including that header instead changes the code nvcc generates for
+// darcy_grad_kernel<2, true>
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
@@ -739,17 +739,6 @@ static DarcyGeom make_geom(float domain_length, int reverse_d1, int flags) {
     return g;
 }
 
-static int darcy_sm_count(int& sm_count) {
-    static int cached = 0;
-    if (!cached) {
-        int dev = 0;
-        PIDM_CUDA(cudaGetDevice(&dev));
-        PIDM_CUDA(cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev));
-    }
-    sm_count = cached;
-    return 0;
-}
-
 static int check_flags(int flags) {
     PIDM_REQUIRE((flags & ~(PIDM_DARCY_PIXELS_AT_BOUNDARY | PIDM_DARCY_PERIODIC)) == 0,
                  "darcy: unknown flag bits 0x%x (PIDM_DARCY_PIXELS_AT_BOUNDARY = 1, PIDM_DARCY_PERIODIC = 2)", flags);
@@ -761,16 +750,10 @@ static int launch_darcy_fwd(const float* x0hat, const float* fs, float* residual
                             int reverse_d1, int flags, cudaStream_t stream) {
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
-    int sm_count;
-    if (int e = darcy_sm_count(sm_count)) return e;
     const size_t smem = sizeof(DarcySmem);
-    static bool attr_set = false;
-    if (!attr_set) {
-        PIDM_CUDA(cudaFuncSetAttribute(darcy_fwd_kernel<PER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set = true;
-    }
+    PIDM_CUDA(allow_smem(darcy_fwd_kernel<PER>, smem));
     const int ctas_per_sm = (int)(220 * 1024 / smem);        // smem-limited residency
-    int grid = sm_count * (ctas_per_sm > 0 ? ctas_per_sm : 1);
+    int grid = num_sms() * (ctas_per_sm > 0 ? ctas_per_sm : 1);
     if (grid > B) grid = B;
     PIDM_CUDA(launch_plain(darcy_fwd_kernel<PER>, dim3(grid), dim3(DARCY_THREADS), (size_t)(smem), stream, x0hat, fs, residual,
                            B, make_geom(domain_length, reverse_d1, flags)));
@@ -785,16 +768,9 @@ static int launch_darcy_grad(const float* x0hat, const float* fs, const float* c
                              float domain_length, int reverse_d1, int flags, cudaStream_t stream, float inv_norm = 0.f) {
     PIDM_REQUIRE(pixels == P, "darcy kernels are built for %d x %d fields (got %d)", P, P, pixels);
     PIDM_REQUIRE(B > 0, "empty batch");
-    int sm_count;
-    if (int e = darcy_sm_count(sm_count)) return e;
     const size_t smem = sizeof(DarcyGradSmem);
-    static bool attr_set = false;                             // one flag per <MODE, PER> instantiation
-    if (!attr_set) {
-        PIDM_CUDA(cudaFuncSetAttribute(darcy_grad_kernel<MODE, PER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem));
-        attr_set = true;
-    }
-    int grid = sm_count;                                      // 145 KB of shared memory: one CTA of 512 threads per SM
+    PIDM_CUDA(allow_smem(darcy_grad_kernel<MODE, PER>, smem));
+    int grid = num_sms();                                     // 145 KB of shared memory: one CTA of 512 threads per SM
     if (grid > B) grid = B;
     PIDM_CUDA(launch_plain(darcy_grad_kernel<MODE, PER>, dim3(grid), dim3(DG_THREADS), (size_t)(smem), stream, x0hat, fs,
                            cot, grad_x0hat, target, model_out, grad_model_out, t, p2w, pvar, c_data, c_res, sums, B,
@@ -807,11 +783,7 @@ template <bool PER>
 static int launch_darcy_cocogen(float* x, const float* fs, float* residual, const long long* t, int n_active, int steps,
                                 int B, float domain_length, int reverse_d1, int flags, cudaStream_t stream) {
     const size_t smem = sizeof(DarcyCocogenSmem);
-    static bool attr_set = false;                             // one flag per PER instantiation
-    if (!attr_set) {
-        PIDM_CUDA(cudaFuncSetAttribute(darcy_cocogen_kernel<PER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set = true;
-    }
+    PIDM_CUDA(allow_smem(darcy_cocogen_kernel<PER>, smem));
     PIDM_CUDA(launch_plain(darcy_cocogen_kernel<PER>, dim3(B), dim3(DG_THREADS), smem, stream, x, fs, residual, t,
                            n_active, steps, make_geom(domain_length, reverse_d1, flags)));
     PIDM_LAUNCH_CHECK("darcy_cocogen_kernel");

@@ -554,19 +554,13 @@ extern "C" int pidm_darcy_gen_solve(const double* K, const double* f_s, double* 
         dgen::assemble_kernel<<<dim3(dgen::P / 2, B), dgen::ASM_THREADS, 0, st>>>(K, f_s, band, rhs, h0, h1, bc1_sign);
         PIDM_LAUNCH_CHECK("pidm_darcy_gen_solve (assemble)");
     }
-    static bool attr = false;
-    if (!attr) {
-        PIDM_CUDA(cudaFuncSetAttribute(dgen::factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)dgen::FACTOR_SMEM));
-        PIDM_CUDA(cudaFuncSetAttribute(dgen::post_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)dgen::POST_SMEM));
-        attr = true;
-    }
     if (stages & PIDM_DARCY_GEN_FACTOR) {
+        PIDM_CUDA(allow_smem(dgen::factor_kernel, dgen::FACTOR_SMEM));
         dgen::factor_kernel<<<B, dgen::FT, dgen::FACTOR_SMEM, st>>>(band, rhs);
         PIDM_LAUNCH_CHECK("pidm_darcy_gen_solve (factor)");
     }
     if (stages & PIDM_DARCY_GEN_POST) {
+        PIDM_CUDA(allow_smem(dgen::post_kernel, dgen::POST_SMEM));
         dgen::post_kernel<<<B, dgen::POST_THREADS, dgen::POST_SMEM, st>>>(band, rhs, K, f_s, p, res, batch, h0, h1,
                                                                          pab ? 1 : 0);
         PIDM_LAUNCH_CHECK("pidm_darcy_gen_solve (post)");

@@ -282,11 +282,6 @@ __global__ void ddim_coefs_kernel(const long long* __restrict__ t, const long lo
 //      evaluated from the fp32 cond [B,HW,2] directly instead of as a channel-padded GEMM.  Thread layout: (pixel row,
 //      channel octet); a thread writes 8 channels of one pixel (16 bytes in bf16).  Samples in null_mask take cond = 0:
 //      their pre-activation is b0 exactly.
-__device__ __forceinline__ float gelu_erf_f(float z) { return z * 0.5f * (1.f + erff(z * 0.70710678118654752f)); }
-__device__ __forceinline__ float gelu_erf_grad_f(float z) {
-    return 0.5f * (1.f + erff(z * 0.70710678118654752f)) + z * 0.3989422804014327f * expf(-0.5f * z * z);
-}
-
 __device__ __forceinline__ float2 cond_at(const float* __restrict__ cond, const unsigned char* __restrict__ null_mask,
                                           int m, int HW) {
     if (null_mask != nullptr && null_mask[m / HW]) return make_float2(0.f, 0.f);

@@ -1,12 +1,11 @@
 // Hopper (sm_90a) building blocks of the tensor-core convolution kernels (conv_tc.cu, wgrad_tc.cu, wgrad_tc3.cu):
-// mbarrier ring plumbing, TMA tensor loads, wgmma shared-memory descriptors and the warpgroup MMA itself.
+// mbarrier ring plumbing, TMA tensor loads, wgmma shared-memory descriptors and the warpgroup MMA itself; on the host,
+// the activation tensor maps and the pixel tiling those kernels share.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
 
 namespace pidm {
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -121,7 +120,40 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t da, uint64_t
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda); nullptr if unavailable
-EncodeTiledFn tensor_map_encoder();
+// cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda).  It is a driver-API call:
+// the primary context is bound to the calling thread first, since that thread (e.g. the autograd worker) may not have
+// run a runtime call yet.  Returns 0, or an error code through set_error naming `who`.
+int tensor_map_encoder(const char* who, EncodeTiledFn* enc);
+
+// Tensor map of a bf16 NHWC activation [B, H, W, C], box {atom, box_w, box_h, box_n} with element stride
+// `elem_stride` on W and H (a strided box spans box_w x box_h elements and loads every elem_stride-th).  128-byte
+// swizzle for a 64-channel atom, 64-byte for a 32-channel one.
+int encode_nhwc_map(CUtensorMap* map, const char* who, const void* ptr, int B, int H, int W, int C, int atom, int box_w,
+                    int box_h, int box_n, int elem_stride);
+
+// Cut a GH x GW pixel grid into tiles of px pixels: TW = GW (whole rows), TH = min(px / GW, GH) rows, and TN samples
+// when one tile holds whole images.  False when such tiles do not cover the grid exactly or a tile side spans more
+// than the 256-element TMA box limit at element stride elem_stride.
+static inline bool box_tiling(int GH, int GW, int px, int elem_stride, int& TW, int& TH, int& TN) {
+    if (GW > px || GW < 1 || px % GW != 0) return false;
+    TW = GW;
+    TH = px / GW < GH ? px / GW : GH;
+    if (GH % TH != 0) return false;
+    TN = px / (TW * TH);
+    if (TW * TH * TN != px) return false;
+    return TW * elem_stride <= 256 && TH * elem_stride <= 256;
+}
+
+// Split n_pix_tiles pixel tiles into contiguous ranges so that `ctas` CTAs per range make one wave (one CTA per SM:
+// the ring takes the shared memory); fewer, longer CTAs also mean fewer reductions of partial tiles.  Returns the
+// tiles per range and sets `splits` to the number of ranges.
+static inline int one_wave_split(int n_pix_tiles, int ctas, int& splits) {
+    int s = num_sms() / ctas;
+    if (s > n_pix_tiles) s = n_pix_tiles;
+    if (s < 1) s = 1;
+    const int per = (n_pix_tiles + s - 1) / s;
+    splits = (n_pix_tiles + per - 1) / per;
+    return per;
+}
 
 }  // namespace pidm

@@ -8,11 +8,6 @@
 
 namespace pidm {
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
-__device__ __forceinline__ float gelu_erf_grad(float x) {
-    return 0.5f * (1.f + erff(x * 0.70710678118654752f)) + x * 0.3989422804014327f * expf(-0.5f * x * x);
-}
-
 // one CTA per sample, blockDim = td
 __global__ void time_embed_fwd_kernel(const long long* __restrict__ t, const float* __restrict__ W1,
                                       const float* __restrict__ b1, const float* __restrict__ W2,
@@ -51,7 +46,7 @@ __global__ void time_embed_fwd_kernel(const long long* __restrict__ t, const flo
         acc += (a0 + a1_) + (a2 + a3);
     }
     h1[(size_t)b * td + j] = acc;
-    a1[j] = gelu_erf(acc);
+    a1[j] = gelu_erf_f(acc);
     __syncthreads();
     float o = b2[j];
     {
@@ -86,7 +81,7 @@ __global__ void time_embed_bwd_act_kernel(const float* __restrict__ d_silu, cons
     float da = 0.f;
 #pragma unroll 32
     for (int i = 0; i < td; ++i) da += dt[i] * __ldg(W2 + (size_t)i * td + j);
-    dh_out[(size_t)b * td + j] = da * gelu_erf_grad(h1[(size_t)b * td + j]);
+    dh_out[(size_t)b * td + j] = da * gelu_erf_grad_f(h1[(size_t)b * td + j]);
 }
 
 // backward, stage 2 (one CTA per output row j, blockDim = td = columns k): the weight gradients are small
@@ -103,7 +98,7 @@ __global__ void time_embed_bwd_wgrad_kernel(const float* __restrict__ dt, const 
     float w2 = 0.f, w1 = 0.f, s2 = 0.f, s1 = 0.f;
     for (int b = 0; b < B; ++b) {
         const float dtj = dt[(size_t)b * td + j], dhj = dh[(size_t)b * td + j];      // broadcast loads
-        w2 += dtj * gelu_erf(h1[(size_t)b * td + k]);
+        w2 += dtj * gelu_erf_f(h1[(size_t)b * td + k]);
         if (k < dim) w1 += dhj * emb[(size_t)b * dim + k];
         s2 += dtj; s1 += dhj;
     }
@@ -320,22 +315,12 @@ extern "C" int pidm_time_embed_bwd(const float* d_silu_t, const float* emb, cons
 
 extern "C" int pidm_mlp_entry_size(void) { return (int)sizeof(MlpEntry); }
 
-static int mlp_smem_attr(size_t bytes) {
-    static bool done = false;
-    if (!done && bytes > 48 * 1024) {
-        PIDM_CUDA(cudaFuncSetAttribute(block_mlps_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        PIDM_CUDA(cudaFuncSetAttribute(block_mlps_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        done = true;
-    }
-    return 0;
-}
-
 extern "C" int pidm_block_mlps_fwd(const void* table_dev, int n_entries, int max_rows, const float* silu_t, int B,
                                    int td, void* stream) {
     PIDM_REQUIRE(td <= MLP_TD_MAX && td % 32 == 0, "block_mlps: td must be a multiple of 32, <= %d", MLP_TD_MAX);
     size_t smem = (size_t)MLP_BCHUNK * (td + 1) * sizeof(float);
-    if (int e = mlp_smem_attr(smem)) return e;
     dim3 grid(n_entries, ceil_div(max_rows, MLP_ROWS));
+    PIDM_CUDA(allow_smem(block_mlps_fwd_kernel, 96 * 1024));
     PIDM_CUDA(launch_plain(block_mlps_fwd_kernel, dim3(grid), dim3(256), (size_t)(smem), (cudaStream_t)stream, (const MlpEntry*)table_dev, silu_t, B, td));
     PIDM_LAUNCH_CHECK("block_mlps_fwd");
     return 0;
@@ -349,9 +334,9 @@ extern "C" int pidm_block_mlps_bwd(const void* table_dev, int n_entries, int max
     PIDM_REQUIRE(td <= MLP_TD_MAX && td % 32 == 0, "block_mlps: td must be a multiple of 32, <= %d", MLP_TD_MAX);
     cudaStream_t st = (cudaStream_t)stream;
     size_t smem = (size_t)MLP_BCHUNK * (td + 1) * sizeof(float);
-    if (int e = mlp_smem_attr(smem)) return e;
     if (parts & 1) {
         dim3 grid(n_entries, ceil_div(max_rows, MLP_ROWS));
+        PIDM_CUDA(allow_smem(block_mlps_wgrad_kernel, 96 * 1024));
         PIDM_CUDA(launch_plain(block_mlps_wgrad_kernel, dim3(grid), dim3(256), (size_t)(smem), st, (const MlpEntry*)table_dev, silu_t, B, td));
     }
     if (parts & 2) {

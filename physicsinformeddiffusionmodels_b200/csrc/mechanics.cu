@@ -603,7 +603,7 @@ extern "C" int pidm_mech_fem_pcg(const float* rho, const float* bcs, const float
     PIDM_CUDA(cudaGetSymbolAddress(&kd, g_KEd));
     PIDM_CUDA(cudaMemcpyToSymbolAsync(c_KEd, kd, 64 * sizeof(double), 0, cudaMemcpyDeviceToDevice, st));
     const size_t smem = (size_t)(4 * nn * nn + 4 * (PCG_THREADS / 32)) * sizeof(double) + (size_t)nel * nel * sizeof(float);
-    PIDM_CUDA(cudaFuncSetAttribute(mech_pcg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PIDM_CUDA(allow_smem(mech_pcg_kernel, smem));
     mech_pcg_kernel<<<B, PCG_THREADS, smem, st>>>(rho, bcs, u, iters, relres, tol, max_iter, nel);
     PIDM_LAUNCH_CHECK("mech_fem_pcg");
     return 0;
@@ -612,7 +612,7 @@ extern "C" int pidm_mech_fem_pcg(const float* rho, const float* bcs, const float
 extern "C" int pidm_mech_floating_material(const float* rho, long long* fm, int B, int nel, void* stream) {
     PIDM_REQUIRE(B > 0 && nel >= 1 && nel <= 128, "mech_floating_material: 1 <= nel <= 128 required (B=%d nel=%d)", B, nel);
     const size_t smem = (size_t)nel * nel * sizeof(int);
-    PIDM_CUDA(cudaFuncSetAttribute(mech_fm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PIDM_CUDA(allow_smem(mech_fm_kernel, smem));
     mech_fm_kernel<<<B, 1024, smem, (cudaStream_t)stream>>>(rho, fm, nel);
     PIDM_LAUNCH_CHECK("mech_floating_material");
     return 0;

@@ -1,5 +1,5 @@
 // Warp-level tensor-core helpers shared by the linear-attention kernels (attention_mma.cu, attention_fused.cu):
-// mma.sync m16n8k16 bf16, ldmatrix fragment loaders, per-warp cp.async tile movers.
+// mma.sync m16n8k16 bf16, ldmatrix fragment loaders, per-warp cp.async tile movers, and their pixel chunking.
 #pragma once
 #include "common.cuh"
 
@@ -11,7 +11,17 @@ constexpr int LM_PITCH = LM_HID + 8;          // bf16 elements per smem row (528
 constexpr int LM_CPITCH = LM_D + 8;           // ctx rows [d][e] in bf16
 constexpr int LM_CHUNK = 256;                 // pixels per CTA
 
-__device__ __forceinline__ uint32_t lm_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// pixels per CTA: about ctas_per_sm CTAs per SM over the whole batch, a multiple of 32, never more than the image.
+// Chunks are per sample: k chunks per sample with B * k <= resident CTA slots (one wave), 32-pixel granularity.
+static inline int chunk_px(int B, int N, int ctas_per_sm) {
+    int k = (num_sms() * ctas_per_sm) / B;
+    if (k < 1) k = 1;
+    int px = ((N + k - 1) / k + 31) / 32 * 32;
+    if (px < 64) px = 64;
+    if (px > N) px = N;
+    return px;
+}
+
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
@@ -37,29 +47,29 @@ __device__ __forceinline__ void st8_smem(__nv_bfloat16* p, const float v[8]) {
 // A fragment (16 rows x 16 k) from a row-major smem tile S[row][col]: rows = M index, cols = K index
 __device__ __forceinline__ void frag_a_rowmajor(uint32_t (&a)[4], const __nv_bfloat16* S, int pitch, int m0, int k0, int lane) {
     const int mi = lane >> 3, r = lane & 7;
-    ldsm_x4(a, lm_smem(S + (size_t)(m0 + r + 8 * (mi & 1)) * pitch + k0 + 8 * (mi >> 1)));
+    ldsm_x4(a, smem_u32(S + (size_t)(m0 + r + 8 * (mi & 1)) * pitch + k0 + 8 * (mi >> 1)));
 }
 // A fragment when smem holds the transpose: S[k][m] (rows = K index, cols = M index)
 __device__ __forceinline__ void frag_a_kmajor(uint32_t (&a)[4], const __nv_bfloat16* S, int pitch, int k0, int m0, int lane) {
     const int mi = lane >> 3, r = lane & 7;
-    ldsm_x4_t(a, lm_smem(S + (size_t)(k0 + r + 8 * (mi >> 1)) * pitch + m0 + 8 * (mi & 1)));
+    ldsm_x4_t(a, smem_u32(S + (size_t)(k0 + r + 8 * (mi >> 1)) * pitch + m0 + 8 * (mi & 1)));
 }
 // B fragments of TWO adjacent n-tiles (n0..n0+15) for one k16 step, from S[k][n] (rows = K index): b[0..1] tile 0, b[2..3] tile 1
 __device__ __forceinline__ void frag_b_krows(uint32_t (&b)[4], const __nv_bfloat16* S, int pitch, int k0, int n0, int lane) {
     const int mi = lane >> 3, r = lane & 7;
-    ldsm_x4_t(b, lm_smem(S + (size_t)(k0 + r + 8 * (mi & 1)) * pitch + n0 + 8 * (mi >> 1)));
+    ldsm_x4_t(b, smem_u32(S + (size_t)(k0 + r + 8 * (mi & 1)) * pitch + n0 + 8 * (mi >> 1)));
 }
 // same from S[n][k] (rows = N index, cols = K index)
 __device__ __forceinline__ void frag_b_nrows(uint32_t (&b)[4], const __nv_bfloat16* S, int pitch, int n0, int k0, int lane) {
     const int mi = lane >> 3, r = lane & 7;
-    ldsm_x4(b, lm_smem(S + (size_t)(n0 + r + 8 * (mi >> 1)) * pitch + k0 + 8 * (mi & 1)));
+    ldsm_x4(b, smem_u32(S + (size_t)(n0 + r + 8 * (mi >> 1)) * pitch + k0 + 8 * (mi & 1)));
 }
 
 constexpr int LW_PITCH = LM_D + 8;            // bf16 per smem row of a head tile: 80 B -> conflict-free ldmatrix / row access
 constexpr int LW_TILE = 32 * LW_PITCH;        // one [32 px][32 ch] tile
 
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(lm_smem(dst)), "l"(src) : "memory");
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int PENDING>

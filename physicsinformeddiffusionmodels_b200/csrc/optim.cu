@@ -2,10 +2,12 @@
 //   global-norm clip (torch.nn.utils.clip_grad_norm_(params, 1.0), main.py:165)
 //   Adam(lr, betas=(0.9,0.999), eps=1e-8)                          (main.py:143,166)
 //   EMA shadow update mu=0.99                                       (denoising_utils.py:174-177, main.py:178-179)
-// and the error plumbing shared by all translation units.
+// and the host plumbing (errors, SM count, shared-memory opt-in) shared by all translation units.
 #include "common.cuh"
 #include "pidm.h"
 #include <stdarg.h>
+#include <mutex>
+#include <unordered_map>
 
 namespace pidm {
 
@@ -19,6 +21,17 @@ int num_sms() {
             n = 132;
     }
     return n;
+}
+
+cudaError_t allow_smem(const void* kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::unordered_map<const void*, size_t> allowed;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& cur = allowed[kernel];
+    if (bytes <= cur) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) cur = bytes;
+    return e;
 }
 
 int set_error(int code, const char* fmt, ...) {

@@ -188,47 +188,19 @@ struct WgPlan { int TW, TH, TN, NP, AA, AB; };
 
 // GH x GW: pixel grid of the reduction (the B-side tensor's spatial size); the A side is sampled at a_stride*g-pad+tap
 static bool wg_plan(int B, int GH, int GW, int CA, int CB, int a_stride, WgPlan& pl) {
-    if (GW > 128 || GW < 1 || (128 % GW) != 0) return false;
     if (CA % 32 != 0 || CB % 32 != 0) return false;
     if (a_stride != 1 && a_stride != 2) return false;
-    pl.TW = GW;
-    int th = 128 / GW;
-    if (th > GH) th = GH;
-    if (GH % th != 0) return false;
-    pl.TH = th;
-    pl.TN = 128 / (pl.TW * pl.TH);
-    if (pl.TW * pl.TH * pl.TN != 128) return false;
-    if (pl.TW * a_stride > 256 || pl.TH * a_stride > 256) return false;
+    if (!box_tiling(GH, GW, 128, a_stride, pl.TW, pl.TH, pl.TN)) return false;
     pl.AA = (CA % 64 == 0) ? 64 : 32;
     pl.AB = (CB % 64 == 0) ? 64 : 32;
     pl.NP = (CB % 128 == 0) ? 128 : ((CB % 64 == 0) ? 64 : 32);
     return true;
 }
 
-static int wg_encode(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int atom, int TW, int TH, int TN,
-                     int es_) {
-    EncodeTiledFn enc = tensor_map_encoder();
-    PIDM_REQUIRE(enc != nullptr, "wgrad_tc: cuTensorMapEncodeTiled is not available from the driver");
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)atom, (cuuint32_t)(TW * es_), (cuuint32_t)(TH * es_), (cuuint32_t)TN};
-    cuuint32_t es[4] = {1, (cuuint32_t)es_, (cuuint32_t)es_, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, atom == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PIDM_REQUIRE(r == CUDA_SUCCESS, "wgrad_tc: cuTensorMapEncodeTiled failed with %d", (int)r);
-    return 0;
-}
-
 template <int NP, int AA, int AB>
 static int wg_launch(const CUtensorMap& mx, const CUtensorMap& my, const WgParams& p, dim3 grid, cudaStream_t st) {
     using Cfg = WgCfg<NP, AA, AB>;
-    static bool attr = false;
-    if (!attr) {
-        PIDM_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<NP, AA, AB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       Cfg::SMEM_BYTES));
-        attr = true;
-    }
+    PIDM_CUDA(allow_smem(wgrad_tc_kernel<NP, AA, AB>, Cfg::SMEM_BYTES));
     PIDM_CUDA(launch_pdl(wgrad_tc_kernel<NP, AA, AB>, grid, dim3(WG_THREADS), Cfg::SMEM_BYTES, st, mx, my, p));
     PIDM_LAUNCH_CHECK("conv2d_wgrad_tc");
     return 0;
@@ -251,13 +223,8 @@ static bool wg_geometry(int B, int GH, int GW, int CA, int CB, int KH, int KW, i
     const int n_pairs = KH * KW * (CA / pl.AA);
     const int m_tiles = (n_pairs + na - 1) / na;
     const int n_tiles = CB / pl.NP;
-    // split the pixel range so that the grid is one wave (one CTA per SM: the ring takes the shared memory); fewer,
-    // longer CTAs also mean fewer red.global.add of partial tiles
-    int splits = num_sms() / (m_tiles * n_tiles);
-    if (splits > p.n_pix_tiles) splits = p.n_pix_tiles;
-    if (splits < 1) splits = 1;
-    p.tiles_per_split = (p.n_pix_tiles + splits - 1) / splits;
-    splits = (p.n_pix_tiles + p.tiles_per_split - 1) / p.tiles_per_split;
+    int splits;
+    p.tiles_per_split = one_wave_split(p.n_pix_tiles, m_tiles * n_tiles, splits);
     grid = dim3(m_tiles, n_tiles, splits);
     return true;
 }
@@ -300,15 +267,12 @@ extern "C" int pidm_conv2d_wgrad_tc(const void* a, const void* b, float* dw, int
     WgParams p;
     dim3 grid;
     PIDM_REQUIRE(wg_geometry(B, GH, GW, CA, CB, KH, KW, a_stride, pl, p, grid), "conv2d_wgrad_tc: unsupported geometry");
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        PIDM_CUDA(cudaFree(0));
-        ctx_bound = true;
-    }
     cudaStream_t st = (cudaStream_t)stream;
     CUtensorMap mx, my;
-    if (int e = wg_encode(&mx, a, B, HA, WA, CA, pl.AA, pl.TW, pl.TH, pl.TN, a_stride)) return e;
-    if (int e = wg_encode(&my, b, B, GH, GW, CB, pl.AB, pl.TW, pl.TH, pl.TN, 1)) return e;
+    if (int e = encode_nhwc_map(&mx, "wgrad_tc", a, B, HA, WA, CA, pl.AA, pl.TW * a_stride, pl.TH * a_stride, pl.TN,
+                                a_stride))
+        return e;
+    if (int e = encode_nhwc_map(&my, "wgrad_tc", b, B, GH, GW, CB, pl.AB, pl.TW, pl.TH, pl.TN, 1)) return e;
     p.B = B; p.Cin = CA; p.Cout = CB; p.c_real = CA_real; p.KH = KH; p.KW = KW; p.pad = pad; p.a_stride = a_stride;
     p.dw = dw; p.s_row = s_row; p.s_col = s_col;
 #define WG_CASE(np, aa, ab) if (pl.NP == np && pl.AA == aa && pl.AB == ab) return wg_launch<np, aa, ab>(mx, my, p, grid, st)

@@ -180,29 +180,10 @@ __global__ void __launch_bounds__(W3_THREADS, 1) wgrad3_kernel(const __grid_cons
     }
 }
 
-static int w3_encode(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int atom, int bw, int bh, int bn) {
-    EncodeTiledFn enc = tensor_map_encoder();
-    PIDM_REQUIRE(enc != nullptr, "wgrad3: cuTensorMapEncodeTiled is not available from the driver");
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)atom, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, atom == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    PIDM_REQUIRE(r == CUDA_SUCCESS, "wgrad3: cuTensorMapEncodeTiled failed with %d", (int)r);
-    return 0;
-}
-
 template <int NP, int AB, bool RG>
 static int w3_launch(const CUtensorMap& mx, const CUtensorMap& my, const W3Params& p, dim3 grid, cudaStream_t st) {
     using Cfg = W3Cfg<NP, AB, RG>;
-    static bool attr = false;
-    if (!attr) {
-        PIDM_CUDA(cudaFuncSetAttribute(wgrad3_kernel<NP, AB, RG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       Cfg::SMEM_BYTES));
-        attr = true;
-    }
+    PIDM_CUDA(allow_smem(wgrad3_kernel<NP, AB, RG>, Cfg::SMEM_BYTES));
     PIDM_CUDA(launch_pdl(wgrad3_kernel<NP, AB, RG>, grid, dim3(W3_THREADS), Cfg::SMEM_BYTES, st, mx, my, p));
     PIDM_LAUNCH_CHECK("conv2d_wgrad_tc(3x3)");
     return 0;
@@ -218,11 +199,8 @@ bool wgrad3_supported(int B, int HA, int WA, int CA, int CA_real, int GH, int GW
     const bool halo = pad == 0 && HA == GH + 2 && WA == GW + 2;
     if (CA % 32 != 0 || CA_real != CA || CB % 32 != 0 || !(same || halo)) return false;
     if (GW % 8 == 0 && GH % 16 == 0) return true;                       // RG
-    if (GW > 64 || 64 % GW != 0) return false;
-    const int th = 64 / GW;
-    if (th <= GH) return GH % th == 0;
-    const int tn = 64 / (GW * GH);
-    return GW * GH * tn == 64 && B % tn == 0;
+    int TW, TH, TN;
+    return box_tiling(GH, GW, 64, 1, TW, TH, TN) && B % TN == 0;
 }
 
 // tile plan and launch grid of a supported call
@@ -230,23 +208,14 @@ static void w3_geometry(int B, int GH, int GW, int CA, int CB, W3Params& p, bool
     rg = (GW % 8 == 0 && GH % 16 == 0);
     p.B = B;
     if (rg) { p.TW = 8; p.TH = 16; p.TN = 1; }
-    else {
-        p.TW = GW;
-        int th = 64 / GW;
-        if (th > GH) th = GH;
-        p.TH = th;
-        p.TN = 64 / (p.TW * p.TH);
-    }
+    else box_tiling(GH, GW, 64, 1, p.TW, p.TH, p.TN);      // true: wgrad3_supported
     p.tiles_h = GH / p.TH; p.tiles_w = GW / p.TW;
     p.n_pix_tiles = (B / p.TN) * p.tiles_h * p.tiles_w;
     NP = (CB % 64 == 0) ? 64 : 32;          // 3 x NP / 2 accumulator registers per consumer thread
     AB = (CB % 64 == 0) ? 64 : 32;
     const int chunks = CA / 32, n_tiles = CB / NP;
-    int splits = num_sms() / (chunks * n_tiles);
-    if (splits > p.n_pix_tiles) splits = p.n_pix_tiles;
-    if (splits < 1) splits = 1;
-    p.tiles_per_split = (p.n_pix_tiles + splits - 1) / splits;
-    splits = (p.n_pix_tiles + p.tiles_per_split - 1) / p.tiles_per_split;
+    int splits;
+    p.tiles_per_split = one_wave_split(p.n_pix_tiles, chunks * n_tiles, splits);
     grid = dim3(chunks, n_tiles, splits);
 }
 
@@ -261,11 +230,6 @@ void wgrad3_geometry(int B, int GH, int GW, int CA, int CB, int* plan) {
 
 int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, int CA, int GH, int GW, int CB, int pad,
                long long s_col, cudaStream_t st) {
-    static thread_local bool ctx_bound = false;
-    if (!ctx_bound) {
-        PIDM_CUDA(cudaFree(0));
-        ctx_bound = true;
-    }
     W3Params p;
     bool rg;
     int NP, AB;
@@ -274,8 +238,8 @@ int wgrad3_run(const void* a, const void* b, float* dw, int B, int HA, int WA, i
     p.pad = pad;
     p.dw = dw; p.s_col = s_col;
     CUtensorMap mx, my;
-    if (int e = w3_encode(&mx, a, B, HA, WA, CA, 32, p.TW, rg ? p.TH + 3 : p.TH, p.TN)) return e;
-    if (int e = w3_encode(&my, b, B, GH, GW, CB, AB, p.TW, p.TH, p.TN)) return e;
+    if (int e = encode_nhwc_map(&mx, "wgrad3", a, B, HA, WA, CA, 32, p.TW, rg ? p.TH + 3 : p.TH, p.TN, 1)) return e;
+    if (int e = encode_nhwc_map(&my, "wgrad3", b, B, GH, GW, CB, AB, p.TW, p.TH, p.TN, 1)) return e;
 #define W3_CASE(np, ab) \
     if (NP == np && AB == ab) return rg ? w3_launch<np, ab, true>(mx, my, p, grid, st) : w3_launch<np, ab, false>(mx, my, p, grid, st)
     W3_CASE(64, 64); W3_CASE(32, 32);
