@@ -127,10 +127,8 @@ int pidm_darcy_gen_solve(const double* K, const double* f_s, double* p, double* 
                          int stages, void* stream);
 
 /* ---- layout ------------------------------------------------------------------------------------------- */
-/* image_to_b_xy_c / b_xy_c_to_image (src/denoising_utils.py:36-55) fused with the dtype change + channel padding */
+/* image_to_b_xy_c (src/denoising_utils.py:36-42) fused with the dtype change + channel padding */
 int pidm_nchw_to_nhwc(const float* src, void* dst, int B, int C, int HW, int Cpad, int dtype, void* stream);
-int pidm_nhwc_to_nchw(const void* src, float* dst, int B, int C, int HW, int Cpad, int dtype, void* stream);
-int pidm_add(const void* a, const void* b, void* out, long long n, int dtype, void* stream);
 /* emb_conv[0] + GELU of the residual-gradient guidance branch (src/unet_model.py:520-524,585-603):
  * out[b,hw,:] = GELU_erf(W0 cond[b,hw,:] + b0) as NHWC activations [B,HW,C] (dtype), cond [B,HW,2] fp32, W0 [C,2], b0 [C]
  * fp32.  null_mask [B] (bool bytes, may be NULL = none): those samples take cond = 0 (cond is not read), i.e. GELU(b0).

@@ -337,7 +337,7 @@ def darcy_fixtures(out):
     cocogen_fixture(out, 'cocogen.pt', res, x0p)
     loss_fixture(out, 'darcy_loss_mean.pt', model, res, DARCY_LOSS_KEYS, nograd_name='params_without_grad.txt')
 
-    # sample-mode loss (A12: ddim_sample_x0, ddim_steps=0)
+    # sample-mode loss (A12: ddim_sample_x0, ddim_steps=0) and the DDIM walk at ddim_steps = 1, 3
     x0 = smooth_fields(2, seed=9)
     loss_s, data_s, res_abs_s = darcy_loss(x0, darcy_residuals(model, use_ddim_x0=True, ddim_steps=0), 321)
     t_s, e_s = loss_draws(321, x0)
@@ -345,7 +345,8 @@ def darcy_fixtures(out):
     save(out, 'darcy_loss_sample.pt', dict(x0=x0, t=t_s, noise=e_s, loss=loss_s.detach(), data_loss=torch.tensor(data_s),
                                            residual_abs=torch.tensor(res_abs_s),
                                            grad_final_w=named['final_conv.1.weight'].grad.clone(),
-                                           grad_init_w=named['init_conv.weight'].grad.clone()))
+                                           grad_init_w=named['init_conv.weight'].grad.clone(),
+                                           **ddim_walk_keys(model)))
 
     guidance_fixture(out, 'darcy_guidance.pt', model, 'none',
                      dict(grad_emb0='emb_conv.0.weight', grad_combine='combine_conv.weight',
@@ -692,6 +693,31 @@ def darcy_gen_fixtures(out):
     save(out, 'darcy_gen.pt', dict(eigenvalues=t(eigenvalues), f_s=t(f_s), int_cond=t(int_cond).reshape(-1),
                                    seed=torch.tensor(fx['seed'], dtype=torch.int64), z=t(fx['z']), K=t(fx['K']),
                                    p=t(fx['p']), res=t(fx['res'])))
+
+
+DDIM_WALK = dict(n_steps=100, t=(0, 2, 57, 99), seed=13, sample=4096)
+
+
+def ddim_walk_input():
+    """x_t [4,2,64,64] of the DDIM walk in darcy_loss_sample.pt, regenerated from its seed (the fixture keeps its
+    checksum)"""
+    return torch.randn(len(DDIM_WALK['t']), 2, 64, 64, generator=torch.Generator().manual_seed(DDIM_WALK['seed']))
+
+
+def ddim_walk_keys(model):
+    """the walk_* keys of darcy_loss_sample.pt: the reference's DenoisingDiffusion.ddim_sample_x0 (eta = 0) on the Darcy
+    test model for ddim_steps = 1 and 3 at per-sample t = 0, 2 (the grids repeat points: linspace(0, 2, 5) -> 0, 0, 1,
+    1, 2), 57 and n_steps - 1; golden_sample(cur_x) and golden_sample(model_out) per ddim_steps"""
+    diff = diffusion(DDIM_WALK['n_steps'])
+    xt = ddim_walk_input()
+    t = torch.tensor(DDIM_WALK['t'])
+    fx = dict(walk_t=t, walk_seed=torch.tensor(DDIM_WALK['seed']), walk_x_t_checksum=xt.double().sum())
+    with torch.no_grad():
+        for s in (1, 3):
+            cur_x, model_out = diff.ddim_sample_x0(xt, t, model, xt.shape, s, 0.)
+            fx[f'walk_cur_x_{s}'] = O.golden_sample(cur_x, DDIM_WALK['sample'])
+            fx[f'walk_model_out_{s}'] = O.golden_sample(model_out, DDIM_WALK['sample'])
+    return fx
 
 
 # family -> (recipe, the files under tests/golden/ it writes)

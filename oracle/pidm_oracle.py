@@ -22,6 +22,7 @@ defaults run the reference's default path.
 import math
 from collections import OrderedDict
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -641,7 +642,9 @@ def ddim_x0(sd, cfg, xt, t, tables, ddim_steps=0, mechanics=False):
     dt = xt.dtype
     seqs, seqs_next = [], []
     for ti in t.tolist():
-        seq = [int(v) for v in torch.linspace(0, ti, ddim_steps + 2, dtype=torch.float64).tolist()]
+        # np.linspace as the reference: torch.linspace rounds some points differently (t = 58, ddim_steps = 13 gives 28
+        # where numpy's int() gives 29)
+        seq = [int(v) for v in np.linspace(0, ti, ddim_steps + 2, endpoint=True, dtype=float)]
         seqs.append(list(reversed(seq)))
         seqs_next.append(list(reversed([-1] + seq[:-1])))
     cur_t = torch.tensor(seqs).T

@@ -33,8 +33,6 @@ _SIGS = {
     'pidm_darcy_abs_residual_grad': [P, P, P, I, L, I, F, I, I, P],
     'pidm_darcy_pidm_loss': [P, P, P, P, P, P, P, F, F, P, P, P, I, I, F, I, I, P],
     'pidm_nchw_to_nhwc': [P, P, I, I, I, I, I, P],
-    'pidm_nhwc_to_nchw': [P, P, I, I, I, I, I, P],
-    'pidm_add': [P, P, P, L, I, P],
     'pidm_cond_embed_fwd': [P, P, P, P, P, I, I, I, I, P],
     'pidm_cond_embed_wgrad': [P, P, P, P, P, P, P, I, I, I, I, P],
     'pidm_concat_channels': [P, P, P, L, I, I, I, P],

@@ -1,5 +1,5 @@
-// HBM-bound element-wise pieces of the PIDM step: q_sample, ancestral posterior step, layout changes
-// (NCHW fp32 <-> NHWC activations), channel concat/split, residual add, and the tiny-N output head
+// HBM-bound element-wise pieces of the PIDM step: q_sample, ancestral posterior step, layout change
+// (NCHW fp32 -> NHWC activations), channel concat/split, and the tiny-N output head
 // (final 1x1 conv -> NCHW fp32, optional sigmoid on the last channel).  128-bit vectorised accesses.
 #include "common.cuh"
 #include "pidm.h"
@@ -89,36 +89,8 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, T* __restrict
         }
     }
 }
-template <typename T>
-__global__ void nhwc_to_nchw_kernel(const T* __restrict__ src, float* __restrict__ dst, int C, int HW, int Cpad,
-                                    long long total) {
-    pdl_trigger();
-    pdl_wait();  // total = B*C*HW
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        int hw = (int)(i % HW);
-        long long bc = i / HW;
-        int c = (int)(bc % C);
-        long long b = bc / C;
-        dst[i] = Act<T>::ld(src + (b * HW + hw) * Cpad + c);
-    }
-}
 
-// ---- add, concat, split along channels (NHWC rows) ------------------------------------------------------
-template <typename T>
-__global__ void add_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ o, long long n8) {
-    pdl_trigger();
-    pdl_wait();
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8;
-         i += (long long)gridDim.x * blockDim.x) {
-        float x[8], y[8];
-        ld8(a + i * 8, x);
-        ld8(b + i * 8, y);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) x[k] += y[k];
-        st8(o + i * 8, x);
-    }
-}
+// ---- concat, split along channels (NHWC rows) ----------------------------------------------------------
 // out[m, 0:Ca] = a[m], out[m, Ca:Ca+Cb] = b[m]   (channels multiples of 8)
 template <typename T>
 __global__ void concat_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ o, int Ca8, int Cb8,
@@ -579,20 +551,6 @@ extern "C" int pidm_nchw_to_nhwc(const float* src, void* dst, int B, int C, int 
     long long n_pix = (long long)B * HW;
     PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(nchw_to_nhwc_kernel<T>, dim3(grid_for(n_pix, 128)), dim3(128), (size_t)(0), (cudaStream_t)stream, src, (T*)dst, C, HW, Cpad, n_pix)));
     PIDM_LAUNCH_CHECK("nchw_to_nhwc");
-    return 0;
-}
-
-extern "C" int pidm_nhwc_to_nchw(const void* src, float* dst, int B, int C, int HW, int Cpad, int dtype, void* stream) {
-    long long total = (long long)B * HW * C;
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(nhwc_to_nchw_kernel<T>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)src, dst, C, HW, Cpad, total)));
-    PIDM_LAUNCH_CHECK("nhwc_to_nchw");
-    return 0;
-}
-
-extern "C" int pidm_add(const void* a, const void* b, void* out, long long n, int dtype, void* stream) {
-    PIDM_REQUIRE(n % 8 == 0, "add: size must be a multiple of 8");
-    PIDM_DISPATCH_DTYPE(dtype, PIDM_CUDA(launch_plain(add_kernel<T>, dim3(grid_for(n / 8, 256)), dim3(256), (size_t)(0), (cudaStream_t)stream, (const T*)a, (const T*)b, (T*)out, n / 8)));
-    PIDM_LAUNCH_CHECK("add");
     return 0;
 }
 

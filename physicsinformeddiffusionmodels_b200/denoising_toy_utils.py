@@ -234,7 +234,11 @@ def ddim_sample_x0(xt, t, model, shape, reduced_n_steps, ddim_sampling_eta, diff
     batch_t = (torch.ones(batch, device=dev, dtype=torch.long) * t) if len(t) == 1 else t
     n_pts = reduced_n_steps + 2
     k = torch.arange(n_pts, device=dev, dtype=torch.float64)
-    grid = (k[None, :] * (batch_t.double() / (n_pts - 1))[:, None]).long()             # int() truncation of np.linspace
+    # int() truncation of np.linspace, whose step is t / (n_pts - 1): divided by a device tensor, since a CUDA
+    # tensor divided by a Python scalar is multiplied by its reciprocal, which can round the step low and a grid
+    # point one lower (t = 14 on 7 points gives 6 for 7)
+    step = batch_t.double() / torch.full_like(batch_t, n_pts - 1, dtype=torch.float64)
+    grid = (k[None, :] * step[:, None]).long()
     grid[:, -1] = batch_t
     cur_times = grid.flip(1).T.contiguous()
     next_times = torch.cat([grid.new_full((batch, 1), -1), grid[:, :-1]], dim=1).flip(1).T.contiguous()

@@ -75,30 +75,6 @@ def nchw_to_nhwc(x, cpad, dtype=None):
     return y
 
 
-def nhwc_to_nchw(x, C=None):
-    B, H, W, Cp = x.shape
-    C = C or Cp
-    y = torch.empty(B, C, H, W, device=x.device, dtype=torch.float32)
-    call('pidm_nhwc_to_nchw', x, y, B, C, H * W, Cp, _code(x), stream())
-    return y
-
-
-class _Add(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, a, b):
-        o = torch.empty_like(a)
-        call('pidm_add', a, b, o, a.numel(), _code(a), stream())
-        return o
-
-    @staticmethod
-    def backward(ctx, g):
-        return g, g
-
-
-def add(a, b):
-    return _Add.apply(a.contiguous(), b.contiguous())
-
-
 class _CondEmbed(torch.autograd.Function):
     """GELU(emb_conv[0](cond)) of the residual-gradient guidance branch (reference unet_model.py:520-524,585-603) as NHWC
     activations, from cond [B, HW, 2] fp32 (data: no gradient) with the samples in null_mask [B] (bool) taking cond = 0.

@@ -1,13 +1,16 @@
-"""The census of the benchmarked steps, shared by the six per-element census files (tests/test_gpu_*_census.py).
+"""The census of the benchmarked and sampling steps, shared by the seven per-element census files
+(tests/test_gpu_*_census.py).
 
 One eager step of every workload bench.py times (Darcy training at batch 32, one Darcy sampling step at batch 16 / 64 /
-256, mechanics training at batch 32 with Unet3D(dim=128)) is run with the C ABI's `call` swapped for a recorder, which
-keeps every entry point called and, for the entry points in KEYS, the distinct (family, key) pairs of their arguments.
-Keys are integer and flag arguments, which optional pointers are set and geometry decoded from device tables, never
-pointers.  There are two recordings: census() runs the workloads as bench.py does (bf16), census_exact() runs them and
-the guidance and circular training steps in the fp32 exact mode that every oracle-parity test uses, where every
-convolution runs on the CUDA-core kernels of conv_simt.cu.  Each census file commits one table per family and checks it
-against its recording (census_exact() for the files in EXACT_FILES) both ways; `python tests/census.py --print-table`
+256 in mean mode and at batch 16 in sample mode with ddim_steps = 0, mechanics training at batch 32 with Unet3D(dim=128))
+is run with the C ABI's `call` swapped for a recorder, which keeps every entry point called and, for the entry points in
+KEYS, the distinct (family, key) pairs of their arguments.  Keys are integer and flag arguments, which optional pointers
+are set and geometry decoded from device tables, never pointers.  There are three recordings: census() runs the
+workloads as bench.py does (bf16), census_exact() runs them and the guidance and circular training steps in the fp32
+exact mode that every oracle-parity test uses, where every convolution runs on the CUDA-core kernels of conv_simt.cu,
+and census_sampling() runs one step of each sampling-side workload the package offers beside them (DDIM walks, CoCoGen
+corrections, the drop-in p_sample, conditional mechanics sampling and the toy study) in bf16.  Each census file commits
+one table per family and checks it against its recording (RECORDING) both ways; `python tests/census.py --print-table`
 regenerates every table.  The product package is imported inside the functions, so importing this module builds
 nothing."""
 import functools
@@ -120,6 +123,12 @@ KEYS = {
     # test_gpu_simt_census.py (the dtype is left out: every row is replayed in both)
     'pidm_conv2d_simt': lambda a: [('simt', tuple(int(v) for v in a[5:17]) + (_has(a[2]), _has(a[3])))],
     'pidm_conv2d_wgrad_simt': lambda a: [('simt_wgrad', tuple(int(v) for v in a[4:19]) + (_has(a[3]),))],
+    # test_gpu_sampling_census.py
+    'pidm_ddim_coefs': lambda a: [('ddim', (int(a[9]),))],
+    'pidm_posterior_step': lambda a: [('posterior', (int(a[7]),))],
+    'pidm_darcy_cocogen': lambda a: [('cocogen', (int(a[6]), int(a[7]), float(a[8]), int(a[9]), int(a[10]), int(a[5]),
+                                                  int(a[4]), _has(a[3])))],
+    'pidm_toy_pidm_loss': lambda a: [('toy_loss', (int(a[17]), int(a[18]), _has(a[3]), _has(a[4]), _has(a[6])))],
 }
 
 # the families of KEYS by the census file that holds their tables, in the order of its tables
@@ -132,9 +141,10 @@ FAMILIES = {
     'test_gpu_glue_census.py': ('time_fwd', 'time_bwd', 'mlp_fwd', 'mlp_bwd', 'sumsq', 'adam', 'pack', 'pair',
                                 'pair_launch', 'qsample', 'axpby', 'scale', 'concat', 'split', 'nchw'),
     'test_gpu_simt_census.py': ('simt', 'simt_wgrad'),
+    'test_gpu_sampling_census.py': ('ddim', 'posterior', 'cocogen', 'toy_loss'),
 }
-# the files whose tables are checked against census_exact(); every other file against census()
-EXACT_FILES = ('test_gpu_simt_census.py',)
+# the recording each census file's tables are checked against, where it is not census()
+RECORDING = {'test_gpu_simt_census.py': 'census_exact', 'test_gpu_sampling_census.py': 'census_sampling'}
 
 # Entry points the benchmarked steps call that launch nothing: host-side capability and size queries.
 LAUNCHES_NOTHING = [
@@ -147,6 +157,32 @@ LAUNCHES_NOTHING = [
     'pidm_pack_entry_size',
     'pidm_pack_pair_entry_size',
 ]
+
+# Entry points of the exact mode and of the sampling steps that no census family keys, with the per-element or bitwise
+# test that checks them
+CHECKED_ELSEWHERE = {
+    'pidm_wrap_pad_nhwc': 'test_gpu_circular.py::test_wrap_pad_is_bitwise_circular_pad',
+    'pidm_cond_embed_fwd': 'test_gpu_guidance.py::test_cond_embed_per_element',
+    'pidm_cond_embed_wgrad': 'test_gpu_guidance.py::test_cond_embed_wgrad_per_element',
+    'pidm_darcy_abs_residual_grad': 'test_gpu_guidance.py::test_abs_residual_grad_per_element',
+    'pidm_mech_sample_input': 'test_gpu_mech_sample.py::test_sample_kernels_match_their_torch_composition',
+    'pidm_mech_posterior_step': 'test_gpu_mech_sample.py::test_sample_kernels_match_their_torch_composition',
+    'pidm_mech_fem_pcg': 'test_gpu_mech_sample.py::test_fused_solver_against_sparse_direct_solve',
+    'pidm_mech_floating_material': 'test_gpu_mech_sample.py::test_floating_material_kernel_matches_host_labelling',
+}
+
+
+def assert_checked_or_listed(names, what):
+    """every entry point in `names` is keyed, launches nothing or is CHECKED_ELSEWHERE by a test that exists"""
+    import re
+    unchecked = sorted(set(names) - set(KEYS) - set(LAUNCHES_NOTHING) - set(CHECKED_ELSEWHERE))
+    assert not unchecked, (f'entry points of {what} that no test checks per element: add a census family, or name the '
+                           'test that checks them in census.CHECKED_ELSEWHERE:\n' + '\n'.join(unchecked))
+    here = os.path.dirname(os.path.abspath(__file__))
+    for name, test in CHECKED_ELSEWHERE.items():
+        file, fn = test.split('::')
+        with open(os.path.join(here, file)) as f:
+            assert re.search(rf'^def {fn}\(', f.read(), re.M), f'{name}: {test} does not exist'
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -186,11 +222,36 @@ def _darcy_model(dev):
     return Unet3D(dim=32, channels=2).to(dev)
 
 
+def _darcy_sample_engine(model, diff, B, t=None, **options):
+    """an eager Darcy SampleEngine of batch B, as bench.py's sampling_bench builds it, on normal x at t [B] (default
+    n_steps - 1) with the packed weights fresh; `options` go to ResidualsDarcy, or to SampleEngine for the CoCoGen
+    ones"""
+    from physicsinformeddiffusionmodels_b200 import ops
+    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
+    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
+    engine_options = {k: options.pop(k) for k in ('N_correction', 'M_correction', 'correction_mode') if k in options}
+    res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
+                         device=DEV, **{'bcs': 'none', 'domain_length': 1., **options})
+    se = SampleEngine(model, diff, res, batch=B, use_graph=False, **engine_options)
+    packer = getattr(model, '_packer', None)
+    if packer is not None:
+        packer.refresh_if_stale(ops.act_dtype())
+    se.x.normal_()
+    se.t.copy_(torch.full((B,), diff.n_steps - 1) if t is None else torch.as_tensor(t))
+    return se
+
+
+def _ddim0_step(model, diff):
+    """bench.py's sample-mode step: x0 by the DDIM walk with ddim_steps = 0, batch 16"""
+    return {'darcy_sample_ddim0_b16': _record(_darcy_sample_engine(model, diff, 16, use_ddim_x0=True,
+                                                                   ddim_steps=0)._step_body)}
+
+
 def run_census(precision='bf16'):
     """{workload: _record(one eager step of it)} for every workload bench.py times, in ops precision `precision`"""
     from physicsinformeddiffusionmodels_b200 import ops
     from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
-    from physicsinformeddiffusionmodels_b200.engine import SampleEngine, TrainEngine
+    from physicsinformeddiffusionmodels_b200.engine import TrainEngine
     from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
     from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
     from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
@@ -209,16 +270,8 @@ def run_census(precision='bf16'):
     model.eval()
     diff = DenoisingDiffusion(250, dev)
     for B in (16, 64, 256):
-        res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True,
-                             device=dev, bcs='none', domain_length=1., use_ddim_x0=False, ddim_steps=0)
-        se = SampleEngine(model, diff, res, batch=B, use_graph=False)
-        packer = getattr(model, '_packer', None)
-        if packer is not None:
-            packer.refresh_if_stale(ops.act_dtype())
-        se.x.normal_()
-        se.t.fill_(diff.n_steps - 1)
-        out[f'darcy_sample_b{B}'] = _record(se._step_body)
-        del se
+        out[f'darcy_sample_b{B}'] = _record(_darcy_sample_engine(model, diff, B)._step_body)
+    out.update(_ddim0_step(model, diff))
     del model
     torch.manual_seed(0)
     mech = Unet3D(dim=128, channels=10, out_dim=3, sigmoid_last_channel=True).to(dev)
@@ -273,6 +326,85 @@ def run_census_exact():
     return out
 
 
+def _toy_residual(x):
+    return torch.sum(x ** 2, dim=1) - 1.0
+
+
+def _toy_ineq(x):
+    density = torch.sum(torch.abs(x), dim=1)
+    return torch.relu(density - 1.0), density
+
+
+def _toy_opt(x):
+    return x[:, 0]
+
+
+def run_census_sampling():
+    """{workload: _record(one eager step of it)} of the sampling side in bf16: bench.py's sample-mode step, a Darcy
+    SampleEngine step with ddim_steps = 3 at per-sample t, CoCoGen SampleEngine steps in both correction modes for both
+    boundary conditions at per-sample t that leave some samples inactive, the M_correction launch after the loop, one
+    drop-in DenoisingDiffusion.p_sample step, conditional mechanics SampleEngine steps in mean and sample mode and the
+    evaluation of their last x0 prediction (topopt_eval, with a solution), the toy training loss in x0 and eps mode, and
+    one toy p_sample step at an odd batch (whose posterior step takes the scalar path)"""
+    import mech_sample_inputs as MI
+    from physicsinformeddiffusionmodels_b200 import denoising_toy_utils as T
+    from physicsinformeddiffusionmodels_b200 import ops
+    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
+    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
+    from physicsinformeddiffusionmodels_b200.residuals_darcy import ResidualsDarcy
+    from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import ResidualsMechanics
+    from physicsinformeddiffusionmodels_b200.unet_model import Unet3D
+    dev = torch.device(DEV)
+    ops.set_precision('bf16')
+    ops.set_tensor_core_conv(True)
+    out = {}
+    model = _darcy_model(dev)
+    model.eval()
+    diff = DenoisingDiffusion(250, dev)
+    out.update(_ddim0_step(model, diff))
+    out['darcy_sample_ddim3_b4'] = _record(_darcy_sample_engine(model, diff, 4, [249, 100, 3, 0], use_ddim_x0=True,
+                                                                ddim_steps=3)._step_body)
+    diff6 = DenoisingDiffusion(6, dev)
+    for bcs in ('none', 'periodic'):
+        for mode in ('xt', 'x0'):
+            se = _darcy_sample_engine(model, diff6, 4, [3, 1, 0, 2], bcs=bcs, N_correction=2, M_correction=3,
+                                      correction_mode=mode)
+            out[f'cocogen_{mode}_{bcs}_b4'] = _record(se._step_body)
+        out[f'cocogen_M3_{bcs}_b4'] = _record(lambda: se.residuals.cocogen(se.x, se.residual, se.M_correction))
+    res = ResidualsDarcy(model=model, fd_acc=2, pixels_per_dim=64, pixels_at_boundary=True, reverse_d1=True, device=dev)
+    x = torch.randn(2, 2, 64, 64, device=dev)
+    out['p_sample_b2'] = _record(lambda: diff6.p_sample(x, None, 5, residual_func=res, surpress_noise=True))
+    del model, se
+    torch.manual_seed(0)
+    mech = Unet3D(dim=32, channels=10, out_dim=3, sigmoid_last_channel=True).to(dev)
+    mech.eval()
+    cond, bcs, rho = MI.conditioning_batch()
+    solution = torch.zeros(MI.B, 3, 65, 65)
+    solution[:, 2, :-1, :-1] = rho
+    ci = (cond.to(dev), bcs.to(dev), solution.to(dev))
+    for mode in ('mean', 'sample'):
+        res = ResidualsMechanics(model=mech, pixels_per_dim=64, pixels_at_boundary=True, no_BC_folder='', device=dev,
+                                 topopt_eval=True, use_ddim_x0=mode == 'sample', ddim_steps=0)
+        se = SampleEngine(mech, diff6, res, batch=MI.B, image_shape=(3, 65, 65), use_graph=False)
+        n = se._mech_condition(ci)
+        se.x.normal_()
+        se.t.fill_(diff6.n_steps - 1)
+        out[f'mech_sample_{mode}_b{MI.B}'] = _record(se._step_body)
+    out[f'mech_aux_b{MI.B}'] = _record(lambda: se._mech_aux(ci, n))
+    del mech, se
+    torch.manual_seed(0)
+    toy = T.ConditionalModel(2, 100).to(dev)
+    dd = T.create_diff_dict(100, dev)
+    x0 = torch.randn(128, 2, device=dev)
+    for mode, extra in (('x0', dict(ineq_func=_toy_ineq, opt_func=_toy_opt)), ('eps', {})):
+        out[f'toy_loss_{mode}_b128'] = _record(lambda: T.model_estimation_loss(
+            toy, x0, 100, dd, model_pred_mode=mode, residual_func=_toy_residual, c_data=1.0, c_residual=0.005,
+            c_ineq=0.3, lambda_opt=0.01, **extra)[0].backward())
+    out['toy_p_sample_b63'] = _record(lambda: T.p_sample(toy, torch.randn(63, 2, device=dev), 5, dd, model_pred_mode='x0'))
+    torch.cuda.empty_cache()
+    return out
+
+
 def _summary(raw):
     return {wl: keys for wl, (keys, _) in raw.items()}, set().union(*(names for _, names in raw.values()))
 
@@ -289,8 +421,14 @@ def census_exact():
     return _summary(run_census_exact())
 
 
+@functools.cache
+def census_sampling():
+    """census() of the sampling-side workloads (run_census_sampling), recorded once per process"""
+    return _summary(run_census_sampling())
+
+
 def _recording(file):
-    return census_exact if file in EXACT_FILES else census
+    return globals()[RECORDING.get(file, 'census')]
 
 
 def _file_of(tables):

@@ -27,6 +27,40 @@ def test_library_builds_loads_and_exports_header_symbols():
     assert _lib.call('pidm_pack_entry_size') == 56 and _lib.call('pidm_mlp_entry_size') == 56
 
 
+# Entry points of include/pidm.h that no census recording calls: host queries that launch nothing, and kernels with a
+# named per-element or bitwise test of their own
+HOST_QUERIES = ['pidm_version', 'pidm_last_error', 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan',
+                'pidm_groupnorm_plan', 'pidm_linattn_block_plan', 'pidm_linattn_plan', 'pidm_darcy_gen_workspace_bytes']
+TESTED_OUTSIDE_THE_RECORDINGS = {
+    'pidm_darcy_gen_kle': 'test_gpu_darcy_gen.py::test_kle',                  # the Darcy training-data generator
+    'pidm_darcy_gen_solve': 'test_gpu_darcy_gen.py::test_fixture_solve',
+    'pidm_swap_f32': 'test_gpu_ema_eval.py::test_swap_is_an_exact_exchange',  # the EMA weight swap
+    'pidm_fd_stencil': 'test_gpu_physics_census.py::test_darcy_fd_stencil_replay',
+    'pidm_darcy_jacobian_max': 'test_gpu_physics_census.py::test_darcy_jacobian_max_replay',
+}
+
+
+def test_every_header_entry_point_is_accounted_for():
+    """every pidm_* of include/pidm.h is keyed by a census family, launches nothing, is checked elsewhere, is a host
+    query or has a named test; an entry point nothing calls is removed, not listed"""
+    import census
+    hdr = open(os.path.join(ROOT, 'include', 'pidm.h')).read()
+    declared = set(re.findall(r'\b(pidm_[a-z0-9_]+)\s*\(', hdr))
+    lists = {'census.KEYS': set(census.KEYS), 'census.LAUNCHES_NOTHING': set(census.LAUNCHES_NOTHING),
+             'census.CHECKED_ELSEWHERE': set(census.CHECKED_ELSEWHERE), 'HOST_QUERIES': set(HOST_QUERIES),
+             'TESTED_OUTSIDE_THE_RECORDINGS': set(TESTED_OUTSIDE_THE_RECORDINGS)}
+    covered = set().union(*lists.values())
+    assert not declared - covered, f'entry points of pidm.h that nothing accounts for: {sorted(declared - covered)}'
+    assert not covered - declared, f'listed entry points that pidm.h does not declare: {sorted(covered - declared)}'
+    for a in ('HOST_QUERIES', 'TESTED_OUTSIDE_THE_RECORDINGS'):
+        for b, names in lists.items():
+            assert a == b or not lists[a] & names, f'{sorted(lists[a] & names)} listed in both {a} and {b}'
+    for name, test in TESTED_OUTSIDE_THE_RECORDINGS.items():
+        file, fn = test.split('::')
+        with open(os.path.join(ROOT, 'tests', file)) as f:
+            assert re.search(rf'^def {fn}\(', f.read(), re.M), f'{name}: {test} does not exist'
+
+
 def test_no_oracle_import_on_product_path():
     """The product package must never reach into oracle/ (selftest.smoke is the one sanctioned checker)."""
     pkg = os.path.join(ROOT, 'physicsinformeddiffusionmodels_b200')

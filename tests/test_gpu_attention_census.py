@@ -69,9 +69,9 @@ BWD_PATHS = {0: 'mma', 1: 'simt'}
 # ----------------------------------------------------------------------------------------------------------------------
 # pidm_linattn_fwd / _bwd: B, N, heads, dtype
 LA_FWD_TABLE = [
-    (16, 64, 8, 'bf16'),  # darcy_sample_b16
-    (16, 256, 8, 'bf16'),  # darcy_sample_b16
-    (16, 1024, 8, 'bf16'),  # darcy_sample_b16
+    (16, 64, 8, 'bf16'),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 8, 'bf16'),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 8, 'bf16'),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 64, 8, 'bf16'),  # darcy_train_b32 mech_train_b32
     (32, 256, 8, 'bf16'),  # darcy_train_b32 mech_train_b32
     (32, 1024, 8, 'bf16'),  # darcy_train_b32 mech_train_b32
@@ -91,7 +91,7 @@ LA_BWD_TABLE = [
 ]
 # pidm_attn_fwd / _bwd: B, n_tokens, heads, dtype
 ATTN_FWD_TABLE = [
-    (16, 64, 8, 'bf16'),  # darcy_sample_b16
+    (16, 64, 8, 'bf16'),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 64, 8, 'bf16'),  # darcy_train_b32 mech_train_b32
     (64, 64, 8, 'bf16'),  # darcy_sample_b64
     (256, 64, 8, 'bf16'),  # darcy_sample_b256
@@ -101,7 +101,7 @@ ATTN_BWD_TABLE = [
 ]
 # pidm_head_fwd / _bwd: B, HW, C, O, sigmoid_last, dtype
 HEAD_FWD_TABLE = [
-    (16, 4096, 32, 2, 0, 'bf16'),  # darcy_sample_b16
+    (16, 4096, 32, 2, 0, 'bf16'),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 4096, 32, 2, 0, 'bf16'),  # darcy_train_b32
     (32, 4096, 128, 3, 1, 'bf16'),  # mech_train_b32
     (64, 4096, 32, 2, 0, 'bf16'),  # darcy_sample_b64

@@ -109,6 +109,78 @@ def test_sample_mode_loss_matches_reference(ops, golden):
     assert rel(model.init_conv.weight.grad, gd['grad_init_w']) < 2e-3
 
 
+def ddim_walk_case(golden):
+    from oracle import make_golden
+    gd = golden('darcy_loss_sample.pt')
+    xt = make_golden.ddim_walk_input()
+    assert torch.equal(xt.double().sum(), gd['walk_x_t_checksum'])
+    return gd, xt.to(DEV), make_golden.DDIM_WALK
+
+
+def check_ddim_walk(gd, sample, ddim_steps, cur_x, model_out):
+    """the walk's result and first network output against the reference's, at the fp32 U-Net tolerance"""
+    assert rel(O.golden_sample(model_out.cpu(), sample), gd[f'walk_model_out_{ddim_steps}']) < 1e-4
+    assert rel(O.golden_sample(cur_x.cpu(), sample), gd[f'walk_cur_x_{ddim_steps}']) < 1e-4
+
+
+@pytest.mark.parametrize('ddim_steps', [1, 3])
+def test_ddim_walk_matches_reference(ops, golden, ddim_steps):
+    """ddim_sample_x0 at ddim_steps > 0, per-sample t = 0, 2 (repeated grid points), 57 and n_steps - 1"""
+    ops.set_precision('fp32')
+    gd, xt, spec = ddim_walk_case(golden)
+    model, diff, _ = build_darcy(n_steps=spec['n_steps'])
+    model.eval()
+    with torch.no_grad():
+        cur_x, model_out = diff.ddim_sample_x0(xt, gd['walk_t'].to(DEV), model, xt.shape, ddim_steps, 0.)
+    check_ddim_walk(gd, spec['sample'], ddim_steps, cur_x, model_out)
+
+
+def test_sample_engine_ddim3_step_matches_reference(ops, golden):
+    """one sample-mode SampleEngine step with ddim_steps = 3: its x0 estimate is the reference's walk, its residual is
+    that of the walk's result and its posterior step takes the walk's first network output"""
+    from physicsinformeddiffusionmodels_b200.engine import SampleEngine
+    ops.set_precision('fp32')
+    gd, xt, spec = ddim_walk_case(golden)
+    model, diff, res = build_darcy(n_steps=spec['n_steps'], use_ddim_x0=True)
+    res.ddim_steps = 3
+    model.eval()
+    walks = []
+    walk = diff.ddim_sample_x0
+    diff.ddim_sample_x0 = lambda *a, **k: walks.append(walk(*a, **k)) or walks[-1]
+    se = SampleEngine(model, diff, res, batch=xt.shape[0], use_graph=False, external_noise=True)
+    se.z.normal_()
+    se.x.copy_(xt)
+    t = gd['walk_t'].to(DEV)
+    se.t.copy_(t)
+    se._step_body()
+    (cur_x, model_out), = walks
+    check_ddim_walk(gd, spec['sample'], 3, cur_x, model_out)
+    assert torch.equal(se.residual, ops.darcy_residual(cur_x, res.f_s_flat, *res.geometry))
+    c1, c2, sig = se.c1[t].view(-1, 1, 1, 1), se.c2[t].view(-1, 1, 1, 1), se.sigma[t].view(-1, 1, 1, 1)
+    assert torch.allclose(se.x, c1 * model_out + c2 * xt + sig * se.z[0], rtol=1e-5, atol=1e-5)
+    assert torch.equal(se.t, t - 1)
+
+
+def test_ddim_device_grid_is_the_reference_linspace():
+    """the time grid ddim_sample_x0 builds on the device is int(np.linspace(0, t, s + 2)) for every t < 1000 and
+    s <= 20: a stub network records the t of each call"""
+    import numpy as np
+    from physicsinformeddiffusionmodels_b200.denoising_utils import DenoisingDiffusion
+    diff = DenoisingDiffusion(1000, DEV)
+    t = torch.arange(1000, device=DEV)
+    x = torch.zeros(1000, 2, 4, 4, device=DEV)
+    for s in range(21):
+        seen = []
+
+        def stub(inp, tt, self_cond=None):
+            seen.append(tt.cpu())
+            return torch.zeros_like(inp)
+        diff.ddim_sample_x0(x, t, stub, x.shape, s, 0.)
+        got = torch.stack(seen).flip(0).T                              # [t, grid point], ascending
+        want = torch.tensor([[int(v) for v in np.linspace(0, ti, s + 2, dtype=float)] for ti in range(1000)])
+        assert torch.equal(got, want), (s, (got != want).nonzero()[:5].tolist())
+
+
 def test_sampling_loop_matches_reference(ops, golden, monkeypatch):
     """p_sample_loop with the reference's own draws injected (x_T, then one z per step incl. t=0)."""
     ops.set_precision('fp32')

@@ -110,8 +110,8 @@ def test_swap_rejects_misuse_without_launching():
 
 def test_ema_context_is_exact_and_leaves_training_unchanged(ops):
     """Inside the context every parameter is the EMA weight; on exit every training buffer is bitwise what it was, and
-    the next graph-replayed step is that of the same state without the context (bitwise where two replays from one
-    state agree bitwise; otherwise to the run-to-run spread of the fp32 atomics)."""
+    the next graph-replayed step is that of the same state without the context (bitwise where replays from one state
+    agree bitwise; otherwise to the run-to-run spread of the fp32 atomics)."""
     ops.set_precision('fp32')
     x = darcy_batch(2, 1)
     eng = trained_engine('mean', steps=3, use_graph=True)
@@ -140,11 +140,18 @@ def test_ema_context_is_exact_and_leaves_training_unchanged(ops):
         out = torch.stack(eng.step(x))
         torch.cuda.synchronize()
         return torch.cat((out, fp.flat, fp.ema, fp.exp_avg, fp.exp_avg_sq)).clone()
-    plain, again, entered = next_step(False), next_step(False), next_step(True)
-    if torch.equal(plain, again):
-        assert torch.equal(entered, plain)
-    else:
-        assert rel(entered, plain) <= 4 * rel(again, plain), (rel(entered, plain), rel(again, plain))
+    # The run-to-run spread of the fp32 atomics (GroupNorm statistics, weight-gradient splits) is not one value: two
+    # replays may agree bitwise, differ in a few small elements, or differ by an ulp of the loss, which dominates the
+    # norm.  So the spread is taken over every pair of replays within each group, five interleaved replays with and
+    # five without the context, and every replay with the context must lie within 4x of it from every replay
+    # without: bitwise where all within-group pairs agree bitwise.
+    runs = {enter: [] for enter in (False, True)}
+    for _ in range(5):
+        for enter in (False, True):
+            runs[enter].append(next_step(enter))
+    spread = max(rel(a, b) for g in runs.values() for i, a in enumerate(g) for b in g[i + 1:])
+    cross = max(rel(e, p) for e in runs[True] for p in runs[False])
+    assert cross <= 4 * spread, (cross, spread)
 
 
 def test_ema_context_guards(ops):

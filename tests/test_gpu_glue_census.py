@@ -61,7 +61,7 @@ GELU_LIP, SILU_LIP = 1.13, 1.10        # max |gelu'|, max |silu'|
 # pair_launch: dtype, tile_base, n_tiles, max_taps
 # qsample / axpby: B, per_sample;  scale: n;  concat / split: rows, Ca, Cb, dtype;  nchw: B, C, HW, Cpad, dtype
 TIME_FWD_TABLE = [
-    (16, 32, 128),  # darcy_sample_b16
+    (16, 32, 128),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 32, 128),  # darcy_train_b32
     (32, 128, 512),  # mech_train_b32
     (64, 32, 128),  # darcy_sample_b64
@@ -74,7 +74,7 @@ TIME_BWD_TABLE = [
     (32, 128, 512, 2),  # mech_train_b32
 ]
 MLP_FWD_TABLE = [
-    (16, 128, 512, (64, 64, 128, 128, 256, 256, 512, 512, 512, 512, 256, 256, 128, 128, 64, 64, 64, 64)),  # darcy_sample_b16
+    (16, 128, 512, (64, 64, 128, 128, 256, 256, 512, 512, 512, 512, 256, 256, 128, 128, 64, 64, 64, 64)),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 128, 512, (64, 64, 128, 128, 256, 256, 512, 512, 512, 512, 256, 256, 128, 128, 64, 64, 64, 64)),  # darcy_train_b32
     (32, 512, 2048, (256, 256, 512, 512, 1024, 1024, 2048, 2048, 2048, 2048, 1024, 1024, 512, 512, 256, 256, 256, 256)),  # mech_train_b32
     (64, 128, 512, (64, 64, 128, 128, 256, 256, 512, 512, 512, 512, 256, 256, 128, 128, 64, 64, 64, 64)),  # darcy_sample_b64
@@ -160,7 +160,7 @@ QSAMPLE_TABLE = [
     (32, 12675),  # mech_train_b32
 ]
 AXPBY_TABLE = [
-    (16, 8192),  # darcy_sample_b16
+    (16, 8192),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (64, 8192),  # darcy_sample_b64
     (256, 8192),  # darcy_sample_b256
 ]
@@ -171,19 +171,19 @@ SCALE_TABLE = [
     (270400,),  # mech_train_b32
 ]
 CONCAT_TABLE = [
-    (1024, 256, 256, 1),  # darcy_sample_b16
+    (1024, 256, 256, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (2048, 256, 256, 1),  # darcy_train_b32
     (2048, 1024, 1024, 1),  # mech_train_b32
-    (4096, 128, 128, 1),  # darcy_sample_b16
+    (4096, 128, 128, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (4096, 256, 256, 1),  # darcy_sample_b64
     (8192, 128, 128, 1),  # darcy_train_b32
     (8192, 512, 512, 1),  # mech_train_b32
-    (16384, 64, 64, 1),  # darcy_sample_b16
+    (16384, 64, 64, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (16384, 128, 128, 1),  # darcy_sample_b64
     (16384, 256, 256, 1),  # darcy_sample_b256
     (32768, 64, 64, 1),  # darcy_train_b32
     (32768, 256, 256, 1),  # mech_train_b32
-    (65536, 32, 32, 1),  # darcy_sample_b16
+    (65536, 32, 32, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (65536, 64, 64, 1),  # darcy_sample_b64
     (65536, 128, 128, 1),  # darcy_sample_b256
     (131072, 32, 32, 1),  # darcy_train_b32
@@ -203,7 +203,7 @@ SPLIT_TABLE = [
     (131072, 128, 128, 1),  # mech_train_b32
 ]
 NCHW_TABLE = [
-    (16, 2, 4096, 32, 1),  # darcy_sample_b16
+    (16, 2, 4096, 32, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 2, 4096, 32, 1),  # darcy_train_b32
     (32, 10, 4096, 32, 1),  # mech_train_b32
     (64, 2, 4096, 32, 1),  # darcy_sample_b64

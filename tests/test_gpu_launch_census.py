@@ -53,49 +53,50 @@ GUARD_BF16 = 0x7FBF            # a NaN bit pattern: an unwritten output element 
 #   darcy_sample_b16: conv 38, wgrad 0, laf 2
 #   darcy_sample_b64: conv 38, wgrad 0, laf 2
 #   darcy_sample_b256: conv 38, wgrad 0, laf 2
+#   darcy_sample_ddim0_b16: conv 38, wgrad 0, laf 2
 #   mech_train_b32: conv 87, wgrad 37, laf 0
 #   distinct: conv 282, wgrad 71, laf 12
 # ----------------------------------------------------------------------------------------------------------------------
 # conv: B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad, transposed, bias, residual, gn_sums, gn_groups, gn_sums_zeroed
 CONV_TABLE = [
-    (16, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 8, 8, 128, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 128, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 8, 8, 128, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 128, 16, 16, 128, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 0, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 512, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 512, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 64, 32, 32, 64, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 128, 8, 8, 128, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 128, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 16, 16, 128, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 256, 16, 16, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 256, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 16, 16, 256, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 32, 32, 32, 64, 64, 32, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 64, 16, 16, 64, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 64, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
-    (16, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16
-    (16, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16
+    (16, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 16, 16, 128, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 0, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 512, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 512, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 32, 32, 64, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 128, 8, 8, 128, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 128, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 128, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 256, 16, 16, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 256, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 256, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 64, 64, 32, 4, 4, 2, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 64, 16, 16, 64, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 64, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 0, 0, 0, 0, 0),  # darcy_train_b32
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 0, 1, 0, 0, 0),  # darcy_train_b32
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0, 1, 8, 1),  # darcy_train_b32
@@ -419,8 +420,8 @@ WGRAD_TABLE = [
 LAF_TABLE = [
     ('bwd', 32, 1024, 0, 0, 0, 0),  # darcy_train_b32
     ('bwd', 32, 4096, 0, 0, 0, 0),  # darcy_train_b32
-    ('fwd', 16, 1024, 0, 0, 0, 0),  # darcy_sample_b16
-    ('fwd', 16, 4096, 0, 0, 0, 0),  # darcy_sample_b16
+    ('fwd', 16, 1024, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    ('fwd', 16, 4096, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
     ('fwd', 32, 1024, 0, 0, 0, 0),  # darcy_train_b32
     ('fwd', 32, 4096, 0, 0, 0, 0),  # darcy_train_b32
     ('fwd', 64, 1024, 0, 0, 0, 0),  # darcy_sample_b64

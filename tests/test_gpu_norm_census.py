@@ -56,27 +56,27 @@ PATHS = {0: 'fallback', 1: 'piece1', 2: 'piece2', 3: 'packed4', 4: 'stream'}
 # ----------------------------------------------------------------------------------------------------------------------
 # pidm_groupnorm_silu_fwd: B, HW, C, G, scale_shift, residual, stats_precomputed
 GN_FWD_TABLE = [
-    (16, 64, 128, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 64, 128, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 64, 128, 8, 1, 0, 1),  # darcy_sample_b16
-    (16, 64, 256, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 64, 256, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 64, 256, 8, 1, 0, 1),  # darcy_sample_b16
-    (16, 256, 64, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 256, 64, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 256, 64, 8, 1, 0, 1),  # darcy_sample_b16
-    (16, 256, 128, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 256, 128, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 256, 128, 8, 1, 0, 1),  # darcy_sample_b16
-    (16, 1024, 32, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 1024, 32, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 1024, 32, 8, 1, 0, 1),  # darcy_sample_b16
-    (16, 1024, 64, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 1024, 64, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 1024, 64, 8, 1, 0, 1),  # darcy_sample_b16
-    (16, 4096, 32, 8, 0, 0, 1),  # darcy_sample_b16
-    (16, 4096, 32, 8, 0, 1, 1),  # darcy_sample_b16
-    (16, 4096, 32, 8, 1, 0, 1),  # darcy_sample_b16
+    (16, 64, 128, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 128, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 128, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 256, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 256, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 256, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 64, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 64, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 64, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 128, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 128, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 256, 128, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 32, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 32, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 32, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 64, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 64, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 1024, 64, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 4096, 32, 8, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 4096, 32, 8, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 4096, 32, 8, 1, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 64, 128, 8, 0, 0, 1),  # darcy_train_b32
     (32, 64, 128, 8, 0, 1, 1),  # darcy_train_b32
     (32, 64, 128, 8, 1, 0, 1),  # darcy_train_b32
@@ -195,28 +195,28 @@ GN_BWD_TABLE = [
 ]
 # pidm_layernorm_c_fwd: M, C
 LN_FWD_TABLE = [
-    (1024, 128),  # darcy_sample_b16
-    (1024, 256),  # darcy_sample_b16
+    (1024, 128),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (1024, 256),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (2048, 128),  # darcy_train_b32
     (2048, 256),  # darcy_train_b32
     (2048, 512),  # mech_train_b32
     (2048, 1024),  # mech_train_b32
-    (4096, 64),  # darcy_sample_b16
-    (4096, 128),  # darcy_sample_b16 darcy_sample_b64
+    (4096, 64),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (4096, 128),  # darcy_sample_b16 darcy_sample_b64 darcy_sample_ddim0_b16
     (4096, 256),  # darcy_sample_b64
     (8192, 64),  # darcy_train_b32
     (8192, 128),  # darcy_train_b32
     (8192, 256),  # mech_train_b32
     (8192, 512),  # mech_train_b32
-    (16384, 32),  # darcy_sample_b16
-    (16384, 64),  # darcy_sample_b16 darcy_sample_b64
+    (16384, 32),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16384, 64),  # darcy_sample_b16 darcy_sample_b64 darcy_sample_ddim0_b16
     (16384, 128),  # darcy_sample_b256 darcy_sample_b64
     (16384, 256),  # darcy_sample_b256
     (32768, 32),  # darcy_train_b32
     (32768, 64),  # darcy_train_b32
     (32768, 128),  # mech_train_b32
     (32768, 256),  # mech_train_b32
-    (65536, 32),  # darcy_sample_b16 darcy_sample_b64
+    (65536, 32),  # darcy_sample_b16 darcy_sample_b64 darcy_sample_ddim0_b16
     (65536, 64),  # darcy_sample_b256 darcy_sample_b64
     (65536, 128),  # darcy_sample_b256
     (131072, 32),  # darcy_train_b32

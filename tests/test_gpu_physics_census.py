@@ -51,7 +51,7 @@ CHUNK = 2048                     # samples per fp64 reference chunk on the devic
 # mech_fwd: B, nel, compliance set;  mech_bwd: B, nel, grad_residual set, grad_compliance set;  mech_loss: B, nel
 # resize_fwd / resize_bwd: planes, in, out
 DARCY_FWD_TABLE = [
-    (16, 64, 1.0, 1, 1),  # darcy_sample_b16
+    (16, 64, 1.0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (64, 64, 1.0, 1, 1),  # darcy_sample_b64
     (256, 64, 1.0, 1, 1),  # darcy_sample_b256
 ]

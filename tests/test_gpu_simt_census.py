@@ -29,14 +29,12 @@ in the four parts of the other census files:
      layouts.
 """
 import math
-import os
-import re
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from census import KEYS, LAUNCHES_NOTHING, assert_census_in_tables, assert_tables_in_census, census_exact
+from census import assert_census_in_tables, assert_checked_or_listed, assert_tables_in_census, census_exact
 from checks import CODE, DTYPES, NAME, U, call_sync, conv_ref, gen, guarded, guards_intact, note, ratio, sms
 
 pytestmark = pytest.mark.gpu
@@ -54,6 +52,7 @@ C_WG = 1.0
 #   darcy_sample_b16: simt 42, simt_wgrad 0
 #   darcy_sample_b64: simt 42, simt_wgrad 0
 #   darcy_sample_b256: simt 42, simt_wgrad 0
+#   darcy_sample_ddim0_b16: simt 42, simt_wgrad 0
 #   mech_train_b32: simt 87, simt_wgrad 41
 #   guidance_train_b32: simt 90, simt_wgrad 43
 #   circular_train_b32: simt 92, simt_wgrad 43
@@ -62,48 +61,48 @@ C_WG = 1.0
 # ----------------------------------------------------------------------------------------------------------------------
 # simt: B, H, W, Cin, Ho, Wo, Cout, KH, KW, stride, pad, transposed, bias, residual
 SIMT_TABLE = [
-    (16, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 8, 8, 128, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 8, 8, 128, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 8, 8, 128, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 128, 16, 16, 128, 4, 4, 2, 1, 1, 1, 0),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 0, 1),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 8, 8, 256, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 8, 8, 512, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 8, 8, 512, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 64, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 64, 32, 32, 64, 4, 4, 2, 1, 1, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 128, 8, 8, 128, 4, 4, 2, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 128, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 128, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 16, 16, 256, 16, 16, 64, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 16, 16, 256, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 16, 16, 256, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 32, 32, 32, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 32, 64, 64, 32, 4, 4, 2, 1, 1, 1, 0),  # darcy_sample_b16
-    (16, 32, 32, 64, 16, 16, 64, 4, 4, 2, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 32, 32, 64, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 32, 32, 256, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0),  # darcy_sample_b16
-    (16, 64, 64, 32, 64, 64, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16
-    (16, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
-    (16, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16
-    (16, 64, 64, 256, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16
+    (16, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 128, 16, 16, 128, 4, 4, 2, 1, 1, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 0, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 256, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 256, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 256, 8, 8, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 512, 8, 8, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 8, 8, 512, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 64, 32, 32, 64, 4, 4, 2, 1, 1, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 128, 8, 8, 128, 4, 4, 2, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 128, 16, 16, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 128, 16, 16, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 256, 16, 16, 64, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 256, 16, 16, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 16, 16, 256, 16, 16, 128, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 32, 64, 64, 32, 4, 4, 2, 1, 1, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 64, 16, 16, 64, 4, 4, 2, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 64, 32, 32, 64, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 64, 32, 32, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 128, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 128, 32, 32, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 256, 32, 32, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 32, 32, 256, 32, 32, 64, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 32, 32, 32, 4, 4, 2, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 64, 64, 32, 7, 7, 1, 3, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 32, 64, 64, 768, 1, 1, 1, 0, 0, 0, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 64, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 64, 64, 64, 32, 3, 3, 1, 1, 0, 1, 0),  # darcy_sample_b16 darcy_sample_ddim0_b16
+    (16, 64, 64, 256, 64, 64, 32, 1, 1, 1, 0, 0, 1, 1),  # darcy_sample_b16 darcy_sample_ddim0_b16
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 0, 0),  # darcy_train_b32 guidance_train_b32
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 0, 1),  # darcy_train_b32 guidance_train_b32
     (32, 8, 8, 128, 8, 8, 128, 3, 3, 1, 1, 0, 1, 0),  # darcy_train_b32 guidance_train_b32
@@ -612,15 +611,6 @@ SIMT_WGRAD_SYNTHETIC = [
     (3, 7, 7, 12, 12, 7, 7, 12, 3, 3, 1, 1, 1, 9, 108, 1),     # transposed stride 1, square (Cout = Cin) blocks
 ]
 
-# Entry points of the exact mode that no census family keys, with the per-element or bitwise test that checks them
-CHECKED_ELSEWHERE = {
-    'pidm_wrap_pad_nhwc': 'test_gpu_circular.py::test_wrap_pad_is_bitwise_circular_pad',
-    'pidm_cond_embed_fwd': 'test_gpu_guidance.py::test_cond_embed_per_element',
-    'pidm_cond_embed_wgrad': 'test_gpu_guidance.py::test_cond_embed_wgrad_per_element',
-    'pidm_darcy_abs_residual_grad': 'test_gpu_guidance.py::test_abs_residual_grad_per_element',
-}
-
-
 def simt_id(k):
     B, H, W, Cin, Ho, Wo, Cout, KH, KW, s, p, tr, hb, hr = k
     return (f'B{B}_{H}x{W}_{Cin}to{Cout}_o{Ho}x{Wo}_k{KH}s{s}p{p}' + ('T' if tr else '') + ('_bias' if hb else '')
@@ -645,17 +635,7 @@ def test_every_table_row_is_produced_by_the_census():
 
 
 def test_every_exact_mode_entry_point_is_checked_or_listed():
-    _, names = census_exact()
-    unchecked = sorted(names - set(KEYS) - set(LAUNCHES_NOTHING) - set(CHECKED_ELSEWHERE))
-    assert not unchecked, ('entry points of the exact mode that no test checks per element: add a census family, or '
-                           'name the test that checks them in CHECKED_ELSEWHERE:\n' + '\n'.join(unchecked))
-    stale = sorted(set(CHECKED_ELSEWHERE) - names)
-    assert not stale, f'CHECKED_ELSEWHERE lists entry points the exact mode no longer calls: {stale}'
-    here = os.path.dirname(os.path.abspath(__file__))
-    for name, test in CHECKED_ELSEWHERE.items():
-        file, fn = test.split('::')
-        with open(os.path.join(here, file)) as f:
-            assert re.search(rf'^def {fn}\(', f.read(), re.M), f'{name}: {test} does not exist'
+    assert_checked_or_listed(census_exact()[1], 'the exact mode')
 
 
 # ----------------------------------------------------------------------------------------------------------------------

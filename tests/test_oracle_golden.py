@@ -145,6 +145,21 @@ def test_sample_mode_loss_matches_reference(golden):
     assert rel(sd['init_conv.weight'].grad, gd['grad_init_w']) < 5e-4
 
 
+@pytest.mark.parametrize('ddim_steps', [1, 3])
+def test_ddim_walk_matches_reference(golden, ddim_steps):
+    """the oracle's DDIM walk (ddim_sample_x0, eta = 0) at ddim_steps > 0 and per-sample t whose grids repeat points"""
+    gd = golden('darcy_loss_sample.pt')
+    xt = make_golden.ddim_walk_input()
+    assert torch.equal(xt.double().sum(), gd['walk_x_t_checksum'])
+    cfg = O.unet_config(dim=32, channels=2)
+    with torch.no_grad():
+        cur_x, model_out = O.ddim_x0(O.make_test_state_dict(cfg, 0), cfg, xt, gd['walk_t'], O.diffusion_tables(100),
+                                     ddim_steps=ddim_steps)
+    n = make_golden.DDIM_WALK['sample']
+    assert rel(O.golden_sample(model_out, n), gd[f'walk_model_out_{ddim_steps}']) < 1e-5
+    assert rel(O.golden_sample(cur_x, n), gd[f'walk_cur_x_{ddim_steps}']) < 1e-5
+
+
 @pytest.mark.parametrize('name,s', [('sample_loop_6', 'none'), ('sample_loop_periodic', 'periodic'),
                                     ('sample_loop_circular', 'circular')])
 def test_sampling_loop_matches_reference(golden, name, s):
