@@ -117,7 +117,9 @@ long long pidm_darcy_gen_workspace_bytes(int B, int pixels);
  * batch [B, 2, P, P] fp32 = (p, K).  h = domain_length / (P-1) with PIDM_DARCY_PIXELS_AT_BOUNDARY in flags (trapezoid
  * weights {1,2,4} h^2/4), else domain_length / P (plain mean); reverse_dy: h1 = -h and the y BC rows +D1 | -D1 (:149-152).
  * stages: PIDM_DARCY_GEN_ASSEMBLE | _FACTOR | _POST, run in that order (PIDM_DARCY_GEN_ALL for a solve); the workspace
- * carries the band and right-hand side between them. */
+ * carries the band and right-hand side between them.  Workspace layout, fp64: band [B, P*P, 3P+4] first, band[b][r][d] =
+ * N[r][r-d] (d = 0 .. 3P+3; entries of negative column r - d < 0 are written 0 by the assembly and never read after it),
+ * then rhs [B, P*P] = A^T f_s; the factorisation overwrites band with L (same layout) and rhs with y = L^-1 rhs. */
 #define PIDM_DARCY_GEN_ASSEMBLE 1
 #define PIDM_DARCY_GEN_FACTOR 2
 #define PIDM_DARCY_GEN_POST 4

@@ -659,6 +659,10 @@ def darcy_gen_fixtures(out):
     f_s [4096], int_cond [4096]   create_f_s and the trapezoid weights of create_int_cond
     seed [4], z [4, 64], K [4, 4096], p [4, 4096], res [4]   generate_sample on four argument tuples
 
+    geometry_*         the same generate_sample at pixels_at_boundary=False, reverse_dy=False, domain_length=2 (its own
+                       eigenpairs, grid, source and weights): the three options, f_s, int_cond, seed [2], K, p [2, 4096],
+                       res [2]
+
     generate_sample draws its seed from os.getpid() * time.time(); the recipe replaces the module's `os` and `time`
     names by stand-ins (pid = seed, clock = 1 ms), so that unique_seed = seed.  The reference file itself is not
     touched."""
@@ -690,9 +694,34 @@ def darcy_gen_fixtures(out):
         fx['res'].append(res)
         print(f'seed {s}: res {res:.6e}  max|p| {np.abs(p).max():.4f}')
     t = lambda a: torch.tensor(np.asarray(a), dtype=torch.float64)  # noqa: E731
-    save(out, 'darcy_gen.pt', dict(eigenvalues=t(eigenvalues), f_s=t(f_s), int_cond=t(int_cond).reshape(-1),
-                                   seed=torch.tensor(fx['seed'], dtype=torch.int64), z=t(fx['z']), K=t(fx['K']),
-                                   p=t(fx['p']), res=t(fx['res'])))
+    out_fx = dict(eigenvalues=t(eigenvalues), f_s=t(f_s), int_cond=t(int_cond).reshape(-1),
+                  seed=torch.tensor(fx['seed'], dtype=torch.int64), z=t(fx['z']), K=t(fx['K']), p=t(fx['p']),
+                  res=t(fx['res']))
+
+    # geometry_*: the same generate_sample away from the default geometry (pixel centres, h = L / P, the plain-mean
+    # integral row, d1 = +h with the -D1 | +D1 BC rows), two samples
+    pab, reverse_dy, dl = False, False, 2.
+    pts = G.uniform_points_pixelwise(P, dl, pab)
+    d0 = d1 = dl / P
+    eigenvalues, eigenvectors = G.compute_eigenpairs(G.complete_covariance_matrix(pts, l), q)
+    f_s = G.create_f_s(pts[:, 0], pts[:, 1])
+    int_cond = G.create_int_cond(pab, shape, d0)
+    fx = dict(seed=[], K=[], p=[], res=[])
+    for s in (3, 90210):
+        G.os = types.SimpleNamespace(getpid=lambda s=s: s)
+        G.time = types.SimpleNamespace(time=lambda: 0.001)
+        args = (0, eigenvalues, eigenvectors, q, P, shape, acc, d0, d1, f_s, int_cond, xmin_bd, xmax_bd, ymin_bd,
+                ymax_bd, reverse_dy)
+        K, p, res, seed = G.generate_sample(args)
+        assert seed == s, (seed, s)
+        for k, v in zip(('seed', 'K', 'p', 'res'), (seed, K, p, res)):
+            fx[k].append(v)
+        print(f'geometry seed {s}: res {res:.6e}  max|p| {np.abs(p).max():.4f}')
+    geometry = dict(pixels_at_boundary=torch.tensor(pab), reverse_dy=torch.tensor(reverse_dy),
+                    domain_length=torch.tensor(dl, dtype=torch.float64), f_s=t(f_s), int_cond=t(int_cond).reshape(-1),
+                    seed=torch.tensor(fx['seed'], dtype=torch.int64), K=t(fx['K']), p=t(fx['p']), res=t(fx['res']))
+    out_fx.update({f'geometry_{k}': v for k, v in geometry.items()})
+    save(out, 'darcy_gen.pt', out_fx)
 
 
 DDIM_WALK = dict(n_steps=100, t=(0, 2, 57, 99), seed=13, sample=4096)

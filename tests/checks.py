@@ -120,3 +120,57 @@ def conv_ref(x, wp, bias, res, k):
     if res is not None:
         y = y + res
     return y
+
+
+# ---- known-answer operands of the Darcy data generator (tests/test_gpu_darcy_gen_replay.py; their exactness is
+# checked on the host in tests/test_oracle_darcy_gen.py) ----------------------------------------------------------------
+DGEN_BW = 3 * P + 3                 # half-bandwidth of the normal equations; the row-band layout holds d = 0 .. DGEN_BW
+# spacing exactly 1 (twice) and 2^-6: every A coefficient, N = M^T M entry and A^T f_s of the dyadic operands below is
+# exact in fp64, so the kernel's assembly must equal the oracle's bit for bit
+DGEN_EXACT_GEOMETRIES = [dict(pixels_at_boundary=True, reverse_dy=True, domain_length=63.),
+                         dict(pixels_at_boundary=False, reverse_dy=True, domain_length=64.),
+                         dict(pixels_at_boundary=False, reverse_dy=True, domain_length=1.)]
+
+
+def dgen_dyadic_K(B, g, device='cuda'):
+    """K = k / 16, k in [16, 256): [B, P*P] fp64"""
+    return torch.randint(16, 256, (B, P * P), generator=g, device=device).double() / 16
+
+
+def dgen_dyadic_source(g, device='cuda'):
+    """a dense integer source in [-8, 8]: [P*P] fp64"""
+    return torch.randint(-8, 9, (P * P,), generator=g, device=device).double()
+
+
+def dgen_dyadic_factor(B, g, device='cuda', fill=float('nan')):
+    """L0 in row-band layout [B, P*P, DGEN_BW + 1]: diagonal 4, the other band entries in {-2..2} / 256 and `fill` where
+    the column r - d is negative.  L0 L0^T is exact in fp64 and diagonally dominant, so its Cholesky factor is L0 in
+    any order of operations"""
+    n = P * P
+    L = torch.randint(-2, 3, (B, n, DGEN_BW + 1), generator=g, device=device).double() / 256
+    L[:, :, 0] = 4.
+    r = torch.arange(n, device=device)[:, None]
+    d = torch.arange(DGEN_BW + 1, device=device)[None, :]
+    L[:, (r - d < 0)] = fill
+    return L
+
+
+def dgen_band_to_dense(band):
+    """lower-triangular dense [P*P, P*P] from one row-band matrix [P*P, DGEN_BW + 1] (entries of negative column
+    ignored)"""
+    n = band.shape[0]
+    r = torch.arange(n, device=band.device)[:, None].expand(n, DGEN_BW + 1)
+    c = r - torch.arange(DGEN_BW + 1, device=band.device)[None, :]
+    ok = c >= 0
+    dense = torch.zeros(n, n, dtype=band.dtype, device=band.device)
+    dense[r[ok], c[ok]] = band[ok]
+    return dense
+
+
+def dgen_dense_to_band(dense, fill=0.):
+    """row-band layout of the lower triangle of dense [P*P, P*P]: band[r, d] = dense[r, r - d], `fill` where r < d"""
+    n = dense.shape[0]
+    r = torch.arange(n, device=dense.device)[:, None]
+    c = r - torch.arange(DGEN_BW + 1, device=dense.device)[None, :]
+    band = dense[r, c.clamp_min(0)]
+    return torch.where(c >= 0, band, torch.full_like(band, fill))

@@ -32,8 +32,8 @@ def test_library_builds_loads_and_exports_header_symbols():
 HOST_QUERIES = ['pidm_version', 'pidm_last_error', 'pidm_conv2d_tc_plan', 'pidm_conv2d_wgrad_tc_plan',
                 'pidm_groupnorm_plan', 'pidm_linattn_block_plan', 'pidm_linattn_plan', 'pidm_darcy_gen_workspace_bytes']
 TESTED_OUTSIDE_THE_RECORDINGS = {
-    'pidm_darcy_gen_kle': 'test_gpu_darcy_gen.py::test_kle',                  # the Darcy training-data generator
-    'pidm_darcy_gen_solve': 'test_gpu_darcy_gen.py::test_fixture_solve',
+    'pidm_darcy_gen_kle': 'test_gpu_darcy_gen_replay.py::test_kle_known_answer',  # the Darcy training-data generator
+    'pidm_darcy_gen_solve': 'test_gpu_darcy_gen_replay.py::test_stages_within_bounds',
     'pidm_swap_f32': 'test_gpu_ema_eval.py::test_swap_is_an_exact_exchange',  # the EMA weight swap
     'pidm_fd_stencil': 'test_gpu_physics_census.py::test_darcy_fd_stencil_replay',
     'pidm_darcy_jacobian_max': 'test_gpu_physics_census.py::test_darcy_jacobian_max_replay',

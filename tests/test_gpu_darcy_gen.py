@@ -181,3 +181,50 @@ def test_csv_round_trip(gen, tmp_path):
     assert np.array_equal(exact('seeds.csv')[:, 0], np.arange(40, 45))
     assert np.array_equal(exact('res_data.csv')[:, 0], res.cpu().numpy())
     assert np.array_equal(exact('p_data.csv'), p.cpu().numpy()) and np.array_equal(exact('K_data.csv'), K.cpu().numpy())
+
+
+# ---- a second geometry: pixel centres, h = L / P, the plain mean, reverse_dy = False -----------------------------------
+@pytest.fixture(scope='module')
+def fxg(golden):
+    return {k[len('geometry_'):]: v for k, v in golden('darcy_gen.pt').items() if k.startswith('geometry_')}
+
+
+def _geometry(fxg):
+    return dict(pixels_at_boundary=bool(fxg['pixels_at_boundary']), reverse_dy=bool(fxg['reverse_dy']),
+                domain_length=float(fxg['domain_length']))
+
+
+def test_fixture_solve_at_another_geometry(gen, fxg):
+    from physicsinformeddiffusionmodels_b200.darcy_data_generation import DarcyDataGenerator
+    geo = _geometry(fxg)
+    g = DarcyDataGenerator(eigenpairs=(gen.eigenvalues, gen.eigenvectors), **geo)
+    assert np.array_equal(g.f_s_np, fxg['f_s'].numpy())
+    assert np.array_equal(g.int_cond.reshape(-1), fxg['int_cond'].numpy())
+    p, res = g.solve_pressure(fxg['K'].to(DEV))
+    p, res = p.cpu().numpy(), res.cpu().numpy()
+    for b in range(len(fxg['seed'])):
+        assert _close_p(p[b], fxg['p'][b].numpy())
+        assert abs(res[b] - fxg['res'][b].item()) <= 1e-4 * fxg['res'][b].item()
+
+
+@pytest.mark.parametrize('pab, dl', [(False, 2.), (True, 0.3)])
+def test_generate_sample_infers_the_geometry(gen, pab, dl):
+    """the reference's argument tuple carries the geometry as d0 and the shape of int_cond: generate_sample must solve
+    at the geometry that tuple describes, bit for bit what DarcyDataGenerator at that geometry computes"""
+    from physicsinformeddiffusionmodels_b200 import darcy_data_generation as G
+    shape, q = (P, P), gen.q
+    d0 = dl / (P - 1) if pab else dl / P
+    grid = G.uniform_points_pixelwise(P, dl, pab)
+    f_s = G.create_f_s(grid[:, 0], grid[:, 1])
+    int_cond = G.create_int_cond(pab, shape, d0)
+    args = (17, gen.eigenvalues, gen.eigenvectors, q, P, shape, 2, d0, d0, f_s, int_cond, *G.create_boundary_idcs(shape),
+            False)
+    K, p, res, seed = G.generate_sample(args)
+    g = G.DarcyDataGenerator(domain_length=dl, reverse_dy=False, pixels_at_boundary=pab,
+                             eigenpairs=(gen.eigenvalues, gen.eigenvectors))
+    K_ref, p_ref, res_ref, seeds = g.generate([17])
+    assert seed == 17 == int(seeds[0])
+    assert np.array_equal(K, K_ref[0].cpu().numpy()) and np.array_equal(p, p_ref[0].cpu().numpy())
+    assert res == res_ref[0].item()
+    # and not the default geometry's answer
+    assert not np.array_equal(p, gen.solve_pressure(K_ref)[0][0].cpu().numpy())
