@@ -1,4 +1,4 @@
-"""The census of the benchmarked and sampling steps, shared by the seven per-element census files
+"""The census of the benchmarked and sampling steps, shared by the eight per-element census files
 (tests/test_gpu_*_census.py).
 
 One eager step of every workload bench.py times (Darcy training at batch 32, one Darcy sampling step at batch 16 / 64 /
@@ -129,6 +129,11 @@ KEYS = {
     'pidm_darcy_cocogen': lambda a: [('cocogen', (int(a[6]), int(a[7]), float(a[8]), int(a[9]), int(a[10]), int(a[5]),
                                                   int(a[4]), _has(a[3])))],
     'pidm_toy_pidm_loss': lambda a: [('toy_loss', (int(a[17]), int(a[18]), _has(a[3]), _has(a[4]), _has(a[6])))],
+    # test_gpu_mech_eval_census.py
+    'pidm_mech_sample_input': lambda a: [('mech_input', (int(a[3]), int(a[4]), int(a[5])))],
+    'pidm_mech_posterior_step': lambda a: [('mech_post', (int(a[8]), int(a[9])))],
+    'pidm_mech_fem_pcg': lambda a: [('pcg', (int(a[8]), int(a[9]), float(a[6]), int(a[7])))],
+    'pidm_mech_floating_material': lambda a: [('fm', (int(a[2]), int(a[3])))],
 }
 
 # the families of KEYS by the census file that holds their tables, in the order of its tables
@@ -142,9 +147,11 @@ FAMILIES = {
                                 'pair_launch', 'qsample', 'axpby', 'scale', 'concat', 'split', 'nchw'),
     'test_gpu_simt_census.py': ('simt', 'simt_wgrad'),
     'test_gpu_sampling_census.py': ('ddim', 'posterior', 'cocogen', 'toy_loss'),
+    'test_gpu_mech_eval_census.py': ('mech_input', 'mech_post', 'pcg', 'fm'),
 }
 # the recording each census file's tables are checked against, where it is not census()
-RECORDING = {'test_gpu_simt_census.py': 'census_exact', 'test_gpu_sampling_census.py': 'census_sampling'}
+RECORDING = {'test_gpu_simt_census.py': 'census_exact', 'test_gpu_sampling_census.py': 'census_sampling',
+             'test_gpu_mech_eval_census.py': 'census_sampling'}
 
 # Entry points the benchmarked steps call that launch nothing: host-side capability and size queries.
 LAUNCHES_NOTHING = [
@@ -158,17 +165,12 @@ LAUNCHES_NOTHING = [
     'pidm_pack_pair_entry_size',
 ]
 
-# Entry points of the exact mode and of the sampling steps that no census family keys, with the per-element or bitwise
-# test that checks them
+# Entry points of the exact mode that no census family keys, with the per-element or bitwise test that checks them
 CHECKED_ELSEWHERE = {
     'pidm_wrap_pad_nhwc': 'test_gpu_circular.py::test_wrap_pad_is_bitwise_circular_pad',
     'pidm_cond_embed_fwd': 'test_gpu_guidance.py::test_cond_embed_per_element',
     'pidm_cond_embed_wgrad': 'test_gpu_guidance.py::test_cond_embed_wgrad_per_element',
     'pidm_darcy_abs_residual_grad': 'test_gpu_guidance.py::test_abs_residual_grad_per_element',
-    'pidm_mech_sample_input': 'test_gpu_mech_sample.py::test_sample_kernels_match_their_torch_composition',
-    'pidm_mech_posterior_step': 'test_gpu_mech_sample.py::test_sample_kernels_match_their_torch_composition',
-    'pidm_mech_fem_pcg': 'test_gpu_mech_sample.py::test_fused_solver_against_sparse_direct_solve',
-    'pidm_mech_floating_material': 'test_gpu_mech_sample.py::test_floating_material_kernel_matches_host_labelling',
 }
 
 

@@ -122,6 +122,30 @@ def conv_ref(x, wp, bias, res, k):
     return y
 
 
+# ---- bilinear resize (align_corners=False, no antialias), shared by the physics and mechanics-evaluation census files ---
+def resize_src_index(n_out, n_in, clamp_hi=None):
+    """bil_src in fp64: source rows i0, i1, the weight of i1 and the error of bil_src's fp32 source coordinate
+    s = (o + 0.5) * fl(in / out) - 0.5: each of fl(in / out), the product and the subtraction rounds once, so
+    |s32 - s| <= 2^-24 (3 (o + 0.5) in / out + 1).  clamp_hi: the largest i0 (the mutant clamps one pixel early)."""
+    o = torch.arange(n_out, dtype=torch.float64)
+    s = ((o + 0.5) * (n_in / n_out) - 0.5).clamp_min(0)
+    i0 = s.floor().clamp_max(n_in - 1 if clamp_hi is None else clamp_hi).long()
+    i1 = torch.where(i0 < n_in - 1, i0 + 1, i0)
+    return i0, i1, s - i0, U * (3 * (o + 0.5) * n_in / n_out + 1)
+
+
+def resize_bounds(x, n_out):
+    """(C-free part A, coordinate term) of the forward bound: |y - r| <= C u A + (e_h + e_w) D, D = twice the largest
+    |x| on source rows / columns i0 - 1 .. i0 + 1 (a coordinate error e moves y by at most e times the largest
+    neighbour difference, also when it moves s across a pixel boundary)"""
+    n_in = x.shape[-1]
+    A = F.interpolate(x.abs()[:, None], size=(n_out, n_out), mode='bilinear', align_corners=False)[:, 0]
+    i0, _, _, e = resize_src_index(n_out, n_in)
+    M = F.max_pool2d(x.abs()[:, None], 3, stride=1, padding=1)[:, 0]
+    D = 2 * M[:, i0][:, :, i0]
+    return A, (e[:, None] + e[None, :]) * D
+
+
 # ---- known-answer operands of the Darcy data generator (tests/test_gpu_darcy_gen_replay.py; their exactness is
 # checked on the host in tests/test_oracle_darcy_gen.py) ----------------------------------------------------------------
 DGEN_BW = 3 * P + 3                 # half-bandwidth of the normal equations; the row-band layout holds d = 0 .. DGEN_BW

@@ -4,7 +4,9 @@ the reference) and by the tests.
 
 * `conditioning_batch()`: the B = 2 conditioning fields, boundary conditions and data densities of the fixture.
 * `replay_draws(gd, mode)`: the reference loop's draws regenerated from the fixture's seed on the CPU generator, checked
-  against the fixture's per-draw checksums, so a generator mismatch is reported as such and not as a parity failure."""
+  against the fixture's per-draw checksums, so a generator mismatch is reported as such and not as a parity failure.
+* `binarised_designs(B, seed)`: binarised densities under four support / load cases, the systems the evaluation solve
+  is checked on."""
 import torch
 
 B = 2
@@ -62,3 +64,35 @@ def inputs(gd):
     assert torch.equal(torch.stack([cond.double().sum(), bcs.double().sum(), rho.double().sum()]), gd['input_checksum'])
     assert torch.equal(gd['solution'][:, 2, :-1, :-1], rho)
     return cond, bcs, gd['solution']
+
+
+def binarised_designs(B, seed):
+    """B designs with rho in {1e-3, 1} (smooth random fields thresholded) under different supports and loads"""
+    g = torch.Generator().manual_seed(seed)
+    i = torch.arange(64, dtype=torch.float32) / 63
+    X, Y = torch.meshgrid(i, i, indexing='ij')
+    rho = torch.empty(B, 64, 64)
+    bcs = torch.zeros(B, 4, 65, 65)
+    for b in range(B):
+        f = torch.zeros(64, 64)
+        for _ in range(5):
+            a, kx, ky, ph = torch.randn(1, generator=g), *torch.randint(1, 5, (2,), generator=g), torch.rand(1, generator=g) * 6
+            f += a * torch.sin(3.1 * kx * X + ph) * torch.cos(3.1 * ky * Y + 0.5 * ph)
+        thr = torch.quantile(f.reshape(-1), 0.3 + 0.3 * torch.rand(1, generator=g).item())
+        rho[b] = torch.where(f > thr, torch.ones_like(f), torch.full_like(f, 1e-3))
+        case = b % 4
+        if case in (0, 1):                                # cantilever: clamped left edge
+            bcs[b, 0, :, 0] = 1.
+            bcs[b, 1, :, 0] = 1.
+        else:                                             # bridge: pinned bottom corners
+            bcs[b, :2, 64, :3] = 1.
+            bcs[b, 1, 64, 62:] = 1.
+        row = int(torch.randint(8, 56, (1,), generator=g))
+        if case == 0:
+            bcs[b, 3, row:row + 3, 64] = -1. / 3
+        elif case == 1:
+            bcs[b, 2, 0, 20 + row // 2] = 0.5
+            bcs[b, 3, 64, 60] = -0.5
+        else:
+            bcs[b, 3, 0, row - 4:row + 4] = -1. / 8
+    return rho, bcs

@@ -61,6 +61,28 @@ def test_every_header_entry_point_is_accounted_for():
             assert re.search(rf'^def {fn}\(', f.read(), re.M), f'{name}: {test} does not exist'
 
 
+@pytest.mark.parametrize('name,args,what', [
+    ('pidm_mech_fem_pcg', dict(nel=67), 'nel'), ('pidm_mech_fem_pcg', dict(nel=1), 'nel'),
+    ('pidm_mech_fem_pcg', dict(B=0), 'B='), ('pidm_mech_fem_pcg', dict(max_iter=-1), 'max_iter'),
+    ('pidm_mech_fem_pcg', dict(tol=-1e-9), 'tol'),
+    ('pidm_mech_floating_material', dict(nel=0), 'nel'), ('pidm_mech_floating_material', dict(nel=129), 'nel'),
+    ('pidm_mech_floating_material', dict(B=0), 'B='),
+    ('pidm_mech_posterior_step', dict(P=1), 'P='), ('pidm_mech_posterior_step', dict(B=0), 'B='),
+    ('pidm_mech_sample_input', dict(P=1), 'P='), ('pidm_mech_sample_input', dict(B=0), 'B='),
+], ids=lambda v: v if isinstance(v, str) else '-'.join(f'{k}{x}' for k, x in v.items()) if isinstance(v, dict) else '')
+def test_mech_eval_sizes_are_refused_before_any_launch(name, args, what):
+    """sizes the topology-optimisation kernels do not support fail the size check (error code 2), which runs before
+    any CUDA call: null pointers and no device are enough"""
+    from physicsinformeddiffusionmodels_b200._lib import call
+    a = {**dict(B=2, nel=64, P=64, tol=1e-6, max_iter=10), **args}
+    argv = {'pidm_mech_fem_pcg': (None,) * 6 + (a['tol'], a['max_iter'], a['B'], a['nel'], None),
+            'pidm_mech_floating_material': (None, None, a['B'], a['nel'], None),
+            'pidm_mech_posterior_step': (None,) * 8 + (a['B'], a['P'], None),
+            'pidm_mech_sample_input': (None,) * 3 + (a['B'], 7, a['P'], None)}[name]
+    with pytest.raises(RuntimeError, match=rf'\(code 2\): {name[5:]}: .*{what}'):
+        call(name, *argv)
+
+
 def test_no_oracle_import_on_product_path():
     """The product package must never reach into oracle/ (selftest.smoke is the one sanctioned checker)."""
     pkg = os.path.join(ROOT, 'physicsinformeddiffusionmodels_b200')

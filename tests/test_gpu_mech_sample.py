@@ -1,6 +1,7 @@
 """Conditional sampling of the topology-optimisation model (configs[2]) on the graph-replayed SampleEngine and its
 evaluation solve, against the unmodified reference (tests/golden/mechanics_sample_loop.pt, mechanics_eval.pt) and the
-fp64 sparse direct solve of oracle/pidm_oracle.py."""
+fp64 sparse direct solve of oracle/pidm_oracle.py.  The four kernels of these steps (sample input, posterior step, PCG
+solve, floating-material flag) are checked per element in tests/test_gpu_mech_eval_census.py."""
 import pytest
 import torch
 
@@ -189,38 +190,6 @@ def test_mech_sample_and_fused_solve_do_not_sync(env, golden):
 
 # ---- the fused solver ------------------------------------------------------------------------------------------------
 
-def binarised_designs(B, seed):
-    """B designs with rho in {1e-3, 1} (smooth random fields thresholded) under different supports and loads"""
-    g = torch.Generator().manual_seed(seed)
-    i = torch.arange(64, dtype=torch.float32) / 63
-    X, Y = torch.meshgrid(i, i, indexing='ij')
-    rho = torch.empty(B, 64, 64)
-    bcs = torch.zeros(B, 4, 65, 65)
-    for b in range(B):
-        f = torch.zeros(64, 64)
-        for _ in range(5):
-            a, kx, ky, ph = torch.randn(1, generator=g), *torch.randint(1, 5, (2,), generator=g), torch.rand(1, generator=g) * 6
-            f += a * torch.sin(3.1 * kx * X + ph) * torch.cos(3.1 * ky * Y + 0.5 * ph)
-        thr = torch.quantile(f.reshape(-1), 0.3 + 0.3 * torch.rand(1, generator=g).item())
-        rho[b] = torch.where(f > thr, torch.ones_like(f), torch.full_like(f, 1e-3))
-        case = b % 4
-        if case in (0, 1):                                # cantilever: clamped left edge
-            bcs[b, 0, :, 0] = 1.
-            bcs[b, 1, :, 0] = 1.
-        else:                                             # bridge: pinned bottom corners
-            bcs[b, :2, 64, :3] = 1.
-            bcs[b, 1, 64, 62:] = 1.
-        row = int(torch.randint(8, 56, (1,), generator=g))
-        if case == 0:
-            bcs[b, 3, row:row + 3, 64] = -1. / 3
-        elif case == 1:
-            bcs[b, 2, 0, 20 + row // 2] = 0.5
-            bcs[b, 3, 64, 60] = -0.5
-        else:
-            bcs[b, 3, 0, row - 4:row + 4] = -1. / 8
-    return rho, bcs
-
-
 def test_fused_solver_against_sparse_direct_solve(env, golden):
     """fem_solve_fused against the fp64 sparse direct solve on the mechanics_eval.pt designs (its data density and the
     binarised x0 of its golden) and on 12 binarised designs under four support / load cases, next to fem_solve on the
@@ -229,7 +198,7 @@ def test_fused_solver_against_sparse_direct_solve(env, golden):
     ev = golden('mechanics_eval.pt')
     res = ResidualsMechanics(model=None, pixels_per_dim=64, pixels_at_boundary=True, no_BC_folder='', device=DEV)
     x0 = ev['x0_pred'][:, 2]
-    rho_bin, bcs = binarised_designs(12, seed=5)
+    rho_bin, bcs = MI.binarised_designs(12, seed=5)
     cases = [('eval_rho_simp', ev['solution'][:, 2, :-1, :-1], ev['bcs']),
              ('eval_x0_binarised', torch.where(x0 > 0.5, torch.ones_like(x0), torch.full_like(x0, 1e-3)), ev['bcs']),
              ('binarised', rho_bin, bcs)]
@@ -273,54 +242,3 @@ def test_fused_metrics_on_reference_golden(env, golden):
     with pytest.raises(AssertionError):
         res.topopt_metrics(*args[:3], bad.to(DEV))
     assert torch.isnan(res.topopt_metrics(*args[:3], bad.to(DEV), solver='fused')['rel_CE_error_full_batch']).all()
-
-
-def test_floating_material_kernel_matches_host_labelling(env):
-    """the device connected-component flag against the reference's cv2 / scipy labelling on designs with 0, 1 and many
-    components, diagonal-only contacts included"""
-    from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import compute_fm, floating_material
-    g = torch.Generator().manual_seed(9)
-    rho = (torch.rand(16, 64, 64, generator=g) > torch.linspace(0.05, 0.95, 16)[:, None, None]).float()
-    rho[0] = 0.
-    rho[1] = 1.
-    rho[2] = 0.
-    rho[2, 10, 10] = rho[2, 11, 11] = 1.                 # touching diagonally: one 8-connected component
-    rho[3] = 0.
-    rho[3, :, ::2] = 1.                                  # 32 separate stripes
-    rho[4] = 0.
-    for k in range(0, 64, 2):                            # one long snake
-        rho[4, k, :] = 1.
-        rho[4, k + 1, 63 if (k // 2) % 2 == 0 else 0] = 1.
-    d = rho.to(DEV)
-    assert torch.equal(floating_material(d).cpu(), compute_fm(d).long())
-    assert floating_material(d)[:5].tolist() == [1, 0, 0, 1, 0]
-
-
-def test_sample_kernels_match_their_torch_composition(env):
-    """pidm_mech_sample_input equals resize(cat(x, cond)) bit for bit; pidm_mech_posterior_step equals the reference's
-    model_out assembly followed by the per-sample axpby."""
-    import torch.nn.functional as F
-    from physicsinformeddiffusionmodels_b200 import ops
-    from physicsinformeddiffusionmodels_b200.residuals_mechanics_K import resize_image
-    g = torch.Generator().manual_seed(1)
-    B = 3
-    x = torch.randn(B, 3, 65, 65, generator=g).to(DEV)
-    cond = torch.randn(B, 3, 65, 65, generator=g).to(DEV)
-    bcs = torch.randn(B, 4, 65, 65, generator=g).to(DEV)
-    planes = torch.cat((resize_image(cond, 64), resize_image(bcs, 64)), dim=1).contiguous()
-    out = torch.empty(B, 10, 64, 64, device=DEV)
-    ops.mech_sample_input(x, planes, out)
-    ref = torch.cat((resize_image(torch.cat((x, cond), dim=1), 64), resize_image(bcs, 64)), dim=1)
-    assert torch.equal(out, ref)
-    y = torch.rand(B, 3, 64, 64, generator=g).to(DEV)
-    z = torch.randn(B, 3, 65, 65, generator=g).to(DEV)
-    t = torch.tensor([0, 7, 3], device=DEV)
-    c1, c2, sig = (torch.rand(10, generator=g).to(DEV) for _ in range(3))
-    xo = torch.empty_like(x)
-    ops.mech_posterior_step(y, x, z, t, c1, c2, sig, xo)
-    mo = torch.cat((resize_image(y[:, :2], 65), F.pad(y[:, 2], (0, 1, 0, 1)).unsqueeze(1)), dim=1)
-    ref = c1[t].view(B, 1, 1, 1) * mo + c2[t].view(B, 1, 1, 1) * x + sig[t].view(B, 1, 1, 1) * z
-    assert (xo - ref).abs().max().item() < 1e-5
-    x_in = x.clone()
-    ops.mech_posterior_step(y, x_in, z, t, c1, c2, sig, x_in)       # in place
-    assert torch.equal(x_in, xo)

@@ -27,7 +27,7 @@ import torch
 import torch.nn.functional as F
 
 from census import KEYS, LAUNCHES_NOTHING, assert_census_in_tables, assert_tables_in_census, census
-from checks import P, U, call_sync, check, gen, guarded, guards_intact, sms
+from checks import P, U, call_sync, check, gen, guarded, guards_intact, resize_bounds, resize_src_index, sms
 from oracle import pidm_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -648,35 +648,12 @@ def _planes(spec, out):
     return spec if isinstance(spec, int) else -(-3 * 8 * sms() * 256 // (out * out))
 
 
-def _src_index(n_out, n_in, clamp_hi=None):
-    """bil_src in fp64: source rows i0, i1, the weight of i1 and the error of bil_src's fp32 source coordinate
-    s = (o + 0.5) * fl(in / out) - 0.5: each of fl(in / out), the product and the subtraction rounds once, so
-    |s32 - s| <= 2^-24 (3 (o + 0.5) in / out + 1).  clamp_hi: the largest i0 (the mutant clamps one pixel early)."""
-    o = torch.arange(n_out, dtype=torch.float64)
-    s = ((o + 0.5) * (n_in / n_out) - 0.5).clamp_min(0)
-    i0 = s.floor().clamp_max(n_in - 1 if clamp_hi is None else clamp_hi).long()
-    i1 = torch.where(i0 < n_in - 1, i0 + 1, i0)
-    return i0, i1, s - i0, U * (3 * (o + 0.5) * n_in / n_out + 1)
-
-
 def resize_gather(x, n_out, clamp_hi=None):
     """bilinear resize from the fp64 index arithmetic (used for the mutants)"""
     n_in = x.shape[-1]
-    i0, i1, w, _ = _src_index(n_out, n_in, clamp_hi)
+    i0, i1, w, _ = resize_src_index(n_out, n_in, clamp_hi)
     rows = x[:, i0] * (1 - w)[:, None] + x[:, i1] * w[:, None]
     return rows[:, :, i0] * (1 - w) + rows[:, :, i1] * w
-
-
-def resize_bounds(x, n_out):
-    """(C-free part A, coordinate term) of the forward bound: |y - r| <= C u A + (e_h + e_w) D, D = twice the largest
-    |x| on source rows / columns i0 - 1 .. i0 + 1 (a coordinate error e moves y by at most e times the largest
-    neighbour difference, also when it moves s across a pixel boundary)"""
-    n_in = x.shape[-1]
-    A = F.interpolate(x.abs()[:, None], size=(n_out, n_out), mode='bilinear', align_corners=False)[:, 0]
-    i0, _, _, e = _src_index(n_out, n_in)
-    M = F.max_pool2d(x.abs()[:, None], 3, stride=1, padding=1)[:, 0]
-    D = 2 * M[:, i0][:, :, i0]
-    return A, (e[:, None] + e[None, :]) * D
 
 
 @pytest.mark.parametrize('row', [k for k in RESIZE_FWD_TABLE] + [(pl, i, o) for i, o in RESIZE_SHAPES for pl in (3, 'multi')],
@@ -698,7 +675,7 @@ def resize_bwd_bounds(dy, n_in):
     rows / columns i0 - 1 .. i0 + 2; at most (out / in + 2)^2 atomics land on one element"""
     n_out = dy.shape[-1]
     A = resize_adjoint(dy.abs(), n_in)
-    i0, _, _, e = _src_index(n_out, n_in)
+    i0, _, _, e = resize_src_index(n_out, n_in)
     w = dy.abs() * (e[:, None] + e[None, :])
     T = torch.zeros(dy.shape[0], n_in, n_in, dtype=torch.float64)
     for dr in range(-1, 3):
