@@ -146,14 +146,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                                                                 const __grid_constant__ CUtensorMap map_w, TcParams p) {
     using Cfg = TcCfg<BN, BK>;
     extern __shared__ unsigned char smem_raw[];
-    // 1024-byte aligned operand ring (required by the 128B swizzle atoms)
-    const uint32_t raw_addr = smem_u32(smem_raw);
-    const uint32_t pad_bytes = (1024 - (raw_addr & 1023)) & 1023;
+    const uint32_t pad_bytes = smem_pad_1024(smem_raw);
     unsigned char* wres = smem_raw + pad_bytes;              // resident weights (res_bytes, may be 0)
     unsigned char* ring = wres + p.res_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + pad_bytes + p.operand_bytes);
-    uint64_t* full = bars;                                   // [TC_MAX_STAGES]
-    uint64_t* empty = bars + TC_MAX_STAGES;                  // [TC_MAX_STAGES]
+    TmaRing tma{bars, bars + TC_MAX_STAGES};                 // full / empty barriers: [TC_MAX_STAGES] each
     uint64_t* acc_full = bars + 2 * TC_MAX_STAGES;           // the accumulator tile is parked in shared memory
     uint64_t* acc_empty = acc_full + 1;                      // ... and has been read back by the epilogue
     uint64_t* wfull = acc_empty + 1;                         // resident weights have landed
@@ -167,16 +164,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     pdl_trigger();
 
     if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+        prefetch_tensormap(&map_x);
+        prefetch_tensormap(&map_w);
     }
     if (warp == 1 && lane == 0) {
-        // a ring stage is free once all 8 consumer warps have retired the wgmmas that read it
-        for (int s = 0; s < n_stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+        tma.init(n_stages);
         mbar_init(acc_full, 256);
         mbar_init(acc_empty, 128);
         mbar_init(wfull, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
     __syncthreads();
     pdl_wait();                 // prologue done; everything below reads what the previous kernel wrote
@@ -193,8 +189,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 mbar_expect_tx(wfull, (uint32_t)(n_k * Cfg::B_BYTES));
                 for (int i = 0; i < n_k; ++i) tma_load_2d(wres + (size_t)i * Cfg::B_BYTES, &map_w, wfull, i * BK, 0);
             }
-            // ring position (stage, phase, whose turn) is carried incrementally: no integer divisions in the loop
-            uint32_t st = 0, ph = 0, turn = 0;
+            // ring position and whose turn it is are carried incrementally: no integer divisions in the loop.  Every
+            // producer walks every stage; only the one whose turn it is loads it.
+            uint32_t turn = 0;
             unsigned char* a_dst = ring;
             const int groups_m0 = p.rg ? p.KW : p.KH * p.KW;
             int tile_m = blockIdx.x % p.m_tiles, rest = blockIdx.x / p.m_tiles;      // tile = rest * m_tiles + tile_m
@@ -220,18 +217,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     int kcol = ktap * p.Cin;
                     for (int kc = 0; kc < kc_per_tap; ++kc, kcol += BK) {
                         if (turn == pidx) {
-                            mbar_wait(&empty[st], ph ^ 1);
-                            mbar_expect_tx(&full[st], (uint32_t)p.stage_bytes);
-                            tma_load_4d(a_dst, &map_x, &full[st], kc * BK, ww0 + dw, hh0 + dh, b0);
+                            uint64_t* full = tma.acquire((uint32_t)p.stage_bytes);
+                            tma_load_4d(a_dst, &map_x, full, kc * BK, ww0 + dw, hh0 + dh, b0);
                             if (!p.resident) {
                                 unsigned char* b_dst = a_dst + p.a_bytes;
                                 int kj = kcol;
                                 for (int j = 0; j < p.nb; ++j, kj += p.KW * p.Cin, b_dst += Cfg::B_BYTES)
-                                    tma_load_2d(b_dst, &map_w, &full[st], kj, n0);   // row-group mode: tap (r = j, q = g)
+                                    tma_load_2d(b_dst, &map_w, full, kj, n0);   // row-group mode: tap (r = j, q = g)
                             }
                         }
                         if (++turn == 4u) turn = 0;
-                        if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_dst = ring; } else a_dst += p.stage_bytes;
+                        if (tma.advance((uint32_t)n_stages)) a_dst = ring; else a_dst += p.stage_bytes;
                     }
                 }
                 tile_m += step_m; rest += step_r;
@@ -258,7 +254,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         const bool resident = p.resident != 0;
         // fragment -> staging tile: this thread's rows 64 cg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
         float* acc_row = acc_tile + (size_t)(64 * cg + 16 * (warp & 3) + (lane >> 2)) * Cfg::ACC_PITCH + 2 * (lane & 3);
-        uint32_t st = 0, ph = 0, a_lo = ring_lo;
+        uint32_t a_lo = ring_lo;
         int rest = blockIdx.x / p.m_tiles, tile_m = blockIdx.x % p.m_tiles;
         const int step_m = gridDim.x % p.m_tiles, step_r = gridDim.x / p.m_tiles;
         int lt = 0;
@@ -268,9 +264,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             if (lt == 0 && resident) mbar_wait(wfull, 0);
             uint32_t accum = 0;
             uint32_t res_lo = wres_lo;                           // resident weights: tile (it) of kernel row 0
-            uint32_t prev_st = 0;
             for (int it = 0; it < n_iters; ++it, res_lo += b_tile_lo) {
-                mbar_wait(&full[st], ph);
+                tma.wait_full();
                 uint32_t aj = a_lo;
                 uint32_t bj = resident ? res_lo : a_lo + b_off_lo;
                 const uint32_t bj_step = resident ? res_j_lo : b_tile_lo;
@@ -282,14 +277,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                         accum = 1;
                     }
                 }
-                wgmma_commit();
-                wgmma_wait<1>();
-                if (it > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
-                prev_st = st;
-                if (++st == (uint32_t)n_stages) { st = 0; ph ^= 1; a_lo = ring_lo; } else a_lo += stage_lo;
+                tma.consumed(it == 0, lane);
+                if (tma.advance((uint32_t)n_stages)) a_lo = ring_lo; else a_lo += stage_lo;
             }
             wgmma_wait<0>();
-            if (n_iters > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
+            if (n_iters > 0) tma.release_held(lane);            // the ring runs on into the next tile
             mbar_wait(acc_empty, (lt & 1) ^ 1);                 // the epilogue has read the previous tile back
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {

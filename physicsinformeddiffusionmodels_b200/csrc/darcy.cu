@@ -28,26 +28,6 @@ constexpr int P = 64;             // pixels per dim (reference: pixels_per_dim =
 constexpr int PP = P * P;
 constexpr int DARCY_THREADS = 256;
 
-// the mbarrier helpers of hopper.cuh: including that header instead changes the code nvcc generates for
-// darcy_grad_kernel<2, true>
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                      smem_u32(dst)),
@@ -230,7 +210,7 @@ __global__ void __launch_bounds__(DARCY_THREADS) darcy_fwd_kernel(const float* _
     if (tid == 0) {
         mbar_init(&S.bar[0], 1);
         mbar_init(&S.bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
     pdl_trigger();
     __syncthreads();
@@ -362,7 +342,7 @@ __global__ void __launch_bounds__(DG_THREADS, MODE == 3 ? 1 : 0) darcy_grad_kern
     if (tid == 0) {
         mbar_init(&S.bar[0], 1);
         mbar_init(&S.bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
     pdl_trigger();
     __syncthreads();

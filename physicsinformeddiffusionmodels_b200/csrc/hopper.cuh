@@ -1,33 +1,12 @@
-// Hopper (sm_90a) building blocks of the tensor-core convolution kernels (conv_tc.cu, wgrad_tc.cu, wgrad_tc3.cu):
-// mbarrier ring plumbing, TMA tensor loads, wgmma shared-memory descriptors and the warpgroup MMA itself; on the host,
-// the activation tensor maps and the pixel tiling those kernels share.
+// Hopper (sm_90a) building blocks of the tensor-core convolution kernels (conv_tc.cu, wgrad_tc.cu): the TMA ring,
+// TMA tensor loads, wgmma shared-memory descriptors and the warpgroup MMA itself; on the host, the activation tensor
+// maps and the pixel tiling those kernels share.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
 
 namespace pidm {
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
     asm volatile(
@@ -74,6 +53,74 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int PENDING>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+
+// ---- TMA ring ---------------------------------------------------------------------------------------------------
+// Operand stages in shared memory between a TMA producer and two consumer warpgroups, each stage with two mbarriers:
+// full[s] takes one arrival (the producer's expect_tx) plus the bytes of its TMA loads; empty[s] one arrival per
+// consumer warp (8) once the wgmmas that read the stage have retired.  Both sides walk the stages in the same order,
+// each with its own TmaRing.  A barrier completes once per pass through the ring: consumers wait for `full` with the
+// parity of the current pass, the producer for `empty` with that of the previous pass (complete on a fresh barrier,
+// so the first pass finds every stage free).  Consumers keep one wgmma group in flight (consumed()).
+// The weight-gradient kernels run one pass of split-K steps per CTA and end there, so their consumers never release
+// the last stage.  The convolution's ring runs across tile boundaries: its consumers release the last stage of every
+// tile (release_held()), and its four producer warps each walk every stage but take turns loading them.
+
+// bytes from the start of the dynamic shared memory to the first 1024-byte boundary, where the ring starts (the 128B
+// swizzle atoms of TMA and wgmma need that alignment)
+__device__ __forceinline__ uint32_t smem_pad_1024(const unsigned char* smem_raw) {
+    return (1024 - (smem_u32(smem_raw) & 1023)) & 1023;
+}
+__device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+
+struct TmaRing {
+    uint64_t* full;
+    uint64_t* empty;
+    uint32_t stage = 0, phase = 0;
+    uint32_t held = 0;       // consumer side only: the stage read by the wgmma group still in flight
+
+    // the first `stages` barrier pairs (one thread; mbar_init_fence() and a CTA barrier must follow)
+    __device__ __forceinline__ void init(int stages) const {
+        for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    }
+    // producer: wait until the current stage is free and arm its `full` barrier with the bytes the loads will bring;
+    // returns that barrier for the loads to complete on
+    __device__ __forceinline__ uint64_t* acquire(uint32_t tx_bytes) const {
+        mbar_wait(&empty[stage], phase ^ 1);
+        mbar_expect_tx(&full[stage], tx_bytes);
+        return &full[stage];
+    }
+    // consumer: wait until the current stage's operands have landed
+    __device__ __forceinline__ void wait_full() const { mbar_wait(&full[stage], phase); }
+    // consumer, after issuing the wgmmas that read the current stage: commit them, wait for the previous group and,
+    // unless this stage is the first of the run, release that group's stage (lane 0 of each warp arrives)
+    __device__ __forceinline__ void consumed(bool first, int lane) {
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (!first && lane == 0) mbar_arrive(&empty[held]);
+        held = stage;
+    }
+    // consumer, once the last group has retired: release its stage too (a ring that runs on past the consumer's run)
+    __device__ __forceinline__ void release_held(int lane) const {
+        if (lane == 0) mbar_arrive(&empty[held]);
+    }
+    // next stage; true when the ring wrapped back to stage 0 (the caller rewinds its stage address)
+    __device__ __forceinline__ bool advance(uint32_t stages) {
+        if (++stage == stages) { stage = 0; phase ^= 1; return true; }
+        return false;
+    }
+};
+
+// Pixel tiles [begin, begin + count) of this CTA's split-K range (blockIdx.z) when n_pix_tiles are cut into ranges
+// of per_split (one_wave_split); count <= 0 for a CTA past the last range
+struct SplitRange { int begin, count; };
+__device__ __forceinline__ SplitRange split_k_range(int per_split, int n_pix_tiles) {
+    const int begin = blockIdx.z * per_split;
+    int end = begin + per_split;
+    if (end > n_pix_tiles) end = n_pix_tiles;
+    return {begin, end - begin};
+}
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands in shared memory, fp32 accumulator fragment in registers
 // (thread t of warp w of the warpgroup holds rows 16w + t/4 (+8), columns 8j + 2(t%4) (+1): d[4j + {0,1,2,3}]).

@@ -1,6 +1,6 @@
 """Every tensor-core launch of the benchmarked steps, replayed element by element against an fp64 reference.
 
-The convolution (conv_tc.cu), the two weight-gradient kernels (wgrad_tc.cu, wgrad_tc3.cu) and the linear-attention block
+The convolution (conv_tc.cu), the two weight-gradient kernels (wgrad_tc.cu) and the linear-attention block
 (attention_fused.cu) choose their plan -- tile widths, persistent-grid waves, pixel splits, pixel chunks -- from the batch
 size and the SM count.  The per-op tests in test_gpu_ops.py run small batches, so they see few of the plans the
 benchmark runs, and they compare whole tensors by a norm ratio, which a bug confined to one tile row cannot move.  Here:
@@ -948,7 +948,7 @@ def test_mutant_attention_block_dw_out_head_transposed():
 # ----------------------------------------------------------------------------------------------------------------------
 TC_CASES = {(128, 64), (64, 64), (32, 64), (128, 32), (64, 32), (32, 32)}        # conv_tc.cu TC_CASE
 WG_CASES = {(128, 64, 64), (128, 32, 64), (64, 64, 64), (64, 32, 64), (32, 64, 32), (32, 32, 32)}   # wgrad_tc.cu WG_CASE
-W3_CASES = {(64, 64), (32, 32)}                                                   # wgrad_tc3.cu W3_CASE
+W3_CASES = {(64, 64), (32, 32)}                                                   # wgrad_tc.cu W3_CASE
 
 
 def conv_coverage():
