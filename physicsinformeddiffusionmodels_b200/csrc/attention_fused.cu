@@ -22,12 +22,6 @@ namespace pidm {
 
 constexpr int LF_C = 32;                       // channels of xn
 
-__device__ __forceinline__ uint32_t movm_t(uint32_t x) {
-    uint32_t y;
-    asm volatile("movmatrix.sync.aligned.m8n8.trans.b16 %0, %1;" : "=r"(y) : "r"(x));
-    return y;
-}
-
 // B fragments of a 32-row block of the K-major projection weights W[n][c] (bf16): B[k = c][n] = W[n][c]
 __device__ __forceinline__ void load_w_frags(uint32_t (&w)[2][4][2], const __nv_bfloat16* __restrict__ Wrows, int lane) {
     const int g = lane >> 2, t = lane & 3;
@@ -56,44 +50,10 @@ __device__ __forceinline__ void project(float (&c)[MT][4][4], const uint32_t (&a
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) c[mt][nt][i] = 0.f;
+            zero(c[mt][nt]);
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) mma_bf16(c[mt][nt], a[mt][ks], w[ks][nt][0], w[ks][nt][1]);
         }
-}
-// softmax over the 32 columns of the two rows (g, g + 8) a thread shares with its quad, times mul
-__device__ __forceinline__ void frag_softmax(float (&c)[4][4], float mul) {
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-        float mx = -INFINITY;
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) mx = fmaxf(mx, fmaxf(c[nt][half * 2], c[nt][half * 2 + 1]));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        float s = 0.f;
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-            c[nt][half * 2] = __expf(c[nt][half * 2] - mx);
-            c[nt][half * 2 + 1] = __expf(c[nt][half * 2 + 1] - mx);
-            s += c[nt][half * 2] + c[nt][half * 2 + 1];
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        const float inv = mul / s;
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) { c[nt][half * 2] *= inv; c[nt][half * 2 + 1] *= inv; }
-    }
-}
-// accumulator fragment [16 px][32] -> the two A fragments (k16 steps over the 32 columns) of the same matrix
-__device__ __forceinline__ void c_to_a(uint32_t (&a)[2][4], const float (&c)[4][4]) {
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-        a[ks][0] = pack_bf16(c[2 * ks][0], c[2 * ks][1]);
-        a[ks][1] = pack_bf16(c[2 * ks][2], c[2 * ks][3]);
-        a[ks][2] = pack_bf16(c[2 * ks + 1][0], c[2 * ks + 1][1]);
-        a[ks][3] = pack_bf16(c[2 * ks + 1][2], c[2 * ks + 1][3]);
-    }
 }
 // per-thread column constants: column (nt, j) = nt*8 + 2*(lane&3) + j
 __device__ __forceinline__ void load_cols(float (&v)[8], const float* __restrict__ src, int lane) {
@@ -112,28 +72,24 @@ __global__ void __launch_bounds__(256) laf_kmax_kernel(const __nv_bfloat16* __re
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFS_STAGES * LW_TILE);
     const int n_begin = chunk * rows_per_chunk, n_end = min(N, n_begin + rows_per_chunk);
     const int n_tiles = (n_end - n_begin) / 32;
     const __nv_bfloat16* xsrc = xn + ((size_t)b * N + n_begin) * LF_C;
-    auto issue = [&](int it) {
-        if (it < n_tiles) lw_issue<32>(ring + (size_t)(it % LFS_STAGES) * LW_TILE, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
-        cp_commit();
+    const CpRing<LFS_STAGES, LW_TILE> ring{reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFS_STAGES * LW_TILE),
+                                           n_tiles};
+    auto load = [&](__nv_bfloat16* buf, int it) {
+        lw_issue<32>(buf, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
     };
-#pragma unroll
-    for (int s = 0; s < LFS_STAGES; ++s) issue(s);
+    ring.prime(load);
     uint32_t wk[2][4][2];
-    load_w_frags(wk, W + (size_t)(LM_HID + h * LM_D) * LF_C, lane);
+    load_w_frags(wk, W + (size_t)(LM_HID + h * DH) * LF_C, lane);
     float m[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) m[i] = -INFINITY;
     for (int it = 0; it < n_tiles; ++it) {
-        cp_wait<LFS_STAGES - 1>();
-        __syncwarp();
         uint32_t ax[2][2][4];
-        load_x_frags<2>(ax, ring + (size_t)(it % LFS_STAGES) * LW_TILE, lane);
-        __syncwarp();
-        issue(it + LFS_STAGES);
+        load_x_frags<2>(ax, ring.wait(it, load), lane);
+        ring.release(it, load);
         float ck[2][4][4];
         project<2>(ck, ax, wk);
 #pragma unroll
@@ -148,7 +104,7 @@ __global__ void __launch_bounds__(256) laf_kmax_kernel(const __nv_bfloat16* __re
 #pragma unroll
         for (int i = 0; i < 8; ++i) m[i] = fmaxf(m[i], __shfl_xor_sync(0xffffffffu, m[i], off));
     if (lane < 4) {
-        float* o = part + ((size_t)b * gridDim.x + chunk) * LM_HID + h * LM_D;
+        float* o = part + ((size_t)b * gridDim.x + chunk) * LM_HID + h * DH;
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
@@ -163,7 +119,7 @@ __global__ void laf_finalize_kernel(float* __restrict__ ctx, float* __restrict__
     const int row = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (row >= n_rows) return;
     const float zi = 1.f / kzinv[row];
-    ctx[(size_t)row * LM_D + lane] *= zi;
+    ctx[(size_t)row * DH + lane] *= zi;
     __syncwarp();
     if (lane == 0) kzinv[row] = zi;
 }
@@ -177,10 +133,7 @@ constexpr int LFP_WO_TILE = LF_C * LW_PITCH;                        // one head'
 
 // c[16 px][32 e] = dy[16 px][32 c] Wo_h[c][e]   (dy as A fragments)
 __device__ __forceinline__ void lfp_dout_acc(float (&c)[4][4], const uint32_t (&ady)[2][4], const __nv_bfloat16* Wo, int lane) {
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) c[nt][i] = 0.f;
+    zero(c);
 #pragma unroll
     for (int kc = 0; kc < 2; ++kc)
 #pragma unroll
@@ -209,7 +162,7 @@ template <int MODE>
 struct LfcCfg {
     static constexpr int STAGES = MODE == 0 ? 4 : 2;                       // tiles are consumed into registers at once
     static constexpr int STAGE_ELEMS = MODE == 0 ? LW_TILE : 2 * LW_TILE;  // xn tile (| dy tile)
-    static constexpr size_t SMEM_BASE = (size_t)LM_HEADS * STAGES * STAGE_ELEMS * 2 + (size_t)LM_HEADS * 2 * LM_D * 4;
+    static constexpr size_t SMEM_BASE = (size_t)LM_HEADS * STAGES * STAGE_ELEMS * 2 + (size_t)LM_HEADS * 2 * DH * 4;
     static constexpr size_t SMEM = SMEM_BASE + (MODE == 1 ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
 };
 template <int MODE>
@@ -223,38 +176,30 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
     extern __shared__ __align__(16) unsigned char raw[];
     constexpr int LFC_STAGES = LfcCfg<MODE>::STAGES, LFC_STAGE_ELEMS = LfcCfg<MODE>::STAGE_ELEMS;
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFC_STAGES * LFC_STAGE_ELEMS);
-    float* sM = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFC_STAGES * LFC_STAGE_ELEMS * 2) + h * 2 * LM_D;
-    float* sZi = sM + LM_D;
+    float* sM = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFC_STAGES * LFC_STAGE_ELEMS * 2) + h * 2 * DH;
     __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + LfcCfg<MODE>::SMEM_BASE) + h * LFP_WO_TILE;   // MODE 1
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / 32;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
     const __nv_bfloat16* gsrc = (MODE == 1) ? dy + pix0 * LF_C : nullptr;
-    if (MODE == 1) {                               // this head's W_out slice: the oldest copy group
-        lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
-        cp_commit();
-    }
-    auto issue = [&](int it) {
-        if (it < n_tiles) {
-            __nv_bfloat16* buf = ring + (size_t)(it % LFC_STAGES) * LFC_STAGE_ELEMS;
-            lw_issue<32>(buf, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
-            if (MODE == 1) lw_issue<32>(buf + LW_TILE, gsrc + (size_t)it * 32 * LF_C, LF_C, lane);
-        }
-        cp_commit();
+    const CpRing<LFC_STAGES, LFC_STAGE_ELEMS> ring{reinterpret_cast<__nv_bfloat16*>(raw) +
+                                                       (size_t)h * (LFC_STAGES * LFC_STAGE_ELEMS),
+                                                   n_tiles};
+    auto load = [&](__nv_bfloat16* buf, int it) {
+        lw_issue<32>(buf, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
+        if (MODE == 1) lw_issue<32>(buf + LW_TILE, gsrc + (size_t)it * 32 * LF_C, LF_C, lane);
     };
-#pragma unroll
-    for (int s = 0; s < LFC_STAGES; ++s) issue(s);
+    if (MODE == 1) ring.prologue([&] { lw_issue<32>(Wo, w_out + h * DH, LM_HID, lane); });    // this head's W_out slice
+    ring.prime(load);
     uint32_t w0[2][4][2], w1[2][4][2];               // MODE 0: Wk, Wv   MODE 1: Wq, (unused)
-    load_w_frags(w0, W + (size_t)((MODE == 0 ? LM_HID : 0) + h * LM_D) * LF_C, lane);
-    if (MODE == 0) load_w_frags(w1, W + (size_t)(2 * LM_HID + h * LM_D) * LF_C, lane);
+    load_w_frags(w0, W + (size_t)((MODE == 0 ? LM_HID : 0) + h * DH) * LF_C, lane);
+    if (MODE == 0) load_w_frags(w1, W + (size_t)(2 * LM_HID + h * DH) * LF_C, lane);
     float Mc[8];
     float zacc[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) zacc[i] = 0.f;
+    zero(zacc);
     if (MODE == 0) {                               // lane = channel d of this head: combine the per-chunk maxima
-        const int c = h * LM_D + lane;
+        const int c = h * DH + lane;
         float M = -INFINITY;
         for (int i = 0; i < n_stat_chunks; ++i) M = fmaxf(M, part[((size_t)b * n_stat_chunks + i) * LM_HID + c]);
         sM[lane] = M;
@@ -263,16 +208,9 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
         load_cols(Mc, sM, lane);
     }
     float acc[2][4][4];
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int k = 0; k < 4; ++k) acc[i][j][k] = 0.f;
+    zero(acc);
     for (int it = 0; it < n_tiles; ++it) {
-        cp_wait<LFC_STAGES - 1>();
-        __syncwarp();
-        const __nv_bfloat16* buf = ring + (size_t)(it % LFC_STAGES) * LFC_STAGE_ELEMS;
+        const __nv_bfloat16* buf = ring.wait(it, load);
         uint32_t ax[2][2][4];
         load_x_frags<2>(ax, buf, lane);
         uint32_t bv[2][4][2];                         // B fragments [k = px][n = e] per 16-pixel step
@@ -284,15 +222,10 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
                 frag_a_rowmajor(ady[1], buf + LW_TILE, LW_PITCH, mt * 16, 16, lane);
                 float cd[4][4];
                 lfp_dout_acc(cd, ady, Wo, lane);
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    bv[mt][nt][0] = movm_t(pack_bf16(cd[nt][0], cd[nt][1]));
-                    bv[mt][nt][1] = movm_t(pack_bf16(cd[nt][2], cd[nt][3]));
-                }
+                c_to_bt(bv[mt], cd);
             }
         }
-        __syncwarp();                              // the tile is in registers
-        issue(it + LFC_STAGES);
+        ring.release(it, load);                    // the tile is in registers
         float cw[2][4][4];
         project<2>(cw, ax, w0);
         if (MODE == 0) {
@@ -308,12 +241,7 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
             float cv[2][4][4];
             project<2>(cv, ax, w1);
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    bv[mt][nt][0] = movm_t(pack_bf16(cv[mt][nt][0], cv[mt][nt][1]));
-                    bv[mt][nt][1] = movm_t(pack_bf16(cv[mt][nt][2], cv[mt][nt][3]));
-                }
+            for (int mt = 0; mt < 2; ++mt) c_to_bt(bv[mt], cv[mt]);
         } else {
             frag_softmax(cw[0], scale);
             frag_softmax(cw[1], scale);
@@ -324,16 +252,12 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
 #pragma unroll
             for (int md = 0; md < 2; ++md) {       // 16-channel m tile
                 uint32_t a[4];
-                a[0] = movm_t(pack_bf16(cw[mt][2 * md][0], cw[mt][2 * md][1]));
-                a[1] = movm_t(pack_bf16(cw[mt][2 * md + 1][0], cw[mt][2 * md + 1][1]));
-                a[2] = movm_t(pack_bf16(cw[mt][2 * md][2], cw[mt][2 * md][3]));
-                a[3] = movm_t(pack_bf16(cw[mt][2 * md + 1][2], cw[mt][2 * md + 1][3]));
+                c_to_at(a, cw[mt], md);
 #pragma unroll
                 for (int ne = 0; ne < 4; ++ne) mma_bf16(acc[md][ne], a, bv[mt][ne][0], bv[mt][ne][1]);
             }
         }
     }
-    const int g = lane >> 2, t = lane & 3;
     if (MODE == 0) {                               // Z_d = sum_n exp(k[n,d] - M_d): column sums over the 8 row-lanes
 #pragma unroll
         for (int off = 4; off < 32; off <<= 1)
@@ -344,30 +268,19 @@ __global__ void __launch_bounds__(256, 2) laf_ctx_kernel(const __nv_bfloat16* __
             for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
                 for (int j = 0; j < 2; ++j)
-                    atomicAdd(kzinv + (size_t)b * LM_HID + h * LM_D + nt * 8 + 2 * lane + j, zacc[nt * 2 + j]);
+                    atomicAdd(kzinv + (size_t)b * LM_HID + h * DH + nt * 8 + 2 * lane + j, zacc[nt * 2 + j]);
         }
     }
-    float* cb = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
-#pragma unroll
-    for (int md = 0; md < 2; ++md)
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int d = md * 16 + g + half * 8;
-            const float f = (MODE == 0) ? 1.f / (float)N : 1.f;      // MODE 0: 1 / Z_d is applied by laf_finalize_kernel
-#pragma unroll
-            for (int ne = 0; ne < 4; ++ne) {
-                const int e = ne * 8 + 2 * t;
-                atomicAdd(cb + d * LM_D + e, acc[md][ne][half * 2] * f);
-                atomicAdd(cb + d * LM_D + e + 1, acc[md][ne][half * 2 + 1] * f);
-            }
-        }
+    // MODE 0: 1 / Z_d is applied by laf_finalize_kernel
+    ctx_atomic_add(ctx + ((size_t)b * LM_HEADS + h) * DH * DH, acc,
+                   [&](int) { return (MODE == 0) ? 1.f / (float)N : 1.f; }, lane);
 }
 
 // ---- y = x + b + sum_h out_h Wo_h^T,  out[n,h,e] = sum_d softmax_d(q[n,:])[d] * s * ctx[h][d][e],  q projected from xn
 // The warps share one xn ring and step through the tiles together; each leaves its fp32 [32 px][32] partial in shared
 // memory, and after a CTA barrier every thread sums two columns of two rows over the eight heads, adds the bias and the
 // residual and writes y once.
-constexpr int LFO_STAGES = 3;      // 68 KB per CTA; 110 registers: two CTAs per SM
+constexpr int LFO_STAGES = 3;      // 68 KB per CTA; 112 registers: two CTAs per SM
 constexpr int LFO_R_PITCH = LF_C + 8;                              // fp32 partial rows: conflict-free float2 stores
 constexpr size_t LAF_OUT_SMEM = (size_t)LFO_STAGES * LW_TILE * 2 + (size_t)LM_HEADS * LFP_WO_TILE * 2 +
                                 (size_t)LM_HEADS * 32 * LFO_R_PITCH * 4;
@@ -380,40 +293,30 @@ __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __res
     pdl_wait();
     extern __shared__ __align__(16) unsigned char raw[];
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw);
-    __nv_bfloat16* Wo = ring + LFO_STAGES * LW_TILE + h * LFP_WO_TILE;
-    float* R = reinterpret_cast<float*>(ring + LFO_STAGES * LW_TILE + LM_HEADS * LFP_WO_TILE);
+    __nv_bfloat16* tiles = reinterpret_cast<__nv_bfloat16*>(raw);
+    __nv_bfloat16* Wo = tiles + LFO_STAGES * LW_TILE + h * LFP_WO_TILE;
+    float* R = reinterpret_cast<float*>(tiles + LFO_STAGES * LW_TILE + LM_HEADS * LFP_WO_TILE);
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / 32;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
-    lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);   // this head's W_out slice: the oldest copy group
-    cp_commit();
-    auto issue = [&](int it) {
-        if (it < n_tiles && h == 0)
-            lw_issue<32>(ring + (size_t)(it % LFO_STAGES) * LW_TILE, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
-        cp_commit();
+    const CpRing<LFO_STAGES, LW_TILE, true> ring{tiles, n_tiles};
+    auto load = [&](__nv_bfloat16* buf, int it) {
+        if (h == 0) lw_issue<32>(buf, xsrc + (size_t)it * 32 * LF_C, LF_C, lane);
     };
-#pragma unroll
-    for (int s = 0; s < LFO_STAGES - 1; ++s) issue(s);
+    ring.prologue([&] { lw_issue<32>(Wo, w_out + h * DH, LM_HID, lane); });   // this head's W_out slice
+    ring.prime(load);
     uint32_t wq[2][4][2];
-    load_w_frags(wq, W + (size_t)(h * LM_D) * LF_C, lane);
-    const float* ch = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
+    load_w_frags(wq, W + (size_t)(h * DH) * LF_C, lane);
     uint32_t bf[2][4][2];
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) frag_b_global<true>(bf[ks][nt], ch, ks * 16, nt * 8, lane);
+    frags_b_global<true>(bf, ctx + ((size_t)b * LM_HEADS + h) * DH * DH, lane);
     const int g = lane >> 2, t = lane & 3;
     const int rrow = threadIdx.x >> 4, rcol = (threadIdx.x & 15) * 2;     // the y elements this thread sums
     const float2 bias = make_float2(b_out[rcol], b_out[rcol + 1]);
     float* Rw = R + h * 32 * LFO_R_PITCH;
     for (int it = 0; it < n_tiles; ++it) {
         uint32_t ax[2][2][4];
-        cp_wait<LFO_STAGES - 2>();
-        __syncthreads();                           // tile `it` is visible to every warp; slot (it - 1) and R are free
-        issue(it + LFO_STAGES - 1);
-        load_x_frags<2>(ax, ring + (size_t)(it % LFO_STAGES) * LW_TILE, lane);
+        load_x_frags<2>(ax, ring.wait(it, load), lane);  // its CTA barrier also frees R
         __nv_bfloat162 res[2];                     // the residual elements this thread adds, loaded early
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh)
@@ -426,20 +329,14 @@ __global__ void __launch_bounds__(256) laf_out_kernel(const __nv_bfloat16* __res
             uint32_t a[2][4];
             c_to_a(a, cq[mt]);
             float c[4][4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int k = 0; k < 4; ++k) c[i][k] = 0.f;
+            zero(c);
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks)
 #pragma unroll
                 for (int nt = 0; nt < 4; ++nt) mma_bf16(c[nt], a[ks], bf[ks][nt][0], bf[ks][nt][1]);
             c_to_a(a, c);                          // yh[16 px][32 c] = out_h Wo_h^T: B[k = e][n = c] = Wo_h[c][e]
             float yh[4][4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int k = 0; k < 4; ++k) yh[i][k] = 0.f;
+            zero(yh);
 #pragma unroll
             for (int ke = 0; ke < 2; ++ke)
 #pragma unroll
@@ -495,8 +392,7 @@ __device__ __forceinline__ void lfb_dq(float (&dq)[4][4], const LfbTile& tl, con
     frag_softmax(c1[0], 1.f);
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) c2[nt][i] = 0.f;
+        zero(c2[nt]);
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) mma_bf16(c2[nt], tl.ag[ks], bc[ks][nt][0], bc[ks][nt][1]);
     }
@@ -506,8 +402,7 @@ __device__ __forceinline__ void lfb_dq(float (&dq)[4][4], const LfbTile& tl, con
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
             dot += c1[0][nt][half * 2] * c2[nt][half * 2] + c1[0][nt][half * 2 + 1] * c2[nt][half * 2 + 1];
-        dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-        dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+        dot = quad_sum(dot);
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
@@ -525,8 +420,7 @@ __device__ __forceinline__ void lfb_dkdv(float (&dk)[4][4], float (&dv)[4][4], c
     c_to_a(a, c1[0]);
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {               // dk~ N = v dctx^T
-#pragma unroll
-        for (int i = 0; i < 4; ++i) dk[nt][i] = 0.f;
+        zero(dk[nt]);
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) mma_bf16(dk[nt], a[ks], bd[ks][nt][0], bd[ks][nt][1]);
     }
@@ -541,25 +435,17 @@ __device__ __forceinline__ void lfb_dkdv(float (&dk)[4][4], float (&dv)[4][4], c
     c_to_a(a, c1[0]);
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) dv[nt][i] = 0.f;
+        zero(dv[nt]);
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) mma_bf16(dv[nt], a[ks], bt[ks][nt][0], bt[ks][nt][1]);
 #pragma unroll
         for (int i = 0; i < 4; ++i) dv[nt][i] *= invN;
     }
 }
-// loop-invariant per-head operands: cd (through a 32-float shared scratch), column statistics, B fragments of ctx / dctx
+// cd as per-thread column constants, through a 32-float shared scratch
 __device__ __forceinline__ void lfb_cd(float (&cdc)[8], float* scd, const float* __restrict__ cg, const float* __restrict__ dg,
                                        int lane) {
-    float s = 0.f;                     // cd[d] = sum_e dctx[d][e] ctx[d][e]   (lane = d)
-#pragma unroll
-    for (int e = 0; e < LM_D; e += 4) {
-        const float4 x = *reinterpret_cast<const float4*>(dg + lane * LM_D + e);
-        const float4 y = *reinterpret_cast<const float4*>(cg + lane * LM_D + e);
-        s += x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
-    }
-    scd[lane] = s;
+    scd[lane] = ctx_dot_row(cg, dg, lane);
     __syncwarp();
     load_cols(cdc, scd, lane);
 }
@@ -575,7 +461,7 @@ constexpr int LFB_R_PITCH = LF_C + 8;                              // fp32 parti
 struct LfbCfg {
     static constexpr int STAGE_ELEMS = 2 * LFB_TILE;                            // xn tile | dy tile
     static constexpr size_t SMEM_BASE = (size_t)LFB_STAGES * STAGE_ELEMS * 2 + (size_t)3 * LM_HID * LFB_W_PITCH * 2 +
-                                        (size_t)LM_HEADS * LFB_ROWS * LFB_R_PITCH * 4 + (size_t)LM_HEADS * LM_D * 4;
+                                        (size_t)LM_HEADS * LFB_ROWS * LFB_R_PITCH * 4 + (size_t)LM_HEADS * DH * 4;
     static constexpr size_t SMEM = SMEM_BASE + (size_t)LM_HEADS * LFP_WO_TILE * 2;
 };
 
@@ -602,69 +488,55 @@ __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __res
     extern __shared__ __align__(16) unsigned char raw[];
     constexpr int LFB_STAGE_ELEMS = LfbCfg::STAGE_ELEMS;
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw);
-    __nv_bfloat16* Ws = ring + LFB_STAGES * LFB_STAGE_ELEMS;
+    __nv_bfloat16* tiles = reinterpret_cast<__nv_bfloat16*>(raw);
+    __nv_bfloat16* Ws = tiles + LFB_STAGES * LFB_STAGE_ELEMS;
     __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + LfbCfg::SMEM_BASE) + h * LFP_WO_TILE;
     float* R = reinterpret_cast<float*>(Ws + 3 * LM_HID * LFB_W_PITCH);
-    float* scd = R + LM_HEADS * LFB_ROWS * LFB_R_PITCH + h * LM_D;
+    float* scd = R + LM_HEADS * LFB_ROWS * LFB_R_PITCH + h * DH;
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / LFB_ROWS;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
     const __nv_bfloat16* gsrc = dy + pix0 * LF_C;
-    for (int i = threadIdx.x; i < 3 * LM_HID * (LF_C / 8); i += blockDim.x)      // W -> smem: the oldest copy group
-        cp_async16(Ws + (i >> 2) * LFB_W_PITCH + (i & 3) * 8, W + (size_t)(i >> 2) * LF_C + (i & 3) * 8);
-    lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
-    cp_commit();
-    auto issue = [&](int it) {
-        if (it < n_tiles) {
-            __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * LFB_STAGE_ELEMS;
-            if (h == 0) lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-            if (h == 1) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-        }
-        cp_commit();
+    const CpRing<LFB_STAGES, LFB_STAGE_ELEMS, true> ring{tiles, n_tiles};
+    auto load = [&](__nv_bfloat16* buf, int it) {
+        if (h == 0) lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
+        if (h == 1) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
     };
-#pragma unroll
-    for (int s = 0; s < LFB_STAGES - 1; ++s) issue(s);
-    const float* cg = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
-    const float* dg = dctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
+    ring.prologue([&] {                            // W and this head's W_out slice
+        for (int i = threadIdx.x; i < 3 * LM_HID * (LF_C / 8); i += blockDim.x)
+            cp_async16(Ws + (i >> 2) * LFB_W_PITCH + (i & 3) * 8, W + (size_t)(i >> 2) * LF_C + (i & 3) * 8);
+        lw_issue<32>(Wo, w_out + h * DH, LM_HID, lane);
+    });
+    ring.prime(load);
+    const float* cg = ctx + ((size_t)b * LM_HEADS + h) * DH * DH;
+    const float* dg = dctx + ((size_t)b * LM_HEADS + h) * DH * DH;
     float Mc[8], Zc[8], cdc[8];
     lfb_cd(cdc, scd, cg, dg, lane);
-    load_cols(Mc, kmax + (size_t)b * LM_HID + h * LM_D, lane);
-    load_cols(Zc, kzinv + (size_t)b * LM_HID + h * LM_D, lane);
+    load_cols(Mc, kmax + (size_t)b * LM_HID + h * DH, lane);
+    load_cols(Zc, kzinv + (size_t)b * LM_HID + h * DH, lane);
     uint32_t wq[2][4][2], wk[2][4][2], wv[2][4][2];
-    load_w_frags(wq, W + (size_t)(h * LM_D) * LF_C, lane);
-    load_w_frags(wk, W + (size_t)(LM_HID + h * LM_D) * LF_C, lane);
-    load_w_frags(wv, W + (size_t)(2 * LM_HID + h * LM_D) * LF_C, lane);
+    load_w_frags(wq, W + (size_t)(h * DH) * LF_C, lane);
+    load_w_frags(wk, W + (size_t)(LM_HID + h * DH) * LF_C, lane);
+    load_w_frags(wv, W + (size_t)(2 * LM_HID + h * DH) * LF_C, lane);
     uint32_t bc[2][4][2], bd[2][4][2], bt[2][4][2];
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-            frag_b_global<false>(bc[ks][nt], cg, ks * 16, nt * 8, lane);      // B[k=e][n=d] = ctx[d][e]
-            frag_b_global<false>(bd[ks][nt], dg, ks * 16, nt * 8, lane);      // B[k=e][n=d] = dctx[d][e]
-            frag_b_global<true>(bt[ks][nt], dg, ks * 16, nt * 8, lane);       // B[k=d][n=e] = dctx[d][e]
-        }
+    frags_b_global<false>(bc, cg, lane);           // B[k=e][n=d] = ctx[d][e]
+    frags_b_global<false>(bd, dg, lane);           // B[k=e][n=d] = dctx[d][e]
+    frags_b_global<true>(bt, dg, lane);            // B[k=d][n=e] = dctx[d][e]
     const int g = lane >> 2, t = lane & 3;
     const float invN = 1.f / (float)N;
-    const __nv_bfloat16* Wq = Ws + (size_t)(h * LM_D) * LFB_W_PITCH;
+    const __nv_bfloat16* Wq = Ws + (size_t)(h * DH) * LFB_W_PITCH;
     const __nv_bfloat16* Wk = Wq + (size_t)LM_HID * LFB_W_PITCH;
     const __nv_bfloat16* Wv = Wk + (size_t)LM_HID * LFB_W_PITCH;
     float* Rw = R + h * LFB_ROWS * LFB_R_PITCH;
     const int rrow = threadIdx.x >> 4, rcol = (threadIdx.x & 15) * 2;     // the two dxn elements this thread sums
     for (int it = 0; it < n_tiles; ++it) {
-        cp_wait<LFB_STAGES - 2>();
-        __syncthreads();                           // tile `it` is visible to every warp; slot (it - 1) is free
-        issue(it + LFB_STAGES - 1);
-        const __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * LFB_STAGE_ELEMS;
+        const __nv_bfloat16* buf = ring.wait(it, load);  // its CTA barrier also frees R
         LfbTile tl;
         load_x_frags<1>(tl.ax, buf, lane);
         lfp_dout(tl.ag, buf + LFB_TILE, Wo, lane);
         float dx[4][4];
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) dx[nt][i] = 0.f;
+        zero(dx);
         uint32_t a[2][4];
         {
             float dq[4][4];
@@ -707,9 +579,9 @@ __global__ void __launch_bounds__(256) laf_bwd_kernel(const __nv_bfloat16* __res
 template <int PART>
 struct LfwCfg {
     static constexpr int STAGE_ELEMS = (PART == 0 ? 2 : 1) * LFB_TILE;     // xn tile (| dy tile)
-    static constexpr int S_PITCH = LM_D + 1;                                 // epilogue staging [32 d][33] fp32
-    static_assert(LFB_STAGES * STAGE_ELEMS * 2 >= LM_D * S_PITCH * 4, "the epilogue staging reuses the tile ring");
-    static constexpr size_t SMEM_BASE = (size_t)LM_HEADS * (LFB_STAGES * STAGE_ELEMS * 2 + LM_D * 4);
+    static constexpr int S_PITCH = DH + 1;                                 // epilogue staging [32 d][33] fp32
+    static_assert(LFB_STAGES * STAGE_ELEMS * 2 >= DH * S_PITCH * 4, "the epilogue staging reuses the tile ring");
+    static constexpr size_t SMEM_BASE = (size_t)LM_HEADS * (LFB_STAGES * STAGE_ELEMS * 2 + DH * 4);
     static constexpr size_t SMEM = SMEM_BASE + (PART == 0 ? (size_t)LM_HEADS * LFP_WO_TILE * 2 : 0);
 };
 
@@ -719,10 +591,7 @@ __device__ __forceinline__ void acc_gtx(float (&acc)[2][4][4], const float (&gf)
 #pragma unroll
     for (int md = 0; md < 2; ++md) {               // A[d][px]: transposed 8x8 blocks of the accumulator fragment
         uint32_t a[4];
-        a[0] = movm_t(pack_bf16(gf[2 * md][0], gf[2 * md][1]));
-        a[1] = movm_t(pack_bf16(gf[2 * md + 1][0], gf[2 * md + 1][1]));
-        a[2] = movm_t(pack_bf16(gf[2 * md][2], gf[2 * md][3]));
-        a[3] = movm_t(pack_bf16(gf[2 * md + 1][2], gf[2 * md + 1][3]));
+        c_to_at(a, gf, md);
 #pragma unroll
         for (int np = 0; np < 2; ++np) {
             mma_bf16(acc[md][2 * np], a, bx[np][0], bx[np][1]);
@@ -745,63 +614,43 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
     using Cfg = LfwCfg<PART>;
     constexpr int STAGE_ELEMS = Cfg::STAGE_ELEMS, S_PITCH = Cfg::S_PITCH;
     const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, h = threadIdx.x >> 5;
-    __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(raw) + (size_t)h * (LFB_STAGES * STAGE_ELEMS);
-    float* scd = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFB_STAGES * STAGE_ELEMS * 2) + h * LM_D;
+    float* scd = reinterpret_cast<float*>(raw + (size_t)LM_HEADS * LFB_STAGES * STAGE_ELEMS * 2) + h * DH;
     __nv_bfloat16* Wo = reinterpret_cast<__nv_bfloat16*>(raw + Cfg::SMEM_BASE) + h * LFP_WO_TILE;        // PART 0
     const int n_begin = chunk * chunk_px, n_end = min(N, n_begin + chunk_px);
     const int n_tiles = (n_end - n_begin) / LFB_ROWS;
     const size_t pix0 = (size_t)b * N + n_begin;
     const __nv_bfloat16* xsrc = xn + pix0 * LF_C;
     const __nv_bfloat16* gsrc = dy + pix0 * LF_C;
-    if (PART == 0) {                               // this head's W_out slice: the oldest copy group
-        lw_issue<32>(Wo, w_out + h * LM_D, LM_HID, lane);
-        cp_commit();
-    }
-    auto issue = [&](int it) {
-        if (it < n_tiles) {
-            __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * STAGE_ELEMS;
-            lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-            if (PART == 0) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
-        }
-        cp_commit();
+    const CpRing<LFB_STAGES, STAGE_ELEMS> ring{reinterpret_cast<__nv_bfloat16*>(raw) +
+                                                   (size_t)h * (LFB_STAGES * STAGE_ELEMS),
+                                               n_tiles};
+    auto load = [&](__nv_bfloat16* buf, int it) {
+        lw_issue<LFB_ROWS>(buf, xsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
+        if (PART == 0) lw_issue<LFB_ROWS>(buf + LFB_TILE, gsrc + (size_t)it * LFB_ROWS * LF_C, LF_C, lane);
     };
-#pragma unroll
-    for (int s = 0; s < LFB_STAGES; ++s) issue(s);
-    const float* cg = ctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
-    const float* dg = dctx + ((size_t)b * LM_HEADS + h) * LM_D * LM_D;
+    if (PART == 0) ring.prologue([&] { lw_issue<32>(Wo, w_out + h * DH, LM_HID, lane); });   // this head's W_out slice
+    ring.prime(load);
+    const float* cg = ctx + ((size_t)b * LM_HEADS + h) * DH * DH;
+    const float* dg = dctx + ((size_t)b * LM_HEADS + h) * DH * DH;
     float Mc[8], Zc[8], cdc[8];
     uint32_t w0[2][4][2], w1[2][4][2];             // PART 0: Wq, (unused)   PART 1: Wk, Wv
     uint32_t b0[2][4][2], b1[2][4][2];             // PART 0: ctx^T, ctx   PART 1: dctx^T, dctx
     if (PART == 0) {
-        load_w_frags(w0, W + (size_t)(h * LM_D) * LF_C, lane);
+        load_w_frags(w0, W + (size_t)(h * DH) * LF_C, lane);
     } else {
         lfb_cd(cdc, scd, cg, dg, lane);
-        load_cols(Mc, kmax + (size_t)b * LM_HID + h * LM_D, lane);
-        load_cols(Zc, kzinv + (size_t)b * LM_HID + h * LM_D, lane);
-        load_w_frags(w0, W + (size_t)(LM_HID + h * LM_D) * LF_C, lane);
-        load_w_frags(w1, W + (size_t)(2 * LM_HID + h * LM_D) * LF_C, lane);
+        load_cols(Mc, kmax + (size_t)b * LM_HID + h * DH, lane);
+        load_cols(Zc, kzinv + (size_t)b * LM_HID + h * DH, lane);
+        load_w_frags(w0, W + (size_t)(LM_HID + h * DH) * LF_C, lane);
+        load_w_frags(w1, W + (size_t)(2 * LM_HID + h * DH) * LF_C, lane);
     }
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-            frag_b_global<false>(b0[ks][nt], PART == 0 ? cg : dg, ks * 16, nt * 8, lane);
-            frag_b_global<true>(b1[ks][nt], PART == 1 ? dg : cg, ks * 16, nt * 8, lane);
-        }
+    frags_b_global<false>(b0, PART == 0 ? cg : dg, lane);
+    frags_b_global<true>(b1, PART == 1 ? dg : cg, lane);
     const float invN = 1.f / (float)N;
     float acc[2][2][4][4];
-#pragma unroll
-    for (int m = 0; m < 2; ++m)
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-#pragma unroll
-                for (int k = 0; k < 4; ++k) acc[m][i][j][k] = 0.f;
+    zero(acc);
     for (int it = 0; it < n_tiles; ++it) {
-        cp_wait<LFB_STAGES - 1>();
-        __syncwarp();
-        const __nv_bfloat16* buf = ring + (size_t)(it % LFB_STAGES) * STAGE_ELEMS;
+        const __nv_bfloat16* buf = ring.wait(it, load);
         LfbTile tl;
         load_x_frags<1>(tl.ax, buf, lane);
         uint32_t bx[2][4];
@@ -814,8 +663,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
             frag_b_krows(bdy[0], buf + LFB_TILE, LW_PITCH, 0, 0, lane);
             frag_b_krows(bdy[1], buf + LFB_TILE, LW_PITCH, 0, 16, lane);
         }
-        __syncwarp();                              // the tile is in registers
-        issue(it + LFB_STAGES);
+        ring.release(it, load);                    // the tile is in registers
         if (PART == 0) {
             {
                 float c[4][4];
@@ -833,8 +681,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
             c_to_a(a, cq[0]);
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) o[nt][i] = 0.f;
+                zero(o[nt]);
 #pragma unroll
                 for (int ks = 0; ks < 2; ++ks) mma_bf16(o[nt], a[ks], b1[ks][nt][0], b1[ks][nt][1]);
             }
@@ -846,9 +693,7 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
             acc_gtx(acc[1], dv, bx);
         }
     }
-    cp_wait<0>();
-    __syncwarp();                                  // the ring is free: stage the sums there
-    float* S = reinterpret_cast<float*>(ring);
+    float* S = reinterpret_cast<float*>(ring.drain());     // the ring is free: stage the sums there
     const int g = lane >> 2, t = lane & 3;
 #pragma unroll
     for (int m = 0; m < 2; ++m) {
@@ -860,14 +705,14 @@ __global__ void __launch_bounds__(256) laf_wgrad_kernel(const __nv_bfloat16* __r
                 for (int i = 0; i < 4; ++i) S[(md * 16 + g + 8 * (i >> 1)) * S_PITCH + nc * 8 + 2 * t + (i & 1)] = acc[m][md][nc][i];
         __syncwarp();
         if (PART == 0 && m == 1) {                    // S[e][c] = dW_out[c][32h + e]: lane = e, one row c at a time
-            float* dst = grad_wo + (long long)(h * LM_D + lane) * wo_stride_c;
+            float* dst = grad_wo + (long long)(h * DH + lane) * wo_stride_c;
 #pragma unroll 4
             for (int c = 0; c < LF_C; ++c) atomicAdd(dst + c * wo_stride_n, S[lane * S_PITCH + c]);
         } else {
             // rows of dW: to_qkv output channel (q | k | v block) * 256 + h * 32 + d;  lane = input channel c
-            float* dst = grad_w + (long long)((PART + m) * LM_HID + h * LM_D) * w_stride_n + lane * w_stride_c;
+            float* dst = grad_w + (long long)((PART + m) * LM_HID + h * DH) * w_stride_n + lane * w_stride_c;
 #pragma unroll 4
-            for (int d = 0; d < LM_D; ++d) atomicAdd(dst + d * w_stride_n, S[d * S_PITCH + lane]);
+            for (int d = 0; d < DH; ++d) atomicAdd(dst + d * w_stride_n, S[d * S_PITCH + lane]);
         }
         __syncwarp();
     }
@@ -906,10 +751,9 @@ extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const v
     PIDM_REQUIRE(w_out && b_out && residual, "linattn_block_fwd: w_out, b_out and residual are required");
     PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
-    const float scale = 0.17677669529663687f;   // 32^-0.5
     const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
     const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
-    PIDM_CUDA(cudaMemsetAsync(ctx, 0, (size_t)B * LM_HEADS * LM_D * LM_D * sizeof(float), st));
+    PIDM_CUDA(cudaMemsetAsync(ctx, 0, (size_t)B * LM_HEADS * DH * DH * sizeof(float), st));
     PIDM_CUDA(cudaMemsetAsync(kzinv, 0, (size_t)B * LM_HID * sizeof(float), st));
     const int chunks = laf_stat_chunks(N);
     const int rpc = N / chunks;
@@ -920,11 +764,11 @@ extern "C" int pidm_linattn_block_fwd(const void* xn, const void* w_qkv, const v
     const dim3 grid((N + px - 1) / px, B);
     PIDM_CUDA(allow_smem(laf_ctx_kernel<0>, LfcCfg<0>::SMEM));
     PIDM_CUDA(launch_plain(laf_ctx_kernel<0>, grid, dim3(256), LfcCfg<0>::SMEM, st, x, w, nullptr, workspace, chunks, kmax, kzinv,
-                           ctx, N, px, scale, nullptr));
+                           ctx, N, px, ATTN_SCALE, nullptr));
     PIDM_CUDA(launch_plain(laf_finalize_kernel, dim3((B * LM_HID + 7) / 8), dim3(256), (size_t)(0), st, ctx, kzinv, B * LM_HID));
     PIDM_CUDA(allow_smem(laf_out_kernel, LAF_OUT_SMEM));
-    PIDM_CUDA(launch_plain(laf_out_kernel, grid, dim3(256), LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)y, N, px, scale,
-                           (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
+    PIDM_CUDA(launch_plain(laf_out_kernel, grid, dim3(256), LAF_OUT_SMEM, st, x, w, ctx, (__nv_bfloat16*)y, N, px,
+                           ATTN_SCALE, (const __nv_bfloat16*)w_out, b_out, (const __nv_bfloat16*)residual));
     PIDM_LAUNCH_CHECK("linattn_block_fwd");
     return 0;
 }
@@ -934,20 +778,19 @@ extern "C" int pidm_linattn_block_bwd(const void* xn, const void* w_qkv, const v
                                       void* stream) {
     PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
-    const float scale = 0.17677669529663687f;
     const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
     const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
     const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
     const __nv_bfloat16* g = (const __nv_bfloat16*)dy;
-    PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * LM_HEADS * LM_D * LM_D * sizeof(float), st));
+    PIDM_CUDA(cudaMemsetAsync(dctx, 0, (size_t)B * LM_HEADS * DH * DH * sizeof(float), st));
     const int cpx = chunk_px(B, N, 2);
     PIDM_CUDA(allow_smem(laf_ctx_kernel<1>, LfcCfg<1>::SMEM));
     PIDM_CUDA(launch_plain(laf_ctx_kernel<1>, dim3(dim3((N + cpx - 1) / cpx, B)), dim3(256), LfcCfg<1>::SMEM, st, x, w, g,
-                           nullptr, 0, nullptr, nullptr, dctx, N, cpx, scale, wo));
+                           nullptr, 0, nullptr, nullptr, dctx, N, cpx, ATTN_SCALE, wo));
     const int bpx = chunk_px(B, N, 1);
     PIDM_CUDA(allow_smem(laf_bwd_kernel, LfbCfg::SMEM));
     PIDM_CUDA(launch_plain(laf_bwd_kernel, dim3(dim3((N + bpx - 1) / bpx, B)), dim3(256), LfbCfg::SMEM, st, x, w, g, ctx, dctx,
-                           kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, scale, wo));
+                           kmax, kzinv, (__nv_bfloat16*)dxn, N, bpx, ATTN_SCALE, wo));
     PIDM_LAUNCH_CHECK("linattn_block_bwd");
     return 0;
 }
@@ -959,7 +802,6 @@ extern "C" int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const
                                         void* stream) {
     PIDM_REQUIRE(N % 128 == 0, "linattn_block: N must be a multiple of 128 (got %d)", N);
     cudaStream_t st = (cudaStream_t)stream;
-    const float scale = 0.17677669529663687f;
     const __nv_bfloat16* x = (const __nv_bfloat16*)xn;
     const __nv_bfloat16* w = (const __nv_bfloat16*)w_qkv;
     const __nv_bfloat16* wo = (const __nv_bfloat16*)w_out;
@@ -968,10 +810,10 @@ extern "C" int pidm_linattn_block_wgrad(const void* xn, const void* w_qkv, const
     const dim3 grid((N + px - 1) / px, B);
     PIDM_CUDA(allow_smem(laf_wgrad_kernel<0>, LfwCfg<0>::SMEM));
     PIDM_CUDA(launch_plain(laf_wgrad_kernel<0>, grid, dim3(256), LfwCfg<0>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
-                           N, px, qkv_stride_n, qkv_stride_c, scale, wo, grad_w_out, out_stride_n, out_stride_c));
+                           N, px, qkv_stride_n, qkv_stride_c, ATTN_SCALE, wo, grad_w_out, out_stride_n, out_stride_c));
     PIDM_CUDA(allow_smem(laf_wgrad_kernel<1>, LfwCfg<1>::SMEM));
     PIDM_CUDA(launch_plain(laf_wgrad_kernel<1>, grid, dim3(256), LfwCfg<1>::SMEM, st, x, w, g, ctx, dctx, kmax, kzinv, grad_w_qkv,
-                           N, px, qkv_stride_n, qkv_stride_c, scale, nullptr, nullptr, 0LL, 0LL));
+                           N, px, qkv_stride_n, qkv_stride_c, ATTN_SCALE, nullptr, nullptr, 0LL, 0LL));
     PIDM_LAUNCH_CHECK("linattn_block_wgrad");
     return 0;
 }

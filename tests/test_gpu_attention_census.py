@@ -1,6 +1,6 @@
 """Every standalone linear-attention, mid softmax-attention and output-head launch of the benchmarked steps, and every
-launch plan of attention.cu / attention_mma.cu / attention_small.cu / attention_mid.cu and the head kernels, replayed
-element by element against an fp64 reference.
+launch plan of attention.cu / attention_mid.cu and the head kernels, replayed element by element against an fp64
+reference.
 
 pidm_linattn_fwd takes one of three forward paths (one CTA per (sample, head) for bf16 at 32 <= N <= 64, mma.sync for
 bf16 with 8 heads and N % 64 == 0, SIMT statistics -> context -> output otherwise) and one of two backward paths, and
